@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """
-bench.py -- nn-classification throughput (6 kb windows/s) on N B200s, next to the reference's CPU path.
+bench.py -- nn-classification throughput (6 kb windows/s) on N H100s, next to the reference's CPU path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {1,2,3,4,5}] [--batch B] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {1,2,3,4,5}] [--batch B] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -20,14 +20,18 @@ Prints ONE JSON line (rank 0).  BASELINE.json's configs:
   --config 5            batch sweep 256 ... 4096 with per-kernel HBM / tensor-pipe roofline fractions.
 
   value    : windows/s with inputs already resident in HBM (CUDA events on the launching stream, max over ranks), after
-             >= 1.5 s of warm-up so the clock has settled under the 1 kW power cap (the burst figure is reported next to it)
+             >= 1.5 s of warm-up so the clock has settled under the card's power cap (the burst figure is reported next to it)
   e2e      : the same metric through the host-buffer C-ABI call gnm_classify_host (pinned host buffers, H2D of every
              step's windows and D2H of its probabilities inside the timed region)
-  roofline : the dominant kernel (tcgen05 Conv1D, conv_t_kernel<false>) against the measured bf16 tensor peak
+  roofline : the dominant kernel (wgmma Conv1D, conv_t_kernel<false>) against the bf16 tensor peak
   cpu_baseline : the oracle's op-for-op restatement of the Keras graph timed on this box's host cores
 
 --impl reference times that CPU restatement (the reference's own implementation is TensorFlow, which cannot be installed
 here -- see DESIGN.md) with all host threads, on bounded 128-window steps.
+
+--dump-outputs DIR (configs 2 / 3) writes what the last timed step returned to its caller, the [batch, 3] per-window class
+probabilities of rank 0, as DIR/probs.npy (float32).  The inputs are a fixed function of the arguments (seeded stream), so two
+builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -62,7 +66,7 @@ def load_peaks():
         d = json.loads(p.read_text())
         return dict(tflops=float(d.get("bf16_tflops_sustained") or d["bf16_tflops"]), tflops_burst=float(d["bf16_tflops"]),
                     hbm_gbs=float(d["hbm_gbs"]), source="measured (MEASURED_PEAKS.json, bf16_tflops_sustained)")
-    return dict(tflops=1400.0, tflops_burst=1590.0, hbm_gbs=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, tflops_burst=989.0, hbm_gbs=3350.0, source="NVIDIA H100 SXM data sheet (dense bf16, 700 W card), not measured")
 
 
 class ClockSampler:
@@ -314,6 +318,8 @@ def main():
     ap.add_argument("--cpu-windows", type=int, default=512, help="--impl reference: windows per step before the time budget shrinks it")
     ap.add_argument("--no-module", action="store_true", help="skip the module_e2e / config4 extras of the default line")
     ap.add_argument("--module-windows", type=int, default=100_000, help="size of the large module_e2e FASTA (windows)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's per-window probabilities to DIR/probs.npy (configs 2 and 3)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -477,6 +483,11 @@ def main():
         sampler.start()
     total_ms = timed(run_device, use_events=True, tail=exchange)
     launches = per_step * K                                        # our kernels inside the K timed steps
+    if args.dump_outputs and rank == 0 and K > 0:
+        last = ((K - 1) % POOL) * B                                # the last timed step's windows: pool[last:last + B]
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / "probs.npy", probs[last:last + B].float().cpu().numpy())
     clocks = sampler.stop() if rank == 0 else None
 
     # per-stage CUDA events over K more steps of the same workload (same stream)
@@ -518,12 +529,6 @@ def main():
         dom_ms = stage_ms.get(dom)
         dom_flop = B * FLOP_CONV
         achieved = dom_flop / (dom_ms * 1e-3) / 1e12 if dom_ms else None
-        traffic, traffic_src = None, None
-        tp = ROOT / "profiles" / "ncu_traffic.json"
-        if tp.exists() and B == 1024:
-            tj = json.loads(tp.read_text())
-            traffic = tj.get("conv2_dram_bytes_per_launch_batch1024")
-            traffic_src = "static: " + tj.get("source", "ncu --set full capture, profiles/ncu_traffic.json") + " (not measured in this run)"
 
         def hbm(key, gbytes, extra=None):
             t = stage_ms.get(key)
@@ -536,7 +541,7 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": total_ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "split operands on tcgen05 (conv: fp16 main pass + two e4m3 correction passes; w_v: 3 fp16 passes), fp32 accumulate; "
+            "dtype": "split operands on wgmma (conv: fp16 main pass + two e4m3 correction passes; w_v: 3 fp16 passes), fp32 accumulate; "
                      "fp32-equivalent (<=1e-4 vs the fp32 oracle, measured ~1e-5)", "data": "synthetic",
             "config": {"workload": (f"BASELINE configs[{args.config - 1}]: {total_windows:,} x 6 kb windows (counter-based stream, seed 1), "
                                     f"batch {B} per GPU, IGLOO1D inference; timed: {K} steps of {B} windows per GPU, issued as API calls of "
@@ -546,7 +551,7 @@ def main():
                                         "before the timed region: `value` is the power-capped steady state",
                        "value_burst": burst, "ms_per_step_burst": burst_ms / K,
                        "l2": "inputs rotate through a 4-batch pool; per-step activation working set "
-                             f"{B * 5997 * 512 * 2 / 1e9:.1f} GB >> 126 MB L2 (no explicit flush needed)",
+                             f"{B * 5997 * 512 * 2 / 1e9:.1f} GB >> 50 MB L2 (no explicit flush needed)",
                        "parallelism": (f"window-sharded x{world}; ONE all_gather of the [windows,3] results per run, inside the timed "
                                        "region (as the module does)") if world > 1 else "single GPU"},
             "e2e": {"value": e2e, "unit": UNIT, "h2d_bytes_per_step": B * 6000, "d2h_bytes_per_step": B * 12,
@@ -555,7 +560,7 @@ def main():
             "clocks": clocks,
             "roofline": {"bound": "tensor", "kernel": "conv_t_kernel<false> (causal Conv1D 128->128 k=6 + LeakyReLU, layer conv2; conv3 is the same kernel)",
                          "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s",
-                         "frac": (achieved / peaks["tflops"]) if achieved else None, "traffic": traffic, "traffic_source": traffic_src,
+                         "frac": (achieved / peaks["tflops"]) if achieved else None,
                          "peak_source": peaks["source"], "launch_ms": dom_ms,
                          "algorithmic_flop_per_launch": dom_flop,
                          "tensor_pass_units": 2.0,

@@ -1,5 +1,5 @@
 """
-genomad_b200 -- B200-native (sm_100a) implementation of geNomad's ``nn-classification`` hot path.
+genomad_b200 -- H100-native (sm_90a) implementation of geNomad's ``nn-classification`` hot path.
 
 Public surface (mirrors the reference's for this path only):
   genomad_b200.nn_classification.main(input_path, output_path, single_window, batch_size, restart,

@@ -1,10 +1,10 @@
 """
-Build libgnm.so (the sm_100a kernels + C ABI) in-tree with nvcc.
+Build libgnm.so (the sm_90a kernels + C ABI) in-tree with nvcc.
 
     python -m genomad_b200.build [--force]
 
-nvcc cross-compiles for sm_100a without a GPU, so this runs in the build container; the resulting
-genomad_b200/libgnm.so is git-ignored but travels to the GPU box with the repository snapshot.
+nvcc cross-compiles for sm_90a without a GPU, so this runs on a machine without one; the resulting
+genomad_b200/libgnm.so is git-ignored and rebuilt whenever a source is newer.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ SOURCES = [CSRC / "api.cu", CSRC / "fasta.cpp", CSRC / "tfrecord.cpp"]
 HEADERS = sorted(CSRC.glob("*.cuh")) + [PKG.parent / "include" / "gnm.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",

@@ -20,9 +20,9 @@ CONTEXT_SETTINGS = dict(help_option_names=["-h", "--help"])
 
 
 @click.group(context_settings=CONTEXT_SETTINGS)
-@click.version_option(version=__version__, prog_name="geNomad-B200")
+@click.version_option(version=__version__, prog_name="geNomad-H100")
 def cli():
-    """geNomad nn-classification on NVIDIA B200."""
+    """geNomad nn-classification on NVIDIA H100."""
 
 
 @cli.command(name="nn-classification", context_settings=CONTEXT_SETTINGS)

@@ -1,5 +1,5 @@
 // fp32 CUDA-core versions of the conv / w_v stages.  These are VALIDATION kernels: they exist so
-// the tcgen05 path (conv_t.cuh) can be checked on the GPU against an independent, obviously
+// the tensor-core path (conv_t.cuh) can be checked on the GPU against an independent, obviously
 // correct implementation at batch sizes the CPU oracle cannot reach (option "conv_impl" = 1).
 // They are not a fallback: the product path never selects them on its own.
 //

@@ -1,5 +1,5 @@
 // K2/K3: causal Conv1D(128->128, k=6) + LeakyReLU, and the IGLOO value projection (y @ w_v, MaxPool1D(8)),
-// as ONE persistent tcgen05 kernel template (conv_t_kernel<false> / conv_t_kernel<true>).
+// as ONE persistent wgmma kernel template (conv_t_kernel<false> / conv_t_kernel<true>).
 //
 // Reference semantics:
 //   Conv1D x2 + LeakyReLU(0.1)      genomad/neural_network/igloo.py:64-72
@@ -9,12 +9,11 @@
 //
 // Arithmetic: fp32-equivalent split.  Every operand x is carried as hi = fp16(x) plus a correction
 // lo = x - hi, and A*B is evaluated on the tensor cores as Ahi*Bhi + Alo*Bhi + Ahi*Blo with fp32
-// accumulation in ONE TMEM accumulator (the dropped Alo*Blo term is ~2^-22).  tools/precision_study.py
-// (profiles/r01_precision_study.md) shows why a single TF32/fp16 pass is not enough for the 1e-4 parity
-// bar (1.4e-4 worst case for the convs, 7e-4 for w_v).
-//   * w_v (feeds max-pool -> mean -> BatchNorm with a 31x gain): all three passes in fp16 (kind::f16), ~7e-6.
+// accumulation in ONE accumulator (the dropped Alo*Blo term is ~2^-22).  tools/precision_study.py
+// shows why a single TF32/fp16 pass is not enough for the 1e-4 parity bar (1.4e-4 worst case for the convs, 7e-4 for w_v).
+//   * w_v (feeds max-pool -> mean -> BatchNorm with a 31x gain): all three passes in fp16, ~7e-6.
 //   * convs: the main pass Ahi*Bhi in fp16; the two correction passes only need ~8 bits, so they run in
-//     e4m3 (kind::f8f6f4, K = 32 per instruction: twice the rate) on pre-scaled operands.  All passes are
+//     e4m3 (K = 32 per instruction: twice the rate) on pre-scaled operands.  All passes are
 //     scaled to a common 2^S so they add up in the same accumulator, and the epilogue multiplies by 2^-S:
 //         main  : (32*Ahi)            x fp16(Whi * 2^d)          S = 5 + d          (d = 16 for |W| < 0.78)
 //         corr1 : e4m3(Alo * 2^12)    x e4m3(Whi * 2^(S-12))
@@ -26,50 +25,33 @@
 // are four slab REGIONS of 272 rows x 128 bytes (conv: hi16 ch 0-63, hi16 ch 64-127, e4m3 pairs of ch 0-63, of ch 64-127;
 // w_v: hi16 and lo16 halves); two TMA boxes of 136 rows bring rows t0-5 .. t0+266 of the window into
 // each SWIZZLE_128B region ONCE; conv tap j is the same slab read j rows further down -- only the
-// UMMA descriptor start address changes (row j is position t0-5+j; TMA zero-fills rows with t < 0 or
-// t >= 5997, which is exactly Keras' causal padding).  Measured on B200 (profiles/r01_bringup.md): the
-// 128B swizzle is a function of the absolute shared-memory address, so a descriptor may start at any
-// 128-byte row of a 1024B-aligned slab with base_offset = 0.
+// wgmma descriptor start address changes (row j is position t0-5+j; TMA zero-fills rows with t < 0 or
+// t >= 5997, which is exactly Keras' causal padding).
 //
-// Operand roles ("transposed" formulation).  Measured (tools/mma_microbench.cu,
-// profiles/r01_mma_microbench.md): a cta_group::1 M=128 x N=128 x K=16 UMMA needs 128 B/cycle of
-// shared-memory operand bandwidth -- all of it -- and in the real kernel (TMA fills and epilogue
-// traffic share the banks) ran at ~109 instead of 64 cycles; N=256 needs 96 B/cycle.  The model has
-// only 128 output channels, so N=256 comes from swapping the roles:
+// Operand roles ("transposed" formulation).  The model has only 128 output channels, so the wide N = 256 side of the
+// instruction comes from swapping the roles:
 //
-//     D^T[cout (M=128 TMEM lanes)][position (N=256 TMEM columns)] += W_tap^T[cout][cin] * Y[position + tap][cin]
+//     D^T[cout (M)][position (N=256)] += W_tap^T[cout][cin] * Y[position + tap][cin]
 //
 //   A operand = one 16 KB weight stage, [128 cout][64 cin] fp16 or [128 cout][128 cin] e4m3, K-major
 //               SWIZZLE_128B (streamed by TMA through a 5-stage ring, host-packed in consumption order);
+//               consumer warpgroup g multiplies its rows 64 g .. 64 g + 63;
 //   B operand = 256 consecutive rows of one slab region.
 //
-// Schedule.  Weight stages are ordered region-major (all 6 taps against region 0, then region 1, ...) so a
-// region is free after its 6 stages and is reloaded for the NEXT unit while the other regions are in use;
-// activations and weights have separate producer threads; 2 accumulator sets x 256 TMEM columns let the
-// epilogue of unit u overlap the MMAs of unit u+1.  The MMA warp stays converged and issues through
-// elect.sync so consecutive tcgen05.mma stay on the uniform datapath (the first version issued from a
-// divergent single lane and spent ~140 cycles per MMA in the compiler's waterfall loop).
+// Schedule.  Weight stages are consumed region-major (all 6 taps against one region, then the next; the two e4m3 regions
+// before the two fp16 ones, see the MMA loop) so a region is free after its 6 stages and is reloaded for the NEXT unit while
+// the other regions are in use;
+// activations and weights have separate producer threads.
 //
-// Warp roles (384 threads, 1 CTA per SM, persistent over units):
-//   warp 0 lane 0 : weight producer (TMA)          warp 3 lane 0 : activation producer (TMA)
-//   warp 1        : tcgen05.mma issuer             warp 2        : TMEM allocator
-//   warps 4..11   : epilogue (two warps per TMEM lane quarter, alternating 32-position chunks).  A thread owns one output CHANNEL (TMEM lane) and reads 32 positions at a time.
+// Warp roles (384 threads = 3 warpgroups, 1 CTA per SM, persistent over units):
+//   warp 0 lane 0 : weight producer (TMA)          warp 1 lane 0 : activation producer (TMA)
+//   warpgroups 1, 2: wgmma (M64 N256, 128 fp32 accumulator registers per thread) and the epilogue of output channels
+//       64 g .. 64 g + 63.  A thread holds channels c and c + 8 at 64 of the unit's positions (wgmma.cuh).
 //       conv : 2^-S scale + bias + LeakyReLU, then the planes the consumer needs (conv2 -> hi16, lo8, hi8 for
-//              conv3; conv3 -> hi16, lo16 for w_v / gather) stored straight to global memory: for a fixed position
-//              a warp's 32 lanes are 32 consecutive channels = one contiguous 64-byte (fp8: 32-byte) piece of the row
-//              (an earlier version transposed through a 16 KB shared staging tile; shared-memory bandwidth is the
-//              scarce resource of this kernel, and dropping the tile also paid for a 5th weight stage; a lane-pair
-//              exchange that halves the store count was measured and brought nothing);
-//       w_v  : the max over 8 consecutive positions is a max over 8 registers (no shuffles); a warp writes
-//              128 contiguous bytes of q[g][:] per pooled row.
-//
-// Round 2: (i) the two e4m3 planes are interleaved as (lo8, hi8) pairs per channel (common.cuh), so the correction passes are one
-// K = 256 contraction per tap against weights interleaved the same way and conv2's epilogue needs one 2-byte store per position
-// instead of two 1-byte stores (conv2 2.30 -> 2.21 ms, profiles/r02_ab_pairs_interleaved.log); (ii) the epilogue tracks the largest
-// |Y| it produced and raises DeviceStatus::act_overflow beyond the operand formats' range; (iii) launching the persistent grid as
-// thread-block clusters of 2 / 4 (hoping L2 would merge the CTAs' identical weight-stage requests) was measured and is slower
-// (2.29 -> 2.40 / 2.43-2.49 ms, option conv_cluster, profiles/r02_ab_conv_cluster.log); (iv) the steady state of the whole step is
-// power-bound (1 kW cap, ~1.45-1.5 GHz during this kernel): tensor pipe 63-68 % active at that clock.
+//              conv3; conv3 -> hi16, lo16 for w_v / gather) stored straight to global memory;
+//       w_v  : the max over 8 consecutive positions (two registers per lane, then a butterfly over the lane quad).
+// The epilogue tracks the largest |Y| it produced and raises DeviceStatus::act_overflow beyond the operand formats' range.
+// Option conv_cluster launches the persistent grid as thread-block clusters (every CTA still issues its own loads).
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -84,7 +66,7 @@ constexpr int kA2Region    = 2 * kARegion;                       // 272-row slab
 constexpr int kNumRegions  = 4;
 constexpr int kA2Bytes     = kNumRegions * kA2Region;            //                                        = 139264
 constexpr int kBStage      = 128 * 128;                          // one weight stage: 128 rows x 128 B     = 16384
-constexpr int kConvThreads = 384;                                // 4 control warps + 8 epilogue warps
+constexpr int kConvThreads = 384;                                // producer warpgroup + 2 MMA / epilogue warpgroups
 constexpr int kConvStages  = 24;                                 // conv: (region, tap)
 constexpr int kWvStages    = 4;                                  // w_v : (K-half, weight hi/lo)
 constexpr int kTWStages    = 5;                                  // weight ring depth (16 KB each)
@@ -102,6 +84,11 @@ struct ConvTcParams {
   DeviceStatus* status;
 };
 
+// conv: consumption step q of a unit -> 16 KB stage of the host pack (packed region-major: hi16.k0, hi16.k1, pairs.k0, pairs.k1,
+// six taps each), e4m3 regions first (see the MMA loop); w_v: the pack order
+template <bool kWvMode> __device__ __forceinline__ int conv_pack_stage(int q) {
+  return kWvMode ? q : ((q / 6 + 2) & 3) * 6 + q % 6;
+}
 // byte offset inside the 768-byte activation row of the data that fills slab region r
 template <bool kWvMode> __device__ __forceinline__ constexpr int region_src(int r) {
   return kWvMode ? (r == 0 ? kOffHi16 : r == 1 ? kOffHi16 + 128 : r == 2 ? kOffLo16 : kOffLo16 + 128)
@@ -113,24 +100,15 @@ __global__ void __launch_bounds__(kConvThreads, 1)
 conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant__ CUtensorMap tm_w,
               const ConvTcParams p) {
   constexpr int kStagesU = kWvMode ? kWvStages : kConvStages;     // stages per unit
-  constexpr uint32_t kIdescFull = umma_idesc_f16(128, 256);
-  // The last unit of a window holds only 5997 - 23 * 256 = 109 positions: N = 112 columns instead of 256 saves 56 % of that
-  // unit's tensor time (2.3 % of the kernel).  Columns 112.. of the accumulator then keep stale values; the epilogue never
-  // stores positions >= 5997 (conv) / pooled rows >= 749 (w_v), which is everything from column 109 on.
-  constexpr int kTailCols = ((kTok - (kUnitsPerWin - 1) * 2 * kTileM) + 15) / 16 * 16;          // 112
-  constexpr uint32_t kIdescTail = umma_idesc_f16(128, kTailCols);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_a = smem;                                   // activation slab: 4 regions x 272 rows x 128 B
   uint8_t* s_w = smem + kA2Bytes;                        // weight ring
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + kTWStages * kBStage);
   uint64_t* a_full = bars;            // [4]  per region
-  uint64_t* a_empty = bars + 4;       // [4]
+  uint64_t* a_empty = bars + 4;       // [4]  one arrival per consumer warp
   uint64_t* w_full = bars + 8;        // [5]
-  uint64_t* w_empty = bars + 13;      // [5]
-  uint64_t* acc_full = bars + 18;     // [2]
-  uint64_t* acc_empty = bars + 20;    // [2]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 22);
+  uint64_t* w_empty = bars + 13;      // [5]  one arrival per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_units = p.n_tiles;      // n_windows * 24
@@ -138,21 +116,13 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_act);
     tma_prefetch_desc(&tm_w);
-    for (int i = 0; i < kNumRegions; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < kTWStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 8); }
+    for (int i = 0; i < kNumRegions; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
+    for (int i = 0; i < kTWStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(s_tmem, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp == 3 && lane == 0) {
+  if (warp == 1 && lane == 0) {
     // ===================================================================== activation producer
     int it = 0;
     const uint64_t pol = l2_policy_evict_first();          // activations stream through L2 once
@@ -162,7 +132,7 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
       const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
 #pragma unroll
       for (int k = 0; k < kNumRegions; ++k) {
-        const int r = kWvMode ? (k == 0 ? 0 : k == 1 ? 2 : k == 2 ? 1 : 3) : k;      // order in which the MMAs need them
+        const int r = kWvMode ? (k == 0 ? 0 : k == 1 ? 2 : k == 2 ? 1 : 3) : (k + 2) & 3;   // order in which the MMAs need them
         mbar_wait(&a_empty[r], ph ^ 1, p.status, 100 + r);
         mbar_arrive_expect_tx(&a_full[r], kA2Region);
         uint8_t* dst = s_a + r * kA2Region;
@@ -180,33 +150,37 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
         const uint32_t wphase = (wcount / kTWStages) & 1;
         mbar_wait(&w_empty[s], wphase ^ 1, p.status, 110 + s);
         mbar_arrive_expect_tx(&w_full[s], kBStage);
-        tma_load_2d_hint(s_w + s * kBStage, &tm_w, &w_full[s], 0, q * 128, pol);
+        tma_load_2d_hint(s_w + s * kBStage, &tm_w, &w_full[s], 0, conv_pack_stage<kWvMode>(q) * 128, pol);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (converged warp, elected lane issues)
+  } else if (warp >= 4) {
+    // ===================================================================== MMA + epilogue (warpgroup g: channels 64 g .. 64 g + 63)
+    const int g = (warp >> 2) - 1, wq = warp & 3;
+    const uint32_t a_base = smem_u32(s_a);
+    const uint32_t w_base = smem_u32(s_w) + g * 64 * 128;  // this warpgroup's 64 rows of every weight stage
+    const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
+    const float bias0 = kWvMode ? 0.f : p.bias[ch0], bias1 = kWvMode ? 0.f : p.bias[ch0 + 8];
+    const float oscale = p.out_scale;
+    float amax = 0.f;                                      // largest |Y| this thread produced (range check, common.cuh)
     uint32_t wcount = 0;
     int it = 0;
-    const uint64_t desc0 = umma_desc_sw128(0);
-    const uint32_t a_base = smem_u32(s_a);
-    const uint32_t w_base = smem_u32(s_w);
-    long long w_acc = 0, w_a = 0, w_w = 0, tq;
+    long long w_a = 0, w_w = 0, t_epi = 0, tq;
     const long long t_begin = clock64();
+    float d[128];
     for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t accphase = (it >> 1) & 1;
       const uint32_t aph = it & 1;
-      const uint32_t acc = tmem_base + as * 256;
-      const uint32_t kIdesc = (unit % kUnitsPerWin == kUnitsPerWin - 1) ? kIdescTail : kIdescFull;
-      tq = clock64();
-      mbar_wait(&acc_empty[as], accphase ^ 1, p.status, 200 + as);
-      w_acc += clock64() - tq;
+      const int w = unit / kUnitsPerWin;
+      const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
+      // resources of the stage whose wgmma is still in flight: released once the next stage's wgmma is issued
+      int prev_s = -1, prev_region = -1;
       for (int q = 0; q < kStagesU; ++q, ++wcount) {
-        // conv: stage q = (region q/6, tap q%6); regions 0,1 are fp16 K-halves, 2 / 3 = e4m3 pairs (lo8, hi8) of channels 0-63 / 64-127
-        //       against weights interleaved the same way (Whi8, Wlo8)
+        // conv: step q = (region ((q/6) + 2) % 4, tap q%6); regions 0,1 are fp16 K-halves, 2 / 3 = e4m3 pairs (lo8, hi8) of channels
+        //       0-63 / 64-127 against weights interleaved the same way (Whi8, Wlo8).  The e4m3 correction passes run FIRST: the
+        //       tensor core adds e4m3 products to the accumulator with less than fp32 precision, which would drop the ~2^-8 smaller
+        //       corrections if the accumulator already held the main pass; the fp16 passes accumulate in full fp32.
         // w_v : stage q = (K-half q/2, weight hi/lo q%2); hi-weight stages multiply both the hi16 and the lo16 region
-        const int reg = kWvMode ? (q >> 1) : (q / 6);
-        const int tap = kWvMode ? 5 : (q - reg * 6);
+        const int reg = kWvMode ? (q >> 1) : ((q / 6 + 2) & 3);
+        const int tap = kWvMode ? 5 : (q % 6);
         const bool first_use = kWvMode ? ((q & 1) == 0) : (tap == 0);
         if (first_use) {
           tq = clock64();
@@ -219,148 +193,113 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
         tq = clock64();
         mbar_wait(&w_full[s], wphase, p.status, 220 + s);
         w_w += clock64() - tq;
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t wdesc = desc0 + ((w_base + s * kBStage) >> 4);                              // A: weights
-          const uint64_t y0 = desc0 + ((a_base + reg * kA2Region + tap * 128) >> 4);                 // B: activations
-          if (kWvMode) {
-            const uint64_t y1 = desc0 + ((a_base + (2 + reg) * kA2Region + tap * 128) >> 4);        // lo16 region
-            const bool w_lo = (q & 1) != 0;
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              umma_f16(acc, wdesc + kk * 2, y0 + kk * 2, kIdesc, (q == 0 && kk == 0) ? 0u : 1u);
-              if (!w_lo) umma_f16(acc, wdesc + kk * 2, y1 + kk * 2, kIdesc, 1u);
-            }
-            umma_commit(&w_empty[s]);
-            if (q == 0) umma_commit(&a_empty[2]);                  // lo16.k0 is only used by stage 0
-            if (q == 1) umma_commit(&a_empty[0]);
-            if (q == 2) umma_commit(&a_empty[3]);
-            if (q == 3) umma_commit(&a_empty[1]);
-          } else {
-            if (reg < 2) {
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) umma_f16(acc, wdesc + kk * 2, y0 + kk * 2, kIdesc, (q == 0 && kk == 0) ? 0u : 1u);
-            } else {
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) umma_f8(acc, wdesc + kk * 2, y0 + kk * 2, kIdesc, 1u);
-            }
-            umma_commit(&w_empty[s]);
-            if (tap == 5) umma_commit(&a_empty[reg]);              // this region of the slab is no longer needed
-          }
-          if (q == kStagesU - 1) umma_commit(&acc_full[as]);
-        }
-        __syncwarp();
-      }
-    }
-    if (p.dbg && lane == 0) {
-      long long* d = p.dbg + blockIdx.x * 8;
-      d[0] = clock64() - t_begin; d[1] = w_acc; d[2] = w_a; d[3] = w_w; d[4] = it;
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue
-    // 8 epilogue warps: warp w may touch TMEM lanes 32*(w%4)..+31 (= 32 output channels); the two warps that share a
-    // lane quarter split the unit's eight 32-position chunks between them (even / odd).
-    const int wq = warp & 3;                                   // TMEM lane quarter = channels 32*wq .. 32*wq+31
-    const int grp = (warp - 4) >> 2;                           // 0: chunks 0,2,4,6   1: chunks 1,3,5,7
-    const int ch = wq * 32 + lane;
-    const float bias = kWvMode ? 0.f : p.bias[ch];
-    const float oscale = p.out_scale;
-    int it = 0;
-    float amax = 0.f;                                          // largest |Y| this thread produced (range check, common.cuh)
-    long long w_full_c = 0, tq;
-    const long long t_begin = clock64();
-    for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t accphase = (it >> 1) & 1;
-      const int w = unit / kUnitsPerWin;
-      const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
-      tq = clock64();
-      mbar_wait(&acc_full[as], accphase, p.status, 300 + as);
-      w_full_c += clock64() - tq;
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16) + as * 256;
-#pragma unroll 1
-      for (int c32 = grp; c32 < 8; c32 += 2) {
-        const int p0 = t0 + c32 * 32;                          // first position of this chunk
-        if (p0 >= kTok) break;                                 // uniform: the rest of the unit is past the window end
-        uint32_t r[32];
-        tmem_ld_32x32(lane_addr + c32 * 32, r);
-        tmem_wait_ld();
+        const uint64_t wdesc = gmma_desc_sw128(w_base + s * kBStage);                              // A: weights
+        const uint64_t y0 = gmma_desc_sw128(a_base + reg * kA2Region + tap * 128);                 // B: activations
+        wgmma_fence();
+        int rel = -1;                                            // slab region this stage is the last user of
         if (kWvMode) {
+          const uint64_t y1 = gmma_desc_sw128(a_base + (2 + reg) * kA2Region + tap * 128);        // lo16 region
+          const bool w_lo = (q & 1) != 0;
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float m = __uint_as_float(r[8 * g]);
-#pragma unroll
-            for (int k = 1; k < 8; ++k) m = fmaxf(m, __uint_as_float(r[8 * g + k]));
-            const int gg = (p0 >> 3) + g;
-            if (gg < kPooled) p.q_out[(static_cast<size_t>(w) * kPooled + gg) * kC + ch] = m * oscale;
+          for (int kk = 0; kk < 4; ++kk) {
+            wgmma_f16_n256(d, wdesc + kk * 2, y0 + kk * 2, (q == 0 && kk == 0) ? 0u : 1u);
+            if (!w_lo) wgmma_f16_n256(d, wdesc + kk * 2, y1 + kk * 2, 1u);
           }
+          rel = q == 0 ? 2 : q == 1 ? 0 : q == 2 ? 3 : 1;        // lo16.k0 is only used by stage 0, hi16.k0 by stages 0, 1, ...
         } else {
-          // Direct global stores: for a fixed position the 32 lanes of a warp hold 32 consecutive channels, so one
-          // 2-byte store per lane is a contiguous 64-byte piece of the row (32 bytes for an fp8 plane).  No shared-memory
-          // staging: the MMAs already use ~75 % of the shared-memory bandwidth for their operands and TMA fills ~23 %.
-          uint8_t* rowp = p.y_out + (static_cast<size_t>(w) * kTok + p0) * kRowBytes;
-          const bool store = !(p.experiment & 2);
-          if (p.out_fp8) {
+          if (reg < 2) {
 #pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              const float y0 = kActScale * lrelu(fmaf(__uint_as_float(r[i]), oscale, bias));
-              const float y1 = kActScale * lrelu(fmaf(__uint_as_float(r[i + 1]), oscale, bias));
-              amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
-              const __half2 h = __floats2half2_rn(y0, y1);
-              const float2 f = __half22float2(h);
+            for (int kk = 0; kk < 4; ++kk) wgmma_f16_n256(d, wdesc + kk * 2, y0 + kk * 2, 1u);
+          } else {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wgmma_e4m3_n256(d, wdesc + kk * 2, y0 + kk * 2, (q == 0 && kk == 0) ? 0u : 1u);
+          }
+          if (tap == 5) rel = reg;                               // this region of the slab is no longer needed
+        }
+        wgmma_commit();
+        // the previous stage's wgmma has completed once at most one group (this stage's) is pending
+        wgmma_wait<1>();
+        __syncwarp();
+        if (lane == 0 && prev_s >= 0) {
+          mbar_arrive(&w_empty[prev_s]);
+          if (prev_region >= 0) mbar_arrive(&a_empty[prev_region]);
+        }
+        prev_s = s; prev_region = rel;
+      }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&w_empty[prev_s]);
+        if (prev_region >= 0) mbar_arrive(&a_empty[prev_region]);
+      }
+      wgmma_fence_regs(d);
+      // ===================================================================== epilogue
+      tq = clock64();
+      if (kWvMode) {
+        // pool group j of the unit = accumulator columns 8 j .. 8 j + 7 = registers 4 j + 2 h + e of the lane quad
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          float m0 = fmaxf(d[4 * j], d[4 * j + 1]), m1 = fmaxf(d[4 * j + 2], d[4 * j + 3]);
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+          const int gg = (t0 >> 3) + j;
+          if ((lane & 3) == 0 && gg < kPooled) {
+            float* qrow = p.q_out + (static_cast<size_t>(w) * kPooled + gg) * kC;
+            qrow[ch0] = m0 * oscale;
+            qrow[ch0 + 8] = m1 * oscale;
+          }
+        }
+      } else {
+        const bool store = !(p.experiment & 2);
+        uint8_t* const unit_rows = p.y_out + (static_cast<size_t>(w) * kTok + t0) * kRowBytes;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const int pos = 8 * j + 2 * (lane & 3);                // positions pos, pos + 1 of the unit
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int ch = ch0 + 8 * h;
+            const float bias = h ? bias1 : bias0;
+            const float y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
+            const float y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
+            amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
+            uint8_t* q0 = unit_rows + static_cast<size_t>(pos) * kRowBytes;
+            uint8_t* q1 = q0 + kRowBytes;
+            if (p.out_fp8) {
+              const __half2 hh = __floats2half2_rn(y0, y1);
+              const float2 f = __half22float2(hh);
               // e4m3 pair (lo8, hi8) of this channel at each of the two positions: one 2-byte store per position
               const uint16_t e0 = pack_e4m3x2((y0 - f.x) * kLo8Scale, f.x * kHi8Scale);
               const uint16_t e1 = pack_e4m3x2((y1 - f.y) * kLo8Scale, f.y * kHi8Scale);
-              if (store && p0 + i < kTok) {
-                uint8_t* q = rowp + i * kRowBytes;
-                reinterpret_cast<__half*>(q + kOffHi16)[ch] = __low2half(h);
-                reinterpret_cast<uint16_t*>(q + kOffP8)[ch] = e0;
+              if (store && t0 + pos < kTok) {
+                reinterpret_cast<__half*>(q0 + kOffHi16)[ch] = __low2half(hh);
+                reinterpret_cast<uint16_t*>(q0 + kOffP8)[ch] = e0;
               }
-              if (store && p0 + i + 1 < kTok) {
-                uint8_t* q = rowp + (i + 1) * kRowBytes;
-                reinterpret_cast<__half*>(q + kOffHi16)[ch] = __high2half(h);
-                reinterpret_cast<uint16_t*>(q + kOffP8)[ch] = e1;
+              if (store && t0 + pos + 1 < kTok) {
+                reinterpret_cast<__half*>(q1 + kOffHi16)[ch] = __high2half(hh);
+                reinterpret_cast<uint16_t*>(q1 + kOffP8)[ch] = e1;
               }
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              const float y0 = kActScale * lrelu(fmaf(__uint_as_float(r[i]), oscale, bias));
-              const float y1 = kActScale * lrelu(fmaf(__uint_as_float(r[i + 1]), oscale, bias));
-              amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
-              __half2 h, l;
-              split2_f16(y0, y1, h, l);
-              if (store && p0 + i < kTok) {
-                uint8_t* q = rowp + i * kRowBytes;
-                reinterpret_cast<__half*>(q + kOffHi16)[ch] = __low2half(h);
-                reinterpret_cast<__half*>(q + kOffLo16)[ch] = __low2half(l);
+            } else {
+              __half2 hh, l;
+              split2_f16(y0, y1, hh, l);
+              if (store && t0 + pos < kTok) {
+                reinterpret_cast<__half*>(q0 + kOffHi16)[ch] = __low2half(hh);
+                reinterpret_cast<__half*>(q0 + kOffLo16)[ch] = __low2half(l);
               }
-              if (store && p0 + i + 1 < kTok) {
-                uint8_t* q = rowp + (i + 1) * kRowBytes;
-                reinterpret_cast<__half*>(q + kOffHi16)[ch] = __high2half(h);
-                reinterpret_cast<__half*>(q + kOffLo16)[ch] = __high2half(l);
+              if (store && t0 + pos + 1 < kTok) {
+                reinterpret_cast<__half*>(q1 + kOffHi16)[ch] = __high2half(hh);
+                reinterpret_cast<__half*>(q1 + kOffLo16)[ch] = __high2half(l);
               }
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[as]);
+      t_epi += clock64() - tq;
     }
     if (!kWvMode) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
-    if (p.dbg && warp == 4 && lane == 0) {   // (group 0's view)
-      long long* d = p.dbg + blockIdx.x * 8;
-      d[5] = clock64() - t_begin; d[6] = w_full_c;
+    if (p.dbg && warp == 4 && lane == 0) {   // warpgroup 1's view
+      long long* dd = p.dbg + blockIdx.x * 8;
+      dd[0] = clock64() - t_begin; dd[2] = w_a; dd[3] = w_w; dd[4] = it; dd[6] = t_epi;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -76,13 +76,7 @@ encode_tokens_kernel(const uint8_t* __restrict__ ascii, uint16_t* __restrict__ t
 // of 6 consecutive bases, so A has only 4^6 = 4096 possible values when those bases are all ACGT, and
 // likewise B: two 2 MB "triple" tables (built on the host with the same fp32 operation order, so a
 // table hit is bit-identical to the three-row sum) replace six 512-byte row reads by two.  Positions
-// next to the window start, or touching a non-ACGT base, fall back to the single-row table.  The first
-// version (six reads per position) was L1-bandwidth bound: l1tex 97 % busy (profiles/r01_small_kernels_ncu.md).
-// Now: 0.76 ms per 1024 windows = 75 % of peak DRAM write bandwidth (4.66 GB), issue slots 83 % busy (~115 warp
-// instructions per position).  Fusing the first IGLOO kernel's patch gather into this kernel (CTA per 64-position segment,
-// folded weights in shared memory, dot products on the row while it is in registers) was built and measured: correct, but
-// 2.1 ms instead of 0.76 + 0.79 ms -- the kernel is instruction-bound (~190 warp instructions per position) and the staged
-// weights cap occupancy at 3 CTAs per SM -- so the gather stays a separate streaming kernel.
+// next to the window start, or touching a non-ACGT base, fall back to the single-row table.
 // ------------------------------------------------------------------------------------------
 constexpr int kEmbSeg = 256;
 constexpr int kEmbThreads = 256;

@@ -16,9 +16,7 @@ namespace gnm {
 // Patch gather, position-ordered streaming form.
 //
 // The 8400 (patch, slot) entries of an IGLOO kernel touch only ~4500 distinct positions, so reading one
-// row per entry moves every popular row ~1.9x through L2 -> SM; the first version (one CTA per 32-patch
-// group, random rows) was bound by exactly that (5 TB/s L2->SM for 2.4 GB of DRAM reads,
-// profiles/r01_small_kernels_ncu.md).  Here the entries are sorted by position on the host and dealt to
+// row per entry moves every popular row ~1.9x through L2 -> SM.  Here the entries are sorted by position on the host and dealt to
 // 700 CTAs x 4 warps x 3 entries (= 8400 exactly; 5 CTAs per SM, one resident wave, no shared memory): a warp's
 // rows are neighbours in memory, repeats of a row are served by L1, and the whole grid sweeps each window
 // front to back.  Every lane keeps its 3 x 8 folded weights in registers and a 3-window deep ring of
@@ -29,11 +27,6 @@ namespace gnm {
 // register cost and the ring's loads mostly hit L2.  Each entry has exactly one writer (part[w][slot]);
 // patch_finish_kernel then adds the four slots of a patch in fixed order k = 0..3 plus the bias, so results are
 // deterministic.
-// Measured per 1024 windows (same-box A/B, profiles/r01_small_kernels_ncu.md): 0.79 ms = 3.0 TB/s with 444 CTAs x 5
-// entries x 4-deep ring and no prefetch (12 warps per SM at 152 registers: long-scoreboard bound) -> 0.56 ms with the
-// L2 prefetch (any distance 2..8; 24 thrashes L2: 0.89 ms) -> 0.51 ms = 4.6 TB/s = 0.70 of the HBM peak with 3 entries per
-// warp and a 3-deep ring (94 registers, 20 warps per SM).  Tried and slower: 512-byte cp.async.bulk row copies into
-// shared memory (0.88 ms), 2 entries per warp (0.60-0.93 ms).
 // HBM-bound: 2.4 MB of distinct activation rows per window per IGLOO kernel (algorithmic 8400 x 512 B = 4.3 MB).
 // ------------------------------------------------------------------------------------------
 constexpr int kGsPerWarp = 3;                                    // entries per warp

@@ -4,31 +4,24 @@
 //                      y @ w_v, MaxPool1D(8)                                genomad/neural_network/igloo.py:207-210
 //
 // Why fuse: y1 is written once (4.7 GB per 1024 windows) and then read three times (patch gather, w_v, conv2).  The w_v
-// read (3.1 GB, 0.6 ms of pure HBM time) disappears if the projection consumes each row while it is still on the SM:
+// read (3.1 GB) disappears if the projection consumes each row while it is still on the SM:
 // the producer warps below write every finished row twice -- to global memory (all four planes, as embed_conv1_kernel
 // does) and, as fp16 hi / lo halves, into a 128-byte-swizzled shared-memory slab in exactly the layout TMA would have
-// produced -- and one thread issues the same 3-pass tcgen05 MMAs conv_t_kernel<true> issues (D^T[cout][pos], weights as the
+// produced -- and two warpgroups issue the same 3-pass wgmma conv_t_kernel<true> issues (D^T[cout][pos], weights as the
 // A operand, the slab as the B operand).  The arithmetic of both halves is unchanged, so y1 and q0 are bit-identical to the
 // unfused kernels' results.
 //
-// Persistent, 1 CTA per SM, 960 threads:
-//   warps 0-23  producers: tokens for the unit (shared memory), then 4 rows each: two table rows from L2 -> y1 row ->
+// Persistent, 1 CTA per SM, 1024 threads:
+//   warps 0-23  producers: tokens for the unit, then 4 rows each: two table rows from L2 -> y1 row ->
 //               4 global plane stores + 2 swizzled shared stores; fence.proxy.async; arrive on a_full[buf]
-//   warp 24     MMA issuer (elected lane): 24 UMMAs M128 N96 K16 per unit into one of two accumulators
-//   warp 25     barrier init, TMEM allocation, the one-time TMA load of w_v's four 16 KB stages (they stay resident)
-//   warps 26-29 epilogue: TMEM -> max over 8 consecutive positions -> q0 (one TMEM lane quarter each)
+//   warps 24-31 two MMA + epilogue warpgroups (output channels 64 g .. 64 g + 63): 2 x 24 wgmma M64 N48 K16 per unit, then
+//               the max over 8 consecutive positions -> q0.  Warp 24 also initialises the barriers and loads w_v's four 16 KB
+//               stages once (they stay resident).
 // Unit = 96 positions (63 per window); the slab is double-buffered (2 x 4 regions x 12 KB), so producers fill unit u+1
-// while the tensor core works on unit u.  Shared memory: 96 KB slab + 64 KB weights + tokens + barriers = 162 KB.
+// while the tensor core works on unit u.  Shared memory: 96 KB slab + 64 KB weights + barriers = 161 KB.
 //
-// STATUS (end of round 1): bit-identical to the two separate kernels (tests/test_gpu_parity.py::test_fused_layer1_wv_option)
-// but not yet faster, so it is OFF by default (option "fuse_l1").  Per 1024 windows, same-box A/B against 0.81 + 0.63 ms:
-//   16 producer warps x 8 rows, CTA-wide token buffer + barrier per unit, 2 rows in flight ............ 2.11 ms
-//   24 producer warps x 4 rows (96-position units), 8 table rows in flight per lane ................... 1.92 ms
-//   + warp-autonomous tokens (shuffles, next unit's bytes prefetched), no CTA barrier ................. 1.68 ms  <- this file
-//   + rolling two-row pipeline (next half-batch's table rows always in flight), hoisted address math ... 1.81 ms (not kept)
-// ~600 warp instructions per warp and unit (14.4 k per SM and unit = 3.6 k issue cycles of the 6.2 k the unit takes): the
-// producers are issue- and dependency-bound with 6 warps per scheduler, where the unfused layer-1 kernel has 16.  Next:
-// cut the per-row instruction count (uniform table indices, packed stores) or hand the row production to TMA-gather.
+// Bit-identical to the two separate kernels (tests/test_gpu_parity.py::test_fused_layer1_wv_option); off by default
+// (option "fuse_l1"): the producers are issue- and dependency-bound, so the fused kernel has not been faster than the pair.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -36,12 +29,12 @@
 
 namespace gnm {
 
-constexpr int kFuUnit = 96;                                      // positions per unit (= UMMA N)
+constexpr int kFuUnit = 96;                                      // positions per unit (two wgmma N = 48 halves)
 constexpr int kFuUnitsPerWin = (kTok + kFuUnit - 1) / kFuUnit;   // 63
 constexpr int kFuProducerWarps = 24;
 constexpr int kFuRowsPerWarp = kFuUnit / kFuProducerWarps;      // 4, all loaded up front (8 table rows in flight per lane)
-constexpr int kFuAccStride = 128;                                // TMEM columns between the two accumulators
-constexpr int kFuThreads = 32 * (kFuProducerWarps + 2 + 4);     // 960
+constexpr int kFuMmaWarps = 8;                                   // two MMA + epilogue warpgroups
+constexpr int kFuThreads = 32 * (kFuProducerWarps + kFuMmaWarps);  // 1024
 constexpr int kFuRegion = kFuUnit * 128;                         // 12 KB: 96 rows x 128 B (one K-half of one plane)
 constexpr int kFuSlab = 4 * kFuRegion;                           // hi.k0 | hi.k1 | lo.k0 | lo.k1
 constexpr int kFuWBytes = 4 * 16384;
@@ -55,7 +48,7 @@ struct FusedParams {
   const float* bias;         // [128]
   uint8_t* y_out;            // [n][5997][768 B]
   float* q_out;              // [n][749][128]
-  int n_units;               // n_windows * 47
+  int n_units;               // n_windows * 63
   DeviceStatus* status;
 };
 
@@ -66,38 +59,23 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 template <bool kFromAscii>
 __global__ void __launch_bounds__(kFuThreads, 1)
 layer1_wv_kernel(const __grid_constant__ CUtensorMap tm_w, const FusedParams p) {
-  constexpr uint32_t kIdesc = umma_idesc_f16(128, kFuUnit);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* s_slab = smem;                                  // [2][4][128 rows][128 B], 128B-swizzled
+  uint8_t* s_slab = smem;                                  // [2][4][96 rows][128 B], 128B-swizzled
   uint8_t* s_w = smem + 2 * kFuSlab;                       // [4][128 rows][128 B]
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + kFuWBytes);
-  uint64_t* a_full = bars;            // [2]  count = 16 producer warps
-  uint64_t* a_empty = bars + 2;       // [2]  count = 1 (MMA commit)
-  uint64_t* acc_full = bars + 4;      // [2]
-  uint64_t* acc_empty = bars + 6;     // [2]  count = 4 epilogue warps
-  uint64_t* w_full = bars + 8;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 9);
+  uint64_t* a_full = bars;            // [2]  count = producer warps
+  uint64_t* a_empty = bars + 2;       // [2]  count = MMA warps
+  uint64_t* w_full = bars + 4;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == kFuProducerWarps + 1) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tm_w);
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&a_full[i], kFuProducerWarps); mbar_init(&a_empty[i], 1);
-        mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 4);
-      }
-      mbar_init(w_full, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(s_tmem, 256);
-    tmem_relinquish();
+  if (warp == kFuProducerWarps && lane == 0) {
+    tma_prefetch_desc(&tm_w);
+    for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], kFuProducerWarps); mbar_init(&a_empty[i], kFuMmaWarps); }
+    mbar_init(w_full, 1);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   if (warp < kFuProducerWarps) {
     // ===================================================================== producers
@@ -193,85 +171,63 @@ layer1_wv_kernel(const __grid_constant__ CUtensorMap tm_w, const FusedParams p) 
       __syncwarp();
       if (lane == 0) mbar_arrive(&a_full[b]);
     }
-  } else if (warp == kFuProducerWarps + 1) {
-    // ===================================================================== weights: once
-    if (lane == 0) {
-      const uint64_t pol = l2_policy_evict_last();
+  } else {
+    // ===================================================================== MMA + epilogue (warpgroup g: channels 64 g .. 64 g + 63)
+    const int g = (warp - kFuProducerWarps) >> 2, wq = warp & 3;
+    if (warp == kFuProducerWarps && lane == 0) {           // the weights, once
       mbar_arrive_expect_tx(w_full, kFuWBytes);
-      for (int q = 0; q < 4; ++q) tma_load_2d_hint(s_w + q * 16384, &tm_w, w_full, 0, q * 128, pol);
+      for (int q = 0; q < 4; ++q) tma_load_2d_hint(s_w + q * 16384, &tm_w, w_full, 0, q * 128, l2_policy_evict_last());
     }
-  } else if (warp == kFuProducerWarps) {
-    // ===================================================================== MMA issuer
-    const uint64_t desc0 = umma_desc_sw128(0);
-    const uint32_t slab_base = smem_u32(s_slab), w_base = smem_u32(s_w);
+    const uint32_t slab_base = smem_u32(s_slab), w_base = smem_u32(s_w) + g * 64 * 128;
+    const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
+    const float oscale = 1.f / kActScale;
     mbar_wait(w_full, 0, p.status, 430);
     int it = 0;
+    float d[24];
     for (int unit = blockIdx.x; unit < p.n_units; unit += gridDim.x, ++it) {
-      const int b = it & 1;                                    // slab buffer == accumulator buffer
-      const uint32_t ph = (it >> 1) & 1;
-      const uint32_t acc = tmem_base + b * kFuAccStride;
-      mbar_wait(&acc_empty[b], ph ^ 1, p.status, 410 + b);
-      mbar_wait(&a_full[b], ph, p.status, 420 + b);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {                           // stage q = (K-half q>>1, weight hi/lo q&1)
-          const int khq = q >> 1;
-          const uint64_t wdesc = desc0 + ((w_base + q * 16384) >> 4);
-          const uint64_t yh = desc0 + ((slab_base + b * kFuSlab + khq * kFuRegion) >> 4);
-          const uint64_t yl = desc0 + ((slab_base + b * kFuSlab + (2 + khq) * kFuRegion) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_f16(acc, wdesc + kk * 2, yh + kk * 2, kIdesc, (q == 0 && kk == 0) ? 0u : 1u);
-            if ((q & 1) == 0) umma_f16(acc, wdesc + kk * 2, yl + kk * 2, kIdesc, 1u);
-          }
-        }
-        umma_commit(&a_empty[b]);
-        umma_commit(&acc_full[b]);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================================================================== epilogue (4 warps)
-    const int wq = warp & 3;                                   // TMEM lane quarter = channels 32*wq .. 32*wq+31
-    const int ch = wq * 32 + lane;
-    const float oscale = 1.f / kActScale;
-    int it = 0;
-    for (int unit = blockIdx.x; unit < p.n_units; unit += gridDim.x, ++it) {
-      const int b = it & 1;
+      const int b = it & 1;                                    // slab buffer
       const uint32_t ph = (it >> 1) & 1;
       const int w = unit / kFuUnitsPerWin;
       const int t0 = (unit - w * kFuUnitsPerWin) * kFuUnit;
-      mbar_wait(&acc_full[b], ph, p.status, 440 + b);
-      tc_fence_after();
-      const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16) + b * kFuAccStride;
+      mbar_wait(&a_full[b], ph, p.status, 420 + b);
 #pragma unroll 1
-      for (int c32 = 0; c32 < kFuUnit / 32; ++c32) {
-        const int p0 = t0 + c32 * 32;
-        if (p0 >= kTok) break;
-        uint32_t r[32];
-        tmem_ld_32x32(lane_addr + c32 * 32, r);
-        tmem_wait_ld();
+      for (int nh = 0; nh < 2; ++nh) {                          // positions 48 nh .. 48 nh + 47 of the unit (24 registers each)
+        const uint32_t rows = slab_base + b * kFuSlab + nh * (kFuUnit / 2) * 128;
+        wgmma_fence();
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float m = __uint_as_float(r[8 * g]);
+        for (int q = 0; q < 4; ++q) {                           // stage q = (K-half q>>1, weight hi/lo q&1)
+          const int khq = q >> 1;
+          const uint64_t wdesc = gmma_desc_sw128(w_base + q * 16384);
+          const uint64_t yh = gmma_desc_sw128(rows + khq * kFuRegion);
+          const uint64_t yl = gmma_desc_sw128(rows + (2 + khq) * kFuRegion);
 #pragma unroll
-          for (int k = 1; k < 8; ++k) m = fmaxf(m, __uint_as_float(r[8 * g + k]));
-          const int gg = (p0 >> 3) + g;
-          if (gg < kPooled) p.q_out[(static_cast<size_t>(w) * kPooled + gg) * kC + ch] = m * oscale;
+          for (int kk = 0; kk < 4; ++kk) {
+            wgmma_f16_n48(d, wdesc + kk * 2, yh + kk * 2, (q == 0 && kk == 0) ? 0u : 1u);
+            if ((q & 1) == 0) wgmma_f16_n48(d, wdesc + kk * 2, yl + kk * 2, 1u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (nh == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&a_empty[b]);
+        }
+        wgmma_fence_regs(d);
+        // pool group j of the half = accumulator columns 8 j .. 8 j + 7 = registers 4 j + 2 h + e of the lane quad
+#pragma unroll
+        for (int j = 0; j < kFuUnit / 2 / kPool; ++j) {
+          float m0 = fmaxf(d[4 * j], d[4 * j + 1]), m1 = fmaxf(d[4 * j + 2], d[4 * j + 3]);
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2)); m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+          const int gg = ((t0 + nh * (kFuUnit / 2)) >> 3) + j;
+          if ((lane & 3) == 0 && gg < kPooled) {
+            float* qrow = p.q_out + (static_cast<size_t>(w) * kPooled + gg) * kC;
+            qrow[ch0] = m0 * oscale;
+            qrow[ch0 + 8] = m1 * oscale;
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[b]);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kFuProducerWarps + 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 

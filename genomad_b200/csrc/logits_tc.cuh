@@ -2,16 +2,17 @@
 // and (round 2) the two Dense(512) projections of the head (reference genomad/neural_network/model.py:28, 40): the same
 // kernel with K = 256 / 512 and N = 512; bias + BatchNorm + ReLU are applied by splitk_reduce_epi_kernel (dense.cuh).
 //
-// fp32 semantics on tcgen05: both operands are split into two TF32 halves, x = hi + lo with hi = x with the low 13 mantissa
-// bits cleared and lo = (x - hi) likewise truncated (so the hardware's fp32 -> tf32 conversion has nothing left to round), and
-// D = Ahi*Bhi + Alo*Bhi + Ahi*Blo accumulates in one fp32 TMEM accumulator (the dropped lo*lo term and the truncation of lo are
-// ~2^-20 relative; TF32 keeps fp32's 8-bit exponent, so the ~1e-32 weights of the shipped model need no scaling).
+// fp32 semantics on the tensor cores: both operands are split into two TF32 halves, x = hi + lo with hi = x with the low 13
+// mantissa bits cleared and lo = (x - hi) likewise truncated (so the hardware's fp32 -> tf32 conversion has nothing left to
+// round), and D = Ahi*Bhi + Alo*Bhi + Ahi*Blo accumulates in one fp32 accumulator (the dropped lo*lo term and the truncation of
+// lo are ~2^-20 relative; TF32 keeps fp32's 8-bit exponent, so the ~1e-32 weights of the shipped model need no scaling).
 // The split halves are written where the operands are produced (patch_finish_kernel for mpi, gnm_create for w_qk^T), TMA
-// brings them in as 128-byte-swizzled K-major tiles, one thread issues 12 UMMAs (M128 N256 K8, kind::tf32) per 32-wide K chunk.
+// brings them in as 128-byte-swizzled K-major tiles, and two consumer warpgroups (64 rows of the 128-row tile each) issue 12
+// wgmma (M64 N256 K8, tf32) per 32-wide K chunk into register accumulators.
 //
 // grid = (3 N tiles of 256 columns, ceil(n/128) M tiles, kLgSplits K splits): 144 CTAs at batch 1024.  Each split writes its
 // partial product to part[z][m][752]; splitk_reduce_kernel adds the partials in fixed order, so a window's logits do not
-// depend on the batch it is in.  Replaces a 64x64-tile fp32 FFMA kernel (0.14 ms per IGLOO kernel and 1024 windows, 23 TFLOP/s).
+// depend on the batch it is in.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -27,7 +28,7 @@ constexpr int kLgStages = 2;
 constexpr int kLgATile = kLgBM * 128, kLgBTile = kLgBN * 128;     // 16 KB, 32 KB
 constexpr int kLgStageBytes = 2 * kLgATile + 2 * kLgBTile;        // A hi | A lo | B hi | B lo = 96 KB
 constexpr int kLgSmem = kLgStages * kLgStageBytes + 1024 + 256;
-constexpr int kLgThreads = 192;                                   // TMA warp, MMA warp, 4 epilogue warps
+constexpr int kLgThreads = 384;                                   // warpgroup 0: TMA thread; warpgroups 1, 2: MMA + epilogue
 
 struct LogitsTcParams {
   float* part;               // [gridDim.z splits][n_rows][ldc]
@@ -39,17 +40,6 @@ struct LogitsTcParams {
   DeviceStatus* status;
 };
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// kind::tf32 instruction descriptor: A, B = TF32 (format 2), D = fp32, both K-major, dense
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
 // x = hi + lo, both exactly representable as TF32 (low 13 mantissa bits zero)
 __host__ __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
 #ifdef __CUDA_ARCH__
@@ -65,14 +55,11 @@ __global__ void __launch_bounds__(kLgThreads, 1)
 logits_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                  const __grid_constant__ CUtensorMap tm_b_hi, const __grid_constant__ CUtensorMap tm_b_lo,
                  const LogitsTcParams p) {
-  constexpr uint32_t kIdesc = umma_idesc_tf32(kLgBM, kLgBN);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kLgStages * kLgStageBytes);
   uint64_t* full = bars;              // [2]
-  uint64_t* empty = bars + 2;         // [2]
-  uint64_t* acc_full = bars + 4;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 5);
+  uint64_t* empty = bars + 2;         // [2]  one arrival per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * kLgBN, m0 = blockIdx.y * kLgBM, z = blockIdx.z;
@@ -81,18 +68,10 @@ logits_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tm_a_hi); tma_prefetch_desc(&tm_a_lo); tma_prefetch_desc(&tm_b_hi); tma_prefetch_desc(&tm_b_lo);
-    for (int i = 0; i < kLgStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < kLgStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(s_tmem, kLgBN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
   if (warp == 0 && lane == 0) {
     // ===================================================================== TMA producer
@@ -109,65 +88,48 @@ logits_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
       tma_load_2d_hint(st + 2 * kLgATile, &tm_b_hi, &full[s], k0, n0, pol_b);
       tma_load_2d_hint(st + 2 * kLgATile + kLgBTile, &tm_b_lo, &full[s], k0, n0, pol_b);
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    const uint64_t desc0 = umma_desc_sw128(0);
+  } else if (warp >= 4) {
+    // ===================================================================== MMA + epilogue: warpgroup g owns rows 64 g .. 64 g + 63
+    const int g = (warp >> 2) - 1, wq = warp & 3;
     const uint32_t base = smem_u32(smem);
+    float d[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) d[i] = 0.f;
     for (int c = 0; c < nc; ++c) {
       const int s = c % kLgStages;
       const uint32_t ph = (c / kLgStages) & 1;
       mbar_wait(&full[s], ph, p.status, 510 + s);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t st = base + s * kLgStageBytes;
-        const uint64_t a_hi = desc0 + (st >> 4), a_lo = desc0 + ((st + kLgATile) >> 4);
-        const uint64_t b_hi = desc0 + ((st + 2 * kLgATile) >> 4), b_lo = desc0 + ((st + 2 * kLgATile + kLgBTile) >> 4);
+      const uint32_t st = base + s * kLgStageBytes;
+      const uint64_t a_hi = gmma_desc_sw128(st + g * 64 * 128), a_lo = gmma_desc_sw128(st + kLgATile + g * 64 * 128);
+      const uint64_t b_hi = gmma_desc_sw128(st + 2 * kLgATile), b_lo = gmma_desc_sw128(st + 2 * kLgATile + kLgBTile);
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < kLgBK / 8; ++kk) {                   // K = 8 TF32 = 32 bytes per instruction
-          umma_tf32(tmem_base, a_hi + kk * 2, b_hi + kk * 2, kIdesc, (c == 0 && kk == 0) ? 0u : 1u);
-          umma_tf32(tmem_base, a_lo + kk * 2, b_hi + kk * 2, kIdesc, 1u);
-          umma_tf32(tmem_base, a_hi + kk * 2, b_lo + kk * 2, kIdesc, 1u);
-        }
-        umma_commit(&empty[s]);
-        if (c == nc - 1) umma_commit(acc_full);
+      for (int kk = 0; kk < kLgBK / 8; ++kk) {                   // K = 8 TF32 = 32 bytes per instruction
+        wgmma_tf32_n256(d, a_hi + kk * 2, b_hi + kk * 2, (c == 0 && kk == 0) ? 0u : 1u);
+        wgmma_tf32_n256(d, a_lo + kk * 2, b_hi + kk * 2, 1u);
+        wgmma_tf32_n256(d, a_hi + kk * 2, b_lo + kk * 2, 1u);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);                       // the stage may be refilled
     }
-  } else if (warp >= 2) {
-    // ===================================================================== epilogue: TMEM lane = window row, columns = logits
-    const int wq = warp & 3;                                     // warps 2..5 -> lane quarters 2, 3, 0, 1
-    const int m = m0 + wq * 32 + lane;
-    mbar_wait(acc_full, 0, p.status, 520);
-    tc_fence_after();
-    float* dst = p.part + (static_cast<size_t>(z) * p.n_rows + m) * p.ldc + n0;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16);
-#pragma unroll 1
-    for (int c32 = 0; c32 < kLgBN / 32; ++c32) {
-      if (n0 + c32 * 32 >= p.n_cols) break;                      // uniform
-      uint32_t r[32];
-      tmem_ld_32x32(lane_addr + c32 * 32, r);
-      tmem_wait_ld();
-      if (m < p.n_rows) {
+    wgmma_fence_regs(d);
+    // ===================================================================== epilogue: rows = windows, columns = logits
+    const int r0 = m0 + g * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const int col = n0 + c32 * 32 + j;
-          if (col + 3 < p.n_cols) {
-            *reinterpret_cast<float4*>(dst + c32 * 32 + j) =
-                make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]), __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-          } else {
+    for (int h = 0; h < 2; ++h) {
+      const int m = r0 + 8 * h;
+      if (m >= p.n_rows) continue;
+      float* dst = p.part + (static_cast<size_t>(z) * p.n_rows + m) * p.ldc;
 #pragma unroll
-            for (int q = 0; q < 4; ++q)
-              if (col + q < p.n_cols) dst[c32 * 32 + j + q] = __uint_as_float(r[j + q]);
-          }
-        }
+      for (int j = 0; j < 32; ++j) {
+        const int col = n0 + 8 * j + 2 * (lane & 3);
+        const float v0 = d[4 * j + 2 * h], v1 = d[4 * j + 2 * h + 1];
+        if (col + 1 < p.n_cols) *reinterpret_cast<float2*>(dst + col) = make_float2(v0, v1);
+        else if (col < p.n_cols) dst[col] = v0;
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kLgBN);
   }
 }
 

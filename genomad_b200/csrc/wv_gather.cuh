@@ -1,50 +1,40 @@
-// K3 + K4 fused: the IGLOO value projection q = maxpool8(y @ w_v) on tcgen05 AND the IGLOO patch gather
-// mpi[p] = sum_k y[P[p,k],:] . Wf[p,k,:], in ONE pass over the activations (round 2; replaces conv_t_kernel<true> +
-// patch_stream_kernel, which each streamed the same hi16/lo16 planes from HBM: 3.1 + 2.4 GB per 1024 windows).
+// K3 + K4 fused: the IGLOO value projection q = maxpool8(y @ w_v) on the tensor cores (wgmma) AND the IGLOO patch gather
+// mpi[p] = sum_k y[P[p,k],:] . Wf[p,k,:], in ONE pass over the activations (replaces conv_t_kernel<true> + patch_stream_kernel,
+// which each stream the same hi16/lo16 planes from HBM).
 //
 // Reference semantics (genomad/neural_network/igloo.py:190-214):
 //   mpi   = gather_nd(transpose(y), patches) * w_mult, reshaped, @ w_summer + w_bias          (lines 192-206)
 //   y_proj = y @ w_v, MaxPool1D(8)                                                              (lines 208-210)
 //
 // Work decomposition: POSITION BANDS.  A unit is one band of 24 consecutive positions of 8 consecutive windows
-// (192 activation rows = one N = 192 tensor-core tile; 250 bands x ceil(n/8) window groups).  Units are numbered
-// band-major and every CTA owns a contiguous range of them, so a CTA stays on one band (at most three) for the whole
-// launch while the grid as a whole sweeps the windows front to back.  That is what makes the gather cheap here: the
-// ~34 (patch, slot) entries whose position falls into the CTA's band use the same 17 KB of folded weights for every unit
-// (L1 / L2 resident), instead of every window re-reading all 4.3 MB.
+// (192 activation rows; 250 bands x ceil(n/8) window groups).  Units are numbered band-major and every CTA owns a contiguous
+// range of them, so a CTA stays on one band (at most three) for the whole launch while the grid as a whole sweeps the windows
+// front to back.  That is what makes the gather cheap here: the ~34 (patch, slot) entries whose position falls into the CTA's
+// band use the same 17 KB of folded weights for every unit (L1 / L2 resident), instead of every window re-reading all 4.3 MB.
 //
 // Slab.  The four regions of a unit (hi16 / lo16 plane x channel half) are ONE 3-D TMA box each, from a tensor map that lists
-// the window axis BEFORE the position axis (api.cu make_band_map; tools/tma_order_probe.cu): the box {128 B, 8 windows, 24
-// positions} lands as [position][window][128 B], i.e. the 8 windows of one position are one 1024-byte swizzle atom.  For the
-// tensor core the region is still a plain K-major SWIZZLE_128B operand of 192 rows (accumulator column n = 8 * position +
-// window); for the gather it means "one position x 8 windows" is one conflict-free ldmatrix.  Eight region buffers = two units
-// in flight: the TMA producer fills unit u+1 while the MMAs and the gather work on unit u (with one unit of buffering every
-// role waited on the same load -> use -> release chain: 7.1 k cycles per 256 rows; now 4.8 k per 192).
+// the window axis BEFORE the position axis (api.cu make_band_map): the box {128 B, 8 windows, 24 positions} lands as
+// [position][window][128 B], i.e. the 8 windows of one position are one 1024-byte swizzle atom.  For the tensor core the
+// region is still a plain K-major SWIZZLE_128B operand of 192 rows (column n = 8 * position + window); for the gather it means
+// "one position x 8 windows" is one conflict-free ldmatrix.  Six region buffers: the TMA producer fills the first half of unit
+// u+1 while the MMAs and the gather work on unit u.
 //
-//   * value projection: 3 fp16 passes Ahi*Whi + Alo*Whi + Ahi*Wlo into one TMEM accumulator, operands swapped so that
-//     D^T[cout][row].  The w_v weights are the A operand and live in TENSOR MEMORY (tcgen05.mma TS form; copied there once per
-//     CTA with tcgen05.st): no shared memory for them (that is what pays for the second unit of buffering) and a third fewer
-//     operand bytes through the shared-memory port.  TMEM: 2 accumulators x 192 columns + 128 columns of weights = 512.
+//   * value projection: 3 fp16 passes Ahi*Whi + Alo*Whi + Ahi*Wlo, operands swapped so that D^T[cout][row].  The w_v weights
+//     (the A operand, 64 KB: hi / lo x two K-halves) are loaded into shared memory once per CTA.  Two MMA warpgroups own 64
+//     output channels each and take the unit one pool group (64 columns = 8 positions x 8 windows) at a time, M64 N64 K16:
+//     a thread's 32 accumulator registers hold 2 channels x 2 windows x the group's 8 positions, so the max-pool is a max over
+//     8 of its own registers and q is written straight from them.
 //   * patch gather: warp-level mma.sync.m16n8k16 on the slab rows.  Entries are grouped by position (<= 4 per group;
 //     8,400 entries hit ~4,500 positions).  For one group and one channel half, A[16 x 64] = the position's 8 windows' hi16 rows
 //     (rows 0-7) and lo16 rows (rows 8-15), read by 4 ldmatrix.x4; B[64 x 8] = the fp16 hi / lo halves of the group's folded
 //     weights (host-packed in fragment order, scaled by a power of two so the lo halves stay normal; L1 / L2 resident); the sum of
-//     the four D entries of (window, entry) is (hi + lo) . (w_hi + w_lo) with fp32 accumulation -- the fp32-equivalent dot product
-//     (tools/tma_order_probe.cu: 8e-8 absolute on O(1) sums).  16 gather warps take <= 2 groups each; pass 0 (channels 0-63) waits
-//     in registers, pass 1 adds channels 64-127 and writes part_t[slot][window] (8 lanes = 32 contiguous bytes).  A K-half's two
-//     regions go back to the producer when the tensor core (tcgen05.commit) and all 16 gather warps have arrived (count 17).
-//     patch_finish_t_kernel adds a patch's four slots in fixed order k = 0..3 plus the bias, as before.
-//   * epilogue: 4 warps (one per TMEM lane quarter) read the accumulator; pool group g of the band is columns 64 g .. 64 g + 63, a
-//     thread (= channel) takes the maximum over the 8 registers of one window and a warp writes 128 contiguous bytes of q.
-//   * what bounds it now (DESIGN.md 5.1, cycle counters of tools/ab_stages.py --wvg-cycles): the gather warps, and inside them the
-//     warp-level mma: it shares the tensor pipe with the tcgen05.mma stream and waits ~190 cycles per instruction (gather phase
-//     3.4 k cycles per unit; 2.1 k with the mma switched off, 3.2 k with the loads switched off).  Splitting every tcgen05.mma
-//     into two N = 96 slices (more instruction boundaries) changes nothing; neither do four independent accumulators.
-//     Earlier forms of this kernel (FFMA gather from a window-major slab, 20 merged gather + epilogue warps, weights in shared
-//     memory, one unit of buffering) are in DESIGN.md 5.1 with their numbers.
+//     the four D entries of (window, entry) is (hi + lo) . (w_hi + w_lo) with fp32 accumulation -- the fp32-equivalent dot product.
+//     15 gather warps take <= 2 groups each; pass 0 (channels 0-63) waits in registers, pass 1 adds channels 64-127 and writes
+//     part_t[slot][window] (8 lanes = 32 contiguous bytes).  A region goes back to the producer when the 8 MMA warps and all 15
+//     gather warps have arrived (count 23).  patch_finish_t_kernel adds a patch's four slots in fixed order k = 0..3 plus the bias.
 //
-// Warp roles (768 threads, 1 CTA per SM):  warp 1: tcgen05.mma issuer | warp 2: TMEM allocator | warp 3 lane 0: activation
-// producer (TMA) | warps 4..19: patch gather (warps 4..7 first copy the weights into tensor memory) | warps 20..23: epilogue.
+// Warp roles (768 threads, 1 CTA per SM):  warps 0..7: two MMA + epilogue warpgroups | warps 8..22: patch gather |
+// warp 23 lane 0: barrier init, the weight load and the activation producer (TMA).
 #pragma once
 #include <cuda.h>
 #include <type_traits>
@@ -56,30 +46,23 @@ namespace gnm {
 
 constexpr int kBandRows   = 24;                                   // positions per band (multiple of the pool size 8)
 constexpr int kBandWins   = 8;                                    // windows per unit
-constexpr int kWgN        = kBandRows * kBandWins;                // activation rows per unit = N of the unit's tcgen05.mma (192)
+constexpr int kWgN        = kBandRows * kBandWins;                // activation rows per unit (192)
 constexpr int kNumBands   = (kTok + kBandRows - 1) / kBandRows;   // 250 (the last band holds 21 valid rows)
 constexpr int kWgRegion   = kWgN * 128;                           // bytes per slab region (192 rows x 128 B)               =  24576
-constexpr int kWgBufs     = 8;                                    // region buffers = TWO units in flight: region k of unit `it` lives in buffer
-                                                                  // (4 it + k) % 8, so the TMA fills the next unit while this one is in use
-constexpr int kWgSlab     = kWgBufs * kWgRegion;                  //                                                        = 196608
-constexpr int kWgWarps    = 16;                                   // patch-gather warps
-constexpr int kWgEpiWarps = 4;                                    // accumulator-epilogue warps (one per TMEM lane quarter)
-constexpr int kWgThreads  = (4 + kWgWarps + kWgEpiWarps) * 32;    // 768
-constexpr int kWgGroupCap = 2;                                    // position groups per warp on the fast path (32 per band; a band has <= 24
+constexpr int kWgBufs     = 6;                                    // region buffers: region k of unit `it` lives in buffer (4 it + k) % 6,
+                                                                  // so the TMA fills the next unit's first K-half while this one is in use
+constexpr int kWgSlab     = kWgBufs * kWgRegion;                  //                                                        = 147456
+constexpr int kWgWBytes   = kWvStages * kBStage;                  // w_v^T hi / lo x two K-halves, the A operand            =  65536
+constexpr int kWgMmaWarps = 8;                                    // two MMA + epilogue warpgroups
+constexpr int kWgWarps    = 15;                                   // patch-gather warps (24 warps in all: 80 registers per thread)
+constexpr int kWgThreads  = (kWgMmaWarps + kWgWarps + 1) * 32;    // 768
+constexpr int kWgGroupCap = 2;                                    // position groups per warp on the fast path (30 per band; a band has <= 24
                                                                   // positions, so only positions with more than 4 entries can exceed it)
 constexpr int kWgGroupMax = 4;                                    // entries per position group: the 8 columns of mma.m16n8k16 = 4 entries x (hi, lo)
-constexpr int kWgSmem     = kWgSlab + 2048;                       //                                                        = 198656
-// tensor memory (512 columns): two accumulators of kWgN columns, then the w_v weights (A operand of the TS-form tcgen05.mma):
-// fp16 pairs along k, 64 columns for the hi halves and 64 for the lo halves
-constexpr int kWgTmemW    = 2 * kWgN;                             // 384
-constexpr int kWgMmaSplit = 1;                                    // experiment: issue every tcgen05.mma of a unit as this many column slices (2 -> N = 96,
-                                                                  // more instruction boundaries for the gather's warp-level mma): measured neutral
-static_assert((kWgN / kWgMmaSplit) % 16 == 0 && ((kWgN / kWgMmaSplit) * 128) % 1024 == 0, "slices must be valid N and start on a swizzle atom");
-static_assert(kWgTmemW + 128 <= 512, "two accumulators + the weights must fit the 512 TMEM columns");
+constexpr int kWgSmem     = kWgSlab + kWgWBytes + 2048;           //                                                        = 215040
 static_assert(kWgSmem <= 232448, "wv_gather_kernel exceeds the 227 KB of shared memory a CTA may use");
-static_assert(kWgN % 16 == 0 && kWgN <= 256 && kBandRows % kPool == 0 && kBandRows <= 32, "unit shape");
+static_assert(kWgN == 3 * 64 && kBandRows == 3 * kPool && kBandWins == 8, "unit shape: three pool groups of 8 positions x 8 windows");
 static_assert(kWgRegion % 1024 == 0, "regions must keep the 1024-byte alignment of the 128-byte swizzle");
-static_assert(kWgEpiWarps == 4 && kWgWarps % 4 == 0 && kWgWarps >= 4, "one epilogue warp per TMEM lane quarter; the first four gather warps load the weights");
 
 struct WvGatherParams {
   float* q_out;                // [n][749][128]
@@ -93,8 +76,7 @@ struct WvGatherParams {
   int groups;                  // window groups per band = n_pad / 8
   int n_units;                 // kNumBands * groups
   const int32_t* cta_split;    // [gridDim.x + 1] unit range of every CTA (api.cu wv_split: near-equal unit counts)
-  int experiment;              // timing experiments only (results become wrong): 32 = no gather work, 64 = no part_t stores, 128 = no q stores, 256 = gather reads its rows and weights but does no arithmetic, 1024 = no weight loads, 2048 = no ldmatrix
-  const uint32_t* wv_t16;      // [2 hi/lo][128 cout][64] packed fp16 pairs of w_v^T: the A operand, copied into tensor memory once per CTA
+  int experiment;              // timing experiments only (results become wrong): 32 = no gather work, 64 = no part_t stores, 128 = no q stores, 256 = gather reads its rows and weights but does no arithmetic, 1024 = no folded-weight loads, 2048 = no ldmatrix
   long long* dbg;              // optional [gridDim.x][8] cycle counters (nullptr = off), see tools/ab_stages.py --wvg-cycles
   DeviceStatus* status;
 };
@@ -116,65 +98,37 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4],
 }
 
 __global__ void __launch_bounds__(kWgThreads, 1)
-wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherParams p) {
-  constexpr uint32_t kIdesc = umma_idesc_f16(128, kWgN / kWgMmaSplit);
+wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_constant__ CUtensorMap tm_w, const WvGatherParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_a = smem;                                   // ring of kWgBufs region buffers, each [24 positions][8 windows] x 128 B
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kWgSlab);
-  uint64_t* a_full = bars;            // [kWgBufs = 8]  per buffer
-  uint64_t* a_empty = bars + 8;       // [kWgBufs = 8]
+  uint8_t* s_w = smem + kWgSlab;                         // w_v stages (K-half, hi / lo), [128 cout][128 B] each
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + kWgWBytes);
+  uint64_t* a_full = bars;            // [kWgBufs]  per buffer
+  uint64_t* a_empty = bars + 8;       // [kWgBufs]
   uint64_t* w_full = bars + 16;       // [1]
-  uint64_t* acc_full = bars + 17;     // [2]
-  uint64_t* acc_empty = bars + 19;    // [2]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 21);
   // Region k of a unit (need order: 0 hi16.k0, 1 lo16.k0, 2 hi16.k1, 3 lo16.k1) is load number g = 4 * it + k of this CTA and
   // lives in buffer g % kWgBufs; every role walks the buffers in the same order, so each keeps the first buffer of the
   // current unit (b0, advanced by 4 mod kWgBufs per unit) and one phase bit per buffer that it flips after each use.
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int kProducerWarp = kWgMmaWarps + kWgWarps;
   // contiguous range of band-major unit numbers; the split points weigh a unit by its band's entry count (host side)
   const int u_begin = p.cta_split[blockIdx.x], u_end = p.cta_split[blockIdx.x + 1];
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_band);
-    for (int i = 0; i < kWgBufs; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1 + kWgWarps); }    // tcgen05.commit + the gather warps
-    mbar_init(w_full, 4);
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], kWgEpiWarps); }
+    tma_prefetch_desc(&tm_w);
+    for (int i = 0; i < kWgBufs; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kWgMmaWarps + kWgWarps); }
+    mbar_init(w_full, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(s_tmem, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp >= 4 && warp < 8) {
-    // ===================================================================== weights -> tensor memory (once): thread = output
-    // channel (TMEM lane), columns kWgTmemW .. +63 = fp16(w_v^T) hi as 64 packed pairs along k, the next 64 = lo
-    const int cout = (warp & 3) * 32 + lane;
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-#pragma unroll 1
-    for (int part = 0; part < 4; ++part) {                  // (hi, lo) x (k 0..63, k 64..127): 32 columns each
-      const uint32_t* src = p.wv_t16 + (static_cast<size_t>(part >> 1) * kC + cout) * 64 + (part & 1) * 32;
-      uint32_t r[32];
-#pragma unroll
-      for (int i = 0; i < 32; i += 4) {
-        const uint4 v = *reinterpret_cast<const uint4*>(src + i);
-        r[i] = v.x; r[i + 1] = v.y; r[i + 2] = v.z; r[i + 3] = v.w;
-      }
-      tmem_st_32x32(lane_addr + kWgTmemW + part * 32, r);
-    }
-    tmem_wait_st();
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(w_full);
-  }
-  if (warp == 3 && lane == 0) {
-    // ===================================================================== activation producer
+  if (warp == kProducerWarp && lane == 0) {
+    // ===================================================================== weights (once), then the activation producer
+    mbar_arrive_expect_tx(w_full, kWgWBytes);
+    for (int q = 0; q < kWvStages; ++q) tma_load_2d_hint(s_w + q * kBStage, &tm_w, w_full, 0, q * 128, l2_policy_evict_last());
     const uint64_t pol = l2_policy_evict_first();
     uint32_t phases = 0;                                   // bit b: parity of buffer b's next "empty" wait is phase ^ 1
     int b0 = 0;
@@ -193,62 +147,74 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherPara
       }
       b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (converged warp, elected lane issues)
-    const uint64_t desc0 = umma_desc_sw128(0);
+  } else if (warp < kWgMmaWarps) {
+    // ===================================================================== MMA + epilogue (warpgroup g: channels 64 g .. 64 g + 63)
+    const int g = warp >> 2, wq = warp & 3;
     const uint32_t a_base = smem_u32(s_a);
-    mbar_wait(w_full, 0, p.status, 510);                      // the weights are in tensor memory
-    tc_fence_after();
-    int it = 0;
+    const uint32_t w_base = smem_u32(s_w) + g * 64 * 128;
+    const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
+    const int win0 = 2 * (lane & 3);                       // accumulator columns: windows win0, win0 + 1 of every position
+    const float oscale = p.out_scale;
+    mbar_wait(w_full, 0, p.status, 510);
     uint32_t phases = 0;
     int b0 = 0;
-    long long m_wait_full = 0, m_wait_acc = 0, tq = 0;
-    for (int unit = u_begin; unit < u_end; ++unit, ++it) {
-      const int as = it & 1;
-      const uint32_t accphase = (it >> 1) & 1;
-      const uint32_t acc = tmem_base + as * kWgN;
-      if (p.dbg) tq = clock64();
-      mbar_wait(&acc_empty[as], accphase ^ 1, p.status, 520 + as);
-      if (p.dbg) m_wait_acc += clock64() - tq;
+    float d[32];
+    for (int unit = u_begin; unit < u_end; ++unit) {
+      const int band = unit / p.groups;
+      const int w0 = (unit - band * p.groups) * kBandWins;
+      int bufs[4];
 #pragma unroll
-      for (int q = 0; q < kWvStages; ++q) {
-        // stage q = (K-half q/2, weight hi/lo q%2); hi-weight stages multiply both the hi16 and the lo16 region
-        const int kh = q >> 1;
-        int bh = b0 + 2 * kh; if (bh >= kWgBufs) bh -= kWgBufs;               // hi16 region of this K-half
-        int bl = b0 + 2 * kh + 1; if (bl >= kWgBufs) bl -= kWgBufs;           // lo16 region
-        if ((q & 1) == 0) {
-          if (p.dbg) tq = clock64();
-          mbar_wait(&a_full[bh], (phases >> bh) & 1, p.status, 530 + bh);
-          mbar_wait(&a_full[bl], (phases >> bl) & 1, p.status, 540 + bl);
-          if (p.dbg) m_wait_full += clock64() - tq;
-          phases ^= (1u << bh) | (1u << bl);
-        }
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t y0 = desc0 + ((a_base + bh * kWgRegion) >> 4);                      // B: hi16 rows
-          const uint64_t y1 = desc0 + ((a_base + bl * kWgRegion) >> 4);                      // B: lo16 rows
-          const bool w_lo = (q & 1) != 0;
-          const uint32_t wt = tmem_base + kWgTmemW + (w_lo ? 64 : 0) + kh * 32;              // A: 16 k-elements = 8 columns per MMA
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-#pragma unroll
-            for (int hs = 0; hs < kWgMmaSplit; ++hs) {           // column slice hs of the unit: rows hs * kWgN / split .. of the regions
-              constexpr uint32_t kSliceDesc = (kWgN / kWgMmaSplit) * 128 >> 4;
-              umma_f16_ts(acc + hs * (kWgN / kWgMmaSplit), wt + kk * 8, y0 + kk * 2 + hs * kSliceDesc, kIdesc, (q == 0 && kk == 0) ? 0u : 1u);
-              if (!w_lo) umma_f16_ts(acc + hs * (kWgN / kWgMmaSplit), wt + kk * 8, y1 + kk * 2 + hs * kSliceDesc, kIdesc, 1u);
-            }
-          if (!w_lo) umma_commit(&a_empty[bl]);                  // the lo16 region is only used by the hi-weight stage
-          else umma_commit(&a_empty[bh]);
-          if (q == 3) umma_commit(&acc_full[as]);
-        }
-        __syncwarp();
+      for (int k = 0; k < 4; ++k) {
+        int b = b0 + k; if (b >= kWgBufs) b -= kWgBufs;
+        bufs[k] = b;
+        mbar_wait(&a_full[b], (phases >> b) & 1, p.status, 530 + b);
+        phases ^= 1u << b;
       }
+#pragma unroll 1
+      for (int pg = 0; pg < kBandRows / kPool; ++pg) {          // pool group pg = rows 64 pg .. 64 pg + 63 of every region
+        wgmma_fence();
+#pragma unroll 1
+        for (int kh = 0; kh < 2; ++kh) {
+          const uint64_t yh = gmma_desc_sw128(a_base + bufs[2 * kh] * kWgRegion + pg * 64 * 128);       // B: hi16 rows
+          const uint64_t yl = gmma_desc_sw128(a_base + bufs[2 * kh + 1] * kWgRegion + pg * 64 * 128);   // B: lo16 rows
+          const uint64_t whi = gmma_desc_sw128(w_base + (2 * kh) * kBStage);                            // A: w_v^T hi
+          const uint64_t wlo = gmma_desc_sw128(w_base + (2 * kh + 1) * kBStage);                        // A: w_v^T lo
+          // the order of conv_t_kernel<true> and layer1_wv_kernel, so that all three produce bit-identical q
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            wgmma_f16_n64(d, whi + kk * 2, yh + kk * 2, (kh == 0 && kk == 0) ? 0u : 1u);
+            wgmma_f16_n64(d, whi + kk * 2, yl + kk * 2, 1u);
+          }
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) wgmma_f16_n64(d, wlo + kk * 2, yh + kk * 2, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(d);
+        // register 4 i + 2 h + e = channel ch0 + 8 h, position i of the pool group, window win0 + e
+        const int gg = band * (kBandRows / kPool) + pg;
+        if (gg < kPooled && !(p.experiment & 128)) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float m = d[2 * h + e];
+#pragma unroll
+              for (int i = 1; i < kPool; ++i) m = fmaxf(m, d[4 * i + 2 * h + e]);
+              const int w = w0 + win0 + e;
+              if (w < p.n_windows) p.q_out[(static_cast<size_t>(w) * kPooled + gg) * kC + ch0 + 8 * h] = m * oscale;
+            }
+        }
+      }
+      __syncwarp();
+      if (lane == 0)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) mbar_arrive(&a_empty[bufs[k]]);
       b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
     }
-    if (p.dbg && lane == 0) { p.dbg[blockIdx.x * 8 + 6] = m_wait_full; p.dbg[blockIdx.x * 8 + 7] = m_wait_acc; }
-  } else if (warp >= 4 && warp < 4 + kWgWarps) {
+  } else if (warp >= kWgMmaWarps && warp < kWgMmaWarps + kWgWarps) {
     // ===================================================================== patch gather
-    const int gw = warp - 4;                                   // 0..15
+    const int gw = warp - kWgMmaWarps;                         // 0..14
     const float gscale = p.gather_unscale;
     // Gather lane roles.  ldmatrix: lanes 8i..8i+7 address matrix i = (plane i & 1: 0 hi16 / 1 lo16, 16-byte chunk i >> 1 of the
     // k-step), row lane & 7 = window.  The A fragment then holds rows 0..7 = the 8 windows' hi16 halves and rows 8..15 = their
@@ -280,8 +246,8 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherPara
         if (p.experiment & 2048) { a[ks][0] = a[ks][1] = a[ks][2] = a[ks][3] = rb; continue; }
         ldsm_x4(rb + (((ks * 2 + lm_chunk) ^ lm_win) << 4), a[ks]);     // 128-byte swizzle: chunk j -> j ^ (row & 7)
       }
-      // four independent accumulators: the warp-level mma shares the tensor pipe with the tcgen05.mma stream and waits long for its
-      // turn, so no mma of a group depends on another one
+      // four independent accumulators: the warp-level mma shares the tensor pipe with the wgmma stream, so no mma of a group
+      // depends on another one
       float d[4][4];
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) d[ks][0] = d[ks][1] = d[ks][2] = d[ks][3] = 0.f;
@@ -300,7 +266,7 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherPara
     for (int unit = u_begin; unit < u_end; ++unit, ++it) {
       const int band = unit / p.groups;
       const int w0 = (unit - band * p.groups) * kBandWins;
-      if (band != cur_band) {                                  // this warp's position groups of the band: gw, gw + 20, ...
+      if (band != cur_band) {                                  // this warp's position groups of the band: gw, gw + 15, ...
         cur_band = band;
         g_first = p.band_gstart[band];
         g_cnt = (p.experiment & 32) ? 0 : p.band_gstart[band + 1] - g_first;
@@ -336,7 +302,7 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherPara
                 p.part_t[static_cast<size_t>(my_e0[i] + tig) * p.n_pad + w0 + gid] = c0[i] + v;
             }
         } else {
-          // generic path (a band with more than 40 position groups: only patch sets that put more than 4 entries on many
+          // generic path (a band with more than 30 position groups: only patch sets that put more than 4 entries on many
           // positions): pass-0 halves are parked in part_t itself (the same thread reads them back in pass 1)
 #pragma unroll 1
           for (int gi = gw; gi < g_cnt; gi += kWgWarps) {
@@ -354,66 +320,10 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const WvGatherPara
       }
       b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
     }
-    if (p.dbg && warp == 4 && lane == 0) {
+    if (p.dbg && warp == kWgMmaWarps && lane == 0) {
       long long* d = p.dbg + blockIdx.x * 8;
       d[0] = clock64() - t_begin; d[1] = c_wait_full; d[2] = c_gather; d[5] = it;
     }
-  } else if (warp >= 4 + kWgWarps) {
-    // ===================================================================== accumulator epilogue
-    const int wq = warp & 3;                                   // TMEM lane quarter = channels 32*wq .. 32*wq+31
-    const int ch = wq * 32 + lane;
-    const float oscale = p.out_scale;
-    long long c_wait_acc = 0, c_epi = 0, tq = 0;
-    int it = 0;
-    for (int unit = u_begin; unit < u_end; ++unit, ++it) {
-      const int band = unit / p.groups;
-      const int w0 = (unit - band * p.groups) * kBandWins;
-      // ---------------- epilogue: q[w][band*3 + g][ch] = max over the 8 positions of pool group g.  Accumulator column
-      // n = 8 * (position inside the band) + window, so pool group g is columns 64 g .. 64 g + 63 and a thread (= channel) takes the
-      // maximum over the 8 registers with stride 8 that belong to one window.
-      const int as = it & 1;
-      const uint32_t accphase = (it >> 1) & 1;
-      if (p.dbg) tq = clock64();
-      mbar_wait(&acc_full[as], accphase, p.status, 570 + as);
-      if (p.dbg) { const long long t = clock64(); c_wait_acc += t - tq; tq = t; }
-      tc_fence_after();
-#pragma unroll 1
-      for (int g = 0; g < kBandRows / kPool; ++g) {
-        const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(wq * 32) << 16) + as * kWgN + g * (kPool * kBandWins);
-        float m[kBandWins];
-        uint32_t r[32], r2[32];
-        tmem_ld_32x32(lane_addr, r);                           // positions 0..3 of the pool group x 8 windows
-        tmem_ld_32x32(lane_addr + 32, r2);                     // positions 4..7
-        tmem_wait_ld();
-#pragma unroll
-        for (int w = 0; w < kBandWins; ++w) {
-          const float ma = fmaxf(fmaxf(__uint_as_float(r[w]), __uint_as_float(r[8 + w])), fmaxf(__uint_as_float(r[16 + w]), __uint_as_float(r[24 + w])));
-          const float mb = fmaxf(fmaxf(__uint_as_float(r2[w]), __uint_as_float(r2[8 + w])), fmaxf(__uint_as_float(r2[16 + w]), __uint_as_float(r2[24 + w])));
-          m[w] = fmaxf(ma, mb);
-        }
-        const int gg = band * (kBandRows / kPool) + g;
-        if (gg < kPooled && !(p.experiment & 128)) {
-#pragma unroll
-          for (int w = 0; w < kBandWins; ++w)
-            if (w0 + w < p.n_windows) p.q_out[(static_cast<size_t>(w0 + w) * kPooled + gg) * kC + ch] = m[w] * oscale;
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[as]);
-      if (p.dbg) c_epi += clock64() - tq;
-    }
-    if (p.dbg && wq == 0 && lane == 0) {
-      long long* d = p.dbg + blockIdx.x * 8;
-      d[3] = c_wait_acc; d[4] = c_epi;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

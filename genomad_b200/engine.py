@@ -4,8 +4,8 @@ ctypes binding of libgnm.so (C ABI: include/gnm.h) and the ``Classifier`` object
 This is the device-facing half of the drop-in: ``Classifier`` plays the role of the Keras model the
 reference builds with ``neural_network.create_classifier()`` + ``load_weights`` and calls with
 ``predict(batch)`` (reference genomad/modules/nn_classification.py:309-317).  Tensors live in PyTorch
-(device memory, streams); all arithmetic happens in the hand-written sm_100a kernels of libgnm.so.
-There is no CPU or PyTorch fallback: if the library or a B200 is missing, construction fails.
+(device memory, streams); all arithmetic happens in the hand-written sm_90a kernels of libgnm.so.
+There is no CPU or PyTorch fallback: if the library or an H100 is missing, construction fails.
 """
 from __future__ import annotations
 
@@ -117,7 +117,7 @@ def _ptr(a: np.ndarray) -> int:
 
 class Classifier:
     """
-    The IGLOO1D classifier on one B200.
+    The IGLOO1D classifier on one H100.
 
     weights : dict from genomad_b200.weights.load_weights() (short names -> numpy arrays in Keras layouts)
     device  : CUDA device index
@@ -127,7 +127,7 @@ class Classifier:
     def __init__(self, weights: Optional[Dict[str, np.ndarray]] = None, device: int = 0, max_batch: int = 1024):
         import torch
         if not torch.cuda.is_available():
-            raise GnmError("no CUDA device visible: genomad_b200 runs on B200 (sm_100a) only, there is no CPU fallback")
+            raise GnmError("no CUDA device visible: genomad_b200 runs on H100 (sm_90a) only, there is no CPU fallback")
         self._torch = torch
         self.lib = load_library()
         self.device = int(device)

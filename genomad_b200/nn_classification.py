@@ -5,11 +5,11 @@
 skip/restart/cleanup semantics, same error behaviour (message + sys.exit(1)).
 
 What changed underneath: the FASTA is indexed once by the native reader (csrc/fasta.cpp: mmap, no copy); its 6 kb
-windows are streamed through pinned chunks to the B200 (the host fills chunk i+1 while the GPU classifies chunk i),
-tokenised and classified by libgnm.so (hand-written sm_100a kernels) and reduced per contig on the device.
+windows are streamed through pinned chunks to the GPU (the host fills chunk i+1 while the GPU classifies chunk i),
+tokenised and classified by libgnm.so (hand-written sm_90a kernels) and reduced per contig on the device.
 ``--batch-size`` keeps the reference's meaning -- an upper bound on the memory one prediction step may use -- but no
 longer sets the device step: the library steps through >= 1024 windows at a time whatever the option says (the
-reference's default of 128 would pay the fixed per-step cost 8x as often for no benefit on a 180 GB part).  TensorFlow, TFRecords and the per-batch ``predict`` call are gone; the
+reference's default of 128 would pay the fixed per-step cost 8x as often for no benefit on an 80 GB part).  TensorFlow, TFRecords and the per-batch ``predict`` call are gone; the
 "encoded sequences" directory only records which window belongs to which sequence.  With torchrun (WORLD_SIZE > 1)
 windows are sharded across GPUs and combined over NCCL (genomad_b200.dist); rank 0 writes the outputs.
 """
@@ -37,8 +37,8 @@ _WORKSPACE_BYTES_PER_WINDOW = 7.0e6          # libgnm workspace per window of ma
 
 def device_step(batch_size: int, free_bytes: int) -> int:
     """Windows per internal GPU step.  `--batch-size` (reference cli.py:757-764: "smaller value to reduce memory") only
-    bounds memory in the reference; here the step is max(batch_size, 1024) capped at 4096 -- throughput is flat from 512 up
-    (profiles/r01_batch_sweep.md) -- and halved until its workspace fits in half of the free HBM."""
+    bounds memory in the reference; here the step is max(batch_size, 1024) capped at 4096, and halved until its workspace fits
+    in half of the free HBM."""
     step = min(DEVICE_STEP_MAX, max(DEVICE_STEP_MIN, int(batch_size)))
     while step > 64 and step * _WORKSPACE_BYTES_PER_WINDOW > 0.5 * free_bytes:
         step //= 2
@@ -56,7 +56,7 @@ def release_classifiers() -> None:
 
 
 def _make_classifier(batch_size: int, device: int):
-    """Factory (patched in CPU tests): the real one needs a B200 and libgnm.so -- no fallback.
+    """Factory (patched in CPU tests): the real one needs an H100 and libgnm.so -- no fallback.
     The classifier (weights re-packed on the device + workspace, ~0.3 s to build and ~0.4 s to free) stays resident between
     main() calls of one process -- `genomad end-to-end`, a service, the provirus twin -- unless GENOMAD_B200_KEEP_MODEL=0."""
     import torch

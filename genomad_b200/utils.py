@@ -162,7 +162,7 @@ def check_provirus_execution(prefix: str, input_file: Path, output_dir: Path) ->
 
 def display_header(console: HybridConsole, version: str, module_name: str, description: str, output_dir: Path,
                    files: Iterable[Path], descriptions: Iterable[str]) -> None:
-    console.print(f"Executing geNomad {module_name} (B200 build v{version}). {description}")
+    console.print(f"Executing geNomad {module_name} (H100 build v{version}). {description}")
     console.print("Outputs:")
     console.print(f"  {output_dir}")
     for f, d in zip(files, descriptions):

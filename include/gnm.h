@@ -1,5 +1,5 @@
 /*
- * gnm.h -- C ABI of libgnm.so: the B200 (sm_100a) implementation of geNomad's
+ * gnm.h -- C ABI of libgnm.so: the H100 (sm_90a) implementation of geNomad's
  * nn-classification hot path.
  *
  * The reference has no FFI: its hot path is Python calling TensorFlow/Keras and numba
@@ -15,7 +15,7 @@
  *     asynchronous with respect to the host unless stated otherwise; the caller owns all
  *     input/output buffers and the stream.
  *   - one handle per (device, stream user); calls on one handle are not thread-safe.
- *   - there is NO CPU fallback: every compute entry point fails if no sm_100 device is present.
+ *   - there is NO CPU fallback: every compute entry point fails if no sm_90 device is present.
  */
 #ifndef GNM_H_
 #define GNM_H_
@@ -73,7 +73,7 @@ typedef struct gnm_weights {
 /* Thread-local description of the last failure on the calling thread. */
 const char* gnm_last_error(void);
 
-/* Library / build information, e.g. "libgnm 0.3 (sm_100a; ...)". */
+/* Library / build information, e.g. "libgnm 0.4 (sm_90a; ...)". */
 const char* gnm_version(void);
 
 /*
@@ -185,7 +185,7 @@ uint32_t gnm_crc32c(const void* data, size_t n);
 
 /* ---- introspection / test hooks (not needed by a drop-in caller) ------------------------- */
 
-/* Options: "conv_impl" 0 = tcgen05 tensor-core path (default), 1 = fp32 CUDA-core validation
+/* Options: "conv_impl" 0 = wgmma tensor-core path (default), 1 = fp32 CUDA-core validation
  * kernels (test hook: lets the tensor-core path be checked on the GPU at large batch);
  * "debug_stop" 0 = full pipeline, 1 = stop after layer 1 + gather#0, 2 = after conv2, 3 = after conv3;
  * "profile_stages" 1 = record a CUDA event between stages (see gnm_stage_times);

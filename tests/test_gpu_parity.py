@@ -1,5 +1,5 @@
 """
-GPU parity tests (run with `-m gpu` on a B200): the CUDA path, called through the C ABI of libgnm.so,
+GPU parity tests (run with `-m gpu` on an H100): the CUDA path, called through the C ABI of libgnm.so,
 against the CPU oracle and the committed golden fixtures.
 
 Tolerances: tokens are bit-exact; per-window probabilities are within 1e-4 (absolute) of the fp32 oracle
@@ -133,7 +133,7 @@ def test_stagewise_parity_synthetic(clf_syn, shipped):
 
 
 def test_tensor_core_path_vs_cuda_core_validation_kernels(clf):
-    """512 windows: tcgen05 fp16x3 path vs the independent fp32 FFMA kernels, both on the GPU."""
+    """512 windows: wgmma fp16x3 path vs the independent fp32 FFMA kernels, both on the GPU."""
     a = torch.from_numpy(_families(512, seed=33)).cuda()
     p_tc = clf.predict_ascii(a).clone()
     try:
@@ -319,7 +319,7 @@ def test_module_tfrecord_intermediates_and_aggregation(tmp_path, shipped, monkey
 
 @pytest.mark.gpu
 def test_fused_layer1_wv_option(shipped):
-    """Option fuse_l1=1 (layer 1 + w_v#0 in one tcgen05 kernel whose B operand is written by SIMT producers in the TMA
+    """Option fuse_l1=1 (layer 1 + w_v#0 in one wgmma kernel whose B operand is written by SIMT producers in the TMA
     swizzle layout) must reproduce the two separate kernels bit for bit: y1, q0 and the final probabilities, from ASCII
     and from tokens, incl. N-rich / padded windows and a batch that leaves the last unit of every window partial."""
     import torch

@@ -125,7 +125,7 @@ def main():
     procs = args.procs or max(1, min(24, cores // 8))
     threads = max(1, min(8, cores // procs))
     lines = [f"# Parity sweep (round 2): CUDA path vs the fp32 CPU oracle\n",
-             f"`python tools/parity_sweep.py --n {args.n} --n-syn {args.n_syn}` on 1 x B200; oracle on {procs} processes x {threads} torch "
+             f"`python tools/parity_sweep.py --n {args.n} --n-syn {args.n_syn}` on 1 x H100; oracle on {procs} processes x {threads} torch "
              f"threads ({cores} host cores); CUDA path through `gnm_forward_ascii` with a max_batch = 1024 handle.  "
              "|dp| = max over the 3 classes of |p_cuda - p_oracle| per window.\n"]
     worst = 0.0

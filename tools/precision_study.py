@@ -3,7 +3,7 @@
 Operand-precision study for the tensor-core stages (CPU emulation, fp64 accumulation).
 
 Question: which operand formats can conv2/conv3 (K=768) and the w_v projection (K=128)
-use on tcgen05 and still keep per-window |dp| <= 1e-4 against the fp32/fp64 oracle?
+use on the tensor cores and still keep per-window |dp| <= 1e-4 against the fp32/fp64 oracle?
 Each recipe rounds the MMA operands the way the kernel would and evaluates the rest of
 the network in fp64.  Output: a markdown table on stdout.
 

@@ -5,7 +5,7 @@
 // plane of the 8 windows, rows 8-15 = lo16 plane; B = fp16 hi / lo halves of up to 8 entries' folded weights) reproduce the patch
 // gather's dot products?  Also checks the fall-back: a 2-D map (bytes of one window, windows) with one 1 KB box per position.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -o /tmp/tma_probe tools/tma_order_probe.cu -lcuda && /tmp/tma_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -o tma_probe tools/tma_order_probe.cu -lcuda && ./tma_probe
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

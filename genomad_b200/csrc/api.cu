@@ -89,6 +89,7 @@ struct gnm_handle {
   int32_t* band_gstart[2] = {nullptr, nullptr};      // [kNumBands + 1] first position group of every band
   uint4* wfrag[2] = {nullptr, nullptr};              // [kGsSlots][2][4][4] folded weights as mma.m16n8k16 B fragments (fp16 hi / lo halves)
   float gather_unscale[2] = {1.f, 1.f};              // 1 / the power of two applied to the folded weights before the fp16 split
+  float wv_out_scale[2] = {1.f, 1.f};                // 2^-e / 32: undoes the power of two applied to w_v before its fp16 split
   std::vector<int32_t> band_groups[2];               // host copy: position groups per band (cost model of wv_gather_kernel's unit split)
   int32_t* cta_split = nullptr;                      // [num_sms + 1] device: unit range per CTA of the current launch
   std::vector<int32_t> split_host[2];                // host copy of the last split per IGLOO kernel (source of the async upload)
@@ -200,24 +201,27 @@ static int make_f32_map(PFN_encodeTiled enc, CUtensorMap* tm, float* base, int i
   return 0;
 }
 
-// One 16 KB fp16 TMA stage: B[n][kk] = fp16(part(W[k = kh*64 + kk][n]) * scale), part = hi or lo of the fp16 split.
+// One 16 KB fp16 TMA stage: B[n][kk] = fp16(part(W[k = kh*64 + kk][n] * scale)), part = hi or lo of the fp16 split.  The split
+// is taken of the scaled weight (scale is a power of two), so weights far below 1 keep their precision instead of falling into
+// fp16's subnormal range.
 static void pack_stage_f16(std::vector<uint8_t>& dst, const float* Wkn /* [128 k][128 n] */, int w_lo, int kh, float scale) {
   for (int n = 0; n < kC; ++n)
     for (int kk = 0; kk < 64; ++kk) {
-      const float x = Wkn[static_cast<size_t>(kh * 64 + kk) * kC + n];
+      const float x = Wkn[static_cast<size_t>(kh * 64 + kk) * kC + n] * scale;
       const __half hi = __float2half_rn(x);
-      const float v = (w_lo ? x - __half2float(hi) : __half2float(hi)) * scale;
+      const float v = w_lo ? x - __half2float(hi) : __half2float(hi);
       const uint16_t bits = __half_as_ushort(__float2half_rn(v));
       dst.push_back(static_cast<uint8_t>(bits & 0xff));
       dst.push_back(static_cast<uint8_t>(bits >> 8));
     }
 }
 // One 16 KB e4m3 TMA stage of the correction passes: B[n][2c + s] for the 64 input channels c of K-half kh, interleaved like the
-// activation pairs (common.cuh): s = 0 multiplies lo8(A) -> e4m3(Whi * scale_hi), s = 1 multiplies hi8(A) -> e4m3(Wlo * scale_lo).
-static void pack_stage_f8_pairs(std::vector<uint8_t>& dst, const float* Wkn, int kh, float scale_hi, float scale_lo) {
+// activation pairs (common.cuh): with x = W * scale split into hi = fp16(x) and lo = x - hi (the main pass's split),
+// s = 0 multiplies lo8(A) -> e4m3(hi * scale_hi), s = 1 multiplies hi8(A) -> e4m3(lo * scale_lo).
+static void pack_stage_f8_pairs(std::vector<uint8_t>& dst, const float* Wkn, int kh, float scale, float scale_hi, float scale_lo) {
   for (int n = 0; n < kC; ++n)
     for (int c = 0; c < 64; ++c) {
-      const float x = Wkn[static_cast<size_t>(kh * 64 + c) * kC + n];
+      const float x = Wkn[static_cast<size_t>(kh * 64 + c) * kC + n] * scale;
       const float hi = __half2float(__float2half_rn(x));
       dst.push_back(static_cast<uint8_t>(__nv_cvt_float_to_fp8(hi * scale_hi, __NV_SATFINITE, __NV_E4M3)));
       dst.push_back(static_cast<uint8_t>(__nv_cvt_float_to_fp8((x - hi) * scale_lo, __NV_SATFINITE, __NV_E4M3)));
@@ -372,12 +376,14 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
   {
     const float* convw[2] = {w->conv2_kernel, w->conv3_kernel};
     for (int L = 0; L < 2; ++L) {
-      // common scale 2^S of the three passes (conv_t.cuh): main weights fp16(Whi * 2^d), d = 16 for |W| < 0.78
+      // common scale 2^S of the three passes (conv_t.cuh): main weights fp16(W * 2^d) with wmax * 2^d in (0.39, 0.78] * 2^16, so
+      // the fp16 plane and both e4m3 planes (|hi| * 2^-7 <= 400 < 448) stay in range.  Small weights get d > 16: with d fixed at
+      // 16 the e4m3 plane of their lo halves fell into the subnormal range and the Ahi * Wlo correction stopped correcting.
       float wmax = 0.f;
       for (size_t i = 0; i < static_cast<size_t>(kTaps) * kC * kC; ++i) wmax = std::max(wmax, std::fabs(convw[L][i]));
       if (!(wmax > 0.f) || !std::isfinite(wmax)) return fail("gnm_create: conv kernel is all-zero or not finite");
-      const int shift = std::max(0, static_cast<int>(std::ceil(std::log2(wmax / 0.78f))));
-      const int d = 16 - shift, S = 5 + d;
+      const int shift = static_cast<int>(std::ceil(std::log2(wmax / 0.78f)));
+      const int d = std::min(16 - shift, 40), S = 5 + d;
       if (d < 1) return fail("gnm_create: conv weights too large for the fp16 operand format");
       h->conv_out_scale[L] = std::ldexp(1.f, -S);
       std::vector<uint8_t> pk;                              // (region, tap): hi16.k0 x6, hi16.k1 x6, pairs.k0 x6, pairs.k1 x6
@@ -386,15 +392,23 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
         for (int tap = 0; tap < kTaps; ++tap)
           pack_stage_f16(pk, convw[L] + static_cast<size_t>(tap) * kC * kC, 0, kh, std::ldexp(1.f, d));
       for (int kh = 0; kh < 2; ++kh)                        // x (lo8, hi8) = (e4m3(Alo * 2^12), e4m3(Ahi * 2^7)):  (e4m3(Whi * 2^(S-12)), e4m3(Wlo * 2^(S-7)))
-        for (int tap = 0; tap < kTaps; ++tap)
-          pack_stage_f8_pairs(pk, convw[L] + static_cast<size_t>(tap) * kC * kC, kh, std::ldexp(1.f, S - 12), std::ldexp(1.f, S - 7));
+        for (int tap = 0; tap < kTaps; ++tap)                //   = (e4m3(hi * 2^(S-12-d)), e4m3(lo * 2^(S-7-d))) of the split of W * 2^d
+          pack_stage_f8_pairs(pk, convw[L] + static_cast<size_t>(tap) * kC * kC, kh, std::ldexp(1.f, d), std::ldexp(1.f, S - 12 - d),
+                              std::ldexp(1.f, S - 7 - d));
       if (dev_upload(h, &h->wpack[L], pk.data(), pk.size())) return 1;
       if (dev_upload(h, &h->conv_w32[L], convw[L], static_cast<size_t>(kTaps) * kC * kC)) return 1;
     }
-    for (int s = 0; s < 2; ++s) {                          // w_v: (K-half, weight hi/lo), unscaled fp16
+    for (int s = 0; s < 2; ++s) {                          // w_v: (K-half, weight hi/lo) of the fp16 split of w_v * 2^e
+      // e moves max |w_v| to [2^13, 2^14) (as for the patch weights): unscaled, the lo halves of small weights (|w| < 0.125)
+      // fall into fp16's subnormal range and the Ahi * Wlo pass stops correcting.  The q epilogues multiply by 2^-e / 32.
+      float wmax = 0.f;
+      for (int i = 0; i < kC * kC; ++i) wmax = std::max(wmax, std::fabs(w->igloo[s].w_v[i]));
+      int e = 0;
+      if (wmax > 0.f && std::isfinite(wmax)) { int ex; std::frexp(wmax, &ex); e = std::max(-24, std::min(40, 14 - ex)); }
+      h->wv_out_scale[s] = std::ldexp(1.f / kActScale, -e);
       std::vector<uint8_t> pk;
       for (int kh = 0; kh < 2; ++kh)
-        for (int w_lo = 0; w_lo < 2; ++w_lo) pack_stage_f16(pk, w->igloo[s].w_v, w_lo, kh, 1.f);
+        for (int w_lo = 0; w_lo < 2; ++w_lo) pack_stage_f16(pk, w->igloo[s].w_v, w_lo, kh, std::ldexp(1.f, e));
       if (dev_upload(h, &h->wpack[2 + s], pk.data(), pk.size())) return 1;
     }
     if (dev_upload(h, &h->conv_bias[0], w->conv2_bias, kC)) return 1;
@@ -631,7 +645,7 @@ static int launch_wv_tc(gnm_handle* h, int s, int buf, int n, cudaStream_t st) {
   p.experiment = 0;
   p.dbg = nullptr;
   p.bias = nullptr; p.y_out = nullptr; p.q_out = h->q[s];
-  p.out_scale = 1.f / kActScale;
+  p.out_scale = h->wv_out_scale[s];
   p.out_fp8 = 0;
   p.n_tiles = n * kUnitsPerWin;
   const int grid = std::min(h->num_sms, p.n_tiles);
@@ -672,7 +686,7 @@ static int wv_split(gnm_handle* h, int s, int groups, int grid, cudaStream_t st)
 // IGLOO kernel s on y[buf]: q[s] = maxpool8(y @ w_v#s) and mpi[s] (patch gather) in ONE pass over the activations
 static int launch_wv_gather(gnm_handle* h, int s, int buf, int n, cudaStream_t st) {
   WvGatherParams p;
-  p.q_out = h->q[s]; p.out_scale = 1.f / kActScale;
+  p.q_out = h->q[s]; p.out_scale = h->wv_out_scale[s];
   p.grp = h->grp[s]; p.band_gstart = h->band_gstart[s]; p.wfrag = h->wfrag[s]; p.gather_unscale = h->gather_unscale[s]; p.part_t = h->part;
   p.n_windows = n;
   p.n_pad = (n + kBandWins - 1) / kBandWins * kBandWins;
@@ -811,7 +825,7 @@ static int forward_main(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d
     timer_mark(h, "layer1_wv0", st);
     FusedParams fp;
     fp.ascii = d_ascii; fp.tokens = d_tok; fp.table = h->conv1_table; fp.triple = h->conv1_triple; fp.bias = h->conv1_bias;
-    fp.y_out = h->ybuf[0]; fp.q_out = h->q[0]; fp.n_units = n * kFuUnitsPerWin; fp.status = h->status;
+    fp.y_out = h->ybuf[0]; fp.q_out = h->q[0]; fp.q_scale = h->wv_out_scale[0]; fp.n_units = n * kFuUnitsPerWin; fp.status = h->status;
     const int grid = std::min(h->num_sms, fp.n_units);
     if (d_ascii) layer1_wv_kernel<true><<<grid, kFuThreads, kFuSmem, st>>>(h->tm_w[2], fp);
     else layer1_wv_kernel<false><<<grid, kFuThreads, kFuSmem, st>>>(h->tm_w[2], fp);
@@ -1134,6 +1148,7 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
   } else if (k == "q0" || k == "q1") { src = h->q[k == "q1"]; count = static_cast<size_t>(n) * kPooled * kC; }
   else if (k == "mpi0" || k == "mpi1") { src = h->mpi[k == "mpi1"]; count = static_cast<size_t>(n) * kPatches; }
   else if (k == "h0") { src = h->h0; count = static_cast<size_t>(n) * 256; }
+  else if (k == "h1" || k == "h2") { src = k == "h1" ? h->h1 : h->h2; count = static_cast<size_t>(n) * kHidden; }
   else if (k == "logits") { src = h->logits; count = static_cast<size_t>(n) * kLogitsLd; }
   else if (k == "conv_dbg") { src = reinterpret_cast<const float*>(h->conv_dbg); count = static_cast<size_t>(h->num_sms) * 16; }
   else return fail("gnm_debug_fetch: unknown buffer " + k);

@@ -15,7 +15,7 @@
 //   * convs: the main pass Ahi*Bhi in fp16; the two correction passes only need ~8 bits, so they run in
 //     e4m3 (K = 32 per instruction: twice the rate) on pre-scaled operands.  All passes are
 //     scaled to a common 2^S so they add up in the same accumulator, and the epilogue multiplies by 2^-S:
-//         main  : (32*Ahi)            x fp16(Whi * 2^d)          S = 5 + d          (d = 16 for |W| < 0.78)
+//         main  : (32*Ahi)            x fp16(W * 2^d)            S = 5 + d          (wmax * 2^d in (0.39, 0.78] * 2^16)
 //         corr1 : e4m3(Alo * 2^12)    x e4m3(Whi * 2^(S-12))
 //         corr2 : e4m3(Ahi * 2^7)     x e4m3(Wlo * 2^(S-7))
 //     CPU emulation of exactly this recipe: max |dp| 6.5e-6 over 256 worst-case-family windows.
@@ -76,7 +76,7 @@ struct ConvTcParams {
   const float* bias;        // [128] (conv) or nullptr (w_v)
   uint8_t* y_out;           // [n][5997][768 B] (conv) or nullptr
   float* q_out;             // [n][749][128] (w_v) or nullptr
-  float out_scale;          // conv: 2^-S (undoes the common operand scaling); w_v: 1/32 (activation scale)
+  float out_scale;          // conv: 2^-S (undoes the common operand scaling); w_v: 2^-e / 32 (w_v operand scaling, activation scale)
   int out_fp8;              // conv: 1 = write hi16 + lo8 + hi8 (consumer is a conv), 0 = write hi16 + lo16
   int n_tiles;              // number of work units = n_windows * 24
   int experiment;           // timing experiments only (results become wrong): 2 = no epilogue global stores

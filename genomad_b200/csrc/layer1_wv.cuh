@@ -48,6 +48,7 @@ struct FusedParams {
   const float* bias;         // [128]
   uint8_t* y_out;            // [n][5997][768 B]
   float* q_out;              // [n][749][128]
+  float q_scale;             // 2^-e / 32: undoes the operand scaling of the w_v pack and the activation scale
   int n_units;               // n_windows * 63
   DeviceStatus* status;
 };
@@ -180,7 +181,7 @@ layer1_wv_kernel(const __grid_constant__ CUtensorMap tm_w, const FusedParams p) 
     }
     const uint32_t slab_base = smem_u32(s_slab), w_base = smem_u32(s_w) + g * 64 * 128;
     const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
-    const float oscale = 1.f / kActScale;
+    const float oscale = p.q_scale;
     mbar_wait(w_full, 0, p.status, 430);
     int it = 0;
     float d[24];

@@ -66,7 +66,7 @@ static_assert(kWgRegion % 1024 == 0, "regions must keep the 1024-byte alignment 
 
 struct WvGatherParams {
   float* q_out;                // [n][749][128]
-  float out_scale;             // 1/32 (activation scale)
+  float out_scale;             // 2^-e / 32 (w_v operand scaling, activation scale)
   const int2* grp;             // [groups of all bands] {first entry slot, row inside the band | entries << 8}: the entries (<= 4) on one position
   const int32_t* band_gstart;  // [kNumBands + 1] first position group of every band
   const uint4* wfrag;          // [kGsSlots][2 K-halves][4 k-steps][4 tig] folded weights * 2^k as mma.m16n8k16 B fragments {hi b0, hi b1, lo b0, lo b1}: a lane reads the (b0, b1) pair of its column

@@ -258,7 +258,7 @@ class Classifier:
     def debug_fetch(self, which: str, n: int):
         t = self._torch
         shapes = {"buf0": (n, TOKENS, 128), "buf1": (n, TOKENS, 128), "q0": (n, 749, 128), "q1": (n, 749, 128),
-                  "mpi0": (n, 2100), "mpi1": (n, 2100), "h0": (n, 256), "logits": (n, 752),
+                  "mpi0": (n, 2100), "mpi1": (n, 2100), "h0": (n, 256), "h1": (n, 512), "h2": (n, 512), "logits": (n, 752),
                   "conv_dbg": (self.get_option("num_sms"), 16)}
         out = t.empty(shapes[which], dtype=t.float32, device=self._dev())
         _check(self.lib, self.lib.gnm_debug_fetch(self._h, which.encode(), n, out.data_ptr(), self._stream()))

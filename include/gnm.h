@@ -238,8 +238,9 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  * Copy an intermediate of the most recent forward step (first n <= max_batch windows) to a device
  * buffer as fp32.  which: "buf0","buf1" = the two activation buffers [n][5997][128] (after a full
  * step buf0 = y3, buf1 = y2; with debug_stop = 1, buf0 = y1); "q0","q1" [n][749][128];
- * "mpi0","mpi1" [n][2100]; "logits" [n][752]; "h0" [n][256]; "conv_dbg" [num_sms][16] (int64 counters viewed as
- * float pairs).  Used by the per-kernel parity tests and tools/gpu_experiment.py.
+ * "mpi0","mpi1" [n][2100]; "logits" [n][752] (of the second IGLOO kernel after a full step); "h0" [n][256];
+ * "h1","h2" [n][512] = the outputs of the two Dense(512) + BatchNorm + ReLU layers of the head;
+ * "conv_dbg" [num_sms][16] (int64 counters viewed as float pairs).  Used by the per-kernel parity tests and tools/gpu_experiment.py.
  */
 int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream);
 

@@ -115,7 +115,8 @@ struct gnm_handle {
   cudaEvent_t in_ready[2] = {nullptr, nullptr}, in_free[2] = {nullptr, nullptr};
   DeviceStatus* status = nullptr;                    // pinned host memory, device-visible
   CUtensorMap tm_act[2];
-  CUtensorMap tm_w[4];
+  CUtensorMap tm_w[4];                               // weight packs, one 16 KB stage per box
+  CUtensorMap tm_w_half[4];                          // the same packs, one warpgroup's 8 KB half-stage per box (conv_t_kernel)
   StageTimer timer;
   std::vector<void*> allocs;
 };
@@ -175,11 +176,11 @@ static int make_band_map(PFN_encodeTiled enc, CUtensorMap* tm, uint8_t* base, in
   if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(activation bands) failed: " + std::to_string(int(r)));
   return 0;
 }
-// packed weights [stages*128 rows][128 B]; box = 128 B x 128 rows
-static int make_w_map(PFN_encodeTiled enc, CUtensorMap* tm, uint8_t* base, int n_stages) {
+// packed weights [stages*128 rows][128 B]; box = 128 B x box_rows
+static int make_w_map(PFN_encodeTiled enc, CUtensorMap* tm, uint8_t* base, int n_stages, int box_rows) {
   cuuint64_t dims[2] = {128, static_cast<cuuint64_t>(n_stages) * 128};
   cuuint64_t strides[1] = {128};
-  cuuint32_t box[2] = {128, 128};
+  cuuint32_t box[2] = {128, static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -526,10 +527,11 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
     if (make_act_map(enc, &h->tm_act[i], h->ybuf[i], max_batch)) return 1;
     if (make_band_map(enc, &h->tm_band[i], h->ybuf[i], h->mb_pad)) return 1;
   }
-  if (make_w_map(enc, &h->tm_w[0], h->wpack[0], kConvStages)) return 1;
-  if (make_w_map(enc, &h->tm_w[1], h->wpack[1], kConvStages)) return 1;
-  if (make_w_map(enc, &h->tm_w[2], h->wpack[2], kWvStages)) return 1;
-  if (make_w_map(enc, &h->tm_w[3], h->wpack[3], kWvStages)) return 1;
+  for (int i = 0; i < 4; ++i) {
+    const int n_stages = i < 2 ? kConvStages : kWvStages;
+    if (make_w_map(enc, &h->tm_w[i], h->wpack[i], n_stages, 128)) return 1;
+    if (make_w_map(enc, &h->tm_w_half[i], h->wpack[i], n_stages, 64)) return 1;
+  }
   for (int s = 0; s < 2; ++s) {
     for (int par = 0; par < 2; ++par) {
       if (make_f32_map(enc, &h->tm_lg_a_set[par][s][0], h->mpi_hi_set[par][s], kPatches, max_batch, kLgBM)) return 1;
@@ -632,10 +634,10 @@ static int launch_conv(gnm_handle* h, int layer, int in_buf, int n, cudaStream_t
     else
       grid = grid / h->conv_cluster * h->conv_cluster;
     cfg.gridDim = dim3(grid);
-    GNM_CUDA(cudaLaunchKernelEx(&cfg, conv_t_kernel<false>, h->tm_act[in_buf], h->tm_w[layer], p));
+    GNM_CUDA(cudaLaunchKernelEx(&cfg, conv_t_kernel<false>, h->tm_act[in_buf], h->tm_w_half[layer], p));
     return check_launch(h, "conv_t_kernel<false>(cluster)");
   }
-  conv_t_kernel<false><<<grid, kConvThreads, kConvTSmem, st>>>(h->tm_act[in_buf], h->tm_w[layer], p);
+  conv_t_kernel<false><<<grid, kConvThreads, kConvTSmem, st>>>(h->tm_act[in_buf], h->tm_w_half[layer], p);
   return check_launch(h, "conv_t_kernel<false>");
 }
 // q[s] = maxpool8(y[buf] @ w_v#s)
@@ -649,7 +651,7 @@ static int launch_wv_tc(gnm_handle* h, int s, int buf, int n, cudaStream_t st) {
   p.out_fp8 = 0;
   p.n_tiles = n * kUnitsPerWin;
   const int grid = std::min(h->num_sms, p.n_tiles);
-  conv_t_kernel<true><<<grid, kConvThreads, kConvTSmem, st>>>(h->tm_act[buf], h->tm_w[2 + s], p);
+  conv_t_kernel<true><<<grid, kConvThreads, kConvTSmem, st>>>(h->tm_act[buf], h->tm_w_half[2 + s], p);
   return check_launch(h, "conv_t_kernel<true>");
 }
 

@@ -34,22 +34,31 @@
 //     D^T[cout (M)][position (N=256)] += W_tap^T[cout][cin] * Y[position + tap][cin]
 //
 //   A operand = one 16 KB weight stage, [128 cout][64 cin] fp16 or [128 cout][128 cin] e4m3, K-major
-//               SWIZZLE_128B (streamed by TMA through a 5-stage ring, host-packed in consumption order);
-//               consumer warpgroup g multiplies its rows 64 g .. 64 g + 63;
+//               SWIZZLE_128B, host-packed in consumption order; consumer warpgroup g multiplies its rows 64 g .. 64 g + 63,
+//               which TMA streams as one contiguous 8 KB HALF-stage through warpgroup g's own ring of 5 slots;
 //   B operand = 256 consecutive rows of one slab region.
 //
 // Schedule.  Weight stages are consumed region-major (all 6 taps against one region, then the next; the two e4m3 regions
-// before the two fp16 ones, see the MMA loop) so a region is free after its 6 stages and is reloaded for the NEXT unit while
-// the other regions are in use;
-// activations and weights have separate producer threads.
+// before the two fp16 ones, see the MMA loop) so a region is free after both warpgroups' 6 stages and is reloaded for the
+// NEXT unit while the other regions are in use; activations and weights have separate producer threads.
+// Ping-pong: ONE weight producer fills the two rings in the order (unit u, g = 0, all stages), (u, g = 1, all stages),
+// (u + 1, g = 0, ...), ...  It can run at most 5 half-stages ahead of the warpgroup it is filling, so warpgroup 1 starts
+// unit u when warpgroup 0 is ~5 stages from the end of it, and warpgroup 0 starts u + 1 when warpgroup 1 is ~5 stages from
+// the end of u: each warpgroup's epilogue runs while its partner issues MMAs, and the tensor cores stay busy (one warpgroup
+// has one warp on each SM sub-partition, so its M64 N256 stream alone can keep all four tensor cores busy).  The rings are
+// separate because a waiter on an mbarrier must never be two phases ahead of it: in one ring shared by both warpgroups,
+// warpgroup 1's first half-stage would take the slot and phase parity of a fill two laps earlier and pass its wait at once.
 //
 // Warp roles (384 threads = 3 warpgroups, 1 CTA per SM, persistent over units):
-//   warp 0 lane 0 : weight producer (TMA)          warp 1 lane 0 : activation producer (TMA)
+//   warpgroup 0: one elected thread of warp 0 produces the weights (TMA), one of warp 1 the activations (TMA)
 //   warpgroups 1, 2: wgmma (M64 N256, 128 fp32 accumulator registers per thread) and the epilogue of output channels
 //       64 g .. 64 g + 63.  A thread holds channels c and c + 8 at 64 of the unit's positions (wgmma.cuh).
 //       conv : 2^-S scale + bias + LeakyReLU, then the planes the consumer needs (conv2 -> hi16, lo8, hi8 for
 //              conv3; conv3 -> hi16, lo16 for w_v / gather) stored straight to global memory;
 //       w_v  : the max over 8 consecutive positions (two registers per lane, then a butterfly over the lane quad).
+//   The warpgroup index is broadcast from lane 0 and every stage of the MMA loop is unrolled at compile time, so ptxas sees
+//   no divergent path between the wgmma of consecutive stages and keeps them in flight (wgmma_wait<1>) instead of draining
+//   each one.
 // The epilogue tracks the largest |Y| it produced and raises DeviceStatus::act_overflow beyond the operand formats' range.
 // Option conv_cluster launches the persistent grid as thread-block clusters (every CTA still issues its own loads).
 #pragma once
@@ -66,11 +75,12 @@ constexpr int kA2Region    = 2 * kARegion;                       // 272-row slab
 constexpr int kNumRegions  = 4;
 constexpr int kA2Bytes     = kNumRegions * kA2Region;            //                                        = 139264
 constexpr int kBStage      = 128 * 128;                          // one weight stage: 128 rows x 128 B     = 16384
+constexpr int kBHalf       = kBStage / 2;                        // one warpgroup's 64 rows of a stage     = 8192
 constexpr int kConvThreads = 384;                                // producer warpgroup + 2 MMA / epilogue warpgroups
 constexpr int kConvStages  = 24;                                 // conv: (region, tap)
 constexpr int kWvStages    = 4;                                  // w_v : (K-half, weight hi/lo)
-constexpr int kTWStages    = 5;                                  // weight ring depth (16 KB each)
-constexpr int kConvTSmem   = kA2Bytes + kTWStages * kBStage + 2048;
+constexpr int kTWSlots     = 5;                                  // depth of each warpgroup's weight ring (8 KB half-stages)
+constexpr int kConvTSmem   = kA2Bytes + 2 * kTWSlots * kBHalf + 2048;
 
 struct ConvTcParams {
   const float* bias;        // [128] (conv) or nullptr (w_v)
@@ -95,6 +105,7 @@ template <bool kWvMode> __device__ __forceinline__ constexpr int region_src(int 
                  : (r == 0 ? kOffHi16 : r == 1 ? kOffHi16 + 128 : r == 2 ? kOffP8 : kOffP8 + 128);
 }
 
+// tm_w: the weight pack with a 64-row box, i.e. one warpgroup's half of a 16 KB stage per load
 template <bool kWvMode>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant__ CUtensorMap tm_w,
@@ -103,82 +114,88 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_a = smem;                                   // activation slab: 4 regions x 272 rows x 128 B
-  uint8_t* s_w = smem + kA2Bytes;                        // weight ring
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + kTWStages * kBStage);
-  uint64_t* a_full = bars;            // [4]  per region
-  uint64_t* a_empty = bars + 4;       // [4]  one arrival per consumer warp
-  uint64_t* w_full = bars + 8;        // [5]
-  uint64_t* w_empty = bars + 13;      // [5]  one arrival per consumer warp
+  uint8_t* s_w = smem + kA2Bytes;                        // weight rings of half-stages: [2 warpgroups][kTWSlots]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + 2 * kTWSlots * kBHalf);
+  uint64_t* a_full = bars;                      // [4]  per region
+  uint64_t* a_empty = bars + 4;                 // [4]  one arrival per consumer warp of both warpgroups
+  uint64_t* w_full = bars + 8;                  // [2][kTWSlots]
+  uint64_t* w_empty = bars + 8 + 2 * kTWSlots;  // [2][kTWSlots]  one arrival per warp of the ring's warpgroup
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x) >> 5, 0);   // warp-uniform for the compiler
+  const int wg = warp >> 2, wq = warp & 3, lane = threadIdx.x & 31;
   const int n_units = p.n_tiles;      // n_windows * 24
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_act);
     tma_prefetch_desc(&tm_w);
     for (int i = 0; i < kNumRegions; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
-    for (int i = 0; i < kTWStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 8); }
+    for (int i = 0; i < 2 * kTWSlots; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 1 && lane == 0) {
-    // ===================================================================== activation producer
-    int it = 0;
-    const uint64_t pol = l2_policy_evict_first();          // activations stream through L2 once
-    for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, ++it) {
-      const uint32_t ph = it & 1;
-      const int w = unit / kUnitsPerWin;
-      const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
+  if (wg == 0) {
+    if (wq == 0 && elect_one()) {
+      // =================================================================== weight producer: (unit, warpgroup, stage) order
+      uint32_t wcount = 0;                                 // fills of each ring so far
+      const uint64_t pol = l2_policy_evict_last();         // the 384 KB of weights are re-read by every CTA for every unit
+      for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, wcount += kStagesU)
+        for (int g = 0; g < 2; ++g)
+          for (int q = 0; q < kStagesU; ++q) {
+            const int s = g * kTWSlots + (wcount + q) % kTWSlots;
+            const uint32_t wphase = ((wcount + q) / kTWSlots) & 1;
+            mbar_wait(&w_empty[s], wphase ^ 1, p.status, 110 + s);
+            mbar_arrive_expect_tx(&w_full[s], kBHalf);
+            tma_load_2d_hint(s_w + s * kBHalf, &tm_w, &w_full[s], 0, conv_pack_stage<kWvMode>(q) * 128 + 64 * g, pol);
+          }
+    } else if (wq == 1 && elect_one()) {
+      // =================================================================== activation producer
+      int it = 0;
+      const uint64_t pol = l2_policy_evict_first();        // activations stream through L2 once
+      for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, ++it) {
+        const uint32_t ph = it & 1;
+        const int w = unit / kUnitsPerWin;
+        const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
 #pragma unroll
-      for (int k = 0; k < kNumRegions; ++k) {
-        const int r = kWvMode ? (k == 0 ? 0 : k == 1 ? 2 : k == 2 ? 1 : 3) : (k + 2) & 3;   // order in which the MMAs need them
-        mbar_wait(&a_empty[r], ph ^ 1, p.status, 100 + r);
-        mbar_arrive_expect_tx(&a_full[r], kA2Region);
-        uint8_t* dst = s_a + r * kA2Region;
-        tma_load_3d_hint(dst, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5, w, pol);
-        tma_load_3d_hint(dst + kARegion, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5 + kSlabRows, w, pol);
+        for (int k = 0; k < kNumRegions; ++k) {
+          const int r = kWvMode ? (k == 0 ? 0 : k == 1 ? 2 : k == 2 ? 1 : 3) : (k + 2) & 3;   // order in which the MMAs need them
+          mbar_wait(&a_empty[r], ph ^ 1, p.status, 100 + r);
+          mbar_arrive_expect_tx(&a_full[r], kA2Region);
+          uint8_t* dst = s_a + r * kA2Region;
+          tma_load_3d_hint(dst, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5, w, pol);
+          tma_load_3d_hint(dst + kARegion, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5 + kSlabRows, w, pol);
+        }
       }
     }
-  } else if (warp == 0 && lane == 0) {
-    // ===================================================================== weight producer
-    uint32_t wcount = 0;
-    const uint64_t pol = l2_policy_evict_last();           // the 384 KB of weights are re-read by every CTA for every unit
-    for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x) {
-      for (int q = 0; q < kStagesU; ++q, ++wcount) {
-        const int s = wcount % kTWStages;
-        const uint32_t wphase = (wcount / kTWStages) & 1;
-        mbar_wait(&w_empty[s], wphase ^ 1, p.status, 110 + s);
-        mbar_arrive_expect_tx(&w_full[s], kBStage);
-        tma_load_2d_hint(s_w + s * kBStage, &tm_w, &w_full[s], 0, conv_pack_stage<kWvMode>(q) * 128, pol);
-      }
-    }
-  } else if (warp >= 4) {
+  } else {
     // ===================================================================== MMA + epilogue (warpgroup g: channels 64 g .. 64 g + 63)
-    const int g = (warp >> 2) - 1, wq = warp & 3;
+    const int g = wg - 1;
     const uint32_t a_base = smem_u32(s_a);
-    const uint32_t w_base = smem_u32(s_w) + g * 64 * 128;  // this warpgroup's 64 rows of every weight stage
+    const uint32_t w_base = smem_u32(s_w);
     const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
     const float bias0 = kWvMode ? 0.f : p.bias[ch0], bias1 = kWvMode ? 0.f : p.bias[ch0 + 8];
     const float oscale = p.out_scale;
     float amax = 0.f;                                      // largest |Y| this thread produced (range check, common.cuh)
-    uint32_t wcount = 0;
     int it = 0;
-    long long w_a = 0, w_w = 0, t_epi = 0, tq;
+    long long w_a = 0, w_w = 0, t_mma = 0, t_epi = 0, tq;
     const long long t_begin = clock64();
     float d[128];
     for (int unit = blockIdx.x; unit < n_units; unit += gridDim.x, ++it) {
       const uint32_t aph = it & 1;
       const int w = unit / kUnitsPerWin;
       const int t0 = (unit - w * kUnitsPerWin) * (2 * kTileM);
+      const uint32_t wc0 = static_cast<uint32_t>(it) * kStagesU;           // fills of this warpgroup's ring before this unit
+      const long long t_unit = clock64();
       // resources of the stage whose wgmma is still in flight: released once the next stage's wgmma is issued
-      int prev_s = -1, prev_region = -1;
-      for (int q = 0; q < kStagesU; ++q, ++wcount) {
+      int prev_s = 0, prev_region = -1;
+#pragma unroll
+      for (int q = 0; q < kStagesU; ++q) {
         // conv: step q = (region ((q/6) + 2) % 4, tap q%6); regions 0,1 are fp16 K-halves, 2 / 3 = e4m3 pairs (lo8, hi8) of channels
         //       0-63 / 64-127 against weights interleaved the same way (Whi8, Wlo8).  The e4m3 correction passes run FIRST: the
         //       tensor core adds e4m3 products to the accumulator with less than fp32 precision, which would drop the ~2^-8 smaller
         //       corrections if the accumulator already held the main pass; the fp16 passes accumulate in full fp32.
         // w_v : stage q = (K-half q/2, weight hi/lo q%2); hi-weight stages multiply both the hi16 and the lo16 region
+        // The loop is unrolled, so region, tap and instruction type are compile-time constants at every wgmma.
         const int reg = kWvMode ? (q >> 1) : ((q / 6 + 2) & 3);
         const int tap = kWvMode ? 5 : (q % 6);
         const bool first_use = kWvMode ? ((q & 1) == 0) : (tap == 0);
@@ -188,12 +205,13 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
           if (kWvMode) mbar_wait(&a_full[2 + reg], aph, p.status, 214 + reg);
           w_a += clock64() - tq;
         }
-        const int s = wcount % kTWStages;
-        const uint32_t wphase = (wcount / kTWStages) & 1;
+        const uint32_t c = wc0 + q;
+        const int s = g * kTWSlots + c % kTWSlots;
+        const uint32_t wphase = (c / kTWSlots) & 1;
         tq = clock64();
         mbar_wait(&w_full[s], wphase, p.status, 220 + s);
         w_w += clock64() - tq;
-        const uint64_t wdesc = gmma_desc_sw128(w_base + s * kBStage);                              // A: weights
+        const uint64_t wdesc = gmma_desc_sw128(w_base + s * kBHalf);                               // A: weights
         const uint64_t y0 = gmma_desc_sw128(a_base + reg * kA2Region + tap * 128);                 // B: activations
         wgmma_fence();
         int rel = -1;                                            // slab region this stage is the last user of
@@ -207,22 +225,24 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
           }
           rel = q == 0 ? 2 : q == 1 ? 0 : q == 2 ? 3 : 1;        // lo16.k0 is only used by stage 0, hi16.k0 by stages 0, 1, ...
         } else {
-          if (reg < 2) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) wgmma_f16_n256(d, wdesc + kk * 2, y0 + kk * 2, 1u);
-          } else {
+          if (reg >= 2) {
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) wgmma_e4m3_n256(d, wdesc + kk * 2, y0 + kk * 2, (q == 0 && kk == 0) ? 0u : 1u);
+          } else {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wgmma_f16_n256(d, wdesc + kk * 2, y0 + kk * 2, 1u);
           }
           if (tap == 5) rel = reg;                               // this region of the slab is no longer needed
         }
         wgmma_commit();
         // the previous stage's wgmma has completed once at most one group (this stage's) is pending
         wgmma_wait<1>();
-        __syncwarp();
-        if (lane == 0 && prev_s >= 0) {
-          mbar_arrive(&w_empty[prev_s]);
-          if (prev_region >= 0) mbar_arrive(&a_empty[prev_region]);
+        if (q > 0) {
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&w_empty[prev_s]);
+            if (prev_region >= 0) mbar_arrive(&a_empty[prev_region]);
+          }
         }
         prev_s = s; prev_region = rel;
       }
@@ -233,8 +253,9 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
         if (prev_region >= 0) mbar_arrive(&a_empty[prev_region]);
       }
       wgmma_fence_regs(d);
-      // ===================================================================== epilogue
       tq = clock64();
+      t_mma += tq - t_unit;
+      // ===================================================================== epilogue (overlaps the partner warpgroup's MMAs)
       if (kWvMode) {
         // pool group j of the unit = accumulator columns 8 j .. 8 j + 7 = registers 4 j + 2 h + e of the lane quad
 #pragma unroll
@@ -296,9 +317,10 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
       t_epi += clock64() - tq;
     }
     if (!kWvMode) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
-    if (p.dbg && warp == 4 && lane == 0) {   // warpgroup 1's view
+    if (p.dbg && wq == 0 && lane == 0) {     // include/gnm.h, "conv_dbg"
       long long* dd = p.dbg + blockIdx.x * 8;
-      dd[0] = clock64() - t_begin; dd[2] = w_a; dd[3] = w_w; dd[4] = it; dd[6] = t_epi;
+      if (g == 0) { dd[0] = clock64() - t_begin; dd[1] = t_mma; dd[2] = w_a; dd[3] = w_w; dd[4] = it; dd[6] = t_epi; }
+      else { dd[5] = t_mma; dd[7] = t_epi; }
     }
   }
 }

@@ -241,6 +241,9 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  * "mpi0","mpi1" [n][2100]; "logits" [n][752] (of the second IGLOO kernel after a full step); "h0" [n][256];
  * "h1","h2" [n][512] = the outputs of the two Dense(512) + BatchNorm + ReLU layers of the head;
  * "conv_dbg" [num_sms][16] (int64 counters viewed as float pairs).  Used by the per-kernel parity tests and tools/gpu_experiment.py.
+ *   conv_t_kernel's counters, per CTA, in clock64 cycles: [0] first consumer warpgroup's total, [1] its MMA phases (first
+ *   barrier wait of a unit to its last wgmma's completion), [2] its waits on a_full, [3] its waits on w_full, [4] units,
+ *   [5] the second consumer warpgroup's MMA phases, [6] the first's epilogues, [7] the second's epilogues.
  */
 int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream);
 

@@ -27,8 +27,9 @@ for exp in [int(x) for x in (sys.argv[1:] or ["0", "2"])]:
     clf.set_option("profile_stages", 0)
     print(f"experiment={exp}: " + "  ".join(f"{k}={sum(v)/len(v):.3f}" for k, v in acc.items()), flush=True)
 
-# cycle breakdown of the MMA issuer / epilogue (experiment bit 4 = conv3, bit 8 = conv2)
-names = ["mma_total", "mma_wait_acc_empty", "mma_wait_a_full", "mma_wait_w_full", "units", "epi_total", "epi_wait_acc_full"]
+# per-CTA cycle breakdown of the two consumer warpgroups (experiment bit 4 = conv3, bit 8 = conv2), layout in include/gnm.h
+names = ["wg1_total", "wg1_mma_phase", "wg1_wait_a_full", "wg1_wait_w_full", "units", "wg2_mma_phase", "wg1_epilogue",
+         "wg2_epilogue"]
 for bit, label in ((8, "conv2"), (4, "conv3")):
     clf.set_option("conv_experiment", bit)
     clf.predict_ascii(a, out); torch.cuda.synchronize()

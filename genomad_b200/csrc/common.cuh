@@ -31,9 +31,9 @@ constexpr float kLeaky  = 0.1f;   // LeakyReLU slope                   (referenc
 //   [256,512)  lo16 = fp16(Y - hi16)                128 halves   -- w_v 3-pass split, patch gather
 //   [512,768)  p8   = 128 e4m3 PAIRS (lo8[c], hi8[c]),  lo8 = e4m3((Y - hi16) * 128), hi8 = e4m3(hi16 * 4)
 //                     -- the operand of the convs' correction passes lo(A) * hi(W) + hi(A) * lo(W), which run as ONE K = 256
-//                     contraction against weights interleaved the same way (Whi8[c], Wlo8[c]).  Interleaving (round 2) lets a
-//                     producer write a channel's two bytes with one store (conv2's epilogue: one 2-byte store per position
-//                     instead of two 1-byte stores; layer 1: one 8-byte store per lane instead of two 4-byte stores).
+//                     contraction against weights interleaved the same way (Whi8[c], Wlo8[c]).  Interleaving (round 2) makes a
+//                     channel's two bytes one b16 element (conv2's epilogue transposes this plane with the same b16 stmatrix
+//                     as hi16; layer 1: one 8-byte store per lane instead of two 4-byte stores).
 constexpr int kRowBytes  = 768;
 constexpr int kOffHi16   = 0, kOffLo16 = 256, kOffP8 = 512;
 constexpr float kActScale = 32.f;          // 2^5
@@ -68,6 +68,20 @@ __device__ __forceinline__ void split2_f16(float a, float b, __half2& hi, __half
 // two floats -> two e4m3 bytes (round to nearest even, saturating)
 __device__ __forceinline__ uint16_t pack_e4m3x2(float a, float b) {
   return static_cast<uint16_t>(__nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3));
+}
+
+// ----------------------------------------------------------------------------- shared-memory transposes
+// Four 8x8 b16 matrices from an mma-style fragment (register i: matrix i; lane l holds row l / 4, columns 2 (l % 4) and
+// 2 (l % 4) + 1, the lower column in the low half), stored TRANSPOSED: row r of matrix i (16 bytes) goes to the address lane
+// 8 i + r passes, and holds column r of the fragment.
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t saddr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
+  return v;
 }
 
 // error flag written by device-side timeouts (see mbar_wait); checked by the host API

@@ -54,7 +54,10 @@
 //   warpgroups 1, 2: wgmma (M64 N256, 128 fp32 accumulator registers per thread) and the epilogue of output channels
 //       64 g .. 64 g + 63.  A thread holds channels c and c + 8 at 64 of the unit's positions (wgmma.cuh).
 //       conv : 2^-S scale + bias + LeakyReLU, then the planes the consumer needs (conv2 -> hi16, lo8, hi8 for
-//              conv3; conv3 -> hi16, lo16 for w_v / gather) stored straight to global memory;
+//              conv3; conv3 -> hi16, lo16 for w_v / gather).  Per column group of 8 positions a warp transposes its
+//              16 channels x 8 positions x 2 planes through a private 512-byte shared-memory tile (one stmatrix.trans),
+//              then each lane writes one full 16-byte half of a 32-byte sector: 32 st.global.v4 per thread and unit
+//              instead of 512 two-byte stores, which is what lets the epilogue fit under the partner's MMA phase;
 //       w_v  : the max over 8 consecutive positions (two registers per lane, then a butterfly over the lane quad).
 //   The warpgroup index is broadcast from lane 0 and every stage of the MMA loop is unrolled at compile time, so ptxas sees
 //   no divergent path between the wgmma of consecutive stages and keeps them in flight (wgmma_wait<1>) instead of draining
@@ -80,7 +83,10 @@ constexpr int kConvThreads = 384;                                // producer war
 constexpr int kConvStages  = 24;                                 // conv: (region, tap)
 constexpr int kWvStages    = 4;                                  // w_v : (K-half, weight hi/lo)
 constexpr int kTWSlots     = 5;                                  // depth of each warpgroup's weight ring (8 KB half-stages)
-constexpr int kConvTSmem   = kA2Bytes + 2 * kTWSlots * kBHalf + 2048;
+constexpr int kEpiTile     = 512;                                // conv epilogue staging: 8 positions x 2 planes x 32 B per warp
+constexpr int kEpiStage    = 8 * 2 * kEpiTile;                   // 8 consumer warps x 2 tiles (double-buffered)    = 8192
+constexpr int kConvTSmem   = kA2Bytes + 2 * kTWSlots * kBHalf + kEpiStage + 2048;
+static_assert(kConvTSmem <= 232448, "conv_t_kernel exceeds the 227 KB of shared memory a CTA may use");
 
 struct ConvTcParams {
   const float* bias;        // [128] (conv) or nullptr (w_v)
@@ -89,7 +95,7 @@ struct ConvTcParams {
   float out_scale;          // conv: 2^-S (undoes the common operand scaling); w_v: 2^-e / 32 (w_v operand scaling, activation scale)
   int out_fp8;              // conv: 1 = write hi16 + lo8 + hi8 (consumer is a conv), 0 = write hi16 + lo16
   int n_tiles;              // number of work units = n_windows * 24
-  int experiment;           // timing experiments only (results become wrong): 2 = no epilogue global stores
+  int experiment;           // timing experiments only (results become wrong): 2 = no epilogue global stores (the shared-memory transpose still runs)
   long long* dbg;           // optional [gridDim.x][8] cycle counters (nullptr = off)
   DeviceStatus* status;
 };
@@ -115,7 +121,8 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* s_a = smem;                                   // activation slab: 4 regions x 272 rows x 128 B
   uint8_t* s_w = smem + kA2Bytes;                        // weight rings of half-stages: [2 warpgroups][kTWSlots]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_w + 2 * kTWSlots * kBHalf);
+  uint8_t* s_epi = s_w + 2 * kTWSlots * kBHalf;          // conv epilogue staging tiles: [8 consumer warps][2][kEpiTile]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_epi + kEpiStage);
   uint64_t* a_full = bars;                      // [4]  per region
   uint64_t* a_empty = bars + 4;                 // [4]  one arrival per consumer warp of both warpgroups
   uint64_t* w_full = bars + 8;                  // [2][kTWSlots]
@@ -271,47 +278,50 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
           }
         }
       } else {
+        // Column group j of the accumulator is this warp's 16 channels x 8 positions 8 j .. 8 j + 7.  Per output plane that is
+        // 8 rows x 32 contiguous bytes, both planes 512 B: one 16-byte store per lane.  Both planes are b16 per (channel,
+        // position) -- hi16 / lo16 halves, or the (lo8, hi8) e4m3 pair of a channel -- so the values of positions (pos, pos + 1)
+        // are packed like a __half2, and one transposing stmatrix.x4 (matrix 2 k + h = plane k, channels ch0 + 8 h) turns the
+        // fragment into position rows in the warp's staging tile: [position][plane][32 B], its 16-byte chunks XOR-swizzled by
+        // position / 2 so that the stmatrix rows and the 16-byte reads are both free of bank conflicts.  The tile is
+        // double-buffered, so the one __syncwarp between a tile's stmatrix and its reads also orders those reads before the
+        // stmatrix that overwrites the tile two steps later.
         const bool store = !(p.experiment & 2);
-        uint8_t* const unit_rows = p.y_out + (static_cast<size_t>(w) * kTok + t0) * kRowBytes;
+        const uint32_t tile = smem_u32(s_epi) + (g * 4 + wq) * 2 * kEpiTile;
+        const int sp = lane & 7, lp = lane >> 2;              // stmatrix row address of this lane / position it stores
+        const uint32_t st_addr = tile + sp * 64 + (((lane >> 3) ^ (sp >> 1)) << 4);
+        const uint32_t ld_addr = tile + lp * 64 + (((lane & 3) ^ (lp >> 1)) << 4);
+        uint8_t* const dst = p.y_out + (static_cast<size_t>(w) * kTok + t0 + lp) * kRowBytes
+                             + ((lane & 2) ? (p.out_fp8 ? kOffP8 : kOffLo16) : kOffHi16) + 2 * (g * 64 + wq * 16) + 16 * (lane & 1);
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          const int pos = 8 * j + 2 * (lane & 3);                // positions pos, pos + 1 of the unit
+          uint32_t r[4];                                         // r[2 k + h]: plane k of channel ch0 + 8 h at 2 positions
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            const int ch = ch0 + 8 * h;
             const float bias = h ? bias1 : bias0;
             const float y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
             const float y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
             amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
-            uint8_t* q0 = unit_rows + static_cast<size_t>(pos) * kRowBytes;
-            uint8_t* q1 = q0 + kRowBytes;
             if (p.out_fp8) {
               const __half2 hh = __floats2half2_rn(y0, y1);
               const float2 f = __half22float2(hh);
-              // e4m3 pair (lo8, hi8) of this channel at each of the two positions: one 2-byte store per position
-              const uint16_t e0 = pack_e4m3x2((y0 - f.x) * kLo8Scale, f.x * kHi8Scale);
-              const uint16_t e1 = pack_e4m3x2((y1 - f.y) * kLo8Scale, f.y * kHi8Scale);
-              if (store && t0 + pos < kTok) {
-                reinterpret_cast<__half*>(q0 + kOffHi16)[ch] = __low2half(hh);
-                reinterpret_cast<uint16_t*>(q0 + kOffP8)[ch] = e0;
-              }
-              if (store && t0 + pos + 1 < kTok) {
-                reinterpret_cast<__half*>(q1 + kOffHi16)[ch] = __high2half(hh);
-                reinterpret_cast<uint16_t*>(q1 + kOffP8)[ch] = e1;
-              }
+              // e4m3 pair (lo8, hi8) of this channel at each of the two positions
+              const uint32_t e0 = pack_e4m3x2((y0 - f.x) * kLo8Scale, f.x * kHi8Scale);
+              const uint32_t e1 = pack_e4m3x2((y1 - f.y) * kLo8Scale, f.y * kHi8Scale);
+              r[h] = pack_h2(__low2half(hh), __high2half(hh));
+              r[2 + h] = e0 | (e1 << 16);
             } else {
               __half2 hh, l;
               split2_f16(y0, y1, hh, l);
-              if (store && t0 + pos < kTok) {
-                reinterpret_cast<__half*>(q0 + kOffHi16)[ch] = __low2half(hh);
-                reinterpret_cast<__half*>(q0 + kOffLo16)[ch] = __low2half(l);
-              }
-              if (store && t0 + pos + 1 < kTok) {
-                reinterpret_cast<__half*>(q1 + kOffHi16)[ch] = __high2half(hh);
-                reinterpret_cast<__half*>(q1 + kOffLo16)[ch] = __high2half(l);
-              }
+              r[h] = pack_h2(__low2half(hh), __high2half(hh));
+              r[2 + h] = pack_h2(__low2half(l), __high2half(l));
             }
           }
+          const uint32_t buf = (j & 1) * kEpiTile;
+          stmatrix_x4_trans(st_addr + buf, r[0], r[1], r[2], r[3]);
+          __syncwarp();
+          const uint4 v = ld_shared_v4(ld_addr + buf);
+          if (store && t0 + 8 * j + lp < kTok) *reinterpret_cast<uint4*>(dst + static_cast<size_t>(8 * j) * kRowBytes) = v;
         }
       }
       t_epi += clock64() - tq;

@@ -27,13 +27,16 @@ for exp in [int(x) for x in (sys.argv[1:] or ["0", "2"])]:
     clf.set_option("profile_stages", 0)
     print(f"experiment={exp}: " + "  ".join(f"{k}={sum(v)/len(v):.3f}" for k, v in acc.items()), flush=True)
 
-# per-CTA cycle breakdown of the two consumer warpgroups (experiment bit 4 = conv3, bit 8 = conv2), layout in include/gnm.h
+# per-CTA cycle breakdown of the two consumer warpgroups (experiment bit 4 = conv3, bit 8 = conv2), layout in include/gnm.h;
+# once as built and once with bit 2 (no epilogue global stores), which gives the epilogue's floor without its stores
 names = ["wg1_total", "wg1_mma_phase", "wg1_wait_a_full", "wg1_wait_w_full", "units", "wg2_mma_phase", "wg1_epilogue",
          "wg2_epilogue"]
-for bit, label in ((8, "conv2"), (4, "conv3")):
-    clf.set_option("conv_experiment", bit)
-    clf.predict_ascii(a, out); torch.cuda.synchronize()
-    d = clf.debug_fetch("conv_dbg", 1).cpu().view(torch.int64).numpy().astype(float)
-    print(f"conv_t cycle breakdown, {label} (mean over CTAs):")
-    for i, nm in enumerate(names):
-        print(f"   {nm:22s} {d[:, i].mean():12.0f}  (per unit {d[:, i].mean() / max(d[:, 4].mean(), 1):9.0f})")
+for extra, what in ((0, "with stores"), (2, "bit 2: no global stores")):
+    for bit, label in ((8, "conv2"), (4, "conv3")):
+        clf.set_option("conv_experiment", bit | extra)
+        clf.predict_ascii(a, out); torch.cuda.synchronize()
+        d = clf.debug_fetch("conv_dbg", 1).cpu().view(torch.int64).numpy().astype(float)
+        print(f"conv_t cycle breakdown, {label}, {what} (mean over CTAs):")
+        for i, nm in enumerate(names):
+            print(f"   {nm:22s} {d[:, i].mean():12.0f}  (per unit {d[:, i].mean() / max(d[:, 4].mean(), 1):9.0f})")
+clf.set_option("conv_experiment", 0)

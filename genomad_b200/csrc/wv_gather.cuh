@@ -17,24 +17,26 @@
 // [position][window][128 B], i.e. the 8 windows of one position are one 1024-byte swizzle atom.  For the tensor core the
 // region is still a plain K-major SWIZZLE_128B operand of 192 rows (column n = 8 * position + window); for the gather it means
 // "one position x 8 windows" is one conflict-free ldmatrix.  Six region buffers: the TMA producer fills the first half of unit
-// u+1 while the MMAs and the gather work on unit u.
+// u+1 while the MMAs and the gather work on unit u, and its second half as soon as every warp is done with unit u's first.
 //
 //   * value projection: 3 fp16 passes Ahi*Whi + Alo*Whi + Ahi*Wlo, operands swapped so that D^T[cout][row].  The w_v weights
 //     (the A operand, 64 KB: hi / lo x two K-halves) are loaded into shared memory once per CTA.  Two MMA warpgroups own 64
-//     output channels each and take the unit one pool group (64 columns = 8 positions x 8 windows) at a time, M64 N64 K16:
-//     a thread's 32 accumulator registers hold 2 channels x 2 windows x the group's 8 positions, so the max-pool is a max over
-//     8 of its own registers and q is written straight from them.
+//     output channels each and take the whole unit per instruction, M64 N192 K16, in K-half-major order: the 12 wgmma of
+//     K-half 0 (one commit group), then the 12 of K-half 1, so K-half 0's two regions go back to the producer while K-half 1
+//     is still in flight.  Registers 32 pg .. 32 pg + 31 of a thread's 96 accumulators hold pool group pg (64 columns =
+//     8 positions x 8 windows): 2 channels x 2 windows x the group's 8 positions, so the max-pool is a max over 8 of its own
+//     registers and q is written straight from them.
 //   * patch gather: warp-level mma.sync.m16n8k16 on the slab rows.  Entries are grouped by position (<= 4 per group;
 //     8,400 entries hit ~4,500 positions).  For one group and one channel half, A[16 x 64] = the position's 8 windows' hi16 rows
 //     (rows 0-7) and lo16 rows (rows 8-15), read by 4 ldmatrix.x4; B[64 x 8] = the fp16 hi / lo halves of the group's folded
 //     weights (host-packed in fragment order, scaled by a power of two so the lo halves stay normal; L1 / L2 resident); the sum of
 //     the four D entries of (window, entry) is (hi + lo) . (w_hi + w_lo) with fp32 accumulation -- the fp32-equivalent dot product.
-//     15 gather warps take <= 2 groups each; pass 0 (channels 0-63) waits in registers, pass 1 adds channels 64-127 and writes
-//     part_t[slot][window] (8 lanes = 32 contiguous bytes).  A region goes back to the producer when the 8 MMA warps and all 15
-//     gather warps have arrived (count 23).  patch_finish_t_kernel adds a patch's four slots in fixed order k = 0..3 plus the bias.
+//     7 gather warps take <= 4 groups each; pass 0 (channels 0-63) waits in registers, pass 1 adds channels 64-127 and writes
+//     part_t[slot][window] (8 lanes = 32 contiguous bytes).  A region goes back to the producer when the 8 MMA warps and all 7
+//     gather warps have arrived (count 15).  patch_finish_t_kernel adds a patch's four slots in fixed order k = 0..3 plus the bias.
 //
-// Warp roles (768 threads, 1 CTA per SM):  warps 0..7: two MMA + epilogue warpgroups | warps 8..22: patch gather |
-// warp 23 lane 0: barrier init, the weight load and the activation producer (TMA).
+// Warp roles (512 threads, 1 CTA per SM, 128 registers per thread):  warps 0..7: two MMA + epilogue warpgroups |
+// warps 8..14: patch gather | warp 15, one elected lane: barrier init, the weight load and the activation producer (TMA).
 #pragma once
 #include <cuda.h>
 #include <type_traits>
@@ -54,10 +56,12 @@ constexpr int kWgBufs     = 6;                                    // region buff
 constexpr int kWgSlab     = kWgBufs * kWgRegion;                  //                                                        = 147456
 constexpr int kWgWBytes   = kWvStages * kBStage;                  // w_v^T hi / lo x two K-halves, the A operand            =  65536
 constexpr int kWgMmaWarps = 8;                                    // two MMA + epilogue warpgroups
-constexpr int kWgWarps    = 15;                                   // patch-gather warps (24 warps in all: 80 registers per thread)
-constexpr int kWgThreads  = (kWgMmaWarps + kWgWarps + 1) * 32;    // 768
-constexpr int kWgGroupCap = 2;                                    // position groups per warp on the fast path (30 per band; a band has <= 24
-                                                                  // positions, so only positions with more than 4 entries can exceed it)
+constexpr int kWgWarps    = 7;                                    // patch-gather warps (16 warps in all: 128 registers per thread, room for
+                                                                  // the MMA warps' 96 accumulators)
+constexpr int kWgThreads  = (kWgMmaWarps + kWgWarps + 1) * 32;    // 512
+constexpr int kWgGroupCap = 4;                                    // position groups per warp on the fast path (28 per band; a band has <= 24
+                                                                  // positions, so only positions with more than 4 entries can exceed it;
+                                                                  // the shipped patch sets have at most 25 groups in a band)
 constexpr int kWgGroupMax = 4;                                    // entries per position group: the 8 columns of mma.m16n8k16 = 4 entries x (hi, lo)
 constexpr int kWgSmem     = kWgSlab + kWgWBytes + 2048;           //                                                        = 215040
 static_assert(kWgSmem <= 232448, "wv_gather_kernel exceeds the 227 KB of shared memory a CTA may use");
@@ -111,12 +115,13 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
   // lives in buffer g % kWgBufs; every role walks the buffers in the same order, so each keeps the first buffer of the
   // current unit (b0, advanced by 4 mod kWgBufs per unit) and one phase bit per buffer that it flips after each use.
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x) >> 5, 0);   // warp-uniform for the compiler
+  const int lane = threadIdx.x & 31;
   constexpr int kProducerWarp = kWgMmaWarps + kWgWarps;
   // contiguous range of band-major unit numbers; the split points weigh a unit by its band's entry count (host side)
   const int u_begin = p.cta_split[blockIdx.x], u_end = p.cta_split[blockIdx.x + 1];
 
-  if (warp == kProducerWarp && lane == 0) {
+  if (warp == kProducerWarp && elect_one()) {
     tma_prefetch_desc(&tm_band);
     tma_prefetch_desc(&tm_w);
     for (int i = 0; i < kWgBufs; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], kWgMmaWarps + kWgWarps); }
@@ -125,27 +130,33 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
   }
   __syncthreads();
 
-  if (warp == kProducerWarp && lane == 0) {
-    // ===================================================================== weights (once), then the activation producer
-    mbar_arrive_expect_tx(w_full, kWgWBytes);
-    for (int q = 0; q < kWvStages; ++q) tma_load_2d_hint(s_w + q * kBStage, &tm_w, w_full, 0, q * 128, l2_policy_evict_last());
-    const uint64_t pol = l2_policy_evict_first();
-    uint32_t phases = 0;                                   // bit b: parity of buffer b's next "empty" wait is phase ^ 1
-    int b0 = 0;
-    for (int unit = u_begin; unit < u_end; ++unit) {
-      const int band = unit / p.groups;
-      const int w0 = (unit - band * p.groups) * kBandWins;
+  if (warp == kProducerWarp) {
+    if (elect_one()) {
+      // =================================================================== weights (once), then the activation producer
+      mbar_arrive_expect_tx(w_full, kWgWBytes);
+      for (int q = 0; q < kWvStages; ++q) tma_load_2d_hint(s_w + q * kBStage, &tm_w, w_full, 0, q * 128, l2_policy_evict_last());
+      const uint64_t pol = l2_policy_evict_first();
+      uint32_t phases = 0;                                 // bit b: parity of buffer b's next "empty" wait is phase ^ 1
+      int b0 = 0;
+      long long c_wait_empty = 0;
+      for (int unit = u_begin; unit < u_end; ++unit) {
+        const int band = unit / p.groups;
+        const int w0 = (unit - band * p.groups) * kBandWins;
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        int b = b0 + k; if (b >= kWgBufs) b -= kWgBufs;
-        mbar_wait(&a_empty[b], ((phases >> b) & 1) ^ 1, p.status, 500 + b);
-        phases ^= 1u << b;
-        mbar_arrive_expect_tx(&a_full[b], kWgRegion);
-        // k: 0 hi16 channels 0-63, 1 lo16 channels 0-63, 2 hi16 channels 64-127, 3 lo16 channels 64-127 (byte offset in the row)
-        const int src = (k & 1 ? kOffLo16 : kOffHi16) + (k >> 1) * 128;
-        tma_load_3d_hint(s_a + b * kWgRegion, &tm_band, &a_full[b], src, w0, band * kBandRows, pol);     // box = {128 B, 8 windows, 24 positions}
+        for (int k = 0; k < 4; ++k) {
+          int b = b0 + k; if (b >= kWgBufs) b -= kWgBufs;
+          const long long tq = clock64();
+          mbar_wait(&a_empty[b], ((phases >> b) & 1) ^ 1, p.status, 500 + b);
+          c_wait_empty += clock64() - tq;
+          phases ^= 1u << b;
+          mbar_arrive_expect_tx(&a_full[b], kWgRegion);
+          // k: 0 hi16 channels 0-63, 1 lo16 channels 0-63, 2 hi16 channels 64-127, 3 lo16 channels 64-127 (byte offset in the row)
+          const int src = (k & 1 ? kOffLo16 : kOffHi16) + (k >> 1) * 128;
+          tma_load_3d_hint(s_a + b * kWgRegion, &tm_band, &a_full[b], src, w0, band * kBandRows, pol);   // box = {128 B, 8 windows, 24 positions}
+        }
+        b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
       }
-      b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
+      if (p.dbg) p.dbg[blockIdx.x * 8 + 7] = c_wait_empty;
     }
   } else if (warp < kWgMmaWarps) {
     // ===================================================================== MMA + epilogue (warpgroup g: channels 64 g .. 64 g + 63)
@@ -158,63 +169,73 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
     mbar_wait(w_full, 0, p.status, 510);
     uint32_t phases = 0;
     int b0 = 0;
-    float d[32];
+    uint32_t w_a = 0, t_mma = 0, t_epi = 0;                 // 32-bit cycle counters: the MMA warps have no registers to spare
+    float d[96];
     for (int unit = u_begin; unit < u_end; ++unit) {
+      auto buf = [&](int k) { const int b = b0 + k; return b >= kWgBufs ? b - kWgBufs : b; };   // buffer of region k
+      const uint32_t t_unit = clock();
+      // K-half-major: every wgmma covers all 192 columns (the three pool groups), so each accumulator element sees the order of
+      // conv_t_kernel<true> and layer1_wv_kernel, K-half 0 then K-half 1, and all three produce bit-identical q
+#pragma unroll
+      for (int kh = 0; kh < 2; ++kh) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {                      // region 2 kh + r: r = 0 hi16, 1 lo16
+          const int b = buf(2 * kh + r);
+          const uint32_t tq = clock();
+          mbar_wait(&a_full[b], (phases >> b) & 1, p.status, 530 + b);
+          w_a += clock() - tq;
+          phases ^= 1u << b;
+        }
+        const uint64_t yh = gmma_desc_sw128(a_base + buf(2 * kh) * kWgRegion);          // B: hi16 rows
+        const uint64_t yl = gmma_desc_sw128(a_base + buf(2 * kh + 1) * kWgRegion);      // B: lo16 rows
+        const uint64_t whi = gmma_desc_sw128(w_base + (2 * kh) * kBStage);              // A: w_v^T hi
+        const uint64_t wlo = gmma_desc_sw128(w_base + (2 * kh + 1) * kBStage);          // A: w_v^T lo
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+          wgmma_f16_n192(d, whi + kk * 2, yh + kk * 2, (kh == 0 && kk == 0) ? 0u : 1u);
+          wgmma_f16_n192(d, whi + kk * 2, yl + kk * 2, 1u);
+        }
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_f16_n192(d, wlo + kk * 2, yh + kk * 2, 1u);
+        wgmma_commit();
+      }
+      // K-half 0 has completed once at most one group (K-half 1) is pending: its regions can take the next unit's K-half 1
+      wgmma_wait<1>();
+      __syncwarp();
+      if (lane == 0) { mbar_arrive(&a_empty[buf(0)]); mbar_arrive(&a_empty[buf(1)]); }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      const uint32_t t_epi0 = clock();
+      t_mma += t_epi0 - t_unit;
       const int band = unit / p.groups;
       const int w0 = (unit - band * p.groups) * kBandWins;
-      int bufs[4];
+      // register 32 pg + 4 i + 2 h + e = channel ch0 + 8 h, position i of pool group pg, window win0 + e
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        int b = b0 + k; if (b >= kWgBufs) b -= kWgBufs;
-        bufs[k] = b;
-        mbar_wait(&a_full[b], (phases >> b) & 1, p.status, 530 + b);
-        phases ^= 1u << b;
-      }
-#pragma unroll 1
-      for (int pg = 0; pg < kBandRows / kPool; ++pg) {          // pool group pg = rows 64 pg .. 64 pg + 63 of every region
-        wgmma_fence();
-#pragma unroll 1
-        for (int kh = 0; kh < 2; ++kh) {
-          const uint64_t yh = gmma_desc_sw128(a_base + bufs[2 * kh] * kWgRegion + pg * 64 * 128);       // B: hi16 rows
-          const uint64_t yl = gmma_desc_sw128(a_base + bufs[2 * kh + 1] * kWgRegion + pg * 64 * 128);   // B: lo16 rows
-          const uint64_t whi = gmma_desc_sw128(w_base + (2 * kh) * kBStage);                            // A: w_v^T hi
-          const uint64_t wlo = gmma_desc_sw128(w_base + (2 * kh + 1) * kBStage);                        // A: w_v^T lo
-          // the order of conv_t_kernel<true> and layer1_wv_kernel, so that all three produce bit-identical q
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            wgmma_f16_n64(d, whi + kk * 2, yh + kk * 2, (kh == 0 && kk == 0) ? 0u : 1u);
-            wgmma_f16_n64(d, whi + kk * 2, yl + kk * 2, 1u);
-          }
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) wgmma_f16_n64(d, wlo + kk * 2, yh + kk * 2, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs(d);
-        // register 4 i + 2 h + e = channel ch0 + 8 h, position i of the pool group, window win0 + e
+      for (int pg = 0; pg < kBandRows / kPool; ++pg) {
         const int gg = band * (kBandRows / kPool) + pg;
         if (gg < kPooled && !(p.experiment & 128)) {
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              float m = d[2 * h + e];
+              float m = d[32 * pg + 2 * h + e];
 #pragma unroll
-              for (int i = 1; i < kPool; ++i) m = fmaxf(m, d[4 * i + 2 * h + e]);
+              for (int i = 1; i < kPool; ++i) m = fmaxf(m, d[32 * pg + 4 * i + 2 * h + e]);
               const int w = w0 + win0 + e;
               if (w < p.n_windows) p.q_out[(static_cast<size_t>(w) * kPooled + gg) * kC + ch0 + 8 * h] = m * oscale;
             }
         }
       }
       __syncwarp();
-      if (lane == 0)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) mbar_arrive(&a_empty[bufs[k]]);
+      if (lane == 0) { mbar_arrive(&a_empty[buf(2)]); mbar_arrive(&a_empty[buf(3)]); }
+      t_epi += clock() - t_epi0;
       b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
     }
-  } else if (warp >= kWgMmaWarps && warp < kWgMmaWarps + kWgWarps) {
+    if (p.dbg && warp == 0 && lane == 0) { long long* o = p.dbg + blockIdx.x * 8; o[3] = t_mma; o[4] = w_a; o[6] = t_epi; }
+  } else {
     // ===================================================================== patch gather
-    const int gw = warp - kWgMmaWarps;                         // 0..14
+    const int gw = warp - kWgMmaWarps;                         // 0..kWgWarps - 1
     const float gscale = p.gather_unscale;
     // Gather lane roles.  ldmatrix: lanes 8i..8i+7 address matrix i = (plane i & 1: 0 hi16 / 1 lo16, 16-byte chunk i >> 1 of the
     // k-step), row lane & 7 = window.  The A fragment then holds rows 0..7 = the 8 windows' hi16 halves and rows 8..15 = their
@@ -228,24 +249,27 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
     long long c_wait_full = 0, c_gather = 0, tq = 0;
     const long long t_begin = clock64();
     int cur_band = -1, g_first = 0, g_cnt = 0, n_mine = 0;
-    int my_e0[kWgGroupCap] = {0, 0}, my_meta[kWgGroupCap] = {0, 0};     // this warp's position groups of the band, fast path
+    int my_e0[kWgGroupCap] = {}, my_meta[kWgGroupCap] = {};             // this warp's position groups of the band, fast path
     bool fast = true;
     // One position group x one K-half: D[16 x 8] = A[16 x 64] * B[64 x 8] as 4 independent k-steps.  B's
-    // columns are (entry 0 hi, entry 0 lo, entry 1 hi, ...): the fp16 hi / lo halves of up to 4 entries' folded weights.  Returns
-    // entry tig of window gid: (hi16 row + lo16 row) x (hi-weight column + lo-weight column).
-    auto gather_group = [&](int e0, int meta, int kh, uint32_t hi_base, uint32_t lo_base) -> float {
+    // columns are (entry 0 hi, entry 0 lo, entry 1 hi, ...): the fp16 hi / lo halves of up to 4 entries' folded weights.
+    // load_group reads a group's fragments, mma_group returns entry tig of window gid: (hi16 row + lo16 row) x (hi-weight
+    // column + lo-weight column).  Split in two so that the fast path can issue a second group's reads before the first
+    // group's mma: the reads and the mma (which queues behind the wgmma stream on the tensor pipe) are latency, not throughput.
+    struct GroupFrag { uint2 b[4]; uint32_t a[4][4]; };
+    auto load_group = [&](int e0, int meta, int kh, uint32_t hi_base, uint32_t lo_base, GroupFrag& f) {
       const int row = meta & 31, ne = meta >> 8;
       const uint2* wf = reinterpret_cast<const uint2*>(p.wfrag) + ((static_cast<size_t>(e0 + (gid >> 1)) * 2 + kh) * 16 + tig) * 2 + (gid & 1);
-      uint2 b[4];
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) b[ks] = ((gid >> 1) < ne && !(p.experiment & 1024)) ? ldg_frag(wf + ks * 8) : make_uint2(0u, 0u);
+      for (int ks = 0; ks < 4; ++ks) f.b[ks] = ((gid >> 1) < ne && !(p.experiment & 1024)) ? ldg_frag(wf + ks * 8) : make_uint2(0u, 0u);
       const uint32_t rb = (lm_plane ? lo_base : hi_base) + row * (kBandWins * 128) + lm_win * 128;
-      uint32_t a[4][4];
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        if (p.experiment & 2048) { a[ks][0] = a[ks][1] = a[ks][2] = a[ks][3] = rb; continue; }
-        ldsm_x4(rb + (((ks * 2 + lm_chunk) ^ lm_win) << 4), a[ks]);     // 128-byte swizzle: chunk j -> j ^ (row & 7)
+        if (p.experiment & 2048) { f.a[ks][0] = f.a[ks][1] = f.a[ks][2] = f.a[ks][3] = rb; continue; }
+        ldsm_x4(rb + (((ks * 2 + lm_chunk) ^ lm_win) << 4), f.a[ks]);     // 128-byte swizzle: chunk j -> j ^ (row & 7)
       }
+    };
+    auto mma_group = [&](const GroupFrag& f) -> float {
       // four independent accumulators: the warp-level mma shares the tensor pipe with the wgmma stream, so no mma of a group
       // depends on another one
       float d[4][4];
@@ -253,10 +277,10 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
       for (int ks = 0; ks < 4; ++ks) d[ks][0] = d[ks][1] = d[ks][2] = d[ks][3] = 0.f;
       if (p.experiment & 256) {                              // timing experiment: rows and weights are read, no arithmetic
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) asm volatile("" :: "r"(a[ks][0] | a[ks][1] | a[ks][2] | a[ks][3] | b[ks].x | b[ks].y));
+        for (int ks = 0; ks < 4; ++ks) asm volatile("" :: "r"(f.a[ks][0] | f.a[ks][1] | f.a[ks][2] | f.a[ks][3] | f.b[ks].x | f.b[ks].y));
       } else {
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) mma_16816(d[ks], a[ks], b[ks].x, b[ks].y);
+        for (int ks = 0; ks < 4; ++ks) mma_16816(d[ks], f.a[ks], f.b[ks].x, f.b[ks].y);
       }
       float v = 0.f;
 #pragma unroll
@@ -266,7 +290,7 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
     for (int unit = u_begin; unit < u_end; ++unit, ++it) {
       const int band = unit / p.groups;
       const int w0 = (unit - band * p.groups) * kBandWins;
-      if (band != cur_band) {                                  // this warp's position groups of the band: gw, gw + 15, ...
+      if (band != cur_band) {                                  // this warp's position groups of the band: gw, gw + 7, ...
         cur_band = band;
         g_first = p.band_gstart[band];
         g_cnt = (p.experiment & 32) ? 0 : p.band_gstart[band + 1] - g_first;
@@ -293,21 +317,33 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
         mbar_wait(&a_full[bl], ph_l, p.status, 560 + bl);          // lo16 K-half kh
         if (p.dbg) { const long long t = clock64(); c_wait_full += t - tq; tq = t; }
         if (fast) {
+          auto finish = [&](int i, float v) {
+            if (kh == 0) c0[i] = v;
+            else if (tig < (my_meta[i] >> 8) && !(p.experiment & 64))           // 8 lanes (gid = window) write 32 contiguous bytes
+              p.part_t[static_cast<size_t>(my_e0[i] + tig) * p.n_pad + w0 + gid] = c0[i] + v;
+          };
 #pragma unroll
-          for (int i = 0; i < kWgGroupCap; ++i)
+          for (int i = 0; i < kWgGroupCap; i += 2)             // two groups at a time: both groups' reads before either mma
             if (i < n_mine) {
-              const float v = gather_group(my_e0[i], my_meta[i], kh, hi_base, lo_base);
-              if (kh == 0) c0[i] = v;
-              else if (tig < (my_meta[i] >> 8) && !(p.experiment & 64))         // 8 lanes (gid = window) write 32 contiguous bytes
-                p.part_t[static_cast<size_t>(my_e0[i] + tig) * p.n_pad + w0 + gid] = c0[i] + v;
+              GroupFrag f0, f1;
+              load_group(my_e0[i], my_meta[i], kh, hi_base, lo_base, f0);
+              if (i + 1 < n_mine) {
+                load_group(my_e0[i + 1], my_meta[i + 1], kh, hi_base, lo_base, f1);
+                finish(i, mma_group(f0));
+                finish(i + 1, mma_group(f1));
+              } else {
+                finish(i, mma_group(f0));
+              }
             }
         } else {
-          // generic path (a band with more than 30 position groups: only patch sets that put more than 4 entries on many
+          // generic path (a band with more than 28 position groups: only patch sets that put more than 4 entries on many
           // positions): pass-0 halves are parked in part_t itself (the same thread reads them back in pass 1)
 #pragma unroll 1
           for (int gi = gw; gi < g_cnt; gi += kWgWarps) {
             const int2 m = p.grp[g_first + gi];
-            const float v = gather_group(m.x, m.y, kh, hi_base, lo_base);
+            GroupFrag f;
+            load_group(m.x, m.y, kh, hi_base, lo_base, f);
+            const float v = mma_group(f);
             if (tig < (m.y >> 8)) {
               float* gp = p.part_t + static_cast<size_t>(m.x + tig) * p.n_pad + w0 + gid;
               *gp = kh == 0 ? v : *gp + v;

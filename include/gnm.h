@@ -244,6 +244,10 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  *   conv_t_kernel's counters, per CTA, in clock64 cycles: [0] first consumer warpgroup's total, [1] its MMA phases (first
  *   barrier wait of a unit to its last wgmma's completion), [2] its waits on a_full, [3] its waits on w_full, [4] units,
  *   [5] the second consumer warpgroup's MMA phases, [6] the first's epilogues, [7] the second's epilogues.
+ *   wv_gather_kernel's counters ("conv_experiment" bit 512, second IGLOO launch), per CTA, in clock64 cycles: [0] the first
+ *   gather warp's total, [1] its waits on a_full, [2] its gather work (reads, mma, part_t stores, release), [3] the first MMA
+ *   warpgroup's MMA phases (first a_full wait of a unit to its last wgmma's completion, waits included), [4] that warpgroup's
+ *   waits on a_full, [5] units, [6] that warpgroup's epilogues (max-pool and q stores), [7] the producer's waits on a_empty.
  */
 int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream);
 

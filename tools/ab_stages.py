@@ -86,14 +86,15 @@ def main():
 
 
 def wvg_cycles(clf, pool, bits=0):
-    names = ["gather warp total", "gather warp wait a_full", "gather warp gather (reads + mma + release)", "epilogue warp wait acc_full",
-             "epilogue warp epilogue", "units", "MMA wait a_full", "MMA wait acc_empty"]
+    # counter layout: include/gnm.h, "conv_dbg"
+    names = ["gather warp total", "gather warp wait a_full", "gather warp gather (reads + mma + release)", "MMA warpgroup MMA phase",
+             "MMA warpgroup wait a_full", "units", "MMA warpgroup epilogue", "producer wait a_empty"]
     clf.set_option("conv_experiment", 512 | bits)
     clf.predict_ascii(pool[0]); torch.cuda.synchronize()
     d = clf.debug_fetch("conv_dbg", 1).cpu().view(torch.int64).numpy().astype(float)
     clf.set_option("conv_experiment", 0)
     units = max(d[:, 5].mean(), 1)
-    print(f"wv_gather_kernel (IGLOO#1) cycle breakdown, experiment bits {bits}, mean over CTAs (warp 4 = a gather warp, warp 20 = an epilogue warp, warp 1 = MMA issuer):")
+    print(f"wv_gather_kernel (IGLOO#1) cycle breakdown, experiment bits {bits}, mean over CTAs (first gather warp, first MMA warpgroup, producer):")
     for i, nm in enumerate(names):
         print(f"   {nm:42s} {d[:, i].mean():12.0f}   per unit {d[:, i].mean() / units:9.0f}   (min {d[:, i].min():.0f}, max {d[:, i].max():.0f})")
 

@@ -21,6 +21,7 @@
 #include "dense.cuh"
 #include "logits_tc.cuh"
 #include "wv_gather.cuh"
+#include "contigs.cuh"
 
 using namespace gnm;
 
@@ -1010,6 +1011,83 @@ extern "C" int gnm_encode(gnm_handle* h, const uint8_t* d_ascii, int n, uint16_t
     if (check_launch(h, "encode_tokens_kernel")) return 1;
   }
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ contigs -> windows
+// Plan (contigs.cuh): count pass -> scan -> one D2H of the total -> capacity check -> write pass.  Scratch: the caller's
+// d_win_offsets only, so a too-small capacity is reported before anything is written to d_win_start / d_win_len.
+extern "C" int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
+                                  int single_window, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
+                                  int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+  if (!h) return fail("gnm_contig_windows: null handle");
+  if (n_contigs < 0) return fail("gnm_contig_windows: negative contig count");
+  if (capacity < 0) return fail("gnm_contig_windows: negative capacity");
+  if (!d_seq_offsets || !d_win_offsets || !h_n_windows || (n_contigs > 0 && !d_seq) ||
+      (capacity > 0 && (!d_win_start || !d_win_len)))
+    return fail("gnm_contig_windows: null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  *h_n_windows = 0;
+  if (n_contigs == 0) {
+    GNM_CUDA(cudaMemsetAsync(d_win_offsets, 0, sizeof(int32_t), st));
+    GNM_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+  contig_plan_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, single_window, d_win_offsets, nullptr, nullptr);
+  if (check_launch(h, "contig_plan_kernel<count>")) return 1;
+  contig_scan_kernel<<<1, kScanThreads, 0, st>>>(d_win_offsets, n_contigs);
+  if (check_launch(h, "contig_scan_kernel")) return 1;
+  int32_t total = 0;
+  GNM_CUDA(cudaMemcpyAsync(&total, d_win_offsets + n_contigs, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  GNM_CUDA(cudaStreamSynchronize(st));
+  if (total == kPlanBadOffsets) return fail("gnm_contig_windows: d_seq_offsets is not non-decreasing");
+  if (total == kPlanOverflow) return fail("gnm_contig_windows: the contigs have more than 2^31-1 windows");
+  *h_n_windows = total;
+  if (total > capacity)
+    return fail("gnm_contig_windows: the contigs have " + std::to_string(total) + " windows, capacity is " +
+                std::to_string(capacity) + " (n_contigs + total_bytes / 6000 is always enough)");
+  if (total == 0) return 0;
+  contig_plan_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, single_window, d_win_offsets, d_win_start, d_win_len);
+  return check_launch(h, "contig_plan_kernel<write>");
+}
+
+static int launch_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                                 uint8_t* d_ascii, cudaStream_t st) {
+  gather_windows_kernel<<<n, kGatherThreads, 0, st>>>(d_seq, d_win_start, d_win_len, d_ascii);
+  return check_launch(h, "gather_windows_kernel");
+}
+
+extern "C" int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                                  uint8_t* d_ascii, void* stream) {
+  if (!h) return fail("gnm_gather_windows: null handle");
+  if (n < 0) return fail("gnm_gather_windows: negative window count");
+  if (n == 0) return 0;
+  if (!d_seq || !d_win_start || !d_win_len || !d_ascii) return fail("gnm_gather_windows: null buffer");
+  if (reinterpret_cast<uintptr_t>(d_ascii) % 16) return fail("gnm_gather_windows: d_ascii must be 16-byte aligned");
+  GNM_CUDA(cudaSetDevice(h->device));
+  return launch_gather_windows(h, d_seq, d_win_start, d_win_len, n, d_ascii, static_cast<cudaStream_t>(stream));
+}
+
+// Steps of max_batch windows: gather into in_stage[step parity], then the unchanged forward step.  The gather runs on the
+// step's main stream, ahead of the layer-1 kernel that reads the stage, so the TailOverlap ordering covers both buffers.
+extern "C" int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                   int n, float* d_probs, void* stream) {
+  if (!h) return fail("gnm_forward_windows: null handle");
+  if (n < 0) return fail("gnm_forward_windows: negative window count");
+  if (n == 0) return 0;
+  if (!d_seq || !d_win_start || !d_win_len || !d_probs) return fail("gnm_forward_windows: null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  if (check_device_status(h)) return 1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  TailOverlap ov(h, st, (n + h->max_batch - 1) / h->max_batch);
+  for (int i = 0, off = 0; off < n; ++i, off += h->max_batch) {
+    const int m = std::min(h->max_batch, n - off);
+    uint8_t* stage = h->in_stage[i & 1];
+    timer_mark(h, "gather_windows", st);
+    if (launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, stage, st)) return 1;
+    if (ov.step(stage, nullptr, m, d_probs + static_cast<size_t>(off) * 3)) return 1;
+  }
+  return ov.join();
 }
 
 static int segment_any(gnm_handle* h, const float* d_probs, const int32_t* d_offsets, int n_contigs, float* d_out,

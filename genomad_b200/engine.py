@@ -63,6 +63,10 @@ EXPORTS = {
     "gnm_segment_sum": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_classify_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "gnm_check_status": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "gnm_contig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64,
+                                     C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "gnm_gather_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_forward_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "gnm_get_option": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]),
     "gnm_kernel_launches": (C.c_longlong, [C.c_void_p]),
@@ -225,6 +229,84 @@ class Classifier:
         _check(self.lib, self.lib.gnm_segment_sum(self._h, probs.contiguous().data_ptr(), offsets.contiguous().data_ptr(),
                                                   n, out.data_ptr(), self._stream()))
         return out
+
+    # ------------------------------------------------------------------ contigs in memory -> windows on the device
+    def contig_buffers(self, seqs):
+        """Contigs -> (uint8 cuda [total_bytes], int64 cuda [n_contigs + 1] offsets), one host-to-device copy each.
+        `seqs` is a list of str / bytes (str is UTF-8 encoded, i.e. the bytes the FASTA reader would see) or a
+        (uint8 tensor or array, int64 offsets) pair on the host or on CUDA."""
+        t = self._torch
+        dev = self._dev()
+        if isinstance(seqs, tuple) and len(seqs) == 2 and not isinstance(seqs[0], (str, bytes, bytearray)):
+            seq = t.as_tensor(seqs[0]).to(device=dev, dtype=t.uint8).reshape(-1)
+            offs = t.as_tensor(seqs[1]).to(device=dev, dtype=t.int64).reshape(-1)
+        else:
+            parts = [s.encode() if isinstance(s, str) else bytes(s) for s in seqs]
+            offs_h = np.zeros(len(parts) + 1, dtype=np.int64)
+            np.cumsum([len(p) for p in parts], out=offs_h[1:])
+            seq = t.from_numpy(np.frombuffer(b"".join(parts), dtype=np.uint8).copy()).to(dev)
+            offs = t.from_numpy(offs_h).to(dev)
+        if seq.numel() == 0:
+            seq = t.zeros(16, dtype=t.uint8, device=dev)          # all contigs empty: the library still wants a buffer
+        return seq.contiguous(), offs.contiguous()
+
+    def contig_windows(self, seq_u8, seq_offsets_i64, single_window: bool = False):
+        """Plan the windows of contigs on the device (gnm_contig_windows): uint8 cuda [total_bytes] + int64 cuda offsets
+        [n_contigs + 1] -> (win_start int64 [W] absolute byte offsets, win_len int32 [W], win_offsets int32 [n_contigs + 1])."""
+        t = self._torch
+        assert seq_u8.dtype == t.uint8 and seq_offsets_i64.dtype == t.int64 and seq_u8.is_cuda and seq_offsets_i64.is_cuda
+        seq, offs = seq_u8.contiguous(), seq_offsets_i64.contiguous()
+        n = offs.numel() - 1
+        assert n >= 0
+        cap = n + seq.numel() // WINDOW                                   # always enough (gnm.h)
+        start = t.empty(cap, dtype=t.int64, device=seq.device)
+        length = t.empty(cap, dtype=t.int32, device=seq.device)
+        woff = t.empty(n + 1, dtype=t.int32, device=seq.device)
+        nw = C.c_int64()
+        _check(self.lib, self.lib.gnm_contig_windows(self._h, seq.data_ptr(), offs.data_ptr(), n, int(bool(single_window)),
+                                                     start.data_ptr(), length.data_ptr(), cap, woff.data_ptr(), C.byref(nw),
+                                                     self._stream()))
+        return start[:nw.value], length[:nw.value], woff
+
+    def gather_windows(self, seq_u8, win_start, win_len):
+        """Kept windows -> uint8 cuda [W, 6000], upper-cased and N-padded (gnm_gather_windows)."""
+        t = self._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        out = t.empty((start.numel(), WINDOW), dtype=t.uint8, device=seq_u8.device)
+        _check(self.lib, self.lib.gnm_gather_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
+                                                     start.numel(), out.data_ptr(), self._stream()))
+        return out
+
+    def predict_windows(self, seq_u8, win_start, win_len, out=None):
+        """Per-window probabilities float32 [W, 3] straight from the sequence buffer (gnm_forward_windows)."""
+        t = self._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        if out is None:
+            out = t.empty((start.numel(), 3), dtype=t.float32, device=seq_u8.device)
+        _check(self.lib, self.lib.gnm_forward_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
+                                                      start.numel(), out.data_ptr(), self._stream()))
+        return out
+
+    def classify_contigs(self, seqs, single_window: bool = False, return_window_probs: bool = False):
+        """Contigs in, one score triple per contig out -- what the reference module computes per contig
+        (nn_classification.py:65-75, 316-320), with windowing on the GPU.
+
+        seqs: list of str / bytes, or a (uint8 tensor, int64 offsets) pair on the host or on CUDA (see contig_buffers).
+        Returns cuda tensors (means float32 [n_contigs, 3], window counts int32 [n_contigs]) and, if asked, the per-window
+        probabilities float32 [W, 3].  A contig that is empty after stripping n/N has count 0 and mean (0, 0, 0); the
+        reference drops such contigs, so drop those rows to mirror its outputs."""
+        t = self._torch
+        seq, offs = self.contig_buffers(seqs)
+        start, length, woff = self.contig_windows(seq, offs, single_window)
+        probs = self.predict_windows(seq, start, length)
+        if probs.numel():
+            means = self.segment_mean(probs, woff)
+        else:                 # no contig has a window (an empty probs tensor has no buffer to hand to gnm_segment_mean)
+            means = t.zeros((woff.numel() - 1, 3), dtype=t.float32, device=seq.device)
+        counts = woff[1:] - woff[:-1]
+        return (means, counts, probs) if return_window_probs else (means, counts)
 
     # ------------------------------------------------------------------ host-buffer API
     def classify_host(self, ascii_windows: np.ndarray) -> np.ndarray:

@@ -133,6 +133,48 @@ int gnm_check_status(gnm_handle* h, void* stream);
  */
 int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs);
 
+/* ---- contigs in memory -> windows, on the GPU ---------------------------------------------- */
+
+/*
+ * The windowing of read_fasta(strip_n=True) -> seq_windows(6000, 2500) -> N rule -> upper-case + pad
+ * (sequence.py:96-167, nn_classification.py:65-72) for contigs already in device memory; the same rules as the FASTA
+ * reader below, byte for byte (csrc/contigs.cuh).
+ *
+ * Input: d_seq holds the contigs' bytes back to back; contig c is d_seq[d_seq_offsets[c] .. d_seq_offsets[c+1]), int64
+ * offsets, n_contigs + 1 of them, non-decreasing, any start address.  A contig is its sequence as read_fasta joins its
+ * lines: no header, no line terminators, NOT yet stripped of leading / trailing n/N.
+ *
+ * gnm_contig_windows: plans the kept windows of every contig.
+ *   d_win_start [capacity]    absolute byte offset in d_seq of each kept window's first byte
+ *   d_win_len   [capacity]    1..6000 bytes of sequence; the rest of the window is 'N' padding
+ *   d_win_offsets [n_contigs + 1]  CSR: the windows of contig c are [off[c], off[c+1]), in order
+ *   *h_n_windows              number of kept windows (also set when the call fails for lack of capacity)
+ *   A contig that is empty after stripping gets ZERO windows; the reference drops such a contig entirely, so a caller that
+ *   mirrors its outputs drops the rows whose window count is 0 (gnm_segment_mean writes zeros for them).
+ *   capacity >= n_contigs + total_bytes / 6000 is always enough.  If the plan needs more than `capacity` windows, or more
+ *   than 2^31 - 1, or the offsets decrease, the call fails with a message and writes nothing to d_win_start / d_win_len.
+ *   d_win_offsets doubles as the planning scratch: no other memory is used or allocated.
+ *   Synchronous: one device-to-host copy of the count; the start / length arrays are written in `stream` order after it.
+ *
+ * gnm_gather_windows: kept windows -> d_ascii uint8 [n][6000] (16-byte aligned), ASCII-upper-cased ('a'..'z' only) and
+ *   'N'-padded: exactly the bytes gnm_forward_ascii takes, and gnm_fasta_export gives for the same contigs as FASTA text.
+ *   Asynchronous.
+ *
+ * gnm_forward_windows: per-window probabilities float [n][3] straight from the sequence buffer.  Each internal step
+ *   gathers its <= max_batch windows into the staging buffers gnm_classify_host copies into (two, alternated by step), then
+ *   runs the same forward step as gnm_forward_ascii: bitwise the same probabilities.  Asynchronous like gnm_forward_ascii;
+ *   synchronise `stream` before calling gnm_classify_host on the same handle.
+ *
+ * Per-contig scores: gnm_segment_mean(h, d_probs, d_win_offsets, n_contigs, d_mean, stream).
+ */
+int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int single_window,
+                       int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
+                       int64_t* h_n_windows, void* stream);
+int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                       uint8_t* d_ascii, void* stream);
+int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                        float* d_probs, void* stream);
+
 /* ---- host-side FASTA front end (no GPU involved) ------------------------------------------ */
 
 /*

@@ -21,6 +21,20 @@ __device__ __forceinline__ uint16_t kmer_token(uint32_t c0, uint32_t c1, uint32_
   return bad ? uint16_t(0) : uint16_t(v);
 }
 
+// A caller's token as a table row index: tf.one_hot(x, 257) turns a token above 256 into an all-zero row, so such a token
+// contributes nothing, exactly like the causal padding (-1).
+__device__ __forceinline__ int vocab_token(uint32_t v) { return v < kVocab ? static_cast<int>(v) : -1; }
+
+// Layer 1's triple-table shortcut for caller-supplied tokens: the row ((tk0-1) << 4) | ((tk2-1) & 15) holds
+// W1[j][k0] + W1[j+1][k1] + W1[j+2][k2] for the three overlapping 4-mers of one all-ACGT 6-base word, so it may replace the
+// three rows only when tk0, tk1, tk2 are such 4-mers (tokenizer output always is; arbitrary tokens mostly are not).
+// 0xFFFF = take the three-row fallback.
+__device__ __forceinline__ int triple_code_checked(int tk0, int tk1, int tk2) {
+  const bool word = tk0 > 0 && tk1 > 0 && tk2 > 0 && ((tk0 - 1) & 15) == ((tk2 - 1) >> 4) &&
+                    tk1 - 1 == ((((tk0 - 1) & 63) << 2) | (((tk2 - 1) >> 2) & 3));
+  return word ? (((tk0 - 1) << 4) | ((tk2 - 1) & 15)) : 0xFFFF;
+}
+
 // ------------------------------------------------------------------------------------------
 // K0 (stand-alone): one CTA per (window, 2048-token segment).  Bytes are staged through shared
 // memory with 16-byte coalesced loads; every thread then emits 8 consecutive tokens as one
@@ -76,7 +90,10 @@ encode_tokens_kernel(const uint8_t* __restrict__ ascii, uint16_t* __restrict__ t
 // of 6 consecutive bases, so A has only 4^6 = 4096 possible values when those bases are all ACGT, and
 // likewise B: two 2 MB "triple" tables (built on the host with the same fp32 operation order, so a
 // table hit is bit-identical to the three-row sum) replace six 512-byte row reads by two.  Positions
-// next to the window start, or touching a non-ACGT base, fall back to the single-row table.
+// next to the window start, or touching a non-ACGT base, fall back to the single-row table.  Tokens
+// supplied by the caller (kFromAscii = false) may be anything: values above 256 become padding (the
+// zero row of tf.one_hot), and a half takes its triple row only when its three tokens are the 4-mers of
+// one 6-base word.
 // ------------------------------------------------------------------------------------------
 constexpr int kEmbSeg = 256;
 constexpr int kEmbThreads = 256;
@@ -115,7 +132,7 @@ embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict
     const uint16_t* src = tokens_in + static_cast<size_t>(w) * kTok;
     for (int i = threadIdx.x; i < kEmbSeg + 5; i += blockDim.x) {
       const int p = t0 - 5 + i;
-      s_tok[i] = (p >= 0 && p < kTok) ? static_cast<int16_t>(src[p]) : int16_t(-1);
+      s_tok[i] = static_cast<int16_t>((p >= 0 && p < kTok) ? vocab_token(src[p]) : -1);
     }
   }
   __syncthreads();
@@ -124,9 +141,15 @@ embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict
   // token logic executed redundantly by all 32 lanes).
   {
     const int i = threadIdx.x;                         // kEmbThreads == kEmbSeg
-    const int tk0 = s_tok[i], tk2 = s_tok[i + 2], tk3 = s_tok[i + 3], tk5 = s_tok[i + 5];
-    const int ca = (tk0 > 0 && tk2 > 0) ? (((tk0 - 1) << 4) | ((tk2 - 1) & 15)) : 0xFFFF;    // bases t-5 .. t all ACGT (implies tk1 > 0)
-    const int cb = (tk3 > 0 && tk5 > 0) ? (((tk3 - 1) << 4) | ((tk5 - 1) & 15)) : 0xFFFF;    // bases t-2 .. t+3 all ACGT (implies tk4 > 0)
+    int ca, cb;
+    if (kFromAscii) {                                  // tokens made from bytes here are consistent 4-mers by construction
+      const int tk0 = s_tok[i], tk2 = s_tok[i + 2], tk3 = s_tok[i + 3], tk5 = s_tok[i + 5];
+      ca = (tk0 > 0 && tk2 > 0) ? (((tk0 - 1) << 4) | ((tk2 - 1) & 15)) : 0xFFFF;    // bases t-5 .. t all ACGT (implies tk1 > 0)
+      cb = (tk3 > 0 && tk5 > 0) ? (((tk3 - 1) << 4) | ((tk5 - 1) & 15)) : 0xFFFF;    // bases t-2 .. t+3 all ACGT (implies tk4 > 0)
+    } else {
+      ca = triple_code_checked(s_tok[i], s_tok[i + 1], s_tok[i + 2]);
+      cb = triple_code_checked(s_tok[i + 3], s_tok[i + 4], s_tok[i + 5]);
+    }
     s_code[i] = ca | (cb << 16);
   }
   __syncthreads();

@@ -90,9 +90,12 @@ layer1_wv_kernel(const __grid_constant__ CUtensorMap tm_w, const FusedParams p) 
     // A (taps 0..2) and B (taps 3..5) of the position whose six tokens start at tk[0]
     auto load_ab = [&](const int16_t* tk, float4& A, float4& B) {
       const int t0_ = tk[0], t1_ = tk[1], t2_ = tk[2], t3_ = tk[3], t4_ = tk[4], t5_ = tk[5];
-      if (t0_ > 0 && t2_ > 0) A = __ldg(tri4 + static_cast<size_t>(((t0_ - 1) << 4) | ((t2_ - 1) & 15)) * (kC / 4) + lane);
+      // bytes -> tokens here are consistent 4-mers by construction; caller tokens need the full check (encode.cuh)
+      const bool hit_a = kFromAscii ? (t0_ > 0 && t2_ > 0) : triple_code_checked(t0_, t1_, t2_) != 0xFFFF;
+      const bool hit_b = kFromAscii ? (t3_ > 0 && t5_ > 0) : triple_code_checked(t3_, t4_, t5_) != 0xFFFF;
+      if (hit_a) A = __ldg(tri4 + static_cast<size_t>(((t0_ - 1) << 4) | ((t2_ - 1) & 15)) * (kC / 4) + lane);
       else A = add4(add4(row1(0, t0_), row1(1, t1_)), row1(2, t2_));
-      if (t3_ > 0 && t5_ > 0) B = __ldg(tri4 + (static_cast<size_t>(kTriple) + (((t3_ - 1) << 4) | ((t5_ - 1) & 15))) * (kC / 4) + lane);
+      if (hit_b) B = __ldg(tri4 + (static_cast<size_t>(kTriple) + (((t3_ - 1) << 4) | ((t5_ - 1) & 15))) * (kC / 4) + lane);
       else B = add4(add4(row1(3, t3_), row1(4, t4_)), row1(5, t5_));
     };
     const int kh = lane >> 4;                                      // which 64-channel K-half this lane's 4 channels are in
@@ -113,7 +116,7 @@ layer1_wv_kernel(const __grid_constant__ CUtensorMap tm_w, const FusedParams p) 
         const uint8_t* src = p.ascii + static_cast<size_t>(w) * kWindow + pos;
         return kmer_token(base_code(__ldg(src)), base_code(__ldg(src + 1)), base_code(__ldg(src + 2)), base_code(__ldg(src + 3)));
       }
-      return static_cast<int>(__ldg(p.tokens + static_cast<size_t>(w) * kTok + pos));
+      return vocab_token(__ldg(p.tokens + static_cast<size_t>(w) * kTok + pos));
     };
     int it = 0;
     int tok_next = fetch_token(blockIdx.x);

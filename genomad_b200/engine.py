@@ -202,7 +202,8 @@ class Classifier:
         return out
 
     def predict_tokens(self, tokens, out=None):
-        """uint16 cuda tensor [n, 5997] -> float32 probabilities [n, 3]; the analogue of nn_model.predict(batch)."""
+        """uint16 cuda tensor [n, 5997] -> float32 probabilities [n, 3]; the analogue of nn_model.predict(batch).  Any uint16 is
+        valid: as in tf.one_hot(x, 257), a token above 256 contributes nothing."""
         t = self._torch
         k = tokens.contiguous()
         assert k.dtype == t.uint16 and k.dim() == 2 and k.shape[1] == TOKENS and k.is_cuda

@@ -101,7 +101,8 @@ int gnm_encode(gnm_handle* h, const uint8_t* d_ascii, int n, uint16_t* d_tokens,
  */
 int gnm_forward_ascii(gnm_handle* h, const uint8_t* d_ascii, int n, float* d_probs, void* stream);
 
-/* Same, from tokens (uint16 [n][5997], values 0..256): nn_model.predict on an int64[B,5997] batch. */
+/* Same, from tokens (uint16 [n][5997]): nn_model.predict on an int64[B,5997] batch.  Any uint16 is accepted, and the
+ * tokens need not come from gnm_encode: as in tf.one_hot(x, 257), a value above 256 contributes nothing. */
 int gnm_forward_tokens(gnm_handle* h, const uint16_t* d_tokens, int n, float* d_probs, void* stream);
 
 /*

@@ -103,20 +103,27 @@ def _lrelu(x):
 
 
 # ----------------------------------------------------------------------------- pieces
+def vocab_tokens(tok: torch.Tensor) -> torch.Tensor:
+    """Tokens as int64 with every value above 256 replaced by 257: tf.one_hot(x, 257) gives such a token an all-zero row,
+    and index 257 selects the zero row that `conv1_*` append to the 257 real ones."""
+    t = tok.long()
+    return torch.where(t > 256, torch.full_like(t, 257), t)
+
+
 def conv1_as_written(tok: torch.Tensor, w, dtype):
     """tf.one_hot(257) -> Conv1D(128, 6, causal) -> LeakyReLU   (model.py:11, igloo.py:45-48)"""
-    oh = F.one_hot(tok.long(), 257).to(dtype)                       # [B, L, 257]
+    oh = F.one_hot(vocab_tokens(tok), 258)[..., :257].to(dtype)     # [B, L, 257]; tokens > 256: zero rows
     x = F.pad(oh.transpose(1, 2), (5, 0))                            # causal: 5 zero rows on the left
     k = _t(w, "c1w", dtype).permute(2, 1, 0).contiguous()            # [k,in,out] -> [out,in,k]
     return _lrelu(F.conv1d(x, k, _t(w, "c1b", dtype))).transpose(1, 2)
 
 
 def conv1_embedding(tok: torch.Tensor, w, dtype):
-    """y1[t] = lrelu(b + sum_j W1[j, tok[t-5+j]]), taps added in order j = 0..5; padded taps add nothing."""
-    W = _t(w, "c1w", dtype)                                          # [6, 257, 128]
+    """y1[t] = lrelu(b + sum_j W1[j, tok[t-5+j]]), taps added in order j = 0..5; padded taps and tokens > 256 add nothing."""
+    W = F.pad(_t(w, "c1w", dtype), (0, 0, 0, 1))                     # [6, 258, 128]: row 257 = 0
     B, L = tok.shape
     acc = torch.zeros(B, L, 128, dtype=dtype)
-    t = tok.long()
+    t = vocab_tokens(tok)
     for j in range(6):
         sh = 5 - j                                                   # tap j reads tok[t - sh]
         acc[:, sh:, :] += W[j][t[:, : L - sh]]

@@ -72,9 +72,11 @@ def _pool(z):
 
 
 def conv1(tokens: np.ndarray, w) -> Ref:
-    """Layer 1 (one-hot -> causal Conv1D -> LeakyReLU) from the tokens: y1[t] = lrelu(b + sum_j W1[j, tok[t-5+j]])."""
-    W = _t(w["c1w"])
+    """Layer 1 (one-hot -> causal Conv1D -> LeakyReLU) from the tokens: y1[t] = lrelu(b + sum_j W1[j, tok[t-5+j]]); a token
+    above 256 is an all-zero one-hot row (tf.one_hot(x, 257)) and adds nothing."""
+    W = F.pad(_t(w["c1w"]), (0, 0, 0, 1))                               # [6, 258, 128]: row 257 = 0
     t = torch.as_tensor(np.asarray(tokens).astype(np.int64))
+    t = torch.where(t > 256, 257, t)
     B, L = t.shape
     acc, sab, s2 = (torch.zeros(B, L, 128, dtype=D) for _ in range(3))
     for j in range(6):
@@ -153,12 +155,15 @@ def head_softmax(h2: torch.Tensor, w) -> Ref:
 
 
 # ------------------------------------------------------------------------------------------ metrics
-def position_regions(n: int, pooled: bool = False) -> Dict[str, tuple]:
+def position_regions(n: int, pooled: bool = False, windows: Optional[list] = None) -> Dict[str, tuple]:
     """Index sets (window slice or indices, position slice) where kernels tend to go wrong: the causal zero fill (positions 0-5),
     the last, partial 256-position conv unit (5888-5996), the last 24-position IGLOO band (5976-5996), and the windows on both
-    sides of the 8-window groups of the fused IGLOO kernel (8k - 1, 8k, 8k + 1).  pooled: the same regions in max-pool groups."""
+    sides of the 8-window groups of the fused IGLOO kernel (8k - 1, 8k, 8k + 1).  pooled: the same regions in max-pool groups.
+    windows: the batch indices of the rows actually compared (a sample of an n-window batch); the window regions then index
+    into that sample."""
     f = (lambda a, b: slice(a // POOL, min(N_POOL, (b + POOL) // POOL))) if pooled else (lambda a, b: slice(a, b + 1))
-    edge = sorted({i for k in range(8, n + 1, 8) for i in (k - 1, k, k + 1) if i < n})
+    edges = {i for k in range(8, n + 1, 8) for i in (k - 1, k, k + 1) if i < n}
+    edge = sorted(edges) if windows is None else [r for r, i in enumerate(windows) if i in edges]
     regions = {"all": (slice(None), slice(None)), "pos 0-5": (slice(None), f(0, 5)),
                "pos 5888-5996": (slice(None), f(5888, 5996)), "pos 5976-5996": (slice(None), f(5976, 5996))}
     if edge:

@@ -37,3 +37,22 @@ def test_conv_t_registers(log, kernel):
     stores, loads, regs = map(int, m.groups())
     assert stores == 0 and loads == 0, f"{kernel} spills ({stores} B stored, {loads} B loaded)"
     assert regs <= 168, f"{kernel} uses {regs} registers; 384 threads per SM allow 168"
+
+
+# Layer 1 from caller tokens checks each half's three tokens before it takes a triple-table row; that check must not cost the
+# kernels their occupancy: embed_conv1_kernel runs 8 CTAs of 256 threads per SM (32 registers), layer1_wv_kernel 1024 threads.
+LAYER1 = {"embed_conv1_kernel<false>": ("_ZN3gnm18embed_conv1_kernelILb0EEEvPKhPKtPKfS6_S6_PhiPNS_12DeviceStatusE", 32),
+          "embed_conv1_kernel<true>": ("_ZN3gnm18embed_conv1_kernelILb1EEEvPKhPKtPKfS6_S6_PhiPNS_12DeviceStatusE", 32),
+          "layer1_wv_kernel<false>": ("_ZN3gnm16layer1_wv_kernelILb0EEEv14CUtensorMap_stNS_11FusedParamsE", 64),
+          "layer1_wv_kernel<true>": ("_ZN3gnm16layer1_wv_kernelILb1EEEv14CUtensorMap_stNS_11FusedParamsE", 64)}
+
+
+@pytest.mark.parametrize("kernel", sorted(LAYER1))
+def test_layer1_registers(log, kernel):
+    mangled, cap = LAYER1[kernel]
+    m = re.search(r"Function properties for " + re.escape(mangled) + r"\n.*?(\d+) bytes spill stores, (\d+) bytes spill loads"
+                  r"\n.*?Used (\d+) registers", log)
+    assert m, f"no ptxas resource report for {kernel} in build.log"
+    stores, loads, regs = map(int, m.groups())
+    assert stores == 0 and loads == 0, f"{kernel} spills ({stores} B stored, {loads} B loaded)"
+    assert regs <= cap, f"{kernel} uses {regs} registers, more than {cap}"

@@ -72,14 +72,16 @@ def _fetch(w, a, max_batch, opts, stops=(2, 3, 0)):
     return got
 
 
-def _check(label, w, a, got, conv_impl=0):
-    """Every stage present in `got` against its bar; prints one table row per stage, returns the misses."""
+def _check(label, w, a, got, conv_impl=0, tokens=None, regions=None):
+    """Every stage present in `got` against its bar; prints one table row per stage, returns the misses.  tokens: layer 1's
+    input when it is not the tokenization of the windows `a`; regions: (positions, pooled positions) region sets of
+    R.position_regions when `got` holds a sample of a larger batch."""
     n = len(a)
-    reg, preg = R.position_regions(n), R.position_regions(n, pooled=True)
+    reg, preg = regions or (R.position_regions(n), R.position_regions(n, pooled=True))
     conv_bar = "conv_fp32" if conv_impl else "conv_tc"
     checks = []
     if "y1" in got:
-        checks += [("y1", "y1", got["y1"], R.conv1(T.tokenize_windows(a), w), reg),
+        checks += [("y1", "y1", got["y1"], R.conv1(T.tokenize_windows(a) if tokens is None else tokens, w), reg),
                    ("y2 (conv2)", conv_bar, got["y2"], R.conv(got["y1"], w["c2w"], w["c2b"]), reg),
                    ("q0 (w_v#0)", "wv", got["q0"], R.wv_pool(got["y1"], w["ig0_w_v"]), preg),
                    ("mpi0", "gather", got["mpi0"], R.gather(got["y1"], w, 0), {})]

@@ -186,12 +186,20 @@ def _skip_restart_scenarios(gold, fa, out):
     assert list(z["contig_names"]) == list(r["contig_names"]) and np.abs(z["predictions"] - r["predictions"]).max() <= 1e-4
 
 
+def _working_copy(src, dst):
+    """A writable copy of the golden input.  copytree keeps the permission bits of the source, so a copy taken from a read-only
+    checkout would be read-only too and the module could not write its output directory into it."""
+    shutil.copytree(src, dst)
+    for p in [dst, *dst.rglob("*")]:
+        p.chmod(p.stat().st_mode | 0o200)
+
+
 def _run_module_and_compare(gold, tmp_path):
     """genomad_b200.nn_classification.main on the golden input, both runs: same files, names, NPZ keys / dtypes, JSON, log messages;
     scores within 1e-4 of the reference module's, TSV equal up to one unit in the 4th decimal."""
     for run, single in RUNS:
         work = tmp_path / run
-        shutil.copytree(gold / "input", work)
+        _working_copy(gold / "input", work)
         out = work / "out"
         out.mkdir()
         shutil.move(str(work / "toy_find_proviruses"), str(out / "toy_find_proviruses"))
@@ -267,7 +275,7 @@ def test_reference_consumer_accepts_our_outputs(gold, golden_dir, tmp_path, weig
     monkeypatch.setattr(nn_classification, "_make_classifier", lambda batch_size, device: object())
     monkeypatch.setattr(nn_classification, "_classify_parsed", oracle_classify)
     work = tmp_path / "case"
-    shutil.copytree(gold / "input", work)
+    _working_copy(gold / "input", work)
     out = work / "out"
     out.mkdir()
     shutil.move(str(work / "toy_find_proviruses"), str(out / "toy_find_proviruses"))

@@ -61,6 +61,15 @@ class NNOutputs:
     def provirus_nn_classification_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification.npz")
 
+    # ---- opt-in (--write-embeddings), not a reference output: per-contig mean encoder embeddings
+    @property
+    def nn_classification_embeddings_output(self) -> Path:
+        return self._nn("nn_classification_embeddings.npz")
+
+    @property
+    def provirus_nn_classification_embeddings_output(self) -> Path:
+        return self._nn("provirus_nn_classification_embeddings.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

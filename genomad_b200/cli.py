@@ -43,14 +43,19 @@ def cli():
 @click.option("--write-tfrecords", is_flag=True, default=False, show_default=True,
               help="Also write the reference's TFRecord intermediates (<count>.tfrec) to the encoded-sequences "
                    "directory. Not an option of the reference: it always writes them; here nothing reads them.")
-def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords):
+@click.option("--write-embeddings", is_flag=True, default=False, show_default=True,
+              help="Also write each sequence's mean encoder embedding (512 values, the network's vector representation) to "
+                   "<prefix>_nn_classification_embeddings.npz. Not an option of the reference.")
+def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
+                      write_embeddings):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
     from . import nn_classification as module
     if write_tfrecords:
         os.environ["GENOMAD_B200_TFRECORDS"] = "1"
-    module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup)
+    module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
+                write_embeddings=True if write_embeddings else None)
 
 
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)

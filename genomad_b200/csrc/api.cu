@@ -790,7 +790,7 @@ static int launch_logits(gnm_handle* h, int s, int n, cudaStream_t st) {
 // 128 CTAs run at batch 1024; the split-K partials go through logits_part (6 x 752 floats per window >= 8 x 512).
 constexpr int kHeadSplits = 8;
 static_assert(kHeadSplits * kHidden <= kLgSplits * kLogitsLd, "logits_part is too small for the head's split-K partials");
-static int launch_dense_tc(gnm_handle* h, int layer, int n, float* out, float* out_hi, float* out_lo, cudaStream_t st) {
+static int launch_dense_tc(gnm_handle* h, int layer, int n, float* out, float* out_hi, float* out_lo, float* emit, cudaStream_t st) {
   const int K = layer == 0 ? 256 : kHidden;
   LogitsTcParams p;
   p.part = h->logits_part; p.ldc = kHidden; p.n_rows = n; p.n_cols = kHidden; p.status = h->status;
@@ -803,7 +803,7 @@ static int launch_dense_tc(gnm_handle* h, int layer, int n, float* out, float* o
   if (check_launch(h, "logits_tc_kernel(dense)")) return 1;
   const size_t total = static_cast<size_t>(n) * kHidden;
   splitk_reduce_epi_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-      h->logits_part, out, out_hi, out_lo, n, kHidden, splits, layer == 0 ? h->d0b : h->d1b,
+      h->logits_part, out, out_hi, out_lo, emit, n, kHidden, splits, layer == 0 ? h->d0b : h->d1b,
       layer == 0 ? h->bn0_scale : h->bn1_scale, layer == 0 ? h->bn0_shift : h->bn1_shift, 1);
   return check_launch(h, "splitk_reduce_epi_kernel");
 }
@@ -888,8 +888,10 @@ static int forward_main(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d
 }
 
 // tail of a step: attention logits, softmax + weighted sum, dense head -> probabilities.  Small kernels
-// that read only q / mpi of the current buffer set and the tail-only buffers (logits, h0..h2)
-static int forward_tail(gnm_handle* h, int n, float* d_probs, cudaStream_t st) {
+// that read only q / mpi of the current buffer set and the tail-only buffers (logits, h0..h2).
+// d_embed (the step's first row, or null): dense layer 0's output h1 -- the encoder's output -- is also stored there; with
+// d_probs null the head stops after that layer.
+static int forward_tail(gnm_handle* h, int n, float* d_probs, float* d_embed, cudaStream_t st) {
   for (int s = 0; s < 2; ++s) {
     timer_mark(h, s ? "logits1" : "logits0", st);
     if (launch_logits(h, s, n, st)) return 1;
@@ -899,10 +901,14 @@ static int forward_tail(gnm_handle* h, int n, float* d_probs, cudaStream_t st) {
   }
   timer_mark(h, "head", st);
   if (h->conv_impl == 0) {       // tensor cores, 3 x TF32 (the model's dense projections; the FFMA kernels stay the validation path)
-    if (launch_dense_tc(h, 0, n, h->h1, h->hA_hi[1], h->hA_lo[1], st)) return 1;
-    if (launch_dense_tc(h, 1, n, h->h2, nullptr, nullptr, st)) return 1;
+    if (launch_dense_tc(h, 0, n, h->h1, h->hA_hi[1], h->hA_lo[1], d_embed, st)) return 1;
+    if (!d_probs) { timer_mark(h, "end", st); return 0; }
+    if (launch_dense_tc(h, 1, n, h->h2, nullptr, nullptr, nullptr, st)) return 1;
   } else {
     if (launch_sgemm(h, h->h0, 256, h->d0w, kHidden, h->h1, kHidden, n, kHidden, 256, h->d0b, h->bn0_scale, h->bn0_shift, 1, st)) return 1;
+    if (d_embed)
+      GNM_CUDA(cudaMemcpyAsync(d_embed, h->h1, static_cast<size_t>(n) * kHidden * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (!d_probs) { timer_mark(h, "end", st); return 0; }
     if (launch_sgemm(h, h->h1, kHidden, h->d1w, kHidden, h->h2, kHidden, n, kHidden, kHidden, h->d1b, h->bn1_scale, h->bn1_shift, 1, st)) return 1;
   }
   dense3_softmax_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(h->h2, h->d2w, h->d2b, d_probs, n);
@@ -912,11 +918,11 @@ static int forward_tail(gnm_handle* h, int n, float* d_probs, cudaStream_t st) {
 }
 
 // One step: n <= max_batch windows, strictly in order on one stream.
-static int forward_step(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs,
+static int forward_step(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, float* d_embed,
                         cudaStream_t st) {
   const int rc = forward_main(h, d_ascii, d_tok, n, st);
   if (rc) return rc == 2 ? 0 : 1;
-  return forward_tail(h, n, d_probs, st);
+  return forward_tail(h, n, d_probs, d_embed, st);
 }
 
 // Steps of a multi-step call with the tails overlapped: the main part of step i+1 (which starts with the issue-bound layer-1
@@ -928,9 +934,9 @@ struct TailOverlap {
   bool on;
   TailOverlap(gnm_handle* h_, cudaStream_t st_, int n_steps)
       : h(h_), st(st_), on(h_->tail_overlap && n_steps > 1 && !h_->profile_stages && h_->debug_stop == 0) {}
-  int step(const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, cudaStream_t* tail_out = nullptr) {
+  int step(const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, float* d_embed, cudaStream_t* tail_out = nullptr) {
     if (tail_out) *tail_out = st;
-    if (!on) return forward_step(h, d_ascii, d_tok, n, d_probs, st);
+    if (!on) return forward_step(h, d_ascii, d_tok, n, d_probs, d_embed, st);
     const int par = steps_done & 1;
     select_set(h, par);
     if (steps_done >= 2) GNM_CUDA(cudaStreamWaitEvent(st, h->tail_done[par], 0));
@@ -938,7 +944,7 @@ struct TailOverlap {
     if (rc) return 1;
     GNM_CUDA(cudaEventRecord(h->main_done[par], st));
     GNM_CUDA(cudaStreamWaitEvent(h->tail_stream, h->main_done[par], 0));
-    if (forward_tail(h, n, d_probs, h->tail_stream)) return 1;
+    if (forward_tail(h, n, d_probs, d_embed, h->tail_stream)) return 1;
     if (tail_out) *tail_out = h->tail_stream;
     GNM_CUDA(cudaEventRecord(h->tail_done[par], h->tail_stream));
     ++steps_done;
@@ -971,11 +977,16 @@ static int check_device_status(gnm_handle* h) {
   return 0;
 }
 
-static int forward_any(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, void* stream) {
+// d_probs + off * 3 / d_embed + off * 512 of the step that starts at window `off` (null stays null)
+static float* probs_at(float* d_probs, int off) { return d_probs ? d_probs + static_cast<size_t>(off) * 3 : nullptr; }
+static float* embed_at(float* d_embed, int off) { return d_embed ? d_embed + static_cast<size_t>(off) * kHidden : nullptr; }
+
+static int forward_any(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, float* d_embed,
+                       void* stream) {
   if (!h) return fail("null handle");
   if (n < 0) return fail("negative window count");
   if (n == 0) return 0;
-  if ((!d_ascii && !d_tok) || !d_probs) return fail("null buffer");
+  if ((!d_ascii && !d_tok) || (!d_probs && !d_embed)) return fail("null buffer");
   GNM_CUDA(cudaSetDevice(h->device));
   if (check_device_status(h)) return 1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -983,16 +994,24 @@ static int forward_any(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_
   for (int off = 0; off < n; off += h->max_batch) {
     const int m = std::min(h->max_batch, n - off);
     if (ov.step(d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : nullptr,
-                d_tok ? d_tok + static_cast<size_t>(off) * kTok : nullptr, m, d_probs + static_cast<size_t>(off) * 3)) return 1;
+                d_tok ? d_tok + static_cast<size_t>(off) * kTok : nullptr, m, probs_at(d_probs, off), embed_at(d_embed, off))) return 1;
   }
   return ov.join();
 }
 
 extern "C" int gnm_forward_ascii(gnm_handle* h, const uint8_t* d_ascii, int n, float* d_probs, void* stream) {
-  return forward_any(h, d_ascii, nullptr, n, d_probs, stream);
+  return forward_any(h, d_ascii, nullptr, n, d_probs, nullptr, stream);
 }
 extern "C" int gnm_forward_tokens(gnm_handle* h, const uint16_t* d_tokens, int n, float* d_probs, void* stream) {
-  return forward_any(h, nullptr, d_tokens, n, d_probs, stream);
+  return forward_any(h, nullptr, d_tokens, n, d_probs, nullptr, stream);
+}
+extern "C" int gnm_embed_ascii(gnm_handle* h, const uint8_t* d_ascii, int n, float* d_probs, float* d_embed, void* stream) {
+  if (!d_embed && n > 0) return fail("gnm_embed_ascii: d_embed is null");
+  return forward_any(h, d_ascii, nullptr, n, d_probs, d_embed, stream);
+}
+extern "C" int gnm_embed_tokens(gnm_handle* h, const uint16_t* d_tokens, int n, float* d_probs, float* d_embed, void* stream) {
+  if (!d_embed && n > 0) return fail("gnm_embed_tokens: d_embed is null");
+  return forward_any(h, nullptr, d_tokens, n, d_probs, d_embed, stream);
 }
 
 extern "C" int gnm_encode(gnm_handle* h, const uint8_t* d_ascii, int n, uint16_t* d_tokens, void* stream) {
@@ -1070,12 +1089,12 @@ extern "C" int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int
 
 // Steps of max_batch windows: gather into in_stage[step parity], then the unchanged forward step.  The gather runs on the
 // step's main stream, ahead of the layer-1 kernel that reads the stage, so the TailOverlap ordering covers both buffers.
-extern "C" int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
-                                   int n, float* d_probs, void* stream) {
+static int forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                           float* d_probs, float* d_embed, void* stream) {
   if (!h) return fail("gnm_forward_windows: null handle");
   if (n < 0) return fail("gnm_forward_windows: negative window count");
   if (n == 0) return 0;
-  if (!d_seq || !d_win_start || !d_win_len || !d_probs) return fail("gnm_forward_windows: null buffer");
+  if (!d_seq || !d_win_start || !d_win_len || (!d_probs && !d_embed)) return fail("gnm_forward_windows: null buffer");
   GNM_CUDA(cudaSetDevice(h->device));
   if (check_device_status(h)) return 1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1085,9 +1104,18 @@ extern "C" int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const in
     uint8_t* stage = h->in_stage[i & 1];
     timer_mark(h, "gather_windows", st);
     if (launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, stage, st)) return 1;
-    if (ov.step(stage, nullptr, m, d_probs + static_cast<size_t>(off) * 3)) return 1;
+    if (ov.step(stage, nullptr, m, probs_at(d_probs, off), embed_at(d_embed, off))) return 1;
   }
   return ov.join();
+}
+extern "C" int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                   int n, float* d_probs, void* stream) {
+  return forward_windows(h, d_seq, d_win_start, d_win_len, n, d_probs, nullptr, stream);
+}
+extern "C" int gnm_embed_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                 int n, float* d_probs, float* d_embed, void* stream) {
+  if (!d_embed && n > 0) return fail("gnm_embed_windows: d_embed is null");
+  return forward_windows(h, d_seq, d_win_start, d_win_len, n, d_probs, d_embed, stream);
 }
 
 static int segment_any(gnm_handle* h, const float* d_probs, const int32_t* d_offsets, int n_contigs, float* d_out,
@@ -1112,6 +1140,25 @@ extern "C" int gnm_segment_sum(gnm_handle* h, const float* d_probs, const int32_
   return segment_any(h, d_probs, d_offsets, n_contigs, d_sum4, stream, false);
 }
 
+// carry_out is copied from the last segment's sum after the kernel, in stream order, so it may alias carry_in
+extern "C" int gnm_segment_sum_rows(gnm_handle* h, const float* d_rows, const int32_t* d_offsets, int k, const float* d_carry_in,
+                                    float* d_sums, float* d_carry_out, void* stream) {
+  if (!h) return fail("gnm_segment_sum_rows: null handle");
+  if (k < 0) return fail("gnm_segment_sum_rows: negative segment count");
+  if (k == 0) return 0;
+  if (!d_offsets || !d_sums) return fail("gnm_segment_sum_rows: null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_rows) | reinterpret_cast<uintptr_t>(d_sums) | reinterpret_cast<uintptr_t>(d_carry_in)) % 16)
+    return fail("gnm_segment_sum_rows: d_rows, d_sums and d_carry_in must be 16-byte aligned");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  segment_sum_rows_kernel<<<k, kSegRowThreads, 0, st>>>(d_rows, d_offsets, d_carry_in, d_sums);
+  if (check_launch(h, "segment_sum_rows_kernel")) return 1;
+  if (d_carry_out)
+    GNM_CUDA(cudaMemcpyAsync(d_carry_out, d_sums + static_cast<size_t>(k - 1) * kHidden, kHidden * sizeof(float),
+                             cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
 // Wait for the work queued on `stream` and report device-side failures of the steps run so far (mbarrier time-outs,
 // activation range overflow).  The asynchronous entry points only see such a flag on the NEXT call.
 extern "C" int gnm_check_status(gnm_handle* h, void* stream) {
@@ -1121,12 +1168,12 @@ extern "C" int gnm_check_status(gnm_handle* h, void* stream) {
   return check_device_status(h);
 }
 
-// Host buffers in, host buffers out; H2D of step i+1 overlaps compute of step i.
-extern "C" int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs) {
+// Host buffers in, host buffers out; H2D of step i+1 overlaps compute of step i.  d_embed (device, or null): embeddings too.
+static int classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs, float* d_embed) {
   if (!h) return fail("null handle");
   if (n < 0) return fail("negative window count");
   if (n == 0) return 0;
-  if (!h_ascii || !h_probs) return fail("null buffer");
+  if (!h_ascii || (!h_probs && !d_embed)) return fail("null buffer");
   GNM_CUDA(cudaSetDevice(h->device));
   if (check_device_status(h)) return 1;
   const int mb = h->max_batch;
@@ -1142,18 +1189,26 @@ extern "C" int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, f
     GNM_CUDA(cudaEventRecord(h->in_ready[b], h->copy_stream));
     GNM_CUDA(cudaStreamWaitEvent(h->compute_stream, h->in_ready[b], 0));
     cudaStream_t tail = h->compute_stream;               // the stream that produced out_stage[b] (tail_stream when overlapped)
-    if (ov.step(h->in_stage[b], nullptr, m, h->out_stage[b], &tail)) return 1;
+    if (ov.step(h->in_stage[b], nullptr, m, h_probs ? h->out_stage[b] : nullptr, embed_at(d_embed, off), &tail)) return 1;
     // the input stage is only read by layer 1, but the event sits after the step's main part (the same stream); the output
     // stage of parity b is rewritten by the tail of step i+2, which is ordered after this copy on the same stream
     GNM_CUDA(cudaEventRecord(h->in_free[b], h->compute_stream));
-    GNM_CUDA(cudaMemcpyAsync(h_probs + static_cast<size_t>(off) * 3, h->out_stage[b], static_cast<size_t>(m) * 3 * sizeof(float),
-                             cudaMemcpyDeviceToHost, tail));
+    if (h_probs)
+      GNM_CUDA(cudaMemcpyAsync(h_probs + static_cast<size_t>(off) * 3, h->out_stage[b], static_cast<size_t>(m) * 3 * sizeof(float),
+                               cudaMemcpyDeviceToHost, tail));
     if (ov.on) GNM_CUDA(cudaEventRecord(h->tail_done[b], tail));     // re-record: the buffer set is free once the copy is queued behind the tail
   }
   if (ov.join()) return 1;
   GNM_CUDA(cudaStreamSynchronize(h->compute_stream));
   if (ov.on) GNM_CUDA(cudaStreamSynchronize(h->tail_stream));
   return check_device_status(h);
+}
+extern "C" int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs) {
+  return classify_host(h, h_ascii, n, h_probs, nullptr);
+}
+extern "C" int gnm_embed_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs, float* d_embed) {
+  if (!d_embed && n > 0) return fail("gnm_embed_host: d_embed is null");
+  return classify_host(h, h_ascii, n, h_probs, d_embed);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -107,10 +107,11 @@ splitk_reduce_kernel(const float* __restrict__ partials, float* __restrict__ C, 
 
 // Dense epilogue after the tensor-core GEMM (logits_tc_kernel): C[m][n] = epi(sum of the split-K partials in fixed order),
 // epi: v += bias[n]; v = v * scale[n] + shift[n] (Keras BatchNormalization, inference form); relu.  Also writes the value's
-// two TF32 halves (low 13 mantissa bits clear) when the result is the A operand of the next tensor-core GEMM.
+// two TF32 halves (low 13 mantissa bits clear) when the result is the A operand of the next tensor-core GEMM, and, when E is set,
+// the value once more into the caller's embedding rows (E already points at the step's first row; the index is 64-bit).
 __global__ void __launch_bounds__(256)
 splitk_reduce_epi_kernel(const float* __restrict__ partials, float* __restrict__ C, float* __restrict__ C_hi, float* __restrict__ C_lo,
-                         int M, int N, int parts, const float* __restrict__ bias, const float* __restrict__ scale,
+                         float* __restrict__ E, int M, int N, int parts, const float* __restrict__ bias, const float* __restrict__ scale,
                          const float* __restrict__ shift, int relu) {
   const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   const size_t total = static_cast<size_t>(M) * N;
@@ -122,6 +123,7 @@ splitk_reduce_epi_kernel(const float* __restrict__ partials, float* __restrict__
   v = v * scale[n] + shift[n];
   if (relu) v = fmaxf(v, 0.f);
   C[i] = v;
+  if (E) E[i] = v;
   if (C_hi) {
     const float hi = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
     C_hi[i] = hi;
@@ -190,6 +192,26 @@ __global__ void segment_reduce_kernel(const float* __restrict__ probs, const int
     out[static_cast<size_t>(c) * 4 + 2] = s2;
     out[static_cast<size_t>(c) * 4 + 3] = cnt;
   }
+}
+
+// Per-segment sums of 512-wide rows (window embeddings -> per-contig sums): one CTA per segment, 128 threads x 4 columns, so
+// each 2 KB row is one fully coalesced 16-byte-per-thread load.  Every column is a plain fp32 running sum in row order (no FMA,
+// no tree: the rule of segment_reduce_kernel), so splitting the rows into calls and chaining them through the carry gives the
+// same bits as one call.  Segment 0 starts from carry_in when it is set; carry_out is written by the caller (see api.cu).
+constexpr int kSegRowThreads = kHidden / 4;
+__global__ void __launch_bounds__(kSegRowThreads)
+segment_sum_rows_kernel(const float* __restrict__ rows, const int32_t* __restrict__ offsets, const float* __restrict__ carry_in,
+                        float* __restrict__ sums) {
+  const int c = blockIdx.x;
+  const int col = threadIdx.x * 4;
+  const int b = offsets[c], e = offsets[c + 1];
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (c == 0 && carry_in) s = *reinterpret_cast<const float4*>(carry_in + col);
+  for (int i = b; i < e; ++i) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(rows + static_cast<size_t>(i) * kHidden + col));
+    s.x = __fadd_rn(s.x, v.x); s.y = __fadd_rn(s.y, v.y); s.z = __fadd_rn(s.z, v.z); s.w = __fadd_rn(s.w, v.w);
+  }
+  *reinterpret_cast<float4*>(sums + static_cast<size_t>(c) * kHidden + col) = s;
 }
 
 }  // namespace gnm

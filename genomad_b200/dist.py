@@ -119,3 +119,131 @@ def allreduce_partials(partials, world_size: int, group=None):
 def finish_mean(partials):
     cnt = partials[:, 3:4].clamp(min=1)
     return partials[:, :3] / cnt
+
+
+# ------------------------------------------------------------------------------------------------ per-contig embeddings
+# Per-contig mean embeddings must not depend on the number of GPUs either, but an all-gather of the [W, 512] window embeddings
+# is out of the question (100 GB at 50 M windows).  Instead every rank sums its rows per contig with a carry chain:
+#   * interior contigs (those that begin on the rank) are reduced from zero as the rank's chunks arrive;
+#   * the HEAD FRAGMENT -- the rows of a contig that began on an earlier rank -- is kept unreduced (bounded by the longest
+#     contig: 167 k windows, 333 MB for a 1 Gbp chromosome);
+#   * at the end a carry runs from rank 0 upward (point-to-point): rank r receives the running sum of its head contig, reduces the
+#     head fragment seeded with it, and passes on that running sum if the contig continues past its shard, else the running sum
+#     of its own last contig;
+#   * the rank that holds a contig's last window completes it; the means (sum / count, fp32) are gathered to rank 0.
+# Every column is one fp32 running sum in window order however the rows are split, so the result is bitwise the one-process
+# result.  `reducer(rows [R, 512], offsets int32 [k + 1], carry [512] or None) -> (sums [k, 512], carry [512])` is the segment sum
+# (Classifier.segment_sum_rows on the GPU; a NumPy statement in the CPU tests).
+
+def _contig_of(offsets: np.ndarray, w: int) -> int:
+    """Index of the (non-empty) contig that holds window w."""
+    return int(np.searchsorted(offsets, w, side="right")) - 1
+
+
+class EmbeddingShard:
+    """Streams one rank's rows [start, end) of the global window list and reduces them per contig (see above)."""
+
+    def __init__(self, offsets: np.ndarray, start: int, end: int, reducer, device="cpu", width: int = 512):
+        import torch
+        self.offsets = np.asarray(offsets, dtype=np.int64)
+        self.start, self.end, self.reducer, self.width = start, end, reducer, width
+        self.device = torch.device(device)
+        self.pos = start
+        self.head = -1                                   # contig of the head fragment, -1 = none
+        self.head_end = start                            # rows [start, head_end) are the head fragment
+        if start < end:
+            c = _contig_of(self.offsets, start)
+            if self.offsets[c] < start:
+                self.head, self.head_end = c, min(end, int(self.offsets[c + 1]))
+        self.head_rows = []
+        # contigs completed on this rank: those whose last window lies in [start, end) -- a contiguous index range
+        self.lo = int(np.searchsorted(self.offsets[1:], start, side="right"))
+        self.hi = int(np.searchsorted(self.offsets[1:], end, side="right"))
+        self.sums = torch.zeros((self.hi - self.lo, width), dtype=torch.float32, device=self.device)
+        self.carry = None                                # running sum of the interior contig that holds row pos - 1
+        self._torch = torch
+
+    def add(self, rows) -> None:
+        """The next rows of the shard, in order (any split into calls gives the same result)."""
+        a, b = self.pos, self.pos + rows.shape[0]
+        assert b <= self.end
+        self.pos = b
+        sums = self.sums
+        if a < self.head_end:                            # head fragment: kept as is (a copy: the caller reuses its buffer)
+            k = min(b, self.head_end) - a
+            self.head_rows.append(rows[:k].clone())
+            rows, a = rows[k:], a + k
+        if a >= b:
+            return
+        off = self.offsets
+        ca, cb = _contig_of(off, a), _contig_of(off, b - 1)
+        seg = (np.clip(off[ca: cb + 2], a, b) - a).astype(np.int32)
+        carry = self.carry if off[ca] < a else None      # segment 0 continues the previous rows' contig
+        s, self.carry = self.reducer(rows, self._torch.from_numpy(seg).to(self.device), carry)
+        done = cb + 1 if off[cb + 1] <= b else cb         # contigs ca .. done-1 end inside these rows
+        if done > ca:
+            sums[ca - self.lo: done - self.lo] = s[: done - ca]
+
+    def finish(self, info: "DistInfo", send=None, recv=None):
+        """Run the carry chain; returns (first completed contig, means [hi - lo, width]) of this rank."""
+        import torch
+        assert self.pos == self.end, "EmbeddingShard.finish before all rows were added"
+        dev = self.device
+        send = send or (lambda t, dst: _p2p_send(t, dst))
+        recv = recv or (lambda t, src: _p2p_recv(t, src))
+        carry_in = torch.zeros(self.width, dtype=torch.float32, device=dev)
+        if info.rank > 0:
+            recv(carry_in, info.rank - 1)
+        out = self.carry if self.carry is not None else torch.zeros_like(carry_in)
+        if self.start == self.end:
+            out = carry_in                               # no rows: pass the running sum on unchanged
+        elif self.head >= 0:
+            rows = torch.cat(self.head_rows) if self.head_rows else torch.zeros((0, self.width), dtype=torch.float32, device=dev)
+            seg = torch.tensor([0, rows.shape[0]], dtype=torch.int32, device=dev)
+            s, run = self.reducer(rows, seg, carry_in)
+            if int(self.offsets[self.head + 1]) > self.end:
+                out = run                                # the head contig also covers the whole shard: forward its carry
+            else:
+                self.sums[self.head - self.lo] = s[0]
+        if info.rank + 1 < info.world_size:
+            send(out.contiguous(), info.rank + 1)
+        cnt = np.diff(self.offsets)[self.lo: self.hi].astype(np.float32)
+        cnt_t = torch.from_numpy(np.maximum(cnt, 1.0)).to(dev)
+        return self.lo, self.sums / cnt_t[:, None]
+
+
+def _p2p_send(t, dst):
+    import torch.distributed as dist
+    dist.send(t, dst)
+
+
+def _p2p_recv(t, src):
+    import torch.distributed as dist
+    dist.recv(t, src)
+
+
+def gather_contig_means(lo: int, means, n_contigs: int, info: DistInfo, group=None):
+    """Each rank's completed contigs [lo, lo + len) -> [n_contigs, width] on rank 0 (None on the others).  Contigs no rank
+    completed (no windows) stay zero."""
+    import torch
+    import torch.distributed as dist
+    width = means.shape[1]
+    if info.world_size == 1:
+        out = torch.zeros((n_contigs, width), dtype=torch.float32, device=means.device)
+        out[lo: lo + means.shape[0]] = means
+        return out
+    meta = torch.tensor([lo, means.shape[0]], dtype=torch.int64, device=means.device)
+    metas = [torch.empty_like(meta) for _ in range(info.world_size)]
+    dist.all_gather(metas, meta, group=group)
+    cap = max(1, max(int(m[1]) for m in metas))
+    buf = torch.zeros((cap, width), dtype=torch.float32, device=means.device)
+    buf[: means.shape[0]] = means
+    parts = [torch.empty_like(buf) for _ in range(info.world_size)]
+    dist.all_gather(parts, buf, group=group)
+    if not info.is_main:
+        return None
+    out = torch.zeros((n_contigs, width), dtype=torch.float32, device=means.device)
+    for m, p in zip(metas, parts):
+        a, k = int(m[0]), int(m[1])
+        out[a: a + k] = p[:k]
+    return out

@@ -24,6 +24,7 @@ _lib = None
 
 WINDOW = 6000
 TOKENS = 5997
+EMBED = 512                      # encoder output width (GNM_EMBED)
 
 
 class GnmError(RuntimeError):
@@ -67,6 +68,11 @@ EXPORTS = {
                                      C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "gnm_gather_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_forward_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_embed_tokens": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_embed_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_embed_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_embed_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_segment_sum_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
     "gnm_get_option": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]),
     "gnm_kernel_launches": (C.c_longlong, [C.c_void_p]),
@@ -231,6 +237,68 @@ class Classifier:
                                                   n, out.data_ptr(), self._stream()))
         return out
 
+    # ------------------------------------------------------------------ encoder embeddings
+    def _embed_out(self, n: int, device):
+        t = self._torch
+        return (t.empty((n, 3), dtype=t.float32, device=device), t.empty((n, EMBED), dtype=t.float32, device=device))
+
+    def embed_tokens(self, tokens):
+        """uint16 cuda [n, 5997] -> (probabilities float32 [n, 3], encoder embeddings float32 [n, 512]) (gnm_embed_tokens)."""
+        t = self._torch
+        k = tokens.contiguous()
+        assert k.dtype == t.uint16 and k.dim() == 2 and k.shape[1] == TOKENS and k.is_cuda
+        probs, emb = self._embed_out(k.shape[0], k.device)
+        _check(self.lib, self.lib.gnm_embed_tokens(self._h, k.data_ptr(), k.shape[0], probs.data_ptr(), emb.data_ptr(),
+                                                   self._stream()))
+        return probs, emb
+
+    def embed_ascii(self, ascii_windows):
+        """uint8 cuda [n, 6000] -> (probabilities [n, 3], embeddings [n, 512]), both float32 on the device (gnm_embed_ascii)."""
+        t = self._torch
+        a = ascii_windows.contiguous()
+        assert a.dtype == t.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        probs, emb = self._embed_out(a.shape[0], a.device)
+        _check(self.lib, self.lib.gnm_embed_ascii(self._h, a.data_ptr(), a.shape[0], probs.data_ptr(), emb.data_ptr(),
+                                                  self._stream()))
+        return probs, emb
+
+    def embed_windows(self, seq_u8, win_start, win_len):
+        """Windows straight from the sequence buffer (see predict_windows) -> (probabilities [W, 3], embeddings [W, 512])."""
+        t = self._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        probs, emb = self._embed_out(start.numel(), seq_u8.device)
+        _check(self.lib, self.lib.gnm_embed_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
+                                                    start.numel(), probs.data_ptr(), emb.data_ptr(), self._stream()))
+        return probs, emb
+
+    def embed_host_into(self, ascii_ptr: int, n: int, probs_ptr: int, d_embed_ptr: int):
+        """Raw-pointer gnm_embed_host: host windows -> host probabilities (probs_ptr may be 0) + device embeddings [n, 512]."""
+        with self._torch.cuda.device(self.device):
+            _check(self.lib, self.lib.gnm_embed_host(self._h, ascii_ptr, n, probs_ptr or None, d_embed_ptr))
+
+    def segment_sum_rows(self, rows, offsets, carry=None):
+        """rows float32 cuda [R, 512], offsets int32 cuda [k + 1] (offsets[0] = 0) -> (sums float32 [k, 512], carry [512]).
+        Plain fp32 running sums in row order; `carry` (a previous call's) seeds segment 0 and the returned carry is the running
+        sum of segment k-1, so chained calls over consecutive row blocks give the bits of one call."""
+        t = self._torch
+        assert rows.dtype == t.float32 and offsets.dtype == t.int32 and rows.is_cuda and offsets.is_cuda
+        assert rows.dim() == 2 and rows.shape[1] == EMBED
+        rows, offs = rows.contiguous(), offsets.contiguous()
+        k = offs.numel() - 1
+        sums = t.empty((k, EMBED), dtype=t.float32, device=rows.device)
+        if carry is not None:
+            assert carry.dtype == t.float32 and carry.numel() == EMBED and carry.is_cuda
+            carry = carry.contiguous()
+        out_carry = t.zeros(EMBED, dtype=t.float32, device=rows.device) if carry is None else carry.clone()
+        if k == 0:
+            return sums, out_carry
+        rows_ptr = rows.data_ptr() if rows.numel() else sums.data_ptr()      # no rows: any aligned buffer, nothing reads it
+        _check(self.lib, self.lib.gnm_segment_sum_rows(self._h, rows_ptr, offs.data_ptr(), k,
+                                                       carry.data_ptr() if carry is not None else None, sums.data_ptr(),
+                                                       out_carry.data_ptr(), self._stream()))
+        return sums, out_carry
+
     # ------------------------------------------------------------------ contigs in memory -> windows on the device
     def contig_buffers(self, seqs):
         """Contigs -> (uint8 cuda [total_bytes], int64 cuda [n_contigs + 1] offsets), one host-to-device copy each.
@@ -290,24 +358,33 @@ class Classifier:
                                                       start.numel(), out.data_ptr(), self._stream()))
         return out
 
-    def classify_contigs(self, seqs, single_window: bool = False, return_window_probs: bool = False):
+    def classify_contigs(self, seqs, single_window: bool = False, return_window_probs: bool = False,
+                         return_embeddings: bool = False):
         """Contigs in, one score triple per contig out -- what the reference module computes per contig
         (nn_classification.py:65-75, 316-320), with windowing on the GPU.
 
         seqs: list of str / bytes, or a (uint8 tensor, int64 offsets) pair on the host or on CUDA (see contig_buffers).
-        Returns cuda tensors (means float32 [n_contigs, 3], window counts int32 [n_contigs]) and, if asked, the per-window
-        probabilities float32 [W, 3].  A contig that is empty after stripping n/N has count 0 and mean (0, 0, 0); the
-        reference drops such contigs, so drop those rows to mirror its outputs."""
+        Returns cuda tensors (means float32 [n_contigs, 3], window counts int32 [n_contigs]), then, if asked, the per-window
+        probabilities float32 [W, 3], then, if asked, the per-contig mean encoder embeddings float32 [n_contigs, 512]
+        (segment_sum_rows / count in fp32).  A contig that is empty after stripping n/N has count 0, mean (0, 0, 0) and a zero
+        embedding; the reference drops such contigs, so drop those rows to mirror its outputs."""
         t = self._torch
         seq, offs = self.contig_buffers(seqs)
         start, length, woff = self.contig_windows(seq, offs, single_window)
-        probs = self.predict_windows(seq, start, length)
+        if return_embeddings:
+            probs, emb = self.embed_windows(seq, start, length)
+        else:
+            probs = self.predict_windows(seq, start, length)
         if probs.numel():
             means = self.segment_mean(probs, woff)
         else:                 # no contig has a window (an empty probs tensor has no buffer to hand to gnm_segment_mean)
             means = t.zeros((woff.numel() - 1, 3), dtype=t.float32, device=seq.device)
         counts = woff[1:] - woff[:-1]
-        return (means, counts, probs) if return_window_probs else (means, counts)
+        out = (means, counts, probs) if return_window_probs else (means, counts)
+        if return_embeddings:
+            sums, _ = self.segment_sum_rows(emb, woff)
+            out = out + (sums / counts.clamp(min=1).to(t.float32)[:, None],)
+        return out
 
     # ------------------------------------------------------------------ host-buffer API
     def classify_host(self, ascii_windows: np.ndarray) -> np.ndarray:

@@ -79,7 +79,8 @@ def _pinned_chunk(n: int):
     return t, t.numpy()
 
 
-def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, contig_reduce: str = "gather") -> np.ndarray:
+def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, contig_reduce: str = "gather",
+                     embeddings: bool = False):
     """
     Indexed FASTA -> float32 [n_contigs, 3] per-contig mean (identical on all ranks).
 
@@ -87,6 +88,11 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
     chunk straight from the mmap'ed file (upper-case + pad, multi-threaded) while the GPU classifies the previous one
     (gnm_classify_host on a worker thread; the C call releases the GIL) into a pinned result buffer, so neither copy
     direction blocks the host.  Windows never exist on disk, and file pages behind the cursor are released.
+
+    With `embeddings`, every chunk goes through gnm_embed_host instead (same probabilities, plus the encoder output of each
+    window in a device chunk buffer), is summed per contig right away (segment_sum_rows, carried from chunk to chunk) and
+    the per-contig means are combined over the ranks by the carry chain of genomad_b200.dist; returns (means, embeddings),
+    the embeddings float32 [n_contigs, 512] on rank 0 and None on the other ranks.
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -95,6 +101,16 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
     chunk = max(4 * clf.max_batch, 4096)
     keep, bufs = zip(*(_pinned_chunk(min(chunk, max(1, end - start))) for _ in range(2)))
     out_t = torch.empty((max(1, end - start), 3), dtype=torch.float32).pin_memory()
+    dev = torch.device("cuda", clf.device)
+    run = clf.classify_host_into
+    if embeddings:
+        shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
+        d_emb = torch.empty((min(chunk, max(1, end - start)), 512), dtype=torch.float32, device=dev)
+
+        def run(ptr, m, out_ptr):                            # the worker owns d_emb: one chunk at a time
+            clf.embed_host_into(ptr, m, out_ptr, d_emb.data_ptr())
+            shard.add(d_emb[:m])
+            torch.cuda.current_stream(dev).synchronize()
     futures = []
     with ThreadPoolExecutor(max_workers=1) as gpu:
         for i, a in enumerate(range(start, end, chunk)):
@@ -103,13 +119,23 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
                 futures[i - 2].result()                          # buffer i%2 is free again
                 parsed.release_before(a - chunk)
             win = parsed.export_windows(a, b - a, bufs[i % 2])
-            futures.append(gpu.submit(clf.classify_host_into, win.ctypes.data, b - a,
-                                      out_t.data_ptr() + (a - start) * 12))
+            futures.append(gpu.submit(run, win.ctypes.data, b - a, out_t.data_ptr() + (a - start) * 12))
         for f in futures:
             f.result()
     del keep
-    dev = torch.device("cuda", clf.device)
     local_t = out_t[: end - start].to(dev, non_blocking=True)
+    if embeddings:
+        preds = _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
+        lo, means = shard.finish(info)
+        emb = gdist.gather_contig_means(lo, means, len(offsets) - 1, info)
+        return preds, (emb.cpu().numpy() if emb is not None else None)
+    return _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
+
+
+def _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce) -> np.ndarray:
+    """This rank's per-window probabilities (device) -> float32 [n_contigs, 3] per-contig means, identical on all ranks."""
+    import torch
+    dev = local_t.device
     if contig_reduce == "allreduce" and info.world_size > 1:
         loc_off = torch.from_numpy(gdist.local_offsets(offsets, start, end)).to(dev)
         partials = gdist.allreduce_partials(clf.segment_sum(local_t, loc_off), info.world_size)
@@ -126,15 +152,8 @@ def _classify_windows(clf, windows: np.ndarray, offsets: np.ndarray, info: gdist
     n = windows.shape[0]
     start, end = gdist.shard_bounds(n, info.world_size, info.rank)
     local = clf.classify_host(windows[start:end])
-    dev = torch.device("cuda", clf.device)
-    local_t = torch.from_numpy(local).to(dev)
-    if contig_reduce == "allreduce" and info.world_size > 1:
-        loc_off = torch.from_numpy(gdist.local_offsets(offsets, start, end)).to(dev)
-        partials = gdist.allreduce_partials(clf.segment_sum(local_t, loc_off), info.world_size)
-        return gdist.finish_mean(partials).cpu().numpy()
-    probs = gdist.gather_window_probs(local_t, n, info.world_size)
-    off_t = torch.from_numpy(offsets.astype(np.int32)).to(dev)
-    return clf.segment_mean(probs, off_t).cpu().numpy()
+    local_t = torch.from_numpy(local).to(torch.device("cuda", clf.device))
+    return _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
 
 
 def _write_tsv(path: Path, names, preds) -> None:
@@ -173,6 +192,17 @@ def _write_tfrecords(clf, parsed, enc_dir: Path) -> int:
     return files
 
 
+def embeddings_enabled() -> bool:
+    """Opt-in (``--write-embeddings`` / GENOMAD_B200_EMBEDDINGS=1): also write the per-contig mean encoder embeddings."""
+    return os.environ.get("GENOMAD_B200_EMBEDDINGS", "0") not in ("", "0")
+
+
+def _write_embeddings(path: Path, names_key: str, names, emb) -> None:
+    # np.savez, not savez_compressed: 2 KB of fp32 per contig barely compresses, and zlib would turn writing a large
+    # input's embeddings into minutes of work
+    np.savez(path, **{names_key: names, "embeddings": np.asarray(emb, dtype=np.float32)})
+
+
 def _encode_stage(console, enc_dir: Path, id_path: Path, names_key, ids_key, what, is_main, parsed, classifier=None):
     """
     The reference's "encoding" stage (nn_classification.py:215-246) wrote TFRecords of tokens; here tokens never exist on
@@ -204,7 +234,8 @@ def contig_reduce_mode(default: str = "gather") -> str:
     return mode
 
 
-def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None):
+def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
+         write_embeddings=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -212,6 +243,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     info = gdist.init_process_group_if_needed()
     is_main = info.is_main
     contig_reduce = contig_reduce or contig_reduce_mode()
+    write_embeddings = embeddings_enabled() if write_embeddings is None else bool(write_embeddings)
     if is_main:
         utils.start_md5(input_path)                      # hashed in the background while the file is indexed (rank 0 only)
     if not output_path.is_dir() and is_main:
@@ -232,11 +264,17 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              outputs.nn_classification_output, outputs.nn_classification_npz_output]
     descr = ["execution parameters", "directory containing encoded sequence data",
              "contig classification: tabular format", "contig classification: binary format"]
+    if write_embeddings:
+        files.append(outputs.nn_classification_embeddings_output)
+        descr.append("contig embeddings: binary format")
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
         descr += ["directory containing encoded sequence data", "provirus classification: tabular format",
                   "provirus classification: binary format"]
+        if write_embeddings:
+            files.append(outputs.provirus_nn_classification_embeddings_output)
+            descr.append("provirus embeddings: binary format")
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -250,11 +288,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     console.log("Executing genomad nn-classification.")
 
     jobs = [("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
-             "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True)]
+             "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
+             outputs.nn_classification_embeddings_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
-                     outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False))
+                     outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
+                     outputs.provirus_nn_classification_embeddings_output))
 
     plan = None
     info_writer = None
@@ -272,7 +312,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             console.log(f"Creating the {outputs.nn_classification_dir} directory.")
             outputs.nn_classification_dir.mkdir()
         # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
-        plan = [(bool(skip and j[4].exists()), bool(skip and j[7].exists())) for j in jobs]
+        # (with embeddings requested, a classification whose embeddings file is missing is redone: same predictions, bit for bit)
+        plan = [(bool(skip and j[4].exists()), bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())))
+                for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
         # so it is written by a helper thread as soon as the background hash is done and joined before main() returns.
@@ -301,7 +343,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     # ---- stage 1, every job: "encode" (here: record the window -> sequence map; the windows themselves are streamed to the GPU in
     # stage 2).  Like the reference, sequences AND proviruses are encoded before either is classified (nn_classification.py:215-281).
     staged = []
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows), \
+    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path), \
             (enc_skip, cls_skip) in zip(jobs, plan):
         parsed = index = None
         if enc_skip:
@@ -312,9 +354,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         staged.append((parsed, index))
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows), \
+    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path), \
             (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
-        names = preds = None
+        names = preds = emb = None
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
         if cls_skip:
@@ -333,15 +375,23 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                         info_writer.join()                    # the reference has written the JSON by this point
                     sys.exit(1)
                 names, preds = index.names, np.zeros((len(index.names), 3), np.float32)
+                emb = np.zeros((len(index.names), 512), np.float32)
             else:
                 t_c = _time.perf_counter()
-                preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce)
+                if write_embeddings:
+                    preds, emb = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, embeddings=True)
+                else:
+                    preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce)
                 last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
                 names = index.names
             console.log(f"{'Sequences' if what == 'sequence' else 'Proviruses'} classified.")
             if is_main:
                 np.savez_compressed(npz_path, **{names_key: names, "predictions": preds.astype(np.float32)})
             console.log(f"{label} classification in binary format written to {npz_path.name}.")
+            if write_embeddings:
+                if is_main:
+                    _write_embeddings(emb_path, names_key, names, emb)
+                console.log(f"{label} embeddings in binary format written to {emb_path.name}.")
         if parsed is not None:
             parsed.close()
         if cleanup and is_main and enc_dir.is_dir():

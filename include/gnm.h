@@ -30,6 +30,7 @@ extern "C" {
 #define GNM_WINDOW 6000   /* nucleotides per window     (nn_classification.py:68)  */
 #define GNM_TOKENS 5997   /* 4-mer tokens per window    (sequence.py:172; model.py:15) */
 #define GNM_CLASSES 3     /* chromosome, plasmid, virus (model.py:44) */
+#define GNM_EMBED 512     /* encoder output: Dense(512) + BatchNorm + ReLU, model.py:28-30 */
 
 typedef struct gnm_handle gnm_handle;
 
@@ -176,6 +177,37 @@ int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win
 int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                         float* d_probs, void* stream);
 
+/* ---- encoder embeddings ------------------------------------------------------------------- */
+
+/*
+ * The output of the reference's encoder sub-model, create_encoder() (model.py:14-31): relu(BN(h0 @ dense0 + b0)), float
+ * [n][GNM_EMBED] per window -- the "vector representation" the classifier head is trained on (docs nn_classification.md).  The
+ * reference computes it inside nn_model.predict and never hands it out; Keras users rebuild it with nn_model.get_layer("model").
+ * Each gnm_embed_* is the matching gnm_forward_* / gnm_classify_host call with d_embed threaded through: the same steps, the
+ * same kernels, bitwise the same probabilities; dense layer 0's epilogue also stores its rows to d_embed (no extra launch),
+ * so the embeddings are bitwise what gnm_debug_fetch("h1") shows for the last step.
+ *   d_embed  DEVICE float [n][GNM_EMBED], caller-owned, may not be NULL; row offsets are 64-bit (n * 2 KB may exceed 2^31 B).
+ *   d_probs / h_probs  may be NULL: then the head stops after the encoder (device calls) or the probabilities are not copied
+ *            back (gnm_embed_host).
+ * gnm_embed_tokens / gnm_embed_ascii / gnm_embed_windows: asynchronous, like gnm_forward_*.
+ * gnm_embed_host: host windows in, host probabilities out, embeddings stay on the device; synchronous, like gnm_classify_host.
+ *
+ * gnm_segment_sum_rows: per-segment sums of 512-wide rows, d_rows float [rows][512], d_offsets int32 [k + 1] with offsets[0] = 0
+ *   (segment c = rows [offsets[c], offsets[c+1])), d_sums float [k][512].  Each column is a plain fp32 running sum in row order
+ *   (no FMA, no tree: gnm_segment_mean's rule).  Segment 0 starts from d_carry_in [512] when it is not NULL; the running sum of
+ *   segment k-1 is written to d_carry_out [512] when it is not NULL (it may alias d_carry_in).  Summing the rows in several calls,
+ *   each seeded with the previous call's carry, gives the same bits as one call over all rows: what a caller that streams chunks,
+ *   or a rank that continues a contig begun on an earlier rank, needs.  d_rows, d_sums and d_carry_in 16-byte aligned.
+ *   Asynchronous.  Per-contig mean embedding = sums / count in fp32 (empty contig: zeros).
+ */
+int gnm_embed_tokens(gnm_handle* h, const uint16_t* d_tokens, int n, float* d_probs, float* d_embed, void* stream);
+int gnm_embed_ascii(gnm_handle* h, const uint8_t* d_ascii, int n, float* d_probs, float* d_embed, void* stream);
+int gnm_embed_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                      float* d_probs, float* d_embed, void* stream);
+int gnm_embed_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs, float* d_embed);
+int gnm_segment_sum_rows(gnm_handle* h, const float* d_rows, const int32_t* d_offsets, int k, const float* d_carry_in,
+                         float* d_sums, float* d_carry_out, void* stream);
+
 /* ---- host-side FASTA front end (no GPU involved) ------------------------------------------ */
 
 /*
@@ -282,7 +314,8 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  * buffer as fp32.  which: "buf0","buf1" = the two activation buffers [n][5997][128] (after a full
  * step buf0 = y3, buf1 = y2; with debug_stop = 1, buf0 = y1); "q0","q1" [n][749][128];
  * "mpi0","mpi1" [n][2100]; "logits" [n][752] (of the second IGLOO kernel after a full step); "h0" [n][256];
- * "h1","h2" [n][512] = the outputs of the two Dense(512) + BatchNorm + ReLU layers of the head;
+ * "h1","h2" [n][512] = the outputs of the two Dense(512) + BatchNorm + ReLU layers of the head (h1 is the encoder output, the
+ * embedding gnm_embed_* return);
  * "conv_dbg" [num_sms][16] (int64 counters viewed as float pairs).  Used by the per-kernel parity tests and tools/gpu_experiment.py.
  *   conv_t_kernel's counters, per CTA, in clock64 cycles: [0] first consumer warpgroup's total, [1] its MMA phases (first
  *   barrier wait of a unit to its last wgmma's completion), [2] its waits on a_full, [3] its waits on w_full, [4] units,

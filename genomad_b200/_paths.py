@@ -70,6 +70,23 @@ class NNOutputs:
     def provirus_nn_classification_embeddings_output(self) -> Path:
         return self._nn("provirus_nn_classification_embeddings.npz")
 
+    # ---- opt-in (--write-window-scores), not a reference output: class scores of every window, with its coordinates
+    @property
+    def nn_classification_windows_output(self) -> Path:
+        return self._nn("nn_classification_windows.tsv")
+
+    @property
+    def nn_classification_windows_npz_output(self) -> Path:
+        return self._nn("nn_classification_windows.npz")
+
+    @property
+    def provirus_nn_classification_windows_output(self) -> Path:
+        return self._nn("provirus_nn_classification_windows.tsv")
+
+    @property
+    def provirus_nn_classification_windows_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_windows.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

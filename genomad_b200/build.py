@@ -17,7 +17,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libgnm.so"
-SOURCES = [CSRC / "api.cu", CSRC / "fasta.cpp", CSRC / "tfrecord.cpp"]
+SOURCES = [CSRC / "api.cu", CSRC / "fasta.cpp", CSRC / "tfrecord.cpp", CSRC / "tsv.cpp"]
 HEADERS = sorted(CSRC.glob("*.cuh")) + [PKG.parent / "include" / "gnm.h"]
 
 NVCC_FLAGS = [

@@ -46,16 +46,29 @@ def cli():
 @click.option("--write-embeddings", is_flag=True, default=False, show_default=True,
               help="Also write each sequence's mean encoder embedding (512 values, the network's vector representation) to "
                    "<prefix>_nn_classification_embeddings.npz. Not an option of the reference.")
+@click.option("--write-window-scores", is_flag=True, default=False, show_default=True,
+              help="Also write the class scores of every window, with its coordinates in the sequence, to "
+                   "<prefix>_nn_classification_windows.{tsv,npz}: where along a sequence the chromosome, plasmid and virus "
+                   "signal lies. Not an option of the reference.")
+@click.option("--window-stride", type=click.IntRange(1, 6000), default=None, show_default="6000",
+              help="Write the window scores (implies --write-window-scores) for a 6,000-base window every N bases (overlapping "
+                   "windows when N < 6000), a finer score profile. Sequence scores always use the reference's windows. Not an "
+                   "option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
-                      write_embeddings):
+                      write_embeddings, write_window_scores, window_stride):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
     from . import nn_classification as module
     if write_tfrecords:
         os.environ["GENOMAD_B200_TFRECORDS"] = "1"
+    extra = {}
+    if write_window_scores:
+        extra["write_window_scores"] = True
+    if window_stride is not None:
+        extra["window_stride"] = window_stride
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
-                write_embeddings=True if write_embeddings else None)
+                write_embeddings=True if write_embeddings else None, **extra)
 
 
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)

@@ -1035,15 +1035,18 @@ extern "C" int gnm_encode(gnm_handle* h, const uint8_t* d_ascii, int n, uint16_t
 // ------------------------------------------------------------------------------------------------ contigs -> windows
 // Plan (contigs.cuh): count pass -> scan -> one D2H of the total -> capacity check -> write pass.  Scratch: the caller's
 // d_win_offsets only, so a too-small capacity is reported before anything is written to d_win_start / d_win_len.
-extern "C" int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
-                                  int single_window, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
-                                  int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
-  if (!h) return fail("gnm_contig_windows: null handle");
-  if (n_contigs < 0) return fail("gnm_contig_windows: negative contig count");
-  if (capacity < 0) return fail("gnm_contig_windows: negative capacity");
+// gnm_contig_windows is the stride-6000 call of the same kernels as gnm_contig_windows_stride.
+static int plan_contig_windows(gnm_handle* h, const char* fn, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
+                               int single_window, int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
+                               int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+  const std::string f(fn);
+  if (!h) return fail(f + ": null handle");
+  if (n_contigs < 0) return fail(f + ": negative contig count");
+  if (capacity < 0) return fail(f + ": negative capacity");
+  if (stride < 1 || stride > kWindow) return fail(f + ": stride must be in [1, 6000], not " + std::to_string(stride));
   if (!d_seq_offsets || !d_win_offsets || !h_n_windows || (n_contigs > 0 && !d_seq) ||
       (capacity > 0 && (!d_win_start || !d_win_len)))
-    return fail("gnm_contig_windows: null buffer");
+    return fail(f + ": null buffer");
   GNM_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   *h_n_windows = 0;
@@ -1052,22 +1055,37 @@ extern "C" int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int
     GNM_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
-  contig_plan_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, single_window, d_win_offsets, nullptr, nullptr);
+  const int step = single_window ? 0 : stride;         // 0: the first window only
+  contig_plan_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, nullptr, nullptr);
   if (check_launch(h, "contig_plan_kernel<count>")) return 1;
   contig_scan_kernel<<<1, kScanThreads, 0, st>>>(d_win_offsets, n_contigs);
   if (check_launch(h, "contig_scan_kernel")) return 1;
   int32_t total = 0;
   GNM_CUDA(cudaMemcpyAsync(&total, d_win_offsets + n_contigs, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   GNM_CUDA(cudaStreamSynchronize(st));
-  if (total == kPlanBadOffsets) return fail("gnm_contig_windows: d_seq_offsets is not non-decreasing");
-  if (total == kPlanOverflow) return fail("gnm_contig_windows: the contigs have more than 2^31-1 windows");
+  if (total == kPlanBadOffsets) return fail(f + ": d_seq_offsets is not non-decreasing");
+  if (total == kPlanOverflow) return fail(f + ": the contigs have more than 2^31-1 windows");
   *h_n_windows = total;
   if (total > capacity)
-    return fail("gnm_contig_windows: the contigs have " + std::to_string(total) + " windows, capacity is " +
-                std::to_string(capacity) + " (n_contigs + total_bytes / 6000 is always enough)");
+    return fail(f + ": the contigs have " + std::to_string(total) + " windows, capacity is " + std::to_string(capacity) +
+                " (n_contigs + total_bytes / " + std::to_string(stride) + " is always enough)");
   if (total == 0) return 0;
-  contig_plan_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, single_window, d_win_offsets, d_win_start, d_win_len);
+  contig_plan_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, d_win_start, d_win_len);
   return check_launch(h, "contig_plan_kernel<write>");
+}
+
+extern "C" int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
+                                  int single_window, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
+                                  int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+  return plan_contig_windows(h, "gnm_contig_windows", d_seq, d_seq_offsets, n_contigs, single_window, kWindow, d_win_start,
+                             d_win_len, capacity, d_win_offsets, h_n_windows, stream);
+}
+
+extern "C" int gnm_contig_windows_stride(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
+                                         int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
+                                         int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+  return plan_contig_windows(h, "gnm_contig_windows_stride", d_seq, d_seq_offsets, n_contigs, 0, stride, d_win_start,
+                             d_win_len, capacity, d_win_offsets, h_n_windows, stream);
 }
 
 static int launch_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,

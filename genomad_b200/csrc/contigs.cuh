@@ -31,6 +31,7 @@ constexpr int kScanPer = 4;                          // counts per thread and ro
 constexpr int kGatherThreads = 128;
 constexpr int32_t kPlanOverflow = -1;                // offsets[n_contigs] after the scan: more than INT32_MAX windows
 constexpr int32_t kPlanBadOffsets = -2;              //   ... a contig's end lies before its start
+constexpr int32_t kCountOverflow = INT32_MIN;        // count pass: this contig alone has more than INT32_MAX windows
 
 // 0xff in every byte of a 32-bit word (whose first byte has index `base`) that lies inside [a, b)
 __device__ __forceinline__ uint32_t byte_range_mask(int64_t base, int64_t a, int64_t b) {
@@ -112,18 +113,22 @@ __device__ __forceinline__ int warp_count_N(const uint8_t* __restrict__ seq, int
   return __reduce_add_sync(0xffffffffu, n);
 }
 
-// Candidate windows of a stripped contig of L > 0 nt (sequence.py:150-167).
-__device__ __forceinline__ int64_t candidate_windows(int64_t L, int single_window) {
-  if (single_window) return 1;
-  const int64_t n = L / kWindow + (L % kWindow >= kMinTail ? 1 : 0);
-  return n > 0 ? n : 1;
+// Candidate windows of a stripped contig of L > 0 nt at window step s (1 <= s <= 6000): candidate k starts at k s and is
+// min(6000, L - k s) long; the first is always a candidate, every other one only if it has >= 2500 nt, so
+// n_cand = 1 + max(0, (L - 2500) / s).  At s = 6000 this is seq_windows(6000, 2500) (sequence.py:150-167):
+// L / 6000 + (L % 6000 >= 2500), at least 1.  s = 0 stands for --single-window: the first window only.
+__device__ __forceinline__ int64_t candidate_windows(int64_t L, int64_t step) {
+  if (step == 0) return 1;
+  return 1 + (L > kMinTail ? (L - kMinTail) / step : 0);
 }
 
+// Windows start every `window_step` bytes of the stripped contig (6000: the reference's windows; smaller: overlapping windows of
+// a score profile, each candidate's N count re-reads its 6000 bytes, i.e. ~6000 / step reads per byte; 0: --single-window).
 // kWrite = false: counts[c] = kept windows of contig c (-1 if its byte range is reversed).
 // kWrite = true : offsets = the scanned counts; contig c writes its kept windows to win_start / win_len [offsets[c], offsets[c+1]).
 template <bool kWrite>
 __global__ void __launch_bounds__(kPlanThreads)
-contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets, int single_window,
+contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets, int window_step,
                    int32_t* __restrict__ offsets, int64_t* __restrict__ win_start, int32_t* __restrict__ win_len) {
   __shared__ unsigned long long s_best;
   __shared__ int s_keep[kPlanWarps];
@@ -145,11 +150,12 @@ contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ 
     return;
   }
   const int64_t L = block_find_non_n<true>(seq, first, s1, &s_best) + 1 - first;
-  const int64_t n_cand = candidate_windows(L, single_window);
-  auto wlen = [&](int64_t w) { return static_cast<int32_t>(min(static_cast<int64_t>(kWindow), L - w * kWindow)); };
+  const int64_t step = window_step;
+  const int64_t n_cand = candidate_windows(L, step);
+  auto wlen = [&](int64_t w) { return static_cast<int32_t>(min(static_cast<int64_t>(kWindow), L - w * step)); };
   if (kWrite && n_kept == n_cand) {                    // nothing dropped by the N rule: window k is candidate k
     for (int64_t w = threadIdx.x; w < n_cand; w += blockDim.x) {
-      win_start[base + w] = first + w * kWindow;
+      win_start[base + w] = first + w * step;
       win_len[base + w] = wlen(w);
     }
     return;
@@ -160,7 +166,7 @@ contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ 
     const int64_t w = w0 + warp;
     int keep = 0;
     if (w < n_cand) {
-      const int64_t a = first + w * kWindow;
+      const int64_t a = first + w * step;
       keep = warp_count_N(seq, a, a + wlen(w)) <= kMaxN;
     }
     if (lane == 0) s_keep[warp] = keep;
@@ -169,24 +175,24 @@ contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ 
 #pragma unroll
     for (int i = 0; i < kPlanWarps; ++i) { before += i < warp ? s_keep[i] : 0; total += s_keep[i]; }
     if (kWrite && keep && lane == 0) {
-      win_start[base + kept + before] = first + w * kWindow;
+      win_start[base + kept + before] = first + w * step;
       win_len[base + kept + before] = wlen(w);
     }
     kept += total;
     __syncthreads();                                   // s_keep is rewritten by the next round
   }
-  if (!kWrite && threadIdx.x == 0) offsets[c] = static_cast<int32_t>(kept);
+  if (!kWrite && threadIdx.x == 0) offsets[c] = kept > INT32_MAX ? kCountOverflow : static_cast<int32_t>(kept);
 }
 
 // offsets[0, n) = per-contig window counts -> exclusive prefix sums in place, offsets[n] = the total, or kPlanOverflow if it
-// exceeds INT32_MAX, or kPlanBadOffsets if a count is negative.  One CTA walks the array in rounds of kScanThreads * kScanPer
-// counts with a 64-bit carry.
+// (or one contig's count, kCountOverflow) exceeds INT32_MAX, or kPlanBadOffsets if a count is otherwise negative.  One CTA
+// walks the array in rounds of kScanThreads * kScanPer counts with a 64-bit carry.
 __global__ void __launch_bounds__(kScanThreads) contig_scan_kernel(int32_t* __restrict__ offsets, int n) {
   __shared__ long long s_warp[kScanThreads / 32];
   __shared__ long long s_carry;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   long long carry = 0;
-  int bad = 0;
+  int bad = 0, over = 0;
   for (long long r0 = 0; r0 < n; r0 += static_cast<long long>(kScanThreads) * kScanPer) {
     const long long i0 = r0 + static_cast<long long>(threadIdx.x) * kScanPer;
     int v[kScanPer];
@@ -194,7 +200,8 @@ __global__ void __launch_bounds__(kScanThreads) contig_scan_kernel(int32_t* __re
 #pragma unroll
     for (int k = 0; k < kScanPer; ++k) {
       v[k] = i0 + k < n ? offsets[i0 + k] : 0;
-      if (v[k] < 0) { bad = 1; v[k] = 0; }
+      if (v[k] == kCountOverflow) { over = 1; v[k] = 0; }
+      else if (v[k] < 0) { bad = 1; v[k] = 0; }
       t += v[k];
     }
     long long incl = t;                                // inclusive scan of the per-thread sums within the warp
@@ -226,7 +233,9 @@ __global__ void __launch_bounds__(kScanThreads) contig_scan_kernel(int32_t* __re
     carry = s_carry;
   }
   bad = __syncthreads_or(bad);
-  if (threadIdx.x == 0) offsets[n] = bad ? kPlanBadOffsets : carry > 0x7fffffffLL ? kPlanOverflow : static_cast<int32_t>(carry);
+  over = __syncthreads_or(over);
+  if (threadIdx.x == 0)
+    offsets[n] = bad ? kPlanBadOffsets : over || carry > 0x7fffffffLL ? kPlanOverflow : static_cast<int32_t>(carry);
 }
 
 // One CTA per window: stage the window's bytes (any start address) in shared memory with aligned 16-byte loads, then write

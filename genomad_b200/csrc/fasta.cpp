@@ -27,6 +27,12 @@
 //     caller memory (a pinned chunk): binary search for the record, file offset of the window start by arithmetic,
 //     line-by-line copy, upper-case, pad.  Under torchrun every rank builds the same index (cheap, deterministic,
 //     no communication) and extracts only its own contiguous block of windows.
+//   * a window list (gnm_fasta_windows) is one enumeration over the index: candidate k of a record starts k * step nt into
+//     its stripped sequence and is min(6000, L - k * step) long; the first is always kept, every other one if it has >= 2500 nt
+//     and <= 4000 'N'.  The index pass builds the reference's list (step 6000, --single-window or not); gnm_fasta_windows_plan
+//     builds a list at any step in [1, 6000] (overlapping windows of a score profile) over the same index.  A list keeps
+//     ~16 bytes per record, 8 bytes per candidate window only for records whose lines are irregular and 4 bytes per window
+//     only for records that lost a window to the N rule: at most 12 bytes per window, 12 MB for a 1 Gbp input at step 1000.
 #include <fcntl.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
@@ -64,8 +70,6 @@ struct Record {
   int64_t seq_len;                 // length after stripping both ends (0 => record dropped)
   int64_t line_len, stride;        // regular layout: every line but the last holds line_len nucleotides and starts
                                    // stride bytes after the previous one; stride == 0 => irregular (see win_off)
-  int64_t n_windows, first_window; // kept windows, index of the first one in the global list
-  int32_t off_idx, kept_idx;       // index into gnm_fasta::win_off / ::kept_wins, or -1
   uint8_t has_cr;                  // body contains '\r' (byte-wise line walking)
 };
 
@@ -88,7 +92,45 @@ inline int64_t count_N(const uint8_t* p, int64_t n) {
   return c;
 }
 
+// Calls fn(line_start, line_end) for every line of the record's body (terminators excluded; "\r\n" is one terminator).
+template <class F>
+void walk_lines(const uint8_t* t, const Record& R, F&& fn) {
+  const int64_t b0 = R.body_begin, b1 = R.body_end;
+  int64_t i = b0;
+  if (!R.has_cr) {
+    while (i < b1) {
+      const void* q = std::memchr(t + i, '\n', static_cast<size_t>(b1 - i));
+      const int64_t j = q ? static_cast<const uint8_t*>(q) - t : b1;
+      fn(i, j);
+      i = j + 1;
+    }
+  } else {
+    while (i < b1) {
+      int64_t j = i;
+      while (j < b1 && !is_eol(t[j])) ++j;
+      fn(i, j);
+      if (j < b1 && t[j] == '\r' && j + 1 < b1 && t[j + 1] == '\n') ++j;      // "\r\n" is one terminator
+      i = j + 1;
+    }
+  }
+}
+
 }  // namespace
+
+// One window list over the index (see the top of the file).  Kept records are numbered in file order.
+struct gnm_fasta_windows {
+  const gnm_fasta* f = nullptr;
+  int64_t step = kWin;
+  int single_window = 0;
+  int64_t n_windows = 0;
+  std::vector<int64_t> first;                   // per kept record: its first window in the list (sorted: window -> record)
+  std::vector<int32_t> off_idx, kept_idx;       // per kept record: index into win_off / kept_wins, or -1
+  std::vector<std::vector<int64_t>> win_off;    // irregular records: file offset of the start of every candidate window
+  std::vector<std::vector<int32_t>> kept_wins;  // records that lost windows to the N rule: candidate numbers kept
+  // bytes of the mapping this list's stream has handed back (madvise): each list streams the file from its start, so each
+  // keeps its own mark (a second pass re-faults the pages a first pass released, and must release them again)
+  mutable std::atomic<int64_t> released{0};
+};
 
 struct gnm_fasta {
   const uint8_t* text = nullptr;
@@ -99,13 +141,9 @@ struct gnm_fasta {
   std::unique_ptr<uint8_t[]> owned;   // inflated text of a gzip input (gnm_fasta_open_gz)
   std::vector<Record> recs;        // every record found (before dropping empties)
   std::vector<int64_t> kept;       // indices of records whose stripped sequence is non-empty
-  std::vector<int64_t> kept_first; // first_window of every kept record (sorted; binary search window -> record)
-  std::vector<std::vector<int64_t>> win_off;    // irregular records: file offset of the start of every candidate window
-  std::vector<std::vector<int32_t>> kept_wins;  // records that lost windows to the N rule: candidate numbers kept
-  int64_t n_windows = 0;
+  gnm_fasta_windows windows;       // the reference's window list (step 6000, single_window)
   int64_t n_nonempty_raw = 0;      // records with a non-empty sequence before stripping (what check_fasta counts)
   int has_dup = 0;
-  mutable std::atomic<int64_t> released{0};      // bytes of the mapping already handed back (madvise)
 };
 
 static thread_local std::string g_fasta_err;
@@ -114,16 +152,16 @@ extern "C" const char* gnm_fasta_last_error(void) { return g_fasta_err.c_str(); 
 // ------------------------------------------------------------------------------------------------ index pass
 // One record: walk its lines once.  Everything the reference derives from the joined, stripped string is derived here
 // from the line structure without building that string.
-static void index_record(gnm_fasta* f, Record& R, std::vector<int64_t>* offs, std::vector<int32_t>* keptw) {
+static void index_record(gnm_fasta* f, Record& R) {
   const uint8_t* t = f->text;
   const int64_t b0 = R.body_begin, b1 = R.body_end;
   R.has_cr = std::memchr(t + b0, '\r', static_cast<size_t>(b1 - b0)) != nullptr;
-  // ---- pass A over the lines: raw length, regularity, leading strip
+  // ---- one pass over the lines: raw length, regularity, leading strip
   int64_t raw = 0, lead = 0;
   bool in_lead = true, regular = true;
   int64_t line_len = -1, stride = 0, nlines = 0, prev_start = -1, prev_len = -1;
   int64_t last_nonstrip_raw = -1;          // raw index of the last byte that is not n/N
-  auto visit = [&](int64_t ls, int64_t le) {   // one line [ls, le), possibly empty
+  walk_lines(t, R, [&](int64_t ls, int64_t le) {   // one line [ls, le), possibly empty
     const int64_t n = le - ls;
     if (nlines == 0) { line_len = n; }
     else {
@@ -141,27 +179,7 @@ static void index_record(gnm_fasta* f, Record& R, std::vector<int64_t>* offs, st
       if (t[ls + k] != 'n' && t[ls + k] != 'N') { last_nonstrip_raw = raw + k; break; }
     raw += n;
     prev_start = ls; prev_len = n; ++nlines;
-  };
-  auto walk = [&](auto&& fn) {
-    int64_t i = b0;
-    if (!R.has_cr) {
-      while (i < b1) {
-        const void* q = std::memchr(t + i, '\n', static_cast<size_t>(b1 - i));
-        const int64_t j = q ? static_cast<const uint8_t*>(q) - t : b1;
-        fn(i, j);
-        i = j + 1;
-      }
-    } else {
-      while (i < b1) {
-        int64_t j = i;
-        while (j < b1 && !is_eol(t[j])) ++j;
-        fn(i, j);
-        if (j < b1 && t[j] == '\r' && j + 1 < b1 && t[j + 1] == '\n') ++j;      // "\r\n" is one terminator
-        i = j + 1;
-      }
-    }
-  };
-  walk(visit);
+  });
   R.raw_len = raw;
   if (last_nonstrip_raw < 0) { R.lead = raw; R.seq_len = 0; }       // nothing but n/N (or empty)
   else { R.lead = lead; R.seq_len = last_nonstrip_raw + 1 - lead; }
@@ -169,46 +187,105 @@ static void index_record(gnm_fasta* f, Record& R, std::vector<int64_t>* offs, st
   if (regular && stride < line_len) regular = false;
   R.line_len = regular ? line_len : 0;
   R.stride = regular ? stride : 0;
-  R.n_windows = 0; R.off_idx = R.kept_idx = -1;
-  if (R.seq_len == 0) return;
-  // ---- candidate windows (sequence.py:150-167)
-  int64_t ncand = 0;
-  for (int64_t w = 0; w * kWin < R.seq_len; ++w) {
-    const int64_t n = std::min(kWin, R.seq_len - w * kWin);
-    if (n < kMinTail) { if (w == 0) ncand = 1; break; }
-    ncand = w + 1;
-    if (f->single_window) break;
-  }
-  // ---- pass B (only when needed): N counts of windows 1.. and window start offsets of irregular records
+}
+
+// Candidate windows of a stripped record of L > 0 nt at window step `step`: 1 + max(0, (L - 2500) / step); at step 6000 this
+// is seq_windows(6000, 2500) (sequence.py:150-167).
+static inline int64_t candidate_windows(int64_t L, int64_t step, int single_window) {
+  return single_window ? 1 : 1 + (L > kMinTail ? (L - kMinTail) / step : 0);
+}
+
+// One kept record's windows in list p: returns how many are kept; fills *offs (irregular records: file offset of every
+// candidate's first byte) and *keptw (only if the N rule dropped one: the candidate numbers kept).  The N count of candidate w
+// is the running count of 'N' at its end minus the one at its start; both are taken in one walk over the lines, so
+// overlapping windows cost no re-reading.  Only the windows open at one position (<= 6000 / step + 1) keep their start count,
+// in a ring, so the walk needs no memory per candidate; a window is kept or dropped as soon as its end is reached.
+static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, int single_window, std::vector<int64_t>* offs,
+                           std::vector<int32_t>* keptw) {
+  const int64_t L = R.seq_len;
+  if (L == 0) return 0;
+  const int64_t ncand = candidate_windows(L, step, single_window);
+  if (ncand == 1 && R.stride != 0) return 1;   // one window (exempt from the N rule) of a regular record: nothing to walk
+  auto wend = [&](int64_t w) { return std::min(L, w * step + kWin); };     // end of candidate w, in the stripped sequence
   const bool need_n = ncand > 1;            // the first window is exempt from the N rule
-  const bool need_off = !regular;
-  std::vector<int64_t> ncount;
-  if (need_n) ncount.assign(static_cast<size_t>(ncand), 0);
+  const bool need_off = R.stride == 0;
+  // ring of the running 'N' count at the start of the open windows: window w - ring has ended before window w starts
+  // (ring * step > 6000 >= any window's length)
+  const int64_t ring = kWin / step + 2;
+  std::vector<int64_t> n_start(need_n ? static_cast<size_t>(std::min(ring, ncand)) : 0);
   if (need_off) offs->assign(static_cast<size_t>(ncand), -1);
-  if (need_n || need_off) {
-    int64_t pos = 0;                        // raw index of the first byte of the current line
-    const int64_t s0 = R.lead, s1 = R.lead + std::min(R.seq_len, ncand * kWin);
-    walk([&](int64_t ls, int64_t le) {
-      const int64_t n = le - ls;
-      int64_t a = std::max(pos, s0), e = std::min(pos + n, s1);            // part of this line inside the windows
-      while (a < e) {
-        const int64_t w = (a - s0) / kWin;
-        const int64_t wend = std::min(e, s0 + (w + 1) * kWin);
-        if (need_off && (a - s0) % kWin == 0) (*offs)[static_cast<size_t>(w)] = ls + (a - pos);
-        if (need_n && w > 0) ncount[static_cast<size_t>(w)] += count_N(t + ls + (a - pos), wend - a);
-        a = wend;
-      }
-      pos += n;
-    });
-  }
-  int64_t nkept = 0;
+  int64_t nkept = 1;                        // window 0 is always kept
   bool dropped = false;
-  for (int64_t w = 0; w < ncand; ++w) {
-    const bool keep = w == 0 || ncount[static_cast<size_t>(w)] <= kMaxN;
-    if (keep) { keptw->push_back(static_cast<int32_t>(w)); ++nkept; } else dropped = true;
+  auto decide = [&](int64_t w, int64_t n_count) {      // windows 1.. in order
+    if (n_count <= kMaxN) {
+      if (dropped) keptw->push_back(static_cast<int32_t>(w));
+      ++nkept;
+    } else if (!dropped) {                   // first drop: the kept candidates so far are 0 .. w-1
+      dropped = true;
+      keptw->resize(static_cast<size_t>(w));
+      for (int64_t k = 0; k < w; ++k) (*keptw)[static_cast<size_t>(k)] = static_cast<int32_t>(k);
+    }
+  };
+  const uint8_t* t = f->text;
+  const int64_t s0 = R.lead, s1 = R.lead + wend(ncand - 1);
+  int64_t pos = 0, cnt = 0, ws = 0, we = 0;   // raw index of the line's first byte; running 'N' count; next start / end event
+  walk_lines(t, R, [&](int64_t ls, int64_t le) {
+    const int64_t n = le - ls;
+    int64_t a = std::max(pos, s0) - s0;
+    const int64_t e = std::min(pos + n, s1) - s0;    // part of this line inside the windows, in the stripped sequence
+    const int64_t base = ls + s0 - pos;              // file offset of stripped position 0 on this line's terms
+    if (a < e) {
+      for (;;) {                                     // window starts in [a, e) and ends in (a, e], in order
+        const int64_t qs = ws < ncand ? ws * step : INT64_MAX;
+        const int64_t qe = need_n && we < ncand ? wend(we) : INT64_MAX;
+        const bool is_start = qs < e && qs <= qe;
+        if (!is_start && qe > e) break;
+        const int64_t q = is_start ? qs : qe;
+        if (need_n) cnt += count_N(t + base + a, q - a);
+        a = q;
+        if (is_start) {
+          if (need_n) n_start[static_cast<size_t>(ws % ring)] = cnt;
+          if (need_off) (*offs)[static_cast<size_t>(ws)] = base + q;
+          ++ws;
+        } else {
+          if (we > 0) decide(we, cnt - n_start[static_cast<size_t>(we % ring)]);
+          ++we;
+        }
+      }
+      if (need_n) cnt += count_N(t + base + a, e - a);
+    }
+    pos += n;
+  });
+  return nkept;
+}
+
+// Windows of a stripped record of L nt at `step`, before the N rule (closed form): what a list can hold at most.
+static int64_t candidate_total(const gnm_fasta* f, int64_t step, int single_window) {
+  int64_t total = 0;
+  for (int64_t r : f->kept) total += candidate_windows(f->recs[static_cast<size_t>(r)].seq_len, step, single_window);
+  return total;
+}
+
+// The window list of every kept record at p->step, records in parallel.
+static void build_windows(const gnm_fasta* f, gnm_fasta_windows* p, int threads) {
+  const size_t nk = f->kept.size();
+  std::vector<std::vector<int64_t>> offs(nk);
+  std::vector<std::vector<int32_t>> keptw(nk);
+  std::vector<int64_t> nw(nk);
+  parallel_for(static_cast<int64_t>(nk), threads, [&](int64_t i) {
+    nw[i] = plan_record(f, f->recs[static_cast<size_t>(f->kept[i])], p->step, p->single_window, &offs[i], &keptw[i]);
+  });
+  p->f = f;
+  p->n_windows = 0;
+  p->first.resize(nk);
+  p->off_idx.assign(nk, -1);
+  p->kept_idx.assign(nk, -1);
+  for (size_t i = 0; i < nk; ++i) {
+    p->first[i] = p->n_windows;
+    p->n_windows += nw[i];
+    if (!offs[i].empty()) { p->off_idx[i] = static_cast<int32_t>(p->win_off.size()); p->win_off.push_back(std::move(offs[i])); }
+    if (!keptw[i].empty()) { p->kept_idx[i] = static_cast<int32_t>(p->kept_wins.size()); p->kept_wins.push_back(std::move(keptw[i])); }
   }
-  if (!dropped) keptw->clear();             // implicit: candidate k is window k
-  R.n_windows = nkept;
 }
 
 static int build_index(gnm_fasta* f, int threads) {
@@ -246,10 +323,8 @@ static int build_index(gnm_fasta* f, int threads) {
   }
   // ---- records in parallel
   const size_t nrec = f->recs.size();
-  std::vector<std::vector<int64_t>> offs(nrec);
-  std::vector<std::vector<int32_t>> keptw(nrec);
-  parallel_for(static_cast<int64_t>(nrec), threads, [&](int64_t r) { index_record(f, f->recs[r], &offs[r], &keptw[r]); });
-  // ---- bookkeeping: kept records, window offsets, duplicate identifiers (first whitespace-delimited token)
+  parallel_for(static_cast<int64_t>(nrec), threads, [&](int64_t r) { index_record(f, f->recs[r]); });
+  // ---- bookkeeping: kept records, duplicate identifiers (first whitespace-delimited token)
   std::unordered_set<std::string> ids;
   ids.reserve(nrec * 2);
   for (size_t r = 0; r < nrec; ++r) {
@@ -263,15 +338,11 @@ static int build_index(gnm_fasta* f, int threads) {
       while (b < e && !ws(text[b])) ++b;
       if (!ids.emplace(reinterpret_cast<const char*>(text + a), static_cast<size_t>(b - a)).second) f->has_dup = 1;
     }
-    if (R.seq_len > 0) {
-      R.first_window = f->n_windows;
-      f->n_windows += R.n_windows;
-      if (!offs[r].empty()) { R.off_idx = static_cast<int32_t>(f->win_off.size()); f->win_off.push_back(std::move(offs[r])); }
-      if (!keptw[r].empty()) { R.kept_idx = static_cast<int32_t>(f->kept_wins.size()); f->kept_wins.push_back(std::move(keptw[r])); }
-      f->kept.push_back(static_cast<int64_t>(r));
-      f->kept_first.push_back(R.first_window);
-    }
+    if (R.seq_len > 0) f->kept.push_back(static_cast<int64_t>(r));
   }
+  // ---- the reference's window list
+  f->windows.single_window = f->single_window;
+  build_windows(f, &f->windows, threads);
   return 0;
 }
 
@@ -429,7 +500,7 @@ extern "C" int gnm_fasta_info(const gnm_fasta* f, int64_t* n_records_nonempty, i
   if (n_records_nonempty) *n_records_nonempty = f->n_nonempty_raw;
   if (has_duplicate_ids) *has_duplicate_ids = f->has_dup;
   if (n_contigs) *n_contigs = static_cast<int64_t>(f->kept.size());
-  if (n_windows) *n_windows = f->n_windows;
+  if (n_windows) *n_windows = f->windows.n_windows;
   if (header_bytes) {
     int64_t b = 0;
     for (int64_t r : f->kept) b += f->recs[r].hdr_end - f->recs[r].hdr_begin + 1;
@@ -444,17 +515,18 @@ static inline int64_t regular_offset(const Record& R, int64_t a) {
   return R.body_begin + (a / R.line_len) * R.stride + a % R.line_len;
 }
 
-// global window index -> dst[6000]
-static void extract_window(const gnm_fasta* f, int64_t wdx, uint8_t* dst) {
-  const size_t ki = static_cast<size_t>(std::upper_bound(f->kept_first.begin(), f->kept_first.end(), wdx) - f->kept_first.begin()) - 1;
+// window wdx of list p -> dst[6000]
+static void extract_window(const gnm_fasta_windows* p, int64_t wdx, uint8_t* dst) {
+  const gnm_fasta* f = p->f;
+  const size_t ki = static_cast<size_t>(std::upper_bound(p->first.begin(), p->first.end(), wdx) - p->first.begin()) - 1;
   const Record& R = f->recs[static_cast<size_t>(f->kept[ki])];
-  int64_t cand = wdx - R.first_window;
-  if (R.kept_idx >= 0) cand = f->kept_wins[static_cast<size_t>(R.kept_idx)][static_cast<size_t>(cand)];
-  const int64_t n = std::min(kWin, R.seq_len - cand * kWin);
+  int64_t cand = wdx - p->first[ki];
+  if (p->kept_idx[ki] >= 0) cand = p->kept_wins[static_cast<size_t>(p->kept_idx[ki])][static_cast<size_t>(cand)];
+  const int64_t n = std::min(kWin, R.seq_len - cand * p->step);
   const uint8_t* t = f->text;
   int64_t got = 0;
   if (R.stride > 0) {
-    const int64_t a = R.lead + cand * kWin;
+    const int64_t a = R.lead + cand * p->step;
     int64_t off = regular_offset(R, a), in_line = R.line_len - a % R.line_len;
     while (got < n) {
       const int64_t c = std::min(n - got, in_line);
@@ -462,7 +534,7 @@ static void extract_window(const gnm_fasta* f, int64_t wdx, uint8_t* dst) {
       got += c; off += c + (R.stride - R.line_len); in_line = R.line_len;
     }
   } else {
-    int64_t i = f->win_off[static_cast<size_t>(R.off_idx)][static_cast<size_t>(cand)];
+    int64_t i = p->win_off[static_cast<size_t>(p->off_idx[ki])][static_cast<size_t>(cand)];
     while (got < n && i < R.body_end) {
       int64_t j = i;
       if (!R.has_cr) {
@@ -484,13 +556,44 @@ static void extract_window(const gnm_fasta* f, int64_t wdx, uint8_t* dst) {
   if (n < kWin) std::memset(dst + n, 'N', static_cast<size_t>(kWin - n));
 }
 
+static int export_windows(const gnm_fasta_windows* p, int64_t first, int64_t count, uint8_t* dst, int threads,
+                          const char* fn) {
+  if (first < 0 || count < 0 || first + count > p->n_windows) { g_fasta_err = std::string(fn) + ": range out of bounds"; return 1; }
+  constexpr int64_t kBlock = 32;                            // windows per work item
+  parallel_for((count + kBlock - 1) / kBlock, threads, [&](int64_t b) {
+    const int64_t lo = first + b * kBlock, hi = std::min(first + count, lo + kBlock);
+    for (int64_t wdx = lo; wdx < hi; ++wdx) extract_window(p, wdx, dst + (wdx - first) * kWin);
+  });
+  return 0;
+}
+
+static int release_before(const gnm_fasta_windows* p, int64_t upto) {
+  const gnm_fasta* f = p->f;
+  if (!f->map_base || f->kept.empty()) return 0;
+  int64_t byte_end;
+  if (upto >= p->n_windows) byte_end = f->len;
+  else if (upto <= 0) return 0;
+  else {
+    const size_t ki = static_cast<size_t>(std::upper_bound(p->first.begin(), p->first.end(), upto) - p->first.begin()) - 1;
+    byte_end = f->recs[static_cast<size_t>(f->kept[ki])].hdr_begin - 1;      // start of the record that holds window `upto`
+  }
+  const int64_t page = 4096;
+  const int64_t aligned = byte_end / page * page;
+  int64_t done = p->released.load();
+  if (aligned > done) {
+    ::madvise(static_cast<uint8_t*>(f->map_base) + done, static_cast<size_t>(aligned - done), MADV_DONTNEED);
+    p->released.store(aligned);
+  }
+  return 0;
+}
+
 extern "C" int gnm_fasta_export(const gnm_fasta* f, uint8_t* windows, int32_t* offsets, char* headers, int threads) {
   if (!f) { g_fasta_err = "gnm_fasta_export: null handle"; return 1; }
-  if (f->n_windows > INT32_MAX) { g_fasta_err = "gnm_fasta_export: more than 2^31-1 windows"; return 1; }
+  if (f->windows.n_windows > INT32_MAX) { g_fasta_err = "gnm_fasta_export: more than 2^31-1 windows"; return 1; }
   const int64_t nk = static_cast<int64_t>(f->kept.size());
   if (offsets) {
-    for (int64_t i = 0; i < nk; ++i) offsets[i] = static_cast<int32_t>(f->recs[f->kept[i]].first_window);
-    offsets[nk] = static_cast<int32_t>(f->n_windows);
+    for (int64_t i = 0; i < nk; ++i) offsets[i] = static_cast<int32_t>(f->windows.first[static_cast<size_t>(i)]);
+    offsets[nk] = static_cast<int32_t>(f->windows.n_windows);
   }
   if (headers) {
     char* h = headers;
@@ -502,7 +605,7 @@ extern "C" int gnm_fasta_export(const gnm_fasta* f, uint8_t* windows, int32_t* o
       h += n + 1;
     }
   }
-  if (windows) return gnm_fasta_export_windows(f, 0, f->n_windows, windows, threads);
+  if (windows) return gnm_fasta_export_windows(f, 0, f->windows.n_windows, windows, threads);
   return 0;
 }
 
@@ -510,36 +613,86 @@ extern "C" int gnm_fasta_export(const gnm_fasta* f, uint8_t* windows, int32_t* o
 // pinned chunk while the GPU classifies the previous one)
 extern "C" int gnm_fasta_export_windows(const gnm_fasta* f, int64_t first, int64_t count, uint8_t* dst, int threads) {
   if (!f || (!dst && count)) { g_fasta_err = "gnm_fasta_export_windows: null argument"; return 1; }
-  if (first < 0 || count < 0 || first + count > f->n_windows) { g_fasta_err = "gnm_fasta_export_windows: range out of bounds"; return 1; }
-  constexpr int64_t kBlock = 32;                            // windows per work item
-  parallel_for((count + kBlock - 1) / kBlock, threads, [&](int64_t b) {
-    const int64_t lo = first + b * kBlock, hi = std::min(first + count, lo + kBlock);
-    for (int64_t wdx = lo; wdx < hi; ++wdx) extract_window(f, wdx, dst + (wdx - first) * kWin);
-  });
-  return 0;
+  return export_windows(&f->windows, first, count, dst, threads, "gnm_fasta_export_windows");
 }
 
-// Hand the pages of the mapping that lie entirely before global window `upto` back to the kernel (they stay in the page
+// Hand the pages of the mapping that lie entirely before window `upto` back to the kernel (they stay in the page
 // cache; the process' resident set stops growing with the file).  No-op for caller-memory text.
 extern "C" int gnm_fasta_release_before(const gnm_fasta* f, int64_t upto) {
   if (!f) { g_fasta_err = "gnm_fasta_release_before: null handle"; return 1; }
-  if (!f->map_base || f->kept.empty()) return 0;
-  int64_t byte_end;
-  if (upto >= f->n_windows) byte_end = f->len;
-  else if (upto <= 0) return 0;
-  else {
-    const size_t ki = static_cast<size_t>(std::upper_bound(f->kept_first.begin(), f->kept_first.end(), upto) - f->kept_first.begin()) - 1;
-    byte_end = f->recs[static_cast<size_t>(f->kept[ki])].hdr_begin - 1;      // start of the record that holds window `upto`
+  return release_before(&f->windows, upto);
+}
+
+// ------------------------------------------------------------------------------------------------ window lists at any step
+extern "C" int gnm_fasta_windows_plan(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out) {
+  if (!f || !out) { g_fasta_err = "gnm_fasta_windows_plan: null argument"; return 1; }
+  if (stride < 1 || stride > kWin) {
+    g_fasta_err = "gnm_fasta_windows_plan: stride must be in [1, 6000], not " + std::to_string(stride);
+    return 1;
   }
-  const int64_t page = 4096;
-  const int64_t aligned = byte_end / page * page;
-  int64_t done = f->released.load();
-  if (aligned > done) {
-    ::madvise(static_cast<uint8_t*>(f->map_base) + done, static_cast<size_t>(aligned - done), MADV_DONTNEED);
-    f->released.store(aligned);
+  // checked before anything is built: the candidate count has a closed form, and the kept windows are at most that many
+  if (candidate_total(f, stride, single_window) > INT32_MAX) {
+    g_fasta_err = "gnm_fasta_windows_plan: more than 2^31-1 windows (before the N rule)";
+    return 1;
   }
+  std::unique_ptr<gnm_fasta_windows> p(new gnm_fasta_windows());
+  p->step = stride;
+  p->single_window = single_window;
+  build_windows(f, p.get(), std::max(1, threads));
+  *out = p.release();
   return 0;
 }
+
+extern "C" int gnm_fasta_windows_info(const gnm_fasta_windows* p, int64_t* n_contigs, int64_t* n_windows) {
+  if (!p) { g_fasta_err = "gnm_fasta_windows_info: null handle"; return 1; }
+  if (n_contigs) *n_contigs = static_cast<int64_t>(p->first.size());
+  if (n_windows) *n_windows = p->n_windows;
+  return 0;
+}
+
+static void window_spans(const gnm_fasta_windows* p, int32_t* offsets, int64_t* starts, int32_t* lengths) {
+  const size_t nk = p->first.size();
+  if (offsets) {
+    for (size_t i = 0; i < nk; ++i) offsets[i] = static_cast<int32_t>(p->first[i]);
+    offsets[nk] = static_cast<int32_t>(p->n_windows);
+  }
+  if (!starts && !lengths) return;
+  for (size_t i = 0; i < nk; ++i) {
+    const Record& R = p->f->recs[static_cast<size_t>(p->f->kept[i])];
+    const int64_t w0 = p->first[i], w1 = i + 1 < nk ? p->first[i + 1] : p->n_windows;
+    const std::vector<int32_t>* kw = p->kept_idx[i] >= 0 ? &p->kept_wins[static_cast<size_t>(p->kept_idx[i])] : nullptr;
+    for (int64_t w = w0; w < w1; ++w) {
+      const int64_t cand = kw ? (*kw)[static_cast<size_t>(w - w0)] : w - w0;
+      if (starts) starts[w] = R.lead + cand * p->step;
+      if (lengths) lengths[w] = static_cast<int32_t>(std::min(kWin, R.seq_len - cand * p->step));
+    }
+  }
+}
+
+extern "C" int gnm_fasta_windows_spans(const gnm_fasta_windows* p, int32_t* offsets, int64_t* starts, int32_t* lengths) {
+  if (!p) { g_fasta_err = "gnm_fasta_windows_spans: null handle"; return 1; }
+  if (p->n_windows > INT32_MAX) { g_fasta_err = "gnm_fasta_windows_spans: more than 2^31-1 windows"; return 1; }
+  window_spans(p, offsets, starts, lengths);
+  return 0;
+}
+
+extern "C" int gnm_fasta_spans(const gnm_fasta* f, int64_t* starts, int32_t* lengths) {
+  if (!f) { g_fasta_err = "gnm_fasta_spans: null handle"; return 1; }
+  window_spans(&f->windows, nullptr, starts, lengths);
+  return 0;
+}
+
+extern "C" int gnm_fasta_windows_export(const gnm_fasta_windows* p, int64_t first, int64_t count, uint8_t* dst, int threads) {
+  if (!p || (!dst && count)) { g_fasta_err = "gnm_fasta_windows_export: null argument"; return 1; }
+  return export_windows(p, first, count, dst, threads, "gnm_fasta_windows_export");
+}
+
+extern "C" int gnm_fasta_windows_release_before(const gnm_fasta_windows* p, int64_t upto) {
+  if (!p) { g_fasta_err = "gnm_fasta_windows_release_before: null handle"; return 1; }
+  return release_before(p, upto);
+}
+
+extern "C" void gnm_fasta_windows_free(gnm_fasta_windows* p) { delete p; }
 
 extern "C" void gnm_fasta_free(gnm_fasta* f) {
   if (!f) return;

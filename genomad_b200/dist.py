@@ -108,6 +108,29 @@ def gather_window_probs(local_probs, n_total: int, world_size: int, group=None):
     return torch.cat(parts, dim=0)
 
 
+def collect_window_probs(local_probs, n_total: int, info: "DistInfo", send=None, recv=None):
+    """Contiguous shards [W_local, 3] -> [n_total, 3] in global window order on rank 0 (None on the other ranks): each rank
+    sends its shard to rank 0, which receives them in rank order.  Only rank 0 ever holds every window (a score profile can
+    have far more windows than the contig pass)."""
+    import torch
+    if info.world_size == 1:
+        return local_probs
+    send = send or (lambda t, dst: _p2p_send(t, dst))
+    recv = recv or (lambda t, src: _p2p_recv(t, src))
+    if not info.is_main:
+        if local_probs.shape[0]:
+            send(local_probs.contiguous(), 0)
+        return None
+    parts = [local_probs]
+    for r in range(1, info.world_size):
+        s, e = shard_bounds(n_total, info.world_size, r)
+        if e > s:
+            buf = torch.empty((e - s, local_probs.shape[1]), dtype=local_probs.dtype, device=local_probs.device)
+            recv(buf, r)
+            parts.append(buf)
+    return torch.cat(parts, dim=0)
+
+
 def allreduce_partials(partials, world_size: int, group=None):
     """[n_contigs, 4] per-rank (sum p0, sum p1, sum p2, count) -> global; then mean = sums / count."""
     import torch.distributed as dist

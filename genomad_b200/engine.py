@@ -12,7 +12,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 from pathlib import Path
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 
@@ -66,6 +66,8 @@ EXPORTS = {
     "gnm_check_status": (C.c_int, [C.c_void_p, C.c_void_p]),
     "gnm_contig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64,
                                      C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "gnm_contig_windows_stride": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                            C.c_int64, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "gnm_gather_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_forward_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_embed_tokens": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -90,6 +92,17 @@ EXPORTS = {
     "gnm_fasta_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "gnm_fasta_export_windows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int]),
     "gnm_fasta_free": (None, [C.c_void_p]),
+    "gnm_fasta_windows_plan": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "gnm_fasta_windows_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "gnm_fasta_windows_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_fasta_windows_export": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int]),
+    "gnm_fasta_windows_release_before": (C.c_int, [C.c_void_p, C.c_int64]),
+    "gnm_fasta_windows_free": (None, [C.c_void_p]),
+    "gnm_fasta_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_tsv_last_error": (C.c_char_p, []),
+    "gnm_write_window_tsv": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_int]),
+    "gnm_format_scores": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_int64)]),
     "gnm_tfrecord_last_error": (C.c_char_p, []),
     "gnm_tfrecord_write": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.c_int]),
     "gnm_tfrecord_read": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]),
@@ -123,6 +136,15 @@ def _check(lib, rc: int):
 
 def _ptr(a: np.ndarray) -> int:
     return a.ctypes.data
+
+
+class WindowScores(NamedTuple):
+    """Result of Classifier.window_scores (cuda tensors)."""
+    probs: "object"           # float32 [W, 3] (chromosome, plasmid, virus)
+    contig: "object"          # int32 [W], index of the window's contig
+    start: "object"           # int64 [W], first byte in the contig (0-based, before stripping n/N)
+    length: "object"          # int32 [W], bytes of sequence (1..6000; the rest of the window is 'N' padding)
+    offsets: "object"         # int32 [n_contigs + 1], CSR: the windows of contig c are [offsets[c], offsets[c+1])
 
 
 class Classifier:
@@ -319,22 +341,34 @@ class Classifier:
             seq = t.zeros(16, dtype=t.uint8, device=dev)          # all contigs empty: the library still wants a buffer
         return seq.contiguous(), offs.contiguous()
 
-    def contig_windows(self, seq_u8, seq_offsets_i64, single_window: bool = False):
-        """Plan the windows of contigs on the device (gnm_contig_windows): uint8 cuda [total_bytes] + int64 cuda offsets
-        [n_contigs + 1] -> (win_start int64 [W] absolute byte offsets, win_len int32 [W], win_offsets int32 [n_contigs + 1])."""
+    def contig_windows(self, seq_u8, seq_offsets_i64, single_window: bool = False, stride: int = WINDOW):
+        """Plan the windows of contigs on the device: uint8 cuda [total_bytes] + int64 cuda offsets [n_contigs + 1] ->
+        (win_start int64 [W] absolute byte offsets, win_len int32 [W], win_offsets int32 [n_contigs + 1]).
+        stride 6000: the reference's windows (gnm_contig_windows); any other stride in [1, 6000]: a window every `stride` nt of
+        the whole contig (gnm_contig_windows_stride; not with single_window)."""
         t = self._torch
         assert seq_u8.dtype == t.uint8 and seq_offsets_i64.dtype == t.int64 and seq_u8.is_cuda and seq_offsets_i64.is_cuda
+        stride = int(stride)
+        if not 1 <= stride <= WINDOW:
+            raise ValueError(f"stride must be in [1, {WINDOW}], not {stride}")
+        if single_window and stride != WINDOW:
+            raise ValueError("single_window plans the reference's windows only (stride 6000)")
         seq, offs = seq_u8.contiguous(), seq_offsets_i64.contiguous()
         n = offs.numel() - 1
         assert n >= 0
-        cap = n + seq.numel() // WINDOW                                   # always enough (gnm.h)
+        cap = n + seq.numel() // stride                                   # always enough (gnm.h)
         start = t.empty(cap, dtype=t.int64, device=seq.device)
         length = t.empty(cap, dtype=t.int32, device=seq.device)
         woff = t.empty(n + 1, dtype=t.int32, device=seq.device)
         nw = C.c_int64()
-        _check(self.lib, self.lib.gnm_contig_windows(self._h, seq.data_ptr(), offs.data_ptr(), n, int(bool(single_window)),
-                                                     start.data_ptr(), length.data_ptr(), cap, woff.data_ptr(), C.byref(nw),
-                                                     self._stream()))
+        if stride == WINDOW:
+            rc = self.lib.gnm_contig_windows(self._h, seq.data_ptr(), offs.data_ptr(), n, int(bool(single_window)),
+                                             start.data_ptr(), length.data_ptr(), cap, woff.data_ptr(), C.byref(nw),
+                                             self._stream())
+        else:
+            rc = self.lib.gnm_contig_windows_stride(self._h, seq.data_ptr(), offs.data_ptr(), n, stride, start.data_ptr(),
+                                                    length.data_ptr(), cap, woff.data_ptr(), C.byref(nw), self._stream())
+        _check(self.lib, rc)
         return start[:nw.value], length[:nw.value], woff
 
     def gather_windows(self, seq_u8, win_start, win_len):
@@ -385,6 +419,26 @@ class Classifier:
             sums, _ = self.segment_sum_rows(emb, woff)
             out = out + (sums / counts.clamp(min=1).to(t.float32)[:, None],)
         return out
+
+    def window_scores(self, seqs, stride: int = WINDOW) -> "WindowScores":
+        """Class scores of every window of every contig, with the window's place in its contig: the per-window probabilities
+        the reference averages away (nn_classification.py:316-320), and at stride < 6000 a window every `stride` nt
+        (overlapping windows, each classified by the unchanged model) for a finer profile along the contig.
+
+        seqs: as for classify_contigs.  Returns cuda tensors WindowScores(probs float32 [W, 3], contig int32 [W],
+        start int64 [W] (0-based, in the contig's bytes as given, i.e. before stripping n/N), length int32 [W] (bytes of
+        sequence, padding excluded), offsets int32 [n_contigs + 1] (CSR: the windows of contig c)).  At stride 6000 these are
+        the windows, and bitwise the probabilities, of classify_contigs(..., return_window_probs=True)."""
+        t = self._torch
+        seq, offs = self.contig_buffers(seqs)
+        start, length, woff = self.contig_windows(seq, offs, stride=stride)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        probs = (self.predict_windows(seq, start, length) if start.numel()
+                 else t.zeros((0, 3), dtype=t.float32, device=seq.device))
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        return WindowScores(probs, contig, rel, length, woff)
 
     # ------------------------------------------------------------------ host-buffer API
     def classify_host(self, ascii_windows: np.ndarray) -> np.ndarray:

@@ -79,10 +79,24 @@ def _pinned_chunk(n: int):
     return t, t.numpy()
 
 
-def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, contig_reduce: str = "gather",
-                     embeddings: bool = False):
+def _pinned_probs(n: int):
+    """float32 [n, 3] in page-locked host memory: where gnm_classify_host writes a rank's per-window probabilities."""
+    import torch
+    return torch.empty((n, 3), dtype=torch.float32).pin_memory()
+
+
+def _device(clf):
+    import torch
+    return torch.device("cuda", clf.device)
+
+
+def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather",
+                     embeddings: bool = False, window_probs: bool = False):
     """
     Indexed FASTA -> float32 [n_contigs, 3] per-contig mean (identical on all ranks).
+
+    `parsed` is the window source: a ParsedFasta (the reference's windows) or a sequence.WindowList (windows at another
+    stride); all the loop needs is n_windows, export_windows and release_before.
 
     This rank's contiguous block of the global window list is streamed in chunks: the native reader fills one pinned
     chunk straight from the mmap'ed file (upper-case + pad, multi-threaded) while the GPU classifies the previous one
@@ -93,6 +107,9 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
     window in a device chunk buffer), is summed per contig right away (segment_sum_rows, carried from chunk to chunk) and
     the per-contig means are combined over the ranks by the carry chain of genomad_b200.dist; returns (means, embeddings),
     the embeddings float32 [n_contigs, 512] on rank 0 and None on the other ranks.
+
+    With `window_probs`, the per-window probabilities float32 [n_windows, 3] are collected on rank 0 (None on the other
+    ranks) and returned last.  With offsets None there is no per-contig reduction: only those are returned.
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -100,8 +117,8 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
     start, end = gdist.shard_bounds(n, info.world_size, info.rank)
     chunk = max(4 * clf.max_batch, 4096)
     keep, bufs = zip(*(_pinned_chunk(min(chunk, max(1, end - start))) for _ in range(2)))
-    out_t = torch.empty((max(1, end - start), 3), dtype=torch.float32).pin_memory()
-    dev = torch.device("cuda", clf.device)
+    out_t = _pinned_probs(max(1, end - start))
+    dev = _device(clf)
     run = clf.classify_host_into
     if embeddings:
         shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
@@ -124,12 +141,17 @@ def _classify_parsed(clf, parsed, offsets: np.ndarray, info: gdist.DistInfo, con
             f.result()
     del keep
     local_t = out_t[: end - start].to(dev, non_blocking=True)
-    if embeddings:
-        preds = _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
-        lo, means = shard.finish(info)
-        emb = gdist.gather_contig_means(lo, means, len(offsets) - 1, info)
-        return preds, (emb.cpu().numpy() if emb is not None else None)
-    return _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
+    out = []
+    if offsets is not None:
+        out.append(_reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce))
+        if embeddings:
+            lo, means = shard.finish(info)
+            emb = gdist.gather_contig_means(lo, means, len(offsets) - 1, info)
+            out.append(emb.cpu().numpy() if emb is not None else None)
+    if window_probs:
+        full = gdist.collect_window_probs(local_t, n, info)
+        out.append(full.cpu().numpy() if full is not None else None)
+    return out[0] if len(out) == 1 else tuple(out)
 
 
 def _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce) -> np.ndarray:
@@ -161,6 +183,84 @@ def _write_tsv(path: Path, names, preds) -> None:
         fout.write(_HEADER)
         for name, s in zip(names, preds):
             fout.write(f"{name}\t{float(s[0]):.4f}\t{float(s[1]):.4f}\t{float(s[2]):.4f}\n")
+
+
+_WINDOW_HEADER = "seq_name\tstart\tend\tchromosome_score\tplasmid_score\tvirus_score\n"
+
+
+def window_scores_enabled() -> bool:
+    """Opt-in (``--write-window-scores`` / GENOMAD_B200_WINDOW_SCORES=1): also write the class scores of every window."""
+    return os.environ.get("GENOMAD_B200_WINDOW_SCORES", "0") not in ("", "0")
+
+
+def _write_window_tsv(path: Path, names, offsets, starts, lengths, probs, threads: int = 1) -> None:
+    """One row per window: name, 1-based start, inclusive end (in the record's sequence before stripping n/N), and the three
+    scores with the digits of f"{x:.4f}" -- formatted natively on `threads` threads (gnm_write_window_tsv): a profile can
+    have hundreds of millions of rows."""
+    from . import engine
+    lib = engine.load_library()
+    blobs = [str(x).encode() for x in names]
+    name_off = np.zeros(len(blobs) + 1, dtype=np.int64)
+    np.cumsum([len(b) for b in blobs], out=name_off[1:])
+    blob = b"".join(blobs) or b"\0"
+    offsets = np.ascontiguousarray(offsets, dtype=np.int32)
+    starts = np.ascontiguousarray(starts, dtype=np.int64)
+    lengths = np.ascontiguousarray(lengths, dtype=np.int32)
+    probs = np.ascontiguousarray(probs, dtype=np.float32)
+    assert len(offsets) == len(blobs) + 1 and len(starts) == len(lengths) == len(probs) == offsets[-1]
+    rc = lib.gnm_write_window_tsv(str(path).encode(), _WINDOW_HEADER.encode(), blob, name_off.ctypes.data, len(blobs),
+                                  offsets.ctypes.data, starts.ctypes.data, lengths.ctypes.data, probs.ctypes.data,
+                                  max(1, int(threads)))
+    if rc != 0:
+        raise RuntimeError(lib.gnm_tsv_last_error().decode())
+
+
+def _write_window_scores(npz_path: Path, tsv_path: Path, names_key: str, names, offsets, starts, lengths, probs, stride: int,
+                         threads: int) -> None:
+    offsets = np.asarray(offsets, dtype=np.int32)
+    np.savez(npz_path, **{names_key: names,
+                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+                          "window_start": np.asarray(starts, dtype=np.int64),
+                          "window_length": np.asarray(lengths, dtype=np.int32),
+                          "predictions": np.asarray(probs, dtype=np.float32).reshape(-1, 3),
+                          "window_stride": np.int32(stride)})
+    _write_window_tsv(tsv_path, names, offsets, starts, lengths, probs, threads)
+
+
+def _window_scores_current(npz_path: Path, tsv_path: Path, stride: int) -> bool:
+    """Both window-score files exist and were written at this stride."""
+    if not (npz_path.exists() and tsv_path.exists()):
+        return False
+    try:
+        with np.load(npz_path) as z:
+            return int(z["window_stride"]) == stride
+    except Exception:
+        return False
+
+
+def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, embeddings: bool):
+    """Per-contig scores (+ embeddings) and the per-window scores at `stride`: (preds, emb or None, offsets, starts, lengths,
+    probs); the window arrays are None off rank 0.  At stride 6000 without --single-window the profile windows are the
+    contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list."""
+    emb = None
+    if stride == sequence.WINDOW and not single_window:
+        res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True)
+        preds, probs = res[0], res[-1]
+        if embeddings:
+            emb = res[1]
+        starts, lengths = parsed.spans() if info.is_main else (None, None)
+        return preds, emb, index.offsets, starts, lengths, probs
+    if embeddings:
+        preds, emb = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=True)
+    else:
+        preds = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce)
+    wl = parsed.windows(stride)
+    try:
+        probs = _classify_parsed(clf, wl, None, info, window_probs=True)
+        offsets, starts, lengths = wl.spans() if info.is_main else (None, None, None)
+    finally:
+        wl.close()
+    return preds, emb, offsets, starts, lengths, probs
 
 
 def tfrecords_enabled() -> bool:
@@ -235,7 +335,7 @@ def contig_reduce_mode(default: str = "gather") -> str:
 
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
-         write_embeddings=None):
+         write_embeddings=None, write_window_scores=None, window_stride=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -244,6 +344,12 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     is_main = info.is_main
     contig_reduce = contig_reduce or contig_reduce_mode()
     write_embeddings = embeddings_enabled() if write_embeddings is None else bool(write_embeddings)
+    # a stride asks for a profile: it implies the window scores unless they are switched off explicitly
+    write_window_scores = ((window_scores_enabled() or window_stride is not None) if write_window_scores is None
+                           else bool(write_window_scores))
+    window_stride = sequence.WINDOW if window_stride is None else int(window_stride)
+    if not 1 <= window_stride <= sequence.WINDOW:
+        raise ValueError(f"window_stride must be in [1, {sequence.WINDOW}], not {window_stride}")
     if is_main:
         utils.start_md5(input_path)                      # hashed in the background while the file is indexed (rank 0 only)
     if not output_path.is_dir() and is_main:
@@ -267,6 +373,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if write_embeddings:
         files.append(outputs.nn_classification_embeddings_output)
         descr.append("contig embeddings: binary format")
+    if write_window_scores:
+        files += [outputs.nn_classification_windows_output, outputs.nn_classification_windows_npz_output]
+        descr += ["window classification: tabular format", "window classification: binary format"]
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -275,6 +384,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if write_embeddings:
             files.append(outputs.provirus_nn_classification_embeddings_output)
             descr.append("provirus embeddings: binary format")
+        if write_window_scores:
+            files += [outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_windows_npz_output]
+            descr += ["provirus window classification: tabular format", "provirus window classification: binary format"]
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -289,12 +401,14 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     jobs = [("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
              "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
-             outputs.nn_classification_embeddings_output)]
+             outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
+             outputs.nn_classification_windows_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
                      outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
-                     outputs.provirus_nn_classification_embeddings_output))
+                     outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
+                     outputs.provirus_nn_classification_windows_output))
 
     plan = None
     info_writer = None
@@ -312,8 +426,11 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             console.log(f"Creating the {outputs.nn_classification_dir} directory.")
             outputs.nn_classification_dir.mkdir()
         # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
-        # (with embeddings requested, a classification whose embeddings file is missing is redone: same predictions, bit for bit)
-        plan = [(bool(skip and j[4].exists()), bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())))
+        # (with embeddings or window scores requested, a classification whose embeddings file is missing, or whose window
+        # scores are missing or were written at another stride, is redone: same predictions, bit for bit)
+        plan = [(bool(skip and j[4].exists()),
+                 bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
+                      and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -343,7 +460,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     # ---- stage 1, every job: "encode" (here: record the window -> sequence map; the windows themselves are streamed to the GPU in
     # stage 2).  Like the reference, sequences AND proviruses are encoded before either is classified (nn_classification.py:215-281).
     staged = []
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path), \
+    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path, *_), \
             (enc_skip, cls_skip) in zip(jobs, plan):
         parsed = index = None
         if enc_skip:
@@ -354,9 +471,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         staged.append((parsed, index))
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path), \
-            (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
+    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
+         win_npz_path, win_tsv_path), (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
         names = preds = emb = None
+        win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
         if cls_skip:
@@ -376,9 +494,14 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     sys.exit(1)
                 names, preds = index.names, np.zeros((len(index.names), 3), np.float32)
                 emb = np.zeros((len(index.names), 512), np.float32)
+                win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
+                       np.zeros((0, 3), np.float32))
             else:
                 t_c = _time.perf_counter()
-                if write_embeddings:
+                if write_window_scores:
+                    preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
+                                                            contig_reduce, write_embeddings)
+                elif write_embeddings:
                     preds, emb = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, embeddings=True)
                 else:
                     preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce)
@@ -392,6 +515,12 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                 if is_main:
                     _write_embeddings(emb_path, names_key, names, emb)
                 console.log(f"{label} embeddings in binary format written to {emb_path.name}.")
+            if write_window_scores:
+                if is_main:
+                    _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,
+                                         threads or 1)
+                console.log(f"{label} window scores (stride {window_stride}) written to {win_tsv_path.name} and "
+                            f"{win_npz_path.name}.")
         if parsed is not None:
             parsed.close()
         if cleanup and is_main and enc_dir.is_dir():

@@ -23,6 +23,10 @@ GPU as they are -- tokenisation happens on the device (csrc/encode.cuh).  gzip i
 memory (BGZF files block-parallel on all reader threads); bz2 / xz / zstd go through Python's bindings.  ``iter_fasta`` / ``window_spans`` /
 ``encode_fasta_py`` are the readable pure-Python statement of the same rules; the tests hold the native code
 to them and both to golden vectors made with the real reference.
+
+Score profiles (``--write-window-scores --window-stride s``) use the same rules with a window every s nt instead of
+every 6000 (``profile_spans``; ``ParsedFasta.windows(s)`` is the native list, ``gnm_contig_windows_stride`` the device
+one).
 """
 from __future__ import annotations
 
@@ -124,6 +128,24 @@ def window_spans(length: int, single_window: bool = False) -> List[Tuple[int, in
         win += 1
         if single_window and win == 1:
             break
+    return spans
+
+
+def profile_spans(length: int, stride: int) -> List[Tuple[int, int]]:
+    """[start, end) of every candidate window of a stripped contig of `length` nt at window stride `stride` (1..6000), before
+    the N rule: candidate k starts at k * stride and is min(6000, length - k * stride) long; the first is always a candidate,
+    any other one only if it has >= 2500 nt.  There are 1 + max(0, (length - 2500) // stride) of them, and at stride 6000
+    they are window_spans(length)."""
+    if not 1 <= stride <= WINDOW:
+        raise ValueError(f"window stride must be in [1, {WINDOW}], not {stride}")
+    spans = []
+    k = 0
+    while k * stride < length:
+        s, e = k * stride, min(k * stride + WINDOW, length)
+        if k > 0 and e - s < MIN_TAIL:
+            break
+        spans.append((s, e))
+        k += 1
     return spans
 
 
@@ -248,11 +270,83 @@ class ParsedFasta:
         """mmap mode: drop the file pages that precede global window `upto` from the resident set."""
         self._lib.gnm_fasta_release_before(self._h, int(upto))
 
+    def spans(self) -> Tuple[np.ndarray, np.ndarray]:
+        """Start (0-based, in the record's sequence before stripping) int64 and length (padding excluded) int32 of every window
+        of the list export_windows() serves."""
+        starts = np.empty(self.n_windows, dtype=np.int64)
+        lengths = np.empty(self.n_windows, dtype=np.int32)
+        if self.n_windows:
+            rc = self._lib.gnm_fasta_spans(self._h, starts.ctypes.data, lengths.ctypes.data)
+            if rc != 0:
+                raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
+        return starts, lengths
+
+    def windows(self, stride: int = WINDOW, single_window: bool = False) -> "WindowList":
+        """The window list at `stride` (1..6000) over this index (native, records on the reader threads).  At stride 6000 with
+        this file's single_window it is the list export_windows() serves."""
+        return WindowList(self, stride, single_window)
+
     def close(self):
         if getattr(self, "_h", None):
             self._lib.gnm_fasta_free(self._h)
             self._h = None
         self._text = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class WindowList:
+    """
+    Windows every `stride` nt of every kept record of a ParsedFasta (gnm_fasta_windows_*): what the module streams for a
+    score profile.  Same interface as ParsedFasta for the classifier's chunk loop (n_windows, export_windows,
+    release_before), plus spans(): the CSR offsets per contig and each window's start (0-based, in the record's sequence
+    before stripping) and length (padding excluded).  The ParsedFasta must stay open while the list is used.
+    """
+
+    def __init__(self, parsed: ParsedFasta, stride: int, single_window: bool = False):
+        import ctypes as C
+        self._parsed, self._lib, self._threads = parsed, parsed._lib, parsed._threads
+        self.stride = int(stride)
+        self._h = C.c_void_p()
+        rc = self._lib.gnm_fasta_windows_plan(parsed._h, self.stride, int(bool(single_window)), self._threads, C.byref(self._h))
+        if rc != 0:
+            raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
+        nc, nw = C.c_int64(), C.c_int64()
+        self._lib.gnm_fasta_windows_info(self._h, C.byref(nc), C.byref(nw))
+        self.n_contigs, self.n_windows = nc.value, nw.value
+
+    def spans(self) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """(offsets int32 [n_contigs + 1], starts int64 [n_windows], lengths int32 [n_windows])."""
+        offsets = np.zeros(self.n_contigs + 1, dtype=np.int32)
+        starts = np.empty(self.n_windows, dtype=np.int64)
+        lengths = np.empty(self.n_windows, dtype=np.int32)
+        rc = self._lib.gnm_fasta_windows_spans(self._h, offsets.ctypes.data, starts.ctypes.data if self.n_windows else None,
+                                               lengths.ctypes.data if self.n_windows else None)
+        if rc != 0:
+            raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
+        return offsets, starts, lengths
+
+    def export_windows(self, first: int, count: int, out: np.ndarray) -> np.ndarray:
+        """Windows [first, first+count) of this list -> out[:count] (uint8 [*, 6000])."""
+        assert out.dtype == np.uint8 and out.shape[1] == WINDOW and out.shape[0] >= count and out.flags.c_contiguous
+        if count:
+            rc = self._lib.gnm_fasta_windows_export(self._h, int(first), int(count), out.ctypes.data, self._threads)
+            if rc != 0:
+                raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
+        return out[:count]
+
+    def release_before(self, upto: int) -> None:
+        self._lib.gnm_fasta_windows_release_before(self._h, int(upto))
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.gnm_fasta_windows_free(self._h)
+            self._h = None
+        self._parsed = None
 
     def __del__(self):
         try:

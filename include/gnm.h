@@ -158,6 +158,14 @@ int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_pro
  *   d_win_offsets doubles as the planning scratch: no other memory is used or allocated.
  *   Synchronous: one device-to-host copy of the count; the start / length arrays are written in `stream` order after it.
  *
+ * gnm_contig_windows_stride: the same plan with a window every `stride` nt (1 <= stride <= 6000) instead of every 6000: the
+ *   overlapping windows of a score profile, always over the whole contig (no single_window).  Candidate k of a stripped contig
+ *   of L nt starts at k * stride and is min(6000, L - k * stride) long; candidate 0 is always kept, any other one if it has
+ *   >= 2500 nt and <= 4000 'N' -- 1 + max(0, (L - 2500) / stride) candidates.  At stride 6000 this is gnm_contig_windows
+ *   (same kernels, bitwise the same plan).  capacity >= n_contigs + total_bytes / stride is always enough; the failures and
+ *   their messages are those of gnm_contig_windows.  Each candidate's N count reads its own 6000 bytes, ~6000 / stride reads
+ *   per byte.
+ *
  * gnm_gather_windows: kept windows -> d_ascii uint8 [n][6000] (16-byte aligned), ASCII-upper-cased ('a'..'z' only) and
  *   'N'-padded: exactly the bytes gnm_forward_ascii takes, and gnm_fasta_export gives for the same contigs as FASTA text.
  *   Asynchronous.
@@ -172,6 +180,9 @@ int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_pro
 int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int single_window,
                        int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
                        int64_t* h_n_windows, void* stream);
+int gnm_contig_windows_stride(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int stride,
+                              int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
+                              int64_t* h_n_windows, void* stream);
 int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                        uint8_t* d_ascii, void* stream);
 int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
@@ -227,6 +238,22 @@ int gnm_segment_sum_rows(gnm_handle* h, const float* d_rows, const int32_t* d_of
  *                      from the text (any block, any order, `threads` threads): what a rank calls for its shard, chunk by chunk.
  *   gnm_fasta_release_before : mmap mode only -- drop the mapped pages that lie before the record holding window `upto`
  *                      from the resident set (they stay in the page cache).
+ *
+ * Window lists at any stride (score profiles): the list above is the stride-6000 case of one enumeration over the index --
+ * candidate k of a kept record starts k * stride nt into its stripped sequence, is min(6000, L - k * stride) long, and is kept
+ * if it is the first or has >= 2500 nt and <= 4000 'N' (the rules of gnm_contig_windows_stride).
+ *   gnm_fasta_windows_plan   : the list at `stride` (1..6000; single_window keeps only the first window of each record) over the
+ *                      index of f, records on `threads` threads; f must outlive it.  ~16 B per record, plus 8 B per candidate
+ *                      window of records with irregular lines and 4 B per window of records that lost one to the N rule.
+ *                      Fails, before anything is built, if the list could have more than 2^31 - 1 windows (its
+ *                      candidates before the N rule, a closed form).  Each list releases the pages behind its own
+ *                      export cursor (gnm_fasta_windows_release_before), so a second pass over the file stays bounded too.
+ *   gnm_fasta_windows_info   : kept records (= contigs) and windows of the list.
+ *   gnm_fasta_windows_spans  : offsets int32 [n_contigs + 1] (CSR: the windows of contig c), starts int64 [n_windows] (0-based,
+ *                      in the record's sequence BEFORE stripping, i.e. its joined lines), lengths int32 [n_windows] (1..6000,
+ *                      padding excluded); any pointer may be NULL.
+ *   gnm_fasta_windows_export / _release_before : gnm_fasta_export_windows / gnm_fasta_release_before on this list.
+ *   gnm_fasta_spans          : starts / lengths, as gnm_fasta_windows_spans gives them, of the list gnm_fasta_export serves.
  */
 typedef struct gnm_fasta gnm_fasta;
 const char* gnm_fasta_last_error(void);
@@ -239,6 +266,31 @@ int gnm_fasta_export(const gnm_fasta* f, uint8_t* windows, int32_t* offsets, cha
 int gnm_fasta_export_windows(const gnm_fasta* f, int64_t first, int64_t count, uint8_t* dst, int threads);
 int gnm_fasta_release_before(const gnm_fasta* f, int64_t upto);
 void gnm_fasta_free(gnm_fasta* f);
+typedef struct gnm_fasta_windows gnm_fasta_windows;
+int gnm_fasta_windows_plan(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out);
+int gnm_fasta_windows_info(const gnm_fasta_windows* w, int64_t* n_contigs, int64_t* n_windows);
+int gnm_fasta_windows_spans(const gnm_fasta_windows* w, int32_t* offsets, int64_t* starts, int32_t* lengths);
+int gnm_fasta_windows_export(const gnm_fasta_windows* w, int64_t first, int64_t count, uint8_t* dst, int threads);
+int gnm_fasta_windows_release_before(const gnm_fasta_windows* w, int64_t upto);
+void gnm_fasta_windows_free(gnm_fasta_windows* w);
+int gnm_fasta_spans(const gnm_fasta* f, int64_t* starts, int32_t* lengths);
+
+/* ---- per-window score table (host side, no GPU involved) ----------------------------------- */
+
+/*
+ * gnm_write_window_tsv: writes `header`, then one line per window w of contig c,
+ *   "<name c>\t<starts[w] + 1>\t<starts[w] + lengths[w]>\t<p0>\t<p1>\t<p2>\n"  (1-based start, inclusive end),
+ *   to `path` (overwritten).  names: the contigs' names back to back, name c = names[name_offsets[c] .. name_offsets[c+1]);
+ *   win_offsets int32 [n_contigs + 1] (CSR); probs float [win_offsets[n_contigs]][3].  Scores carry exactly the digits of
+ *   Python's f"{float(x):.4f}" (the float value rounded half to even at the fourth decimal; no locale).  Rows are formatted on
+ *   `threads` threads and written in order.
+ * gnm_format_scores: the same score formatting, one value per line into out (<= 49 bytes per value); *out_len = bytes written.
+ */
+const char* gnm_tsv_last_error(void);
+int gnm_write_window_tsv(const char* path, const char* header, const char* names, const int64_t* name_offsets, int64_t n_contigs,
+                         const int32_t* win_offsets, const int64_t* starts, const int32_t* lengths, const float* probs,
+                         int threads);
+int gnm_format_scores(const float* x, int64_t n, char* out, int64_t* out_len);
 
 /* ---- TFRecord files of tokenised windows (host side, no GPU involved; off by default) ------ */
 

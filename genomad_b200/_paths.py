@@ -87,6 +87,15 @@ class NNOutputs:
     def provirus_nn_classification_windows_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification_windows.npz")
 
+    # ---- opt-in (--write-attributions), not a reference output: per-token input gradients of one class, per window
+    @property
+    def nn_classification_attributions_output(self) -> Path:
+        return self._nn("nn_classification_attributions.npz")
+
+    @property
+    def provirus_nn_classification_attributions_output(self) -> Path:
+        return self._nn("provirus_nn_classification_attributions.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

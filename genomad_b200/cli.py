@@ -54,8 +54,13 @@ def cli():
               help="Write the window scores (implies --write-window-scores) for a 6,000-base window every N bases (overlapping "
                    "windows when N < 6000), a finer score profile. Sequence scores always use the reference's windows. Not an "
                    "option of the reference.")
+@click.option("--write-attributions", type=click.Choice(["chromosome", "plasmid", "virus"]), default=None,
+              help="Also write, for every window of the classification, the gradient of the log-probability of this class "
+                   "with respect to each one-hot 4-mer (gradient x input; position t covers bases t..t+3 of the window) to "
+                   "<prefix>_nn_classification_attributions.npz: 5,997 float32 values, 24 KB per window, ~4 GB per Gbp of "
+                   "input. About 4x the classification's GPU time. Not an option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
-                      write_embeddings, write_window_scores, window_stride):
+                      write_embeddings, write_window_scores, window_stride, write_attributions):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -67,6 +72,8 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["write_window_scores"] = True
     if window_stride is not None:
         extra["window_stride"] = window_stride
+    if write_attributions is not None:
+        extra["write_attributions"] = write_attributions
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
 

@@ -22,6 +22,7 @@
 #include "logits_tc.cuh"
 #include "wv_gather.cuh"
 #include "contigs.cuh"
+#include "attr.cuh"
 
 using namespace gnm;
 
@@ -120,6 +121,10 @@ struct gnm_handle {
   CUtensorMap tm_w_half[4];                          // the same packs, one warpgroup's 8 KB half-stage per box (conv_t_kernel)
   StageTimer timer;
   std::vector<void*> allocs;
+  const uint8_t* attr_route[2] = {nullptr, nullptr};   // routing / maxima of the last attribution chunk (gnm_debug_fetch "route*", "routeq*")
+  const float* attr_rq[2] = {nullptr, nullptr};
+  const uint8_t* attr_y1 = nullptr;                    // the attribution pass's layer-1 copy (gnm_debug_fetch "attr_y1")
+  int attr_mb = 0;                                     // max_batch of the context those buffers belong to
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -228,6 +233,31 @@ static void pack_stage_f8_pairs(std::vector<uint8_t>& dst, const float* Wkn, int
       dst.push_back(static_cast<uint8_t>(__nv_cvt_float_to_fp8(hi * scale_hi, __NV_SATFINITE, __NV_E4M3)));
       dst.push_back(static_cast<uint8_t>(__nv_cvt_float_to_fp8((x - hi) * scale_lo, __NV_SATFINITE, __NV_E4M3)));
     }
+}
+
+// A conv layer's tensor-core weight pack, in the order conv_t_kernel consumes its 16 KB stages, and its output scale 2^-S.
+// Wk: Keras layout [6 taps][128 in][128 out].  Common scale 2^S of the three passes (conv_t.cuh): main weights fp16(W * 2^d)
+// with wmax * 2^d in (0.39, 0.78] * 2^16, so the fp16 plane and both e4m3 planes (|hi| * 2^-7 <= 400 < 448) stay in range.
+// Small weights get d > 16: with d fixed at 16 the e4m3 plane of their lo halves fell into the subnormal range and the
+// Ahi * Wlo correction stopped correcting.
+static int pack_conv_weights(const float* Wk, std::vector<uint8_t>& pk, float* out_scale, const char* who) {
+  float wmax = 0.f;
+  for (size_t i = 0; i < static_cast<size_t>(kTaps) * kC * kC; ++i) wmax = std::max(wmax, std::fabs(Wk[i]));
+  if (!(wmax > 0.f) || !std::isfinite(wmax)) return fail(std::string(who) + ": conv kernel is all-zero or not finite");
+  const int shift = static_cast<int>(std::ceil(std::log2(wmax / 0.78f)));
+  const int d = std::min(16 - shift, 40), S = 5 + d;
+  if (d < 1) return fail(std::string(who) + ": conv weights too large for the fp16 operand format");
+  *out_scale = std::ldexp(1.f, -S);
+  pk.clear();                                           // (region, tap): hi16.k0 x6, hi16.k1 x6, pairs.k0 x6, pairs.k1 x6
+  pk.reserve(static_cast<size_t>(kConvStages) * kBStage);
+  for (int kh = 0; kh < 2; ++kh)
+    for (int tap = 0; tap < kTaps; ++tap)
+      pack_stage_f16(pk, Wk + static_cast<size_t>(tap) * kC * kC, 0, kh, std::ldexp(1.f, d));
+  for (int kh = 0; kh < 2; ++kh)                        // x (lo8, hi8) = (e4m3(Alo * 2^12), e4m3(Ahi * 2^7)):  (e4m3(Whi * 2^(S-12)), e4m3(Wlo * 2^(S-7)))
+    for (int tap = 0; tap < kTaps; ++tap)                //   = (e4m3(hi * 2^(S-12-d)), e4m3(lo * 2^(S-7-d))) of the split of W * 2^d
+      pack_stage_f8_pairs(pk, Wk + static_cast<size_t>(tap) * kC * kC, kh, std::ldexp(1.f, d), std::ldexp(1.f, S - 12 - d),
+                          std::ldexp(1.f, S - 7 - d));
+  return 0;
 }
 
 // One IGLOO layer's patch set as the gather kernels want it (host only).
@@ -378,25 +408,8 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
   {
     const float* convw[2] = {w->conv2_kernel, w->conv3_kernel};
     for (int L = 0; L < 2; ++L) {
-      // common scale 2^S of the three passes (conv_t.cuh): main weights fp16(W * 2^d) with wmax * 2^d in (0.39, 0.78] * 2^16, so
-      // the fp16 plane and both e4m3 planes (|hi| * 2^-7 <= 400 < 448) stay in range.  Small weights get d > 16: with d fixed at
-      // 16 the e4m3 plane of their lo halves fell into the subnormal range and the Ahi * Wlo correction stopped correcting.
-      float wmax = 0.f;
-      for (size_t i = 0; i < static_cast<size_t>(kTaps) * kC * kC; ++i) wmax = std::max(wmax, std::fabs(convw[L][i]));
-      if (!(wmax > 0.f) || !std::isfinite(wmax)) return fail("gnm_create: conv kernel is all-zero or not finite");
-      const int shift = static_cast<int>(std::ceil(std::log2(wmax / 0.78f)));
-      const int d = std::min(16 - shift, 40), S = 5 + d;
-      if (d < 1) return fail("gnm_create: conv weights too large for the fp16 operand format");
-      h->conv_out_scale[L] = std::ldexp(1.f, -S);
-      std::vector<uint8_t> pk;                              // (region, tap): hi16.k0 x6, hi16.k1 x6, pairs.k0 x6, pairs.k1 x6
-      pk.reserve(static_cast<size_t>(kConvStages) * kBStage);
-      for (int kh = 0; kh < 2; ++kh)
-        for (int tap = 0; tap < kTaps; ++tap)
-          pack_stage_f16(pk, convw[L] + static_cast<size_t>(tap) * kC * kC, 0, kh, std::ldexp(1.f, d));
-      for (int kh = 0; kh < 2; ++kh)                        // x (lo8, hi8) = (e4m3(Alo * 2^12), e4m3(Ahi * 2^7)):  (e4m3(Whi * 2^(S-12)), e4m3(Wlo * 2^(S-7)))
-        for (int tap = 0; tap < kTaps; ++tap)                //   = (e4m3(hi * 2^(S-12-d)), e4m3(lo * 2^(S-7-d))) of the split of W * 2^d
-          pack_stage_f8_pairs(pk, convw[L] + static_cast<size_t>(tap) * kC * kC, kh, std::ldexp(1.f, d), std::ldexp(1.f, S - 12 - d),
-                              std::ldexp(1.f, S - 7 - d));
+      std::vector<uint8_t> pk;
+      if (pack_conv_weights(convw[L], pk, &h->conv_out_scale[L], "gnm_create")) return 1;
       if (dev_upload(h, &h->wpack[L], pk.data(), pk.size())) return 1;
       if (dev_upload(h, &h->conv_w32[L], convw[L], static_cast<size_t>(kTaps) * kC * kC)) return 1;
     }
@@ -961,9 +974,12 @@ struct TailOverlap {
 static int check_device_status(gnm_handle* h) {
   if (h->status && h->status->act_overflow) {
     // not fatal for the device, but the parity promise no longer holds for the step that raised it: fail loudly
-    const int stage = h->status->ov_stage[1] ? 1 : h->status->ov_stage[2] ? 2 : 3;       // the first layer that left the range
+    const int stage = h->status->ov_stage[1] ? 1 : h->status->ov_stage[2] ? 2 : h->status->ov_stage[3] ? 3 : 0;   // the first layer that left the range
     h->status->act_overflow = 0;
     for (int i = 0; i < 4; ++i) h->status->ov_stage[i] = 0;
+    if (stage == 0)
+      return fail("gradient range exceeded in conv3's backward pass of an attribution call: |g_z2| * s_w > 3.5 saturates the "
+                  "e4m3 correction plane -- the attributions of that step are not within their precision bar");
     return fail(std::string("activation range exceeded in ") + (stage == 1 ? "layer 1" : stage == 2 ? "conv2" : "conv3") +
                 ": |y| > 3.5 saturates the e4m3 correction plane (|y| > 2047 overflows fp16) -- these weights are outside the "
                 "range the split-operand tensor-core recipe supports (common.cuh); results of that step are not within 1e-4");
@@ -1293,6 +1309,8 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
   const std::string k(which);
   const float* src = nullptr;
   size_t count = 0;
+  if ((k.rfind("route", 0) == 0 || k == "attr_y1") && n > h->attr_mb)        // the last attribution context's buffers
+    return fail("gnm_debug_fetch: n exceeds the max_batch of the last attribution call's context (" + std::to_string(h->attr_mb) + ")");
   if (k == "buf0" || k == "buf1") {
     const size_t rows = static_cast<size_t>(n) * kTok;
     join_rows_kernel<<<static_cast<unsigned>((rows * kC + 255) / 256), 256, 0, st>>>(h->ybuf[k == "buf1"], d_dst, rows,
@@ -1304,7 +1322,269 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
   else if (k == "h1" || k == "h2") { src = k == "h1" ? h->h1 : h->h2; count = static_cast<size_t>(n) * kHidden; }
   else if (k == "logits") { src = h->logits; count = static_cast<size_t>(n) * kLogitsLd; }
   else if (k == "conv_dbg") { src = reinterpret_cast<const float*>(h->conv_dbg); count = static_cast<size_t>(h->num_sms) * 16; }
+  else if (k == "route0" || k == "route1") {               // uint8 [n][749][128]: n * 749 * 128 BYTES
+    const uint8_t* r = h->attr_route[k == "route1"];
+    if (!r) return fail("gnm_debug_fetch: no attribution call has run on this handle");
+    GNM_CUDA(cudaMemcpyAsync(d_dst, r, static_cast<size_t>(n) * kPooled * kC, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  } else if (k == "attr_y1") {
+    if (!h->attr_y1) return fail("gnm_debug_fetch: no attribution call has run on this handle");
+    const size_t rows = static_cast<size_t>(n) * kTok;
+    join_rows_kernel<<<static_cast<unsigned>((rows * kC + 255) / 256), 256, 0, st>>>(h->attr_y1, d_dst, rows, 0);
+    return check_launch(h, "join_rows_kernel");
+  } else if (k == "routeq0" || k == "routeq1") {
+    src = h->attr_rq[k == "routeq1"];
+    if (!src) return fail("gnm_debug_fetch: no attribution call has run on this handle");
+    count = static_cast<size_t>(n) * kPooled * kC;
+  }
   else return fail("gnm_debug_fetch: unknown buffer " + k);
   GNM_CUDA(cudaMemcpyAsync(d_dst, src, count * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ attributions (attr.cuh)
+// Workspace of the attribution pass, separate from the handle so that plain handles keep their memory.  Per window:
+// y1 copy, g_z3 and g_z2 operand rows (3 x 4.6 MB), fp32 g_y1 / g_z rows (2 x 3.1 MB), routing + routed maxima (2 x 0.48 MB):
+// ~21 MB (kAttrBytesPerWindow).
+struct gnm_attr {
+  gnm_handle* h = nullptr;
+  int max_batch = 0;
+  uint8_t* y1 = nullptr;                                // layer 1 re-run: the forward's y1 (ybuf[0] is overwritten by conv3)
+  uint8_t* gz3 = nullptr; uint8_t* gz2 = nullptr;       // conv operand rows of s_w g_z3, s_w g_z2, time-reversed
+  float* f32a = nullptr;                                // fp32 rows: g_z3 (before packing), then g_z1 (conv2 backward output)
+  float* gy1 = nullptr;                                 // fp32 rows: IGLOO#0's part of g_y1
+  uint8_t* route[2] = {nullptr, nullptr}; float* rq[2] = {nullptr, nullptr};
+  float* g_out = nullptr; float* alpha = nullptr; float* g_logit = nullptr; float* g_mpi = nullptr;
+  float* blockmax = nullptr; float* s_w = nullptr; float* probs = nullptr;
+  uint8_t* wpackT[2] = {nullptr, nullptr};              // W2^T, W3^T packed like the forward's conv weights
+  float out_scaleT[2] = {1.f, 1.f};
+  float* wvT[2] = {nullptr, nullptr}; float* wqkT[2] = {nullptr, nullptr};
+  int32_t* pos_start[2] = {nullptr, nullptr}; int32_t* slot_patch[2] = {nullptr, nullptr};
+  CUtensorMap tm_y1, tm_gz3, tm_gz2, tm_wT[2];
+  std::vector<void*> allocs;
+};
+
+static int attr_alloc(gnm_attr* a, void** p, size_t bytes) {
+  GNM_CUDA(cudaMalloc(p, bytes));
+  a->allocs.push_back(*p);
+  return 0;
+}
+template <class T>
+static int attr_upload(gnm_attr* a, T** dst, const std::vector<T>& src) {
+  if (attr_alloc(a, reinterpret_cast<void**>(dst), src.size() * sizeof(T))) return 1;
+  GNM_CUDA(cudaMemcpy(*dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return 0;
+}
+template <class T>
+static int fetch_host(std::vector<T>& dst, const T* src, size_t count) {
+  dst.resize(count);
+  GNM_CUDA(cudaMemcpy(dst.data(), src, count * sizeof(T), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int gnm_attr_destroy(gnm_attr* a) {
+  if (!a) return 0;
+  cudaSetDevice(a->h->device);
+  cudaDeviceSynchronize();
+  for (int s = 0; s < 2; ++s)
+    if (a->h->attr_route[s] == a->route[s]) {
+      a->h->attr_route[s] = nullptr; a->h->attr_rq[s] = nullptr; a->h->attr_y1 = nullptr; a->h->attr_mb = 0;
+    }
+  for (void* p : a->allocs) cudaFree(p);
+  delete a;
+  return 0;
+}
+
+extern "C" int gnm_attr_create(gnm_handle* h, int max_batch, gnm_attr** out) {
+  if (!h || !out) return fail("gnm_attr_create: null argument");
+  *out = nullptr;
+  if (max_batch < 1 || max_batch > h->max_batch)
+    return fail("gnm_attr_create: max_batch must be in [1, the handle's max_batch = " + std::to_string(h->max_batch) + "]");
+  GNM_CUDA(cudaSetDevice(h->device));
+  gnm_attr* a = new gnm_attr();
+  a->h = h;
+  a->max_batch = max_batch;
+  *out = a;                                             // so the caller can gnm_attr_destroy() after a partial failure
+  const size_t mb = static_cast<size_t>(max_batch), rows = mb * kTok;
+  void** v = nullptr;
+#define ATTR_ALLOC(ptr, bytes) do { v = reinterpret_cast<void**>(&(ptr)); if (attr_alloc(a, v, (bytes))) return 1; } while (0)
+  ATTR_ALLOC(a->y1, rows * kRowBytes);
+  ATTR_ALLOC(a->gz3, rows * kRowBytes);
+  ATTR_ALLOC(a->gz2, rows * kRowBytes);
+  ATTR_ALLOC(a->f32a, rows * kC * sizeof(float));
+  ATTR_ALLOC(a->gy1, rows * kC * sizeof(float));
+  for (int s = 0; s < 2; ++s) {
+    ATTR_ALLOC(a->route[s], mb * kPooled * kC);
+    ATTR_ALLOC(a->rq[s], mb * kPooled * kC * sizeof(float));
+  }
+  ATTR_ALLOC(a->g_out, mb * 256 * sizeof(float));
+  ATTR_ALLOC(a->alpha, mb * kLogitsLd * sizeof(float));
+  ATTR_ALLOC(a->g_logit, mb * kLogitsLd * sizeof(float));
+  ATTR_ALLOC(a->g_mpi, mb * kPatches * sizeof(float));
+  ATTR_ALLOC(a->blockmax, mb * kAttrPosBlocks * sizeof(float));
+  ATTR_ALLOC(a->s_w, mb * sizeof(float));
+  ATTR_ALLOC(a->probs, mb * 3 * sizeof(float));
+#undef ATTR_ALLOC
+  // ---- weights, derived from the handle's device copies
+  for (int L = 0; L < 2; ++L) {                         // conv2, conv3: W[j]^T in the forward's pack, same split and scale
+    std::vector<float> Wk, WT(static_cast<size_t>(kTaps) * kC * kC);
+    if (fetch_host(Wk, h->conv_w32[L], WT.size())) return 1;
+    for (int j = 0; j < kTaps; ++j)
+      for (int i = 0; i < kC; ++i)
+        for (int o = 0; o < kC; ++o)
+          WT[(static_cast<size_t>(j) * kC + o) * kC + i] = Wk[(static_cast<size_t>(j) * kC + i) * kC + o];
+    std::vector<uint8_t> pk;
+    if (pack_conv_weights(WT.data(), pk, &a->out_scaleT[L], "gnm_attr_create")) return 1;
+    if (attr_upload(a, &a->wpackT[L], pk)) return 1;
+  }
+  for (int s = 0; s < 2; ++s) {
+    std::vector<float> wv, wvT(static_cast<size_t>(kC) * kC), qk, qkT(static_cast<size_t>(kPooled) * kPatches);
+    if (fetch_host(wv, h->wv32[s], wvT.size())) return 1;
+    for (int k = 0; k < kC; ++k)
+      for (int c = 0; c < kC; ++c) wvT[static_cast<size_t>(c) * kC + k] = wv[static_cast<size_t>(k) * kC + c];
+    if (attr_upload(a, &a->wvT[s], wvT)) return 1;
+    if (fetch_host(qk, h->wqk[s], qkT.size())) return 1;
+    for (int i = 0; i < kPatches; ++i)
+      for (int p = 0; p < kPooled; ++p) qkT[static_cast<size_t>(p) * kPatches + i] = qk[static_cast<size_t>(i) * kPooled + p];
+    if (attr_upload(a, &a->wqkT[s], qkT)) return 1;
+    // inverse of the gather's packing: the first 8,400 slots are the patch entries sorted by position (pack_patches)
+    std::vector<int32_t> ent_pos, slot_of, pos_start(kTok + 1, 0), slot_patch(static_cast<size_t>(kPatches) * kPatchLen);
+    if (fetch_host(ent_pos, h->ent_pos[s], static_cast<size_t>(kPatches) * kPatchLen)) return 1;
+    if (fetch_host(slot_of, h->slot_of[s], slot_patch.size())) return 1;
+    for (size_t e = 0; e < slot_of.size(); ++e) slot_patch[slot_of[e]] = static_cast<int32_t>(e / kPatchLen);
+    for (int32_t p : ent_pos) pos_start[p + 1]++;
+    for (int t = 0; t < kTok; ++t) pos_start[t + 1] += pos_start[t];
+    if (attr_upload(a, &a->pos_start[s], pos_start)) return 1;
+    if (attr_upload(a, &a->slot_patch[s], slot_patch)) return 1;
+  }
+  PFN_encodeTiled enc = nullptr;
+  if (get_encode_fn(&enc)) return 1;
+  if (make_act_map(enc, &a->tm_y1, a->y1, max_batch)) return 1;
+  if (make_act_map(enc, &a->tm_gz3, a->gz3, max_batch)) return 1;
+  if (make_act_map(enc, &a->tm_gz2, a->gz2, max_batch)) return 1;
+  for (int L = 0; L < 2; ++L)
+    if (make_w_map(enc, &a->tm_wT[L], a->wpackT[L], kConvStages, 64)) return 1;
+  GNM_CUDA(cudaFuncSetAttribute(conv_t_attr_kernel<kConvRoute>, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvTSmem));
+  GNM_CUDA(cudaFuncSetAttribute(conv_t_attr_kernel<kConvBwd>, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvTSmem));
+  GNM_CUDA(cudaDeviceSynchronize());
+  return 0;
+}
+
+// the w_v pass of IGLOO kernel s over `tm` with the routing epilogue: route[s], rq[s] (= the forward's q[s], bit for bit)
+static int launch_route(gnm_handle* h, gnm_attr* a, int s, const CUtensorMap& tm, int n, cudaStream_t st) {
+  ConvTcParams p;
+  p.status = h->status; p.experiment = 0; p.dbg = nullptr;
+  p.bias = nullptr; p.y_out = nullptr; p.q_out = a->rq[s];
+  p.out_scale = h->wv_out_scale[s]; p.out_fp8 = 0;
+  p.n_tiles = n * kUnitsPerWin;
+  ConvAttrExt x = {};
+  x.route_out = a->route[s];
+  conv_t_attr_kernel<kConvRoute><<<std::min(h->num_sms, p.n_tiles), kConvThreads, kConvTSmem, st>>>(tm, h->tm_w_half[2 + s], p, x);
+  return check_launch(h, "conv_t_attr_kernel<route>");
+}
+// backward of conv layer L (0 = conv2, 1 = conv3) over time-reversed gradient rows
+static int launch_conv_bwd(gnm_handle* h, gnm_attr* a, int L, const CUtensorMap& tm_in, const uint8_t* mask_rows,
+                           const float* add_rows, uint8_t* rows_out, float* f32_out, int n, cudaStream_t st) {
+  ConvTcParams p;
+  p.status = h->status; p.experiment = 0; p.dbg = nullptr;
+  p.bias = nullptr; p.y_out = rows_out; p.q_out = nullptr;
+  p.out_scale = a->out_scaleT[L]; p.out_fp8 = 1;
+  p.n_tiles = n * kUnitsPerWin;
+  ConvAttrExt x = {};
+  x.mask_rows = mask_rows; x.add_rows = add_rows; x.s_w = a->s_w; x.f32_out = f32_out;
+  conv_t_attr_kernel<kConvBwd><<<std::min(h->num_sms, p.n_tiles), kConvThreads, kConvTSmem, st>>>(tm_in, a->tm_wT[L], p, x);
+  return check_launch(h, "conv_t_attr_kernel<bwd>");
+}
+// attention part and g_y of IGLOO kernel s (logits of s must be in h->logits)
+static int launch_igloo_bwd(gnm_handle* h, gnm_attr* a, int s, int n, cudaStream_t st) {
+  attr_igloo_prep_kernel<<<n, 256, 0, st>>>(h->logits, h->q[s], a->g_out + s * kC, a->alpha, a->g_logit);
+  if (check_launch(h, "attr_igloo_prep_kernel")) return 1;
+  if (launch_sgemm(h, a->g_logit, kLogitsLd, a->wqkT[s], kPatches, a->g_mpi, kPatches, n, kPatches, kPooled, nullptr, nullptr,
+                   nullptr, 0, st)) return 1;
+  IglooBwdParams P;
+  P.alpha = a->alpha; P.g_out = a->g_out + s * kC; P.route = a->route[s]; P.wvT = a->wvT[s]; P.g_mpi = a->g_mpi;
+  P.pos_start = a->pos_start[s]; P.slot_patch = a->slot_patch[s]; P.ent_w = h->ent_w[s];
+  P.y_rows = h->ybuf[0]; P.out = s ? a->f32a : a->gy1; P.blockmax = a->blockmax;
+  dim3 grid(kAttrPosBlocks, n);
+  if (s) attr_igloo_backward_kernel<true><<<grid, 256, 0, st>>>(P);
+  else attr_igloo_backward_kernel<false><<<grid, 256, 0, st>>>(P);
+  return check_launch(h, "attr_igloo_backward_kernel");
+}
+
+// One chunk: the unchanged forward step, strictly in order, then the backward pass over the state that step left behind
+// (ybuf[0] = y3, ybuf[1] = y2, q / logits of IGLOO#1, h1, h2).
+static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs, float* d_attr,
+                          cudaStream_t st) {
+  float* probs = d_probs ? d_probs : a->probs;
+  if (forward_step(h, d_ascii, nullptr, n, probs, nullptr, st)) return 1;
+  dim3 egrid((kTok + kEmbSeg - 1) / kEmbSeg, n), sgrid((kTok + kAttrSeg - 1) / kAttrSeg, n);
+  timer_mark(h, "attr_layer1", st);
+  embed_conv1_kernel<true><<<egrid, kEmbThreads, 0, st>>>(d_ascii, nullptr, h->conv1_table, h->conv1_triple, h->conv1_bias, a->y1, n, h->status);
+  if (check_launch(h, "embed_conv1_kernel")) return 1;
+  timer_mark(h, "attr_route1", st);
+  if (launch_route(h, a, 1, h->tm_act[0], n, st)) return 1;                  // y3
+  timer_mark(h, "attr_route0", st);
+  if (launch_route(h, a, 0, a->tm_y1, n, st)) return 1;                      // y1
+  timer_mark(h, "attr_head", st);
+  attr_head_backward_kernel<<<n, 256, 0, st>>>(probs, h->h1, h->h2, h->d2w, h->d1w, h->bn1_scale, h->d0w, h->bn0_scale, target, a->g_out);
+  if (check_launch(h, "attr_head_backward_kernel")) return 1;
+  timer_mark(h, "attr_igloo1", st);
+  if (launch_igloo_bwd(h, a, 1, n, st)) return 1;                            // -> fp32 g_z3, block maxima
+  attr_pack_kernel<<<sgrid, 256, 0, st>>>(a->f32a, a->blockmax, a->s_w, a->gz3);
+  if (check_launch(h, "attr_pack_kernel")) return 1;
+  timer_mark(h, "attr_conv3_bwd", st);
+  if (launch_conv_bwd(h, a, 1, a->tm_gz3, h->ybuf[1], nullptr, a->gz2, nullptr, n, st)) return 1;   // mask y2 -> s_w g_z2
+  timer_mark(h, "attr_igloo0", st);
+  if (launch_logits(h, 0, n, st)) return 1;                                  // IGLOO#0's logits (the tail overwrote them)
+  if (launch_igloo_bwd(h, a, 0, n, st)) return 1;                            // -> fp32 g_y1 (IGLOO#0 part)
+  timer_mark(h, "attr_conv2_bwd", st);
+  if (launch_conv_bwd(h, a, 0, a->tm_gz2, a->y1, a->gy1, nullptr, a->f32a, n, st)) return 1;        // + s_w g_y1, mask y1 -> s_w g_z1
+  timer_mark(h, "attr_layer1_attr", st);
+  layer1_attr_kernel<<<sgrid, 256, 0, st>>>(d_ascii, a->f32a, h->conv1_table, a->s_w, d_attr);
+  if (check_launch(h, "layer1_attr_kernel")) return 1;
+  timer_mark(h, "end", st);
+  for (int s = 0; s < 2; ++s) { h->attr_route[s] = a->route[s]; h->attr_rq[s] = a->rq[s]; }
+  h->attr_y1 = a->y1;
+  h->attr_mb = a->max_batch;
+  return 0;
+}
+
+static int attribute_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
+                         const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, float* d_probs, float* d_attr,
+                         void* stream) {
+  const std::string f(fn);
+  if (!h || !a) return fail(f + ": null handle or attribution context");
+  if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
+  if (n < 0) return fail(f + ": negative window count");
+  if (target < 0 || target > 2) return fail(f + ": target must be 0 (chromosome), 1 (plasmid) or 2 (virus)");
+  if (h->conv_impl != 0)
+    return fail(f + ": attributions need the tensor-core path (conv_impl = 0); the fp32 validation kernels have no backward pass");
+  if (h->debug_stop != 0) return fail(f + ": debug_stop must be 0");
+  if (n == 0) return 0;
+  if (!d_attr || (!d_ascii && (!d_seq || !d_win_start || !d_win_len))) return fail(f + ": null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  if (check_device_status(h)) return 1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int off = 0; off < n; off += a->max_batch) {
+    const int m = std::min(a->max_batch, n - off);
+    const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
+    if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
+    if (attribute_step(h, a, asc, m, target, probs_at(d_probs, off), d_attr + static_cast<size_t>(off) * kTok, st)) return 1;
+  }
+  return 0;
+}
+
+extern "C" int gnm_attribute_ascii(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs,
+                                   float* d_attr, void* stream) {
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_ascii: null buffer");
+  return attribute_any(h, a, "gnm_attribute_ascii", d_ascii, nullptr, nullptr, nullptr, n, target, d_probs, d_attr, stream);
+}
+extern "C" int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, const int64_t* d_win_start,
+                                     const int32_t* d_win_len, int n, int target, float* d_probs, float* d_attr, void* stream) {
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_windows: null buffer");
+  return attribute_any(h, a, "gnm_attribute_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, d_probs, d_attr, stream);
+}
+extern "C" long long gnm_attr_bytes_per_window(void) {
+  return static_cast<long long>(kTok) * (3 * kRowBytes + 2 * kC * 4) + 2LL * kPooled * kC * 5 +
+         4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + 4);
 }

@@ -1,0 +1,291 @@
+// Attribution pass: attr[t] = d log p_c / d x[t, tok[t]] for the one-hot input x of the first Conv1D (gradient x input), the
+// exact backward of the forward as written.  The tensor-core parts are instantiations of conv_t.cuh's body (kConvRoute: the
+// w_v pass storing where each pooled maximum sits; kConvBwd: the conv pass over time-reversed gradient rows against W[j]^T);
+// everything here runs on the CUDA cores in fp32 with a fixed summation order and no atomics, so a window's attributions do not
+// depend on its batch, its chunk or the GPU count.
+//
+// Backward, per window (DESIGN.md, "Attributions"):
+//   head     g_logits = e_c - p; back through Dense(3), BN1 + ReLU, Dense(512), BN0 + ReLU, Dense(512)    -> g_out0, g_out1
+//   IGLOO k  out = alpha^T q, alpha = softmax(mpi w_qk), q = maxpool8(y w_v)
+//            g_q[p,c] = alpha[p] g_out[c];  g_alpha[p] = sum_c g_out[c] q[p,c];  g_logit = alpha (g_alpha - <alpha, g_alpha>)
+//            g_mpi = w_qk g_logit (sgemm_epi_kernel);  g_y[t] = sum over the (p,c) routed to t of g_q[p,c] w_v[:,c]
+//                                                            + sum over the patch entries (i,k) on t of g_mpi[i] Wf[i,k,:]
+//   convs    g_z = g_y * lrelu'(y);  g_yprev[s] = sum_j g_z[s+5-j] W[j]^T  (conv_t_attr_kernel<kConvBwd>, rows reversed)
+//   layer 1  attr[t] = sum_{u=t}^{min(t+5,5996)} <g_z1[u], W1[t-u+5, tok[t], :]>
+// From g_z3 on, the gradient is carried times a per-window power of two s_w (max |g_z3| s_w in [0.25, 0.5)) so that the conv
+// operand formats (common.cuh) see values in their range; layer 1 divides it out.
+#pragma once
+#include "common.cuh"
+#include "encode.cuh"
+#include "igloo.cuh"
+
+namespace gnm {
+
+constexpr int kAttrPosBlock = 64;                                         // positions per CTA of the IGLOO backward kernel
+constexpr int kAttrPosBlocks = (kTok + kAttrPosBlock - 1) / kAttrPosBlock; // 94
+constexpr int kAttrSeg = 256;                                             // positions per CTA of the pack / layer-1 kernels
+
+// warp sum in a fixed butterfly order (every lane gets the same bits)
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+
+// ------------------------------------------------------------------------------------------------ head
+// One window per CTA, 256 threads.  g_out[w][0..255] = d log p_c / d h0 (h0 = [out0 | out1]), unscaled.
+__global__ void __launch_bounds__(256)
+attr_head_backward_kernel(const float* __restrict__ probs,      // [n][3]
+                          const float* __restrict__ h1, const float* __restrict__ h2,   // [n][512] (post-ReLU)
+                          const float* __restrict__ d2w,        // [512][3]
+                          const float* __restrict__ d1w,        // [512][512]
+                          const float* __restrict__ bn1_scale,  // [512]
+                          const float* __restrict__ d0w,        // [256][512]
+                          const float* __restrict__ bn0_scale,  // [512]
+                          int target, float* __restrict__ g_out) {
+  __shared__ float s_a1[kHidden], s_a0[kHidden];
+  const int w = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  float gl[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) gl[i] = (i == target ? 1.f : 0.f) - probs[static_cast<size_t>(w) * 3 + i];
+  for (int k = tid; k < kHidden; k += 256) {
+    const float g = fmaf(gl[2], d2w[k * 3 + 2], fmaf(gl[1], d2w[k * 3 + 1], gl[0] * d2w[k * 3]));
+    s_a1[k] = h2[static_cast<size_t>(w) * kHidden + k] > 0.f ? g * bn1_scale[k] : 0.f;
+  }
+  __syncthreads();
+  for (int j = warp; j < kHidden; j += 8) {                     // g_h1[j] = sum_k d1w[j][k] g_a1[k]
+    const float* row = d1w + static_cast<size_t>(j) * kHidden;
+    float a = 0.f;
+#pragma unroll 4
+    for (int k = lane; k < kHidden; k += 32) a = fmaf(row[k], s_a1[k], a);
+    a = warp_sum(a);
+    if (lane == 0) s_a0[j] = h1[static_cast<size_t>(w) * kHidden + j] > 0.f ? a * bn0_scale[j] : 0.f;
+  }
+  __syncthreads();
+  for (int m = warp; m < 256; m += 8) {                         // g_h0[m] = sum_j d0w[m][j] g_a0[j]
+    const float* row = d0w + static_cast<size_t>(m) * kHidden;
+    float a = 0.f;
+#pragma unroll 4
+    for (int j = lane; j < kHidden; j += 32) a = fmaf(row[j], s_a0[j], a);
+    a = warp_sum(a);
+    if (lane == 0) g_out[static_cast<size_t>(w) * 256 + m] = a;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ IGLOO: attention part
+// One window per CTA, 256 threads: alpha = softmax(logits) (as attention_kernel), g_alpha, g_logit -> [n][752] rows.
+__global__ void __launch_bounds__(256)
+attr_igloo_prep_kernel(const float* __restrict__ logits,    // [n][752]
+                       const float* __restrict__ q,         // [n][749][128]
+                       const float* __restrict__ g_out,     // [n][256] + column offset of this IGLOO kernel
+                       float* __restrict__ alpha_out,       // [n][752]
+                       float* __restrict__ g_logit) {       // [n][752]
+  __shared__ __align__(16) float s_go[kC];                        // read as float4
+  __shared__ float s_al[kPooled], s_ga[kPooled], s_red[8];
+  const int w = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* lrow = logits + static_cast<size_t>(w) * kLogitsLd;
+  if (tid < kC) s_go[tid] = g_out[static_cast<size_t>(w) * 256 + tid];
+  float m = -INFINITY;
+  for (int g = tid; g < kPooled; g += 256) { const float v = lrow[g]; s_al[g] = v; m = fmaxf(m, v); }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
+  if (lane == 0) s_red[warp] = m;
+  __syncthreads();
+  m = s_red[0];
+  for (int i = 1; i < 8; ++i) m = fmaxf(m, s_red[i]);
+  __syncthreads();
+  float sum = 0.f;
+  for (int g = tid; g < kPooled; g += 256) { const float e = expf(s_al[g] - m); s_al[g] = e; sum += e; }
+  sum = warp_sum(sum);
+  if (lane == 0) s_red[warp] = sum;
+  __syncthreads();
+  sum = ((s_red[0] + s_red[1]) + (s_red[2] + s_red[3])) + ((s_red[4] + s_red[5]) + (s_red[6] + s_red[7]));
+  const float inv = 1.f / sum;
+  __syncthreads();
+  for (int g = tid; g < kPooled; g += 256) s_al[g] *= inv;
+  // g_alpha[p] = sum_c g_out[c] q[p,c]: one warp per pooled row, lanes over channels
+  const float4 go = reinterpret_cast<const float4*>(s_go)[lane];
+  for (int g = warp; g < kPooled; g += 8) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(q + (static_cast<size_t>(w) * kPooled + g) * kC) + lane);
+    const float a = warp_sum(fmaf(go.w, v.w, fmaf(go.z, v.z, fmaf(go.y, v.y, go.x * v.x))));
+    if (lane == 0) s_ga[g] = a;
+  }
+  __syncthreads();
+  float dot = 0.f;
+  for (int g = tid; g < kPooled; g += 256) dot = fmaf(s_al[g], s_ga[g], dot);
+  dot = warp_sum(dot);
+  if (lane == 0) s_red[warp] = dot;
+  __syncthreads();
+  dot = ((s_red[0] + s_red[1]) + (s_red[2] + s_red[3])) + ((s_red[4] + s_red[5]) + (s_red[6] + s_red[7]));
+  for (int g = tid; g < kLogitsLd; g += 256) {
+    const size_t o = static_cast<size_t>(w) * kLogitsLd + g;
+    alpha_out[o] = g < kPooled ? s_al[g] : 0.f;
+    g_logit[o] = g < kPooled ? s_al[g] * (s_ga[g] - dot) : 0.f;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ IGLOO: g_y
+// grid (94 position blocks, n), 256 threads; warp v handles pool group 8 b + v of the block, i.e. positions 8 (8 b + v) + r.
+// Lane l holds output channels 4 l .. 4 l + 3.
+//   value path: for each row r, the channels c routed to it (ballots over c = lane + 32 i: ascending c), acc += g_q[c] w_v^T[c]
+//   patch path: the patch entries on the position (slots pos_start[t] .. pos_start[t+1] of the position-sorted packing, in
+//               slot order), acc += g_mpi[patch] * 32 * ent_w[slot]   (ent_w holds Wf / 32, api.cu pack_patches)
+// kLast = 1 (IGLOO#1 on y3): g_z3 = g_y3 * lrelu'(y3) to fp32 rows, and the block's max |g_z3| to blockmax[w][b];
+// kLast = 0 (IGLOO#0 on y1): g_y1 to fp32 rows (conv2's backward epilogue adds it and applies the mask).
+struct IglooBwdParams {
+  const float* alpha;          // [n][752]
+  const float* g_out;          // [n][256] (already offset to this IGLOO kernel's 128 columns)
+  const uint8_t* route;        // [n][749][128]
+  const float* wvT;            // [128 c][128 k]
+  const float* g_mpi;          // [n][2100]
+  const int32_t* pos_start;    // [5998] CSR over positions into the sorted entry slots
+  const int32_t* slot_patch;   // [8400] patch index of every entry slot
+  const float* ent_w;          // [slots][128]
+  const uint8_t* y_rows;       // kLast: y3 activation rows (mask)
+  float* out;                  // [n][5997][128]
+  float* blockmax;             // kLast: [n][94]
+};
+
+template <bool kLast>
+__global__ void __launch_bounds__(256)
+attr_igloo_backward_kernel(const IglooBwdParams P) {
+  __shared__ float s_gq[8][kC];
+  __shared__ float s_max[8];
+  const int w = blockIdx.y, b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int pg = b * 8 + warp;                                   // pool group of this warp
+  const float4* wvT4 = reinterpret_cast<const float4*>(P.wvT);
+  const float4* ew4 = reinterpret_cast<const float4*>(P.ent_w);
+  float amax = 0.f;
+  uint32_t rt[4] = {0u, 0u, 0u, 0u};
+  if (pg < kPooled) {
+    const float al = P.alpha[static_cast<size_t>(w) * kLogitsLd + pg];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = lane + 32 * i;
+      s_gq[warp][c] = al * P.g_out[static_cast<size_t>(w) * 256 + c];
+      rt[i] = P.route[(static_cast<size_t>(w) * kPooled + pg) * kC + c];
+    }
+  }
+  __syncwarp();
+  for (int r = 0; r < kPool; ++r) {
+    const int t = pg * kPool + r;
+    if (t >= kTok) break;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (pg < kPooled) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        uint32_t msk = __ballot_sync(0xffffffffu, rt[i] == static_cast<uint32_t>(r));
+        while (msk) {
+          const int c = 32 * i + __ffs(msk) - 1;
+          msk &= msk - 1;
+          const float gq = s_gq[warp][c];
+          const float4 v = __ldg(wvT4 + c * (kC / 4) + lane);
+          acc.x = fmaf(gq, v.x, acc.x); acc.y = fmaf(gq, v.y, acc.y); acc.z = fmaf(gq, v.z, acc.z); acc.w = fmaf(gq, v.w, acc.w);
+        }
+      }
+    }
+    const int e1 = P.pos_start[t + 1];
+    for (int e = P.pos_start[t]; e < e1; ++e) {
+      const float gm = kActScale * P.g_mpi[static_cast<size_t>(w) * kPatches + P.slot_patch[e]];
+      const float4 v = __ldg(ew4 + static_cast<size_t>(e) * (kC / 4) + lane);
+      acc.x = fmaf(gm, v.x, acc.x); acc.y = fmaf(gm, v.y, acc.y); acc.z = fmaf(gm, v.z, acc.z); acc.w = fmaf(gm, v.w, acc.w);
+    }
+    const size_t row = static_cast<size_t>(w) * kTok + t;
+    if (kLast) {
+      const __half2* yh = reinterpret_cast<const __half2*>(P.y_rows + row * kRowBytes + kOffHi16) + 2 * lane;
+      const float2 y01 = __half22float2(yh[0]), y23 = __half22float2(yh[1]);
+      acc.x = y01.x > 0.f ? acc.x : acc.x * kLeaky; acc.y = y01.y > 0.f ? acc.y : acc.y * kLeaky;
+      acc.z = y23.x > 0.f ? acc.z : acc.z * kLeaky; acc.w = y23.y > 0.f ? acc.w : acc.w * kLeaky;
+      amax = fmaxf(amax, fmaxf(fmaxf(fabsf(acc.x), fabsf(acc.y)), fmaxf(fabsf(acc.z), fabsf(acc.w))));
+    }
+    reinterpret_cast<float4*>(P.out + row * kC)[lane] = acc;
+  }
+  if (kLast) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, off));
+    if (lane == 0) s_max[warp] = amax;
+    __syncthreads();
+    if (tid == 0) {
+      float m = s_max[0];
+      for (int i = 1; i < 8; ++i) m = fmaxf(m, s_max[i]);
+      P.blockmax[static_cast<size_t>(w) * kAttrPosBlocks + b] = m;
+    }
+  }
+}
+
+// s_w = 2^k with max |g_z3| * s_w in [0.25, 0.5) (1 for an all-zero gradient)
+__device__ __forceinline__ float attr_scale_of(float gmax) {
+  if (!(gmax > 0.f) || !isfinite(gmax)) return 1.f;
+  int e;
+  frexpf(gmax, &e);                                              // gmax = m 2^e, m in [0.5, 1)
+  return ldexpf(1.f, max(-120, min(120, -e - 1)));
+}
+
+// fp32 g_z3 rows (natural order) -> conv operand rows (hi16 | - | e4m3 pairs) of s_w * g_z3 at row 5996 - t, the input of
+// conv3's backward pass.  grid (24, n), 256 threads, one warp per position; block 0 also stores s_w.
+__global__ void __launch_bounds__(256)
+attr_pack_kernel(const float* __restrict__ g, const float* __restrict__ blockmax, float* __restrict__ s_w_out,
+                 uint8_t* __restrict__ rows_out) {
+  __shared__ float s_sw;
+  const int w = blockIdx.y, t0 = blockIdx.x * kAttrSeg, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    float m = 0.f;
+    for (int i = 0; i < kAttrPosBlocks; ++i) m = fmaxf(m, blockmax[static_cast<size_t>(w) * kAttrPosBlocks + i]);
+    s_sw = attr_scale_of(m);
+    if (blockIdx.x == 0) s_w_out[w] = s_sw;
+  }
+  __syncthreads();
+  const float sc = kActScale * s_sw;
+  const int i_end = min(kAttrSeg, kTok - t0);
+  for (int i = warp; i < i_end; i += 8) {
+    const int t = t0 + i;
+    float4 a = reinterpret_cast<const float4*>(g + (static_cast<size_t>(w) * kTok + t) * kC)[lane];
+    a.x *= sc; a.y *= sc; a.z *= sc; a.w *= sc;
+    __half2 h01, h23, l01, l23;
+    split2_f16(a.x, a.y, h01, l01);
+    split2_f16(a.z, a.w, h23, l23);
+    const float2 fa = __half22float2(h01), fb = __half22float2(h23);
+    uint8_t* rowp = rows_out + (static_cast<size_t>(w) * kTok + (kTok - 1 - t)) * kRowBytes;
+    *reinterpret_cast<uint2*>(rowp + kOffHi16 + lane * 8) =
+        make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
+    *reinterpret_cast<uint2*>(rowp + kOffP8 + lane * 8) = make_uint2(
+        static_cast<uint32_t>(pack_e4m3x2((a.x - fa.x) * kLo8Scale, fa.x * kHi8Scale)) |
+            (static_cast<uint32_t>(pack_e4m3x2((a.y - fa.y) * kLo8Scale, fa.y * kHi8Scale)) << 16),
+        static_cast<uint32_t>(pack_e4m3x2((a.z - fb.x) * kLo8Scale, fb.x * kHi8Scale)) |
+            (static_cast<uint32_t>(pack_e4m3x2((a.w - fb.y) * kLo8Scale, fb.y * kHi8Scale)) << 16));
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ layer 1
+// attr[t] = (1 / s_w) sum_{u=t}^{min(t+5,5996)} <g_z1[u], W1[t-u+5, tok[t], :]>, tok from the window's bytes (token 0 = a
+// 4-mer with a non-ACGT base, a real one-hot row).  grid (24, n), 256 threads, one warp per position, u ascending.
+__global__ void __launch_bounds__(256)
+layer1_attr_kernel(const uint8_t* __restrict__ ascii, const float* __restrict__ g_z1, const float* __restrict__ table,
+                   const float* __restrict__ s_w, float* __restrict__ attr) {
+  __shared__ int16_t s_tok[kAttrSeg];
+  const int w = blockIdx.y, t0 = blockIdx.x * kAttrSeg, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  {
+    const int t = t0 + threadIdx.x;
+    if (t < kTok) {
+      const uint8_t* s = ascii + static_cast<size_t>(w) * kWindow + t;
+      s_tok[threadIdx.x] = static_cast<int16_t>(kmer_token(base_code(s[0]), base_code(s[1]), base_code(s[2]), base_code(s[3])));
+    }
+  }
+  __syncthreads();
+  const float inv = 1.f / s_w[w];
+  const int i_end = min(kAttrSeg, kTok - t0);
+  for (int i = warp; i < i_end; i += 8) {
+    const int t = t0 + i, tk = s_tok[i];
+    float a = 0.f;
+    const int u_end = min(t + 5, kTok - 1);
+    for (int u = t; u <= u_end; ++u) {
+      const float4 gz = reinterpret_cast<const float4*>(g_z1 + (static_cast<size_t>(w) * kTok + u) * kC)[lane];
+      const float4 wr = __ldg(reinterpret_cast<const float4*>(table + (static_cast<size_t>(t - u + 5) * kVocab + tk) * kC) + lane);
+      a = fmaf(gz.w, wr.w, fmaf(gz.z, wr.z, fmaf(gz.y, wr.y, fmaf(gz.x, wr.x, a))));
+    }
+    a = warp_sum(a);
+    if (lane == 0) attr[static_cast<size_t>(w) * kTok + t] = a * inv;
+  }
+}
+
+}  // namespace gnm

@@ -111,11 +111,23 @@ template <bool kWvMode> __device__ __forceinline__ constexpr int region_src(int 
                  : (r == 0 ? kOffHi16 : r == 1 ? kOffHi16 + 128 : r == 2 ? kOffP8 : kOffP8 + 128);
 }
 
-// tm_w: the weight pack with a 64-row box, i.e. one warpgroup's half of a 16 KB stage per load
-template <bool kWvMode>
-__global__ void __launch_bounds__(kConvThreads, 1)
-conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant__ CUtensorMap tm_w,
-              const ConvTcParams p) {
+// Epilogue modes of the kernel body.  kConvFwd / kConvWv are the forward's conv_t_kernel<false> / <true>.  The attribution
+// pass (attr.cuh) adds two: kConvRoute is the w_v pass with an epilogue that also stores WHERE each pooled maximum sits, and
+// kConvBwd is the conv pass run over time-reversed gradient rows against W[j]^T (no bias; lrelu' of the forward activation at the
+// mirrored row; optional fp32 rows added first; fp32 or operand-format output).  MMA loop, producers and rings are shared.
+constexpr int kConvFwd = 0, kConvWv = 1, kConvRoute = 2, kConvBwd = 3;
+struct ConvAttrExt {
+  uint8_t* route_out;         // kConvRoute: [n][749][128] row (0..7) of each pooled maximum, the first one on ties
+  const uint8_t* mask_rows;   // kConvBwd: forward activation rows [n][5997][768 B]; the sign of hi16 at row 5996 - r gives lrelu'
+  const float* add_rows;      // kConvBwd: fp32 rows [n][5997][128] (natural order) added as s_w * add before the mask, or nullptr
+  const float* s_w;           // kConvBwd: [n] per-window gradient scale (with add_rows)
+  float* f32_out;             // kConvBwd: fp32 rows [n][5997][128] at the mirrored (natural) row, or nullptr: operand rows p.y_out
+};
+
+template <int kMode>
+__device__ __forceinline__ void conv_t_body(const CUtensorMap* tm_act_p, const CUtensorMap* tm_w_p, const ConvTcParams& p,
+                                            const ConvAttrExt& x) {
+  constexpr bool kWvMode = kMode == kConvWv || kMode == kConvRoute;
   constexpr int kStagesU = kWvMode ? kWvStages : kConvStages;     // stages per unit
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -133,8 +145,8 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
   const int n_units = p.n_tiles;      // n_windows * 24
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tm_act);
-    tma_prefetch_desc(&tm_w);
+    tma_prefetch_desc(tm_act_p);
+    tma_prefetch_desc(tm_w_p);
     for (int i = 0; i < kNumRegions; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
     for (int i = 0; i < 2 * kTWSlots; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
     fence_barrier_init();
@@ -153,7 +165,7 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
             const uint32_t wphase = ((wcount + q) / kTWSlots) & 1;
             mbar_wait(&w_empty[s], wphase ^ 1, p.status, 110 + s);
             mbar_arrive_expect_tx(&w_full[s], kBHalf);
-            tma_load_2d_hint(s_w + s * kBHalf, &tm_w, &w_full[s], 0, conv_pack_stage<kWvMode>(q) * 128 + 64 * g, pol);
+            tma_load_2d_hint(s_w + s * kBHalf, tm_w_p, &w_full[s], 0, conv_pack_stage<kWvMode>(q) * 128 + 64 * g, pol);
           }
     } else if (wq == 1 && elect_one()) {
       // =================================================================== activation producer
@@ -169,8 +181,8 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
           mbar_wait(&a_empty[r], ph ^ 1, p.status, 100 + r);
           mbar_arrive_expect_tx(&a_full[r], kA2Region);
           uint8_t* dst = s_a + r * kA2Region;
-          tma_load_3d_hint(dst, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5, w, pol);
-          tma_load_3d_hint(dst + kARegion, &tm_act, &a_full[r], region_src<kWvMode>(r), t0 - 5 + kSlabRows, w, pol);
+          tma_load_3d_hint(dst, tm_act_p, &a_full[r], region_src<kWvMode>(r), t0 - 5, w, pol);
+          tma_load_3d_hint(dst + kARegion, tm_act_p, &a_full[r], region_src<kWvMode>(r), t0 - 5 + kSlabRows, w, pol);
         }
       }
     }
@@ -180,7 +192,7 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
     const uint32_t a_base = smem_u32(s_a);
     const uint32_t w_base = smem_u32(s_w);
     const int ch0 = g * 64 + wq * 16 + (lane >> 2);        // accumulator rows of this thread: channels ch0 and ch0 + 8
-    const float bias0 = kWvMode ? 0.f : p.bias[ch0], bias1 = kWvMode ? 0.f : p.bias[ch0 + 8];
+    const float bias0 = (kWvMode || kMode == kConvBwd) ? 0.f : p.bias[ch0], bias1 = (kWvMode || kMode == kConvBwd) ? 0.f : p.bias[ch0 + 8];
     const float oscale = p.out_scale;
     float amax = 0.f;                                      // largest |Y| this thread produced (range check, common.cuh)
     int it = 0;
@@ -263,7 +275,38 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
       tq = clock64();
       t_mma += tq - t_unit;
       // ===================================================================== epilogue (overlaps the partner warpgroup's MMAs)
-      if (kWvMode) {
+      if constexpr (kMode == kConvRoute) {
+        // as below, with the row of the maximum carried along: a lane's two positions 2 (lane % 4) + e, then the lane quad;
+        // a later row wins only if strictly larger, so ties go to the first row (the value is the forward's q bit for bit)
+        const int r0 = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          float v[2];
+          int ix[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float a = d[4 * j + 2 * h], b = d[4 * j + 2 * h + 1];
+            v[h] = b > a ? b : a;
+            ix[h] = b > a ? r0 + 1 : r0;
+          }
+#pragma unroll
+          for (int off = 1; off <= 2; off <<= 1)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float pv = __shfl_xor_sync(0xffffffffu, v[h], off);
+              const int pi = __shfl_xor_sync(0xffffffffu, ix[h], off);
+              if (pv > v[h] || (pv == v[h] && pi < ix[h])) { v[h] = pv; ix[h] = pi; }
+            }
+          const int gg = (t0 >> 3) + j;
+          if ((lane & 3) == 0 && gg < kPooled) {
+            const size_t o = (static_cast<size_t>(w) * kPooled + gg) * kC;
+            p.q_out[o + ch0] = v[0] * oscale;
+            p.q_out[o + ch0 + 8] = v[1] * oscale;
+            x.route_out[o + ch0] = static_cast<uint8_t>(ix[0]);
+            x.route_out[o + ch0 + 8] = static_cast<uint8_t>(ix[1]);
+          }
+        }
+      } else if (kWvMode) {
         // pool group j of the unit = accumulator columns 8 j .. 8 j + 7 = registers 4 j + 2 h + e of the lane quad
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
@@ -277,6 +320,25 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
             qrow[ch0 + 8] = m1 * oscale;
           }
         }
+      } else if (kMode == kConvBwd && x.f32_out) {
+        // backward pass into fp32 rows: accumulator row r is the gradient at position 5996 - r; plain 4-byte stores
+        const float sw = x.add_rows ? x.s_w[w] : 0.f;
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int pos = t0 + 8 * j + 2 * (lane & 3) + e;
+              if (pos < kTok) {
+                const int ch = ch0 + 8 * h;
+                const size_t row = static_cast<size_t>(w) * kTok + (kTok - 1 - pos);
+                float v = d[4 * j + 2 * h + e] * oscale;
+                if (x.add_rows) v = fmaf(sw, x.add_rows[row * kC + ch], v);
+                const __half m = *reinterpret_cast<const __half*>(x.mask_rows + row * kRowBytes + kOffHi16 + 2 * ch);
+                x.f32_out[row * kC + ch] = __hgt(m, __float2half(0.f)) ? v : v * kLeaky;
+              }
+            }
       } else {
         // Column group j of the accumulator is this warp's 16 channels x 8 positions 8 j .. 8 j + 7.  Per output plane that is
         // 8 rows x 32 contiguous bytes, both planes 512 B: one 16-byte store per lane.  Both planes are b16 per (channel,
@@ -299,8 +361,18 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const float bias = h ? bias1 : bias0;
-            const float y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
-            const float y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
+            float y0, y1;
+            if constexpr (kMode == kConvBwd) {
+              // gradient rows, time-reversed in and out: lrelu' of the forward activation at the mirrored position
+              y0 = y1 = 0.f;
+              const int pos = t0 + 8 * j + 2 * (lane & 3);
+              const __half* mrow = reinterpret_cast<const __half*>(x.mask_rows + (static_cast<size_t>(w) * kTok + (kTok - 1 - pos)) * kRowBytes + kOffHi16) + ch0 + 8 * h;
+              if (pos < kTok) y0 = kActScale * d[4 * j + 2 * h] * oscale * (__hgt(mrow[0], __float2half(0.f)) ? 1.f : kLeaky);
+              if (pos + 1 < kTok) y1 = kActScale * d[4 * j + 2 * h + 1] * oscale * (__hgt(mrow[-kRowBytes / 2], __float2half(0.f)) ? 1.f : kLeaky);
+            } else {
+              y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
+              y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
+            }
             amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
             if (p.out_fp8) {
               const __half2 hh = __floats2half2_rn(y0, y1);
@@ -326,13 +398,30 @@ conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant_
       }
       t_epi += clock64() - tq;
     }
-    if (!kWvMode) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
+    if constexpr (kMode == kConvBwd) { if (!x.f32_out) flag_act_overflow(p.status, amax, kHi8Limit, 0); }
+    else if (!kWvMode) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
     if (p.dbg && wq == 0 && lane == 0) {     // include/gnm.h, "conv_dbg"
       long long* dd = p.dbg + blockIdx.x * 8;
       if (g == 0) { dd[0] = clock64() - t_begin; dd[1] = t_mma; dd[2] = w_a; dd[3] = w_w; dd[4] = it; dd[6] = t_epi; }
       else { dd[5] = t_mma; dd[7] = t_epi; }
     }
   }
+}
+
+// tm_w: the weight pack with a 64-row box, i.e. one warpgroup's half of a 16 KB stage per load
+template <bool kWvMode>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_t_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant__ CUtensorMap tm_w,
+              const ConvTcParams p) {
+  conv_t_body<kWvMode ? kConvWv : kConvFwd>(&tm_act, &tm_w, p, ConvAttrExt{});
+}
+
+// the attribution pass's instantiations (attr.cuh): kMode = kConvRoute or kConvBwd
+template <int kMode>
+__global__ void __launch_bounds__(kConvThreads, 1)
+conv_t_attr_kernel(const __grid_constant__ CUtensorMap tm_act, const __grid_constant__ CUtensorMap tm_w,
+                   const ConvTcParams p, const ConvAttrExt x) {
+  conv_t_body<kMode>(&tm_act, &tm_w, p, x);
 }
 
 }  // namespace gnm

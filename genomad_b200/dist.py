@@ -109,9 +109,10 @@ def gather_window_probs(local_probs, n_total: int, world_size: int, group=None):
 
 
 def collect_window_probs(local_probs, n_total: int, info: "DistInfo", send=None, recv=None):
-    """Contiguous shards [W_local, 3] -> [n_total, 3] in global window order on rank 0 (None on the other ranks): each rank
-    sends its shard to rank 0, which receives them in rank order.  Only rank 0 ever holds every window (a score profile can
-    have far more windows than the contig pass)."""
+    """Contiguous shards of per-window rows [W_local, width] -> [n_total, width] in global window order on rank 0 (None on the
+    other ranks): each rank sends its shard to rank 0, which receives them in rank order.  Only rank 0 ever holds every window
+    (a score profile can have far more windows than the contig pass).  Any row width: the class scores (3) or the
+    attributions (5,997); a rank without windows passes a [0, width] tensor."""
     import torch
     if info.world_size == 1:
         return local_probs

@@ -82,6 +82,12 @@ EXPORTS = {
     "gnm_debug_fetch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_pack_patches": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int), C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.c_void_p]),
+    "gnm_attr_create": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]),
+    "gnm_attr_destroy": (C.c_int, [C.c_void_p]),
+    "gnm_attr_bytes_per_window": (C.c_longlong, []),
+    "gnm_attribute_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
     "gnm_fasta_last_error": (C.c_char_p, []),
     "gnm_fasta_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_open_gz": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -147,6 +153,32 @@ class WindowScores(NamedTuple):
     offsets: "object"         # int32 [n_contigs + 1], CSR: the windows of contig c are [offsets[c], offsets[c+1])
 
 
+class Attributions(NamedTuple):
+    """Result of Classifier.attribute_contigs (cuda tensors); the windows are those of window_scores at stride 6000."""
+    probs: "object"           # float32 [W, 3]
+    contig: "object"          # int32 [W]
+    start: "object"           # int64 [W], first byte in the contig (0-based, before stripping n/N)
+    length: "object"          # int32 [W]
+    offsets: "object"         # int32 [n_contigs + 1], CSR
+    attr: "object"            # float32 [W, 5997]: d log p_target / d one-hot token, token t = bases t .. t+3 of the window
+
+
+CLASSES = ("chromosome", "plasmid", "virus")
+ATTR_MAX_BATCH = 256             # windows per attribution chunk (attribution context, ~21 MB per window)
+
+
+def class_index(target) -> int:
+    """0 / 1 / 2 or "chromosome" / "plasmid" / "virus" -> class index."""
+    if isinstance(target, str):
+        if target not in CLASSES:
+            raise ValueError(f"target must be one of {CLASSES}, not {target!r}")
+        return CLASSES.index(target)
+    t = int(target)
+    if t not in (0, 1, 2):
+        raise ValueError(f"target must be 0, 1 or 2, not {t}")
+    return t
+
+
 class Classifier:
     """
     The IGLOO1D classifier on one H100.
@@ -180,6 +212,9 @@ class Classifier:
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
+        if getattr(self, "_attr", None):
+            self.lib.gnm_attr_destroy(self._attr)
+            self._attr = None
         if getattr(self, "_h", None):
             self.lib.gnm_destroy(self._h)
             self._h = C.c_void_p()
@@ -440,6 +475,68 @@ class Classifier:
         rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
         return WindowScores(probs, contig, rel, length, woff)
 
+    # ------------------------------------------------------------------ attributions
+    def _attr_ctx(self, max_batch: Optional[int] = None):
+        """The attribution workspace, created on first use (ATTR_MAX_BATCH windows per chunk, capped at the handle's max_batch)."""
+        if getattr(self, "_attr", None):
+            return self._attr
+        mb = min(int(max_batch or ATTR_MAX_BATCH), self.max_batch)
+        ctx = C.c_void_p()
+        with self._torch.cuda.device(self.device):
+            rc = self.lib.gnm_attr_create(self._h, mb, C.byref(ctx))
+        if rc != 0:
+            msg = self.lib.gnm_last_error().decode(errors="replace")
+            if ctx:
+                self.lib.gnm_attr_destroy(ctx)
+            raise GnmError(msg)
+        self._attr = ctx
+        self.attr_max_batch = mb
+        return ctx
+
+    def attribute_ascii(self, ascii_windows, target):
+        """uint8 cuda [n, 6000], target class (0 / 1 / 2 or its name) -> (probabilities float32 [n, 3], attributions float32
+        [n, 5997]): attr[i, t] = d log p_target / d x[t, tok[t]] for the one-hot tokens x of window i (gnm_attribute_ascii).
+        The probabilities are bitwise those of predict_ascii."""
+        t = self._torch
+        a = ascii_windows.contiguous()
+        assert a.dtype == t.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        c = class_index(target)
+        probs = t.empty((a.shape[0], 3), dtype=t.float32, device=a.device)
+        attr = t.empty((a.shape[0], TOKENS), dtype=t.float32, device=a.device)
+        if a.shape[0]:
+            _check(self.lib, self.lib.gnm_attribute_ascii(self._h, self._attr_ctx(), a.data_ptr(), a.shape[0], c,
+                                                          probs.data_ptr(), attr.data_ptr(), self._stream()))
+        return probs, attr
+
+    def attribute_windows(self, seq_u8, win_start, win_len, target):
+        """Planned windows of a sequence buffer (see predict_windows) -> (probabilities [W, 3], attributions [W, 5997])."""
+        t = self._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        c = class_index(target)
+        n = start.numel()
+        probs = t.empty((n, 3), dtype=t.float32, device=seq_u8.device)
+        attr = t.empty((n, TOKENS), dtype=t.float32, device=seq_u8.device)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_windows(self._h, self._attr_ctx(), seq_u8.data_ptr(), start.data_ptr(),
+                                                            length.data_ptr(), n, c, probs.data_ptr(), attr.data_ptr(),
+                                                            self._stream()))
+        return probs, attr
+
+    def attribute_contigs(self, seqs, target, single_window: bool = False) -> "Attributions":
+        """Attributions of the reference's windows of every contig (the windows whose mean is the contig score), with their
+        place in the contig.  seqs: as for classify_contigs.  Token t of a window covers its bases t .. t+3; sum or spread the
+        values over those bases for a per-base track."""
+        t = self._torch
+        seq, offs = self.contig_buffers(seqs)
+        start, length, woff = self.contig_windows(seq, offs, single_window)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        probs, attr = self.attribute_windows(seq, start, length, target)
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        return Attributions(probs, contig, rel, length, woff, attr)
+
     # ------------------------------------------------------------------ host-buffer API
     def classify_host(self, ascii_windows: np.ndarray) -> np.ndarray:
         """numpy uint8 [n, 6000] (host) -> numpy float32 [n, 3]; copies overlap compute inside the library."""
@@ -473,7 +570,9 @@ class Classifier:
         t = self._torch
         shapes = {"buf0": (n, TOKENS, 128), "buf1": (n, TOKENS, 128), "q0": (n, 749, 128), "q1": (n, 749, 128),
                   "mpi0": (n, 2100), "mpi1": (n, 2100), "h0": (n, 256), "h1": (n, 512), "h2": (n, 512), "logits": (n, 752),
-                  "conv_dbg": (self.get_option("num_sms"), 16)}
-        out = t.empty(shapes[which], dtype=t.float32, device=self._dev())
+                  "conv_dbg": (self.get_option("num_sms"), 16), "routeq0": (n, 749, 128), "routeq1": (n, 749, 128),
+                  "route0": (n, 749, 128), "route1": (n, 749, 128), "attr_y1": (n, TOKENS, 128)}
+        dtype = t.uint8 if which in ("route0", "route1") else t.float32
+        out = t.empty(shapes[which], dtype=dtype, device=self._dev())
         _check(self.lib, self.lib.gnm_debug_fetch(self._h, which.encode(), n, out.data_ptr(), self._stream()))
         return out

@@ -91,7 +91,7 @@ def _device(clf):
 
 
 def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather",
-                     embeddings: bool = False, window_probs: bool = False):
+                     embeddings: bool = False, window_probs: bool = False, attributions: "dict | None" = None):
     """
     Indexed FASTA -> float32 [n_contigs, 3] per-contig mean (identical on all ranks).
 
@@ -110,6 +110,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
 
     With `window_probs`, the per-window probabilities float32 [n_windows, 3] are collected on rank 0 (None on the other
     ranks) and returned last.  With offsets None there is no per-contig reduction: only those are returned.
+
+    With `attributions` ({"target": class name}), every chunk goes through the attribution calls instead
+    (Classifier.attribute_ascii: the same forward step, so bitwise the same probabilities, plus each window's 5,997
+    attributions in a device buffer of this rank's shard); they are collected on rank 0 in window order and stored as
+    attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -119,15 +124,32 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     keep, bufs = zip(*(_pinned_chunk(min(chunk, max(1, end - start))) for _ in range(2)))
     out_t = _pinned_probs(max(1, end - start))
     dev = _device(clf)
-    run = clf.classify_host_into
+
+    def sync():
+        if dev.type == "cuda":
+            torch.cuda.current_stream(dev).synchronize()
+
+    def run(win, m, row):                                    # one chunk: windows win[:m] are rows [row, row + m) of the shard
+        clf.classify_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12)
     if embeddings:
         shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
         d_emb = torch.empty((min(chunk, max(1, end - start)), 512), dtype=torch.float32, device=dev)
+        if attributions is None:
+            def run(win, m, row):                            # the worker owns d_emb: one chunk at a time
+                clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, d_emb.data_ptr())
+                shard.add(d_emb[:m])
+                sync()
+    if attributions is not None:
+        d_attr = torch.empty((end - start, ATTR_TOKENS), dtype=torch.float32, device=dev)
 
-        def run(ptr, m, out_ptr):                            # the worker owns d_emb: one chunk at a time
-            clf.embed_host_into(ptr, m, out_ptr, d_emb.data_ptr())
-            shard.add(d_emb[:m])
-            torch.cuda.current_stream(dev).synchronize()
+        def run(win, m, row):                                # probabilities and attributions from the attribution calls
+            d_win = torch.from_numpy(win[:m]).to(dev)
+            probs, attr = clf.attribute_ascii(d_win, attributions["target"])
+            out_t[row: row + m].copy_(probs)
+            d_attr[row: row + m].copy_(attr)
+            if embeddings:
+                shard.add(clf.embed_ascii(d_win)[1])
+            sync()
     futures = []
     with ThreadPoolExecutor(max_workers=1) as gpu:
         for i, a in enumerate(range(start, end, chunk)):
@@ -136,7 +158,7 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 futures[i - 2].result()                          # buffer i%2 is free again
                 parsed.release_before(a - chunk)
             win = parsed.export_windows(a, b - a, bufs[i % 2])
-            futures.append(gpu.submit(run, win.ctypes.data, b - a, out_t.data_ptr() + (a - start) * 12))
+            futures.append(gpu.submit(run, win, b - a, a - start))
         for f in futures:
             f.result()
     del keep
@@ -151,6 +173,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     if window_probs:
         full = gdist.collect_window_probs(local_t, n, info)
         out.append(full.cpu().numpy() if full is not None else None)
+    if attributions is not None:
+        full = gdist.collect_window_probs(d_attr, n, info)
+        attributions["attr"] = full.cpu().numpy() if full is not None else None
     return out[0] if len(out) == 1 else tuple(out)
 
 
@@ -238,22 +263,24 @@ def _window_scores_current(npz_path: Path, tsv_path: Path, stride: int) -> bool:
         return False
 
 
-def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, embeddings: bool):
+def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, embeddings: bool,
+                         attributions=None):
     """Per-contig scores (+ embeddings) and the per-window scores at `stride`: (preds, emb or None, offsets, starts, lengths,
     probs); the window arrays are None off rank 0.  At stride 6000 without --single-window the profile windows are the
     contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list."""
     emb = None
+    ak = {"attributions": attributions} if attributions is not None else {}      # option off: the call of before
     if stride == sequence.WINDOW and not single_window:
-        res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True)
+        res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True, **ak)
         preds, probs = res[0], res[-1]
         if embeddings:
             emb = res[1]
         starts, lengths = parsed.spans() if info.is_main else (None, None)
         return preds, emb, index.offsets, starts, lengths, probs
     if embeddings:
-        preds, emb = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=True)
+        preds, emb = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=True, **ak)
     else:
-        preds = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce)
+        preds = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, **ak)
     wl = parsed.windows(stride)
     try:
         probs = _classify_parsed(clf, wl, None, info, window_probs=True)
@@ -261,6 +288,45 @@ def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, i
     finally:
         wl.close()
     return preds, emb, offsets, starts, lengths, probs
+
+
+ATTR_TOKENS = 5997
+ATTR_CLASSES = ("chromosome", "plasmid", "virus")
+
+
+def attributions_target(value=None):
+    """The class whose attributions are written (``--write-attributions CLASS`` / GENOMAD_B200_ATTRIBUTIONS=CLASS /
+    main(..., write_attributions=CLASS)), or None.  value None: the environment decides; False / "" / "0": off."""
+    if value is None:
+        value = os.environ.get("GENOMAD_B200_ATTRIBUTIONS", "")
+    if value is False or value is None or str(value).strip() in ("", "0"):
+        return None
+    v = str(value).strip().lower()
+    if v not in ATTR_CLASSES:
+        raise ValueError(f"attributions target must be one of {ATTR_CLASSES}, not {value!r}")
+    return v
+
+
+def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr) -> None:
+    # np.savez, as for the embeddings: 24 KB of fp32 per window barely compresses
+    offsets = np.asarray(offsets, dtype=np.int32)
+    np.savez(path, **{names_key: names,
+                      "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+                      "window_start": np.asarray(starts, dtype=np.int64),
+                      "window_length": np.asarray(lengths, dtype=np.int32),
+                      "target": np.str_(target),
+                      "attributions": np.asarray(attr, dtype=np.float32).reshape(-1, ATTR_TOKENS)})
+
+
+def _attributions_current(path: Path, target: str) -> bool:
+    """The attributions file exists and was written for this class."""
+    if not path.exists():
+        return False
+    try:
+        with np.load(path) as z:
+            return str(z["target"]) == target
+    except Exception:
+        return False
 
 
 def tfrecords_enabled() -> bool:
@@ -335,7 +401,7 @@ def contig_reduce_mode(default: str = "gather") -> str:
 
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
-         write_embeddings=None, write_window_scores=None, window_stride=None):
+         write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -348,6 +414,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     write_window_scores = ((window_scores_enabled() or window_stride is not None) if write_window_scores is None
                            else bool(write_window_scores))
     window_stride = sequence.WINDOW if window_stride is None else int(window_stride)
+    attr_target = attributions_target(write_attributions)
     if not 1 <= window_stride <= sequence.WINDOW:
         raise ValueError(f"window_stride must be in [1, {sequence.WINDOW}], not {window_stride}")
     if is_main:
@@ -376,6 +443,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if write_window_scores:
         files += [outputs.nn_classification_windows_output, outputs.nn_classification_windows_npz_output]
         descr += ["window classification: tabular format", "window classification: binary format"]
+    if attr_target:
+        files.append(outputs.nn_classification_attributions_output)
+        descr.append(f"window attributions ({attr_target}): binary format")
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -387,6 +457,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if write_window_scores:
             files += [outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_windows_npz_output]
             descr += ["provirus window classification: tabular format", "provirus window classification: binary format"]
+        if attr_target:
+            files.append(outputs.provirus_nn_classification_attributions_output)
+            descr.append(f"provirus window attributions ({attr_target}): binary format")
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -402,13 +475,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     jobs = [("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
              "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
              outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
-             outputs.nn_classification_windows_output)]
+             outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
                      outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
                      outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
-                     outputs.provirus_nn_classification_windows_output))
+                     outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output))
 
     plan = None
     info_writer = None
@@ -427,10 +500,12 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             outputs.nn_classification_dir.mkdir()
         # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
         # (with embeddings or window scores requested, a classification whose embeddings file is missing, or whose window
-        # scores are missing or were written at another stride, is redone: same predictions, bit for bit)
+        # scores are missing or were written at another stride, or whose attributions are missing or were written for another
+        # class, is redone: same predictions, bit for bit)
         plan = [(bool(skip and j[4].exists()),
                  bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
-                      and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))))
+                      and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
+                      and (not attr_target or _attributions_current(j[13], attr_target))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -472,8 +547,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
-         win_npz_path, win_tsv_path), (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
+         win_npz_path, win_tsv_path, attr_path), (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
         names = preds = emb = None
+        attr = {"target": attr_target} if attr_target else None      # the contig pass runs through the attribution calls
         win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
@@ -496,15 +572,20 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                 emb = np.zeros((len(index.names), 512), np.float32)
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
+                if attr is not None:
+                    attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), spans=win[:3])
             else:
                 t_c = _time.perf_counter()
+                ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
                 if write_window_scores:
                     preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
-                                                            contig_reduce, write_embeddings)
+                                                            contig_reduce, write_embeddings, **ak)
                 elif write_embeddings:
-                    preds, emb = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, embeddings=True)
+                    preds, emb = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, embeddings=True, **ak)
                 else:
-                    preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce)
+                    preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, **ak)
+                if attr is not None:
+                    attr["spans"] = (index.offsets, *parsed.spans()) if is_main else None
                 last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
                 names = index.names
             console.log(f"{'Sequences' if what == 'sequence' else 'Proviruses'} classified.")
@@ -521,6 +602,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                                          threads or 1)
                 console.log(f"{label} window scores (stride {window_stride}) written to {win_tsv_path.name} and "
                             f"{win_npz_path.name}.")
+            if attr is not None:
+                if is_main:
+                    _write_attributions(attr_path, names_key, names, *attr["spans"], attr_target, attr["attr"])
+                console.log(f"{label} window attributions ({attr_target}) in binary format written to {attr_path.name}.")
         if parsed is not None:
             parsed.close()
         if cleanup and is_main and enc_dir.is_dir():

@@ -376,8 +376,46 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  *   gather warp's total, [1] its waits on a_full, [2] its gather work (reads, mma, part_t stores, release), [3] the first MMA
  *   warpgroup's MMA phases (first a_full wait of a unit to its last wgmma's completion, waits included), [4] that warpgroup's
  *   waits on a_full, [5] units, [6] that warpgroup's epilogues (max-pool and q stores), [7] the producer's waits on a_empty.
+ * After an attribution call (gnm_attribute_*), for its last chunk (n <= the context's max_batch, checked): "route0","route1" = uint8
+ * [n][749][128], the row 0..7 inside each max-pool window of the pooled maximum (first row on ties) -- n * 749 * 128 BYTES are
+ * written to d_dst; "routeq0","routeq1" [n][749][128] = the maxima the routing pass found (bitwise "q0","q1"); "attr_y1"
+ * [n][5997][128] = its layer-1 copy (y1, bitwise what the forward's layer 1 wrote).  An attribution
+ * call re-runs IGLOO#0's logits, so "logits" then holds the first IGLOO kernel's.
  */
 int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream);
+
+/*
+ * Attributions: the input gradient of a class's log-probability, per 4-mer position of a window (gradient x input on the
+ * one-hot tokens).  For a window with tokens tok[0..5996] (the tokenizer's output, 0..256) and a target class c (0 chromosome,
+ * 1 plasmid, 2 virus):
+ *
+ *     attr[t] = d log p_c / d x[t, tok[t]]
+ *
+ * with x the one-hot input of the first Conv1D (reference model.py:9-11), at the window's own input, for the unchanged model.
+ * Token position t covers bases t .. t+3 of the window.  Token 0 (a 4-mer with a non-ACGT base) is a real one-hot row, so the
+ * N-padded tail of a short window gets attributions too.  log p_c rather than p_c: a saturated class still has a gradient.
+ * Max-pool gradients go to the first row of a tie (ties are exact and common inside N runs).  DESIGN.md, "Attributions".
+ *
+ * gnm_attr_create: the attribution workspace for up to max_batch windows per chunk (1 <= max_batch <= the handle's), allocated
+ *   here, not by gnm_create: gnm_attr_bytes_per_window() bytes per window (~21 MB) plus ~14 MB of re-packed weights (W2^T, W3^T packs
+ *   0.8 MB, w_v^T 0.1 MB, w_qk^T 12.6 MB, patch index 0.06 MB).  The
+ *   context belongs to the handle; destroy it before the handle.
+ * gnm_attribute_ascii / gnm_attribute_windows: n windows (ASCII rows as for gnm_forward_ascii, or planned windows of a sequence
+ *   buffer as for gnm_forward_windows) in chunks of the context's max_batch.  Each chunk runs the unchanged forward step, strictly
+ *   in order (no tail overlap), then the backward pass over what that step left on the device.
+ *   d_attr  DEVICE float [n][5997], caller-owned.
+ *   d_probs DEVICE float [n][3] or NULL; when given, bitwise what gnm_forward_ascii / gnm_forward_windows return.
+ *   Asynchronous on `stream`; a gradient range overflow (|g| * s_w beyond the conv operand format) is reported by the next call
+ *   or gnm_check_status, like act_overflow.  Fails with conv_impl = 1: the fp32 validation kernels have no backward pass.
+ */
+typedef struct gnm_attr gnm_attr;
+int gnm_attr_create(gnm_handle* h, int max_batch, gnm_attr** out);
+int gnm_attr_destroy(gnm_attr* a);
+long long gnm_attr_bytes_per_window(void);
+int gnm_attribute_ascii(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs, float* d_attr,
+                        void* stream);
+int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                          int n, int target, float* d_probs, float* d_attr, void* stream);
 
 #ifdef __cplusplus
 }

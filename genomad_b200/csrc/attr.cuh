@@ -5,7 +5,8 @@
 // depend on its batch, its chunk or the GPU count.
 //
 // Backward, per window (DESIGN.md, "Attributions"):
-//   head     g_logits = e_c - p; back through Dense(3), BN1 + ReLU, Dense(512), BN0 + ReLU, Dense(512)    -> g_out0, g_out1
+//   head     g_logits = e_c - p, as -p_i and, for the target, the sum of the other two p_i (never 1 - p_c, which cancels
+//            when p_c is near 1); back through Dense(3), BN1 + ReLU, Dense(512), BN0 + ReLU, Dense(512)  -> g_out0, g_out1
 //   IGLOO k  out = alpha^T q, alpha = softmax(mpi w_qk), q = maxpool8(y w_v)
 //            g_q[p,c] = alpha[p] g_out[c];  g_alpha[p] = sum_c g_out[c] q[p,c];  g_logit = alpha (g_alpha - <alpha, g_alpha>)
 //            g_mpi = w_qk g_logit (sgemm_epi_kernel);  g_y[t] = sum over the (p,c) routed to t of g_q[p,c] w_v[:,c]
@@ -45,9 +46,19 @@ attr_head_backward_kernel(const float* __restrict__ probs,      // [n][3]
                           int target, float* __restrict__ g_out) {
   __shared__ float s_a1[kHidden], s_a0[kHidden];
   const int w = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  float gl[3];
+  // g_logits = e_c - p with the target's component as the sum of the other two probabilities (ascending i), not 1 - p_c:
+  // values just below 1 are 2^-24 apart, so 1 - p_c cancels for a window classified confidently as the target and is
+  // exactly 0 once p_c rounds to 1.0f (log-odds margin ~17.3), while the off-target p_i keep their relative precision
+  float gl[3], other = 0.f;
 #pragma unroll
-  for (int i = 0; i < 3; ++i) gl[i] = (i == target ? 1.f : 0.f) - probs[static_cast<size_t>(w) * 3 + i];
+  for (int i = 0; i < 3; ++i) {
+    const float p = probs[static_cast<size_t>(w) * 3 + i];
+    gl[i] = -p;
+    if (i != target) other += p;
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    if (i == target) gl[i] = other;
   for (int k = tid; k < kHidden; k += 256) {
     const float g = fmaf(gl[2], d2w[k * 3 + 2], fmaf(gl[1], d2w[k * 3 + 1], gl[0] * d2w[k * 3]));
     s_a1[k] = h2[static_cast<size_t>(w) * kHidden + k] > 0.f ? g * bn1_scale[k] : 0.f;

@@ -7,7 +7,10 @@ pieces (oracle/igloo_model.py), and a NumPy restatement of the backward pass as 
 Max-pool routing: by default F.max_pool1d's, which sends the gradient to the first row of a tie (the rule the kernels follow);
 `routes` ([2] arrays [B, 749, 128] of rows 0..7, e.g. the GPU's "route0" / "route1") makes the gradient follow a given routing,
 and `masks` (the signs y > 0 of y1, y2, y3) the LeakyReLU branches of a given forward: both derivatives are discontinuous, and
-an fp32 forward lands on the other side of a near-tie or of z ~ 0 at a few places per window.
+an fp32 forward lands on the other side of a near-tie or of z ~ 0 at a few places per window.  log p_c is differentiated
+in a form that keeps its relative precision when p_c saturates (log_p_target), so windows classified confidently as the target
+have a reference too.  softmax_fp32 / head_gradient_fp32 restate the float32 head: the forward's softmax and the backward's
+first step.
 """
 from __future__ import annotations
 
@@ -23,16 +26,20 @@ L_TOK, N_POOL, POOL = M.L_TOK, M.N_POOL, M.POOL
 
 
 def _igloo(y, w, s, dtype, route=None):
-    """IGLOO1D_kernel.call (igloo.py:190-217) with the max-pool either as written (F.max_pool1d) or along `route`."""
+    """IGLOO1D_kernel.call (igloo.py:190-217) with the max-pool either as written (F.max_pool1d's own choice of row, the first
+    on ties) or along `route`.  Both take q through the same gather from rows of the same layout, so an explicit route equal
+    to F.max_pool1d's gives the same bits on any BLAS (a transposed q would send einsum and its backward through other
+    matmul kernels, whose summation order may differ)."""
     P = torch.as_tensor(np.asarray(w[f"ig{s}_random_patches"]).reshape(M.N_PATCH, 4), dtype=torch.long)
     Wf = M._t(w, f"ig{s}_w_mult", dtype)[0] * M._t(w, f"ig{s}_w_summer", dtype).reshape(1, 4, 128)
     mpi = (y[:, P] * Wf).sum(dim=(2, 3)) + M._t(w, f"ig{s}_w_bias", dtype)
     y_proj = y @ M._t(w, f"ig{s}_w_v", dtype)[0]
     if route is None:
-        q = F.max_pool1d(y_proj.transpose(1, 2), POOL).transpose(1, 2)
-    else:
-        yp = y_proj[:, : N_POOL * POOL].reshape(y.shape[0], N_POOL, POOL, -1)
-        q = yp.gather(2, torch.as_tensor(np.asarray(route), dtype=torch.long)[:, :, None, :]).squeeze(2)
+        with torch.no_grad():
+            _, idx = F.max_pool1d(y_proj.transpose(1, 2), POOL, return_indices=True)     # [B, 128, 749] positions
+        route = (idx - POOL * torch.arange(N_POOL)).transpose(1, 2)                    # [B, 749, 128] rows 0..7
+    yp = y_proj[:, : N_POOL * POOL].reshape(y.shape[0], N_POOL, POOL, -1)
+    q = yp.gather(2, torch.as_tensor(np.asarray(route), dtype=torch.long)[:, :, None, :]).squeeze(2)
     alpha = torch.softmax(mpi @ M._t(w, f"ig{s}_w_qk", dtype), dim=-1)
     return torch.einsum("bg,bgc->bc", alpha, q)
 
@@ -53,6 +60,23 @@ def _act(z, mask):
 
 def log_probs_onehot(x, w, routes: Optional[Sequence] = None, dtype=torch.float64, masks: Optional[Sequence] = None):
     """log softmax of the model on one-hot (or relaxed) input x [B, 5997, 257]; masks = [y1 > 0, y2 > 0, y3 > 0] optional."""
+    return torch.log_softmax(logits_onehot(x, w, routes, dtype, masks), dim=-1)
+
+
+def log_p_target(logits, target: int):
+    """log p_c from the logits [B, 3], with a gradient that keeps its relative precision when p_c saturates.  log_softmax's
+    backward is e_c - p, whose target component 1 - p_c cancels once p_c is near 1 (in fp64 too: p_c == 1.0 from a log-odds
+    margin of about 37).  Where c is the argmax this uses log p_c = -log1p(sum_{i != c} exp(l_i - l_c)), whose derivatives are
+    sum_{i != c} p_i and -p_i: sums of positive terms.  Elsewhere p_c <= 1/2 and log_softmax loses nothing."""
+    lc = logits[:, target: target + 1]
+    d = torch.cat([logits[:, :target], logits[:, target + 1:]], dim=1) - lc
+    top = d.max(dim=1).values <= 0
+    sat = -torch.log1p(torch.exp(d.clamp(max=0)).sum(dim=1))      # the clamp only bites on rows where it is not selected
+    return torch.where(top, sat, torch.log_softmax(logits, dim=-1)[:, target])
+
+
+def logits_onehot(x, w, routes: Optional[Sequence] = None, dtype=torch.float64, masks: Optional[Sequence] = None):
+    """the model's three logits on one-hot (or relaxed) input x [B, 5997, 257] (see log_probs_onehot)"""
     ms = masks if masks is not None else (None, None, None)
     xc = F.pad(x.transpose(1, 2), (5, 0))
     k = M._t(w, "c1w", dtype).permute(2, 1, 0).contiguous()
@@ -71,15 +95,21 @@ def log_probs_onehot(x, w, routes: Optional[Sequence] = None, dtype=torch.float6
         y2 = conv(y1, 2, ms[1])
         y3 = conv(y2, 3, ms[2])
     o1 = _igloo(y3, w, 1, dtype, None if routes is None else routes[1])
-    return torch.log_softmax(M.head(torch.cat([o0, o1], dim=1), w, dtype, return_logits=True), dim=-1)
+    return M.head(torch.cat([o0, o1], dim=1), w, dtype, return_logits=True)
 
 
 def attribution(tokens, w, target: int, routes: Optional[Sequence] = None, dtype=torch.float64,
-                masks: Optional[Sequence] = None) -> np.ndarray:
+                masks: Optional[Sequence] = None, logits_at: Optional[np.ndarray] = None) -> np.ndarray:
     """[B, 5997] tokens (0..256) -> [B, 5997] attributions by autograd; `routes` / `masks` make the max-pools / LeakyReLUs
-    follow a given forward (e.g. the GPU's: "route0/1", and the signs of y1, y2, y3)."""
+    follow a given forward (e.g. the GPU's: "route0/1", and the signs of y1, y2, y3).  `logits_at` ([B, 3], e.g. the GPU
+    forward's) is where log p_c and its gradient are evaluated; the logits' derivatives stay this model's.  For a window
+    classified confidently as the target the attributions scale as e^-mu, so a forward's logit-margin error d moves all of
+    them by the relative d: an fp32 forward with logits of magnitude ~176 (golden row 16) has d ~ 1e-4."""
     x = one_hot(tokens, dtype).requires_grad_(True)
-    lp = log_probs_onehot(x, w, routes, dtype, masks)[:, target].sum()
+    lg = logits_onehot(x, w, routes, dtype, masks)
+    if logits_at is not None:
+        lg = lg - lg.detach() + torch.as_tensor(np.asarray(logits_at), dtype=dtype)
+    lp = log_p_target(lg, target).sum()
     (g,) = torch.autograd.grad(lp, x)
     tok = torch.as_tensor(np.asarray(tokens).astype(np.int64))
     return g.gather(2, tok[..., None]).squeeze(2).numpy()
@@ -103,11 +133,48 @@ def _lrelu_d(y):
     return np.where(y > 0, 1.0, M.LRELU)
 
 
-def decomposed(tokens, w, target: int, routes: Optional[Sequence] = None) -> np.ndarray:
+def softmax_fp32(logits32) -> np.ndarray:
+    """[n, 3] float32 logits -> float32 probabilities as dense3_softmax_kernel (csrc/dense.cuh) computes them: the maximum,
+    exp(a_i - m), one reciprocal of (e0 + e1) + e2, three products."""
+    a = np.asarray(logits32, dtype=np.float32)
+    e = np.exp(a - a.max(axis=1, keepdims=True))
+    inv = np.float32(1) / ((e[:, 0] + e[:, 1]) + e[:, 2])
+    return e * inv[:, None]
+
+
+def head_gradient_from_probs32(p32, target: int) -> np.ndarray:
+    """g_logits = e_c - p as attr_head_backward_kernel computes it from the forward's float32 probabilities: -p_i off the
+    target, and the target's component as the sum of the other two probabilities in ascending i, never as 1 - p_c (which
+    cancels in fp32 once p_c is near 1 and is exactly 0 once p_c rounds to 1.0f)."""
+    p = np.asarray(p32, dtype=np.float32)
+    g = -p
+    o = [i for i in range(3) if i != target]
+    g[:, target] = p[:, o[0]] + p[:, o[1]]
+    return g
+
+
+def head_gradient_fp32(logits32, target: int) -> np.ndarray:
+    """the head's g_logits from float32 logits: the forward's softmax, then the kernel's formula (both in float32)"""
+    return head_gradient_from_probs32(softmax_fp32(logits32), target)
+
+
+def head_gradient_fp64(logits, target: int) -> np.ndarray:
+    """e_c - softmax(logits) in fp64 with full relative precision in every component (no 1 - p_c)"""
+    a = np.asarray(logits, dtype=np.float64)
+    e = np.exp(a - a.max(axis=1, keepdims=True))
+    p = e / e.sum(axis=1, keepdims=True)
+    g = -p
+    g[:, target] = np.delete(p, target, axis=1).sum(axis=1)
+    return g
+
+
+def decomposed(tokens, w, target: int, routes: Optional[Sequence] = None,
+               g_logits: Optional[np.ndarray] = None) -> np.ndarray:
     """The backward pass as csrc/attr.cuh computes it, one window at a time, in fp64: head backward, the attention part,
     the sparse value path (per row t: the channels routed to t), the patch path through the position-sorted entries, the
     per-window power of two s_w, conv backward as a causal conv over time-reversed rows against W[j]^T with the mirrored
-    lrelu' mask, and the layer-1 formula."""
+    lrelu' mask, and the layer-1 formula.  `g_logits` ([B, 3]) replaces the head's gradient e_c - p (by default the fp64
+    head_gradient_fp64), e.g. with one computed from float32 probabilities."""
     f64 = torch.float64
     tokens = np.asarray(tokens).astype(np.int64)
     with torch.no_grad():
@@ -127,8 +194,7 @@ def decomposed(tokens, w, target: int, routes: Optional[Sequence] = None) -> np.
         a1 = h1 @ W["d1w"] + W["d1b"]
         h2 = np.maximum(bn["bn1"] * (a1 - W["bn1m"]) + W["bn1b"], 0)
         lg = h2 @ W["d2w"] + W["d2b"]
-        p = np.exp(lg - lg.max()); p /= p.sum()
-        g_lg = np.eye(3)[target] - p
+        g_lg = head_gradient_fp64(lg[None], target)[0] if g_logits is None else np.asarray(g_logits[b], dtype=np.float64)
         g_a1 = np.where(h2 > 0, W["d2w"] @ g_lg, 0) * bn["bn1"]
         g_a0 = np.where(h1 > 0, W["d1w"] @ g_a1, 0) * bn["bn0"]
         g_h0 = W["d0w"] @ g_a0

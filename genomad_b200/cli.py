@@ -59,8 +59,19 @@ def cli():
                    "with respect to each one-hot 4-mer (gradient x input; position t covers bases t..t+3 of the window) to "
                    "<prefix>_nn_classification_attributions.npz: 5,997 float32 values, 24 KB per window, ~4 GB per Gbp of "
                    "input. About 4x the classification's GPU time. Not an option of the reference.")
+@click.option("--attribution-steps", type=click.IntRange(0, 256), default=None, show_default="0",
+              help="With --write-attributions: 0 writes gradient x input; N >= 1 writes integrated gradients with N steps "
+                   "instead, attributions that add up to the change in log-probability from a baseline to the window, also for "
+                   "windows classified with near certainty (where gradient x input is ~0). About 1 + 4.2 N times the "
+                   "classification's GPU time; the file adds log_p_target (window, baseline). At most 256, and at most the windows per GPU "
+                   "step of the device (checked before any work). Without --write-attributions it has no effect (a warning is "
+                   "logged). Not an option of the reference.")
+@click.option("--attribution-baseline", type=click.Choice(["zero", "N"]), default=None, show_default="zero",
+              help="Baseline of integrated gradients: zero (all-zero one-hot input) or N (a window of N). Not an option of the "
+                   "reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
-                      write_embeddings, write_window_scores, window_stride, write_attributions):
+                      write_embeddings, write_window_scores, window_stride, write_attributions, attribution_steps,
+                      attribution_baseline):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -74,6 +85,10 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["window_stride"] = window_stride
     if write_attributions is not None:
         extra["write_attributions"] = write_attributions
+    if attribution_steps is not None:
+        extra["attribution_steps"] = attribution_steps
+    if attribution_baseline is not None:
+        extra["attribution_baseline"] = attribution_baseline
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
 

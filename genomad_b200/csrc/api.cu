@@ -831,13 +831,26 @@ static void select_set(gnm_handle* h, int par) {
   }
 }
 
+// Layer 1 of an integrated-gradients step (encode.cuh, embed_conv1_ig_kernel): row r is window r / m of d_ascii at
+// alpha = (r mod m + 1/2) / m on the line from the baseline (kIgZero / kIgN) to the window; m = 0: the baseline itself.
+struct L1Interp {
+  int m, baseline;
+};
+
 // main part of a step: layer 1, the two IGLOO kernels' value projection + patch gather, conv2, conv3 (everything that streams
-// the activations); returns 2 when a debug_stop cut the step short
-static int forward_main(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, cudaStream_t st) {
+// the activations); returns 2 when a debug_stop cut the step short.  With `ig`, layer 1 is the interpolated embed kernel
+// whatever fuse_l1 says (ASCII input only), and the rest of the step is unchanged.
+static int forward_main(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, cudaStream_t st,
+                        const L1Interp* ig = nullptr) {
   dim3 egrid((kTok + kEmbSeg - 1) / kEmbSeg, n);
   h->ybuf_fp8lo[0] = h->ybuf_fp8lo[1] = 0;
-  const bool fused = h->fuse_l1 && h->conv_impl == 0;       // layer 1 + w_v#0 in one kernel
-  if (fused) {
+  const bool fused = h->fuse_l1 && h->conv_impl == 0 && !ig;       // layer 1 + w_v#0 in one kernel
+  if (ig) {
+    timer_mark(h, "embed_conv1_ig", st);
+    embed_conv1_ig_kernel<<<egrid, kEmbThreads, 0, st>>>(d_ascii, h->conv1_table, h->conv1_triple, h->conv1_bias, h->ybuf[0],
+                                                         ig->m, ig->baseline, h->status);
+    if (check_launch(h, "embed_conv1_ig_kernel")) return 1;
+  } else if (fused) {
     timer_mark(h, "layer1_wv0", st);
     FusedParams fp;
     fp.ascii = d_ascii; fp.tokens = d_tok; fp.table = h->conv1_table; fp.triple = h->conv1_triple; fp.bias = h->conv1_bias;
@@ -930,10 +943,10 @@ static int forward_tail(gnm_handle* h, int n, float* d_probs, float* d_embed, cu
   return 0;
 }
 
-// One step: n <= max_batch windows, strictly in order on one stream.
+// One step: n <= max_batch windows (or interpolated rows, see forward_main), strictly in order on one stream.
 static int forward_step(gnm_handle* h, const uint8_t* d_ascii, const uint16_t* d_tok, int n, float* d_probs, float* d_embed,
-                        cudaStream_t st) {
-  const int rc = forward_main(h, d_ascii, d_tok, n, st);
+                        cudaStream_t st, const L1Interp* ig = nullptr) {
+  const int rc = forward_main(h, d_ascii, d_tok, n, st, ig);
   if (rc) return rc == 2 ? 0 : 1;
   return forward_tail(h, n, d_probs, d_embed, st);
 }
@@ -1512,15 +1525,23 @@ static int launch_igloo_bwd(gnm_handle* h, gnm_attr* a, int s, int n, cudaStream
 }
 
 // One chunk: the unchanged forward step, strictly in order, then the backward pass over the state that step left behind
-// (ybuf[0] = y3, ybuf[1] = y2, q / logits of IGLOO#1, h1, h2).
+// (ybuf[0] = y3, ybuf[1] = y2, q / logits of IGLOO#1, h1, h2).  With `ig`, the n rows are interpolated inputs (forward_main)
+// and the layer-1 result of row r, g[t, tok[t]] (minus g[t, 0] for the N baseline), goes to the g_y1 rows as [n][5997]
+// (layer1_ig_kernel); d_attr is not used.
 static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs, float* d_attr,
-                          cudaStream_t st) {
+                          cudaStream_t st, const L1Interp* ig = nullptr) {
   float* probs = d_probs ? d_probs : a->probs;
-  if (forward_step(h, d_ascii, nullptr, n, probs, nullptr, st)) return 1;
+  if (forward_step(h, d_ascii, nullptr, n, probs, nullptr, st, ig)) return 1;
   dim3 egrid((kTok + kEmbSeg - 1) / kEmbSeg, n), sgrid((kTok + kAttrSeg - 1) / kAttrSeg, n);
   timer_mark(h, "attr_layer1", st);
+  if (ig) {
+    embed_conv1_ig_kernel<<<egrid, kEmbThreads, 0, st>>>(d_ascii, h->conv1_table, h->conv1_triple, h->conv1_bias, a->y1, ig->m,
+                                                         ig->baseline, h->status);
+    if (check_launch(h, "embed_conv1_ig_kernel")) return 1;
+  } else {
   embed_conv1_kernel<true><<<egrid, kEmbThreads, 0, st>>>(d_ascii, nullptr, h->conv1_table, h->conv1_triple, h->conv1_bias, a->y1, n, h->status);
   if (check_launch(h, "embed_conv1_kernel")) return 1;
+  }
   timer_mark(h, "attr_route1", st);
   if (launch_route(h, a, 1, h->tm_act[0], n, st)) return 1;                  // y3
   timer_mark(h, "attr_route0", st);
@@ -1540,8 +1561,13 @@ static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, in
   timer_mark(h, "attr_conv2_bwd", st);
   if (launch_conv_bwd(h, a, 0, a->tm_gz2, a->y1, a->gy1, nullptr, a->f32a, n, st)) return 1;        // + s_w g_y1, mask y1 -> s_w g_z1
   timer_mark(h, "attr_layer1_attr", st);
+  if (ig) {
+    layer1_ig_kernel<<<sgrid, 256, 0, st>>>(d_ascii, a->f32a, h->conv1_table, a->s_w, ig->m, ig->baseline, a->gy1);
+    if (check_launch(h, "layer1_ig_kernel")) return 1;
+  } else {
   layer1_attr_kernel<<<sgrid, 256, 0, st>>>(d_ascii, a->f32a, h->conv1_table, a->s_w, d_attr);
   if (check_launch(h, "layer1_attr_kernel")) return 1;
+  }
   timer_mark(h, "end", st);
   for (int s = 0; s < 2; ++s) { h->attr_route[s] = a->route[s]; h->attr_rq[s] = a->rq[s]; }
   h->attr_y1 = a->y1;
@@ -1584,6 +1610,76 @@ extern "C" int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* 
   if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_windows: null buffer");
   return attribute_any(h, a, "gnm_attribute_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, d_probs, d_attr, stream);
 }
+// ------------------------------------------------------------------------------------------------ integrated gradients
+// Chunks of floor(max_batch / steps) windows, so that a window's `steps` rows never span chunks.  Per chunk, in order:
+//   1. the unchanged forward of the windows: probabilities (bitwise gnm_forward_*) and log p_c(x);
+//   2. attribute_step over the windows x steps rows (row w steps + k: window w at alpha_k), layer-1 results to the g_y1 rows;
+//   3. ig_reduce_kernel: IG = the rows' mean over k, ascending.
+// log p_c(x') is the same for every window: one one-row forward of the baseline per call, before the first chunk (only when
+// d_logp is given), so the debug buffers still hold the last chunk's rows afterwards.
+static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
+                            const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps, int baseline,
+                            float* d_probs, float* d_logp, float* d_attr, void* stream) {
+  const std::string f(fn);
+  if (!h || !a) return fail(f + ": null handle or attribution context");
+  if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
+  if (n < 0) return fail(f + ": negative window count");
+  if (target < 0 || target > 2) return fail(f + ": target must be 0 (chromosome), 1 (plasmid) or 2 (virus)");
+  if (steps < 1 || steps > a->max_batch)
+    return fail(f + ": steps must be in [1, the attribution context's max_batch = " + std::to_string(a->max_batch) + "]");
+  if (baseline != GNM_IG_BASELINE_ZERO && baseline != GNM_IG_BASELINE_N)
+    return fail(f + ": baseline must be GNM_IG_BASELINE_ZERO (0) or GNM_IG_BASELINE_N (1)");
+  if (h->conv_impl != 0)
+    return fail(f + ": attributions need the tensor-core path (conv_impl = 0); the fp32 validation kernels have no backward pass");
+  if (h->debug_stop != 0) return fail(f + ": debug_stop must be 0");
+  if (n == 0) return 0;
+  if (!d_attr || (!d_ascii && (!d_seq || !d_win_start || !d_win_len))) return fail(f + ": null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  if (check_device_status(h)) return 1;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int per = a->max_batch / steps;                         // windows per chunk
+  if (d_logp) {                                                 // log p_c(x'), into column 1 of every window
+    const L1Interp base = {0, baseline};
+    if (forward_step(h, d_ascii ? d_ascii : h->in_stage[0], nullptr, 1, a->probs, nullptr, st, &base)) return 1;
+    ig_logp_kernel<<<(n + 255) / 256, 256, 0, st>>>(a->probs, 1, n, target, d_logp + 1);
+    if (check_launch(h, "ig_logp_kernel")) return 1;
+  }
+  const L1Interp ig = {steps, baseline};
+  for (int off = 0; off < n; off += per) {
+    const int m = std::min(per, n - off);
+    const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
+    if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
+    if (d_probs || d_logp) {
+      float* probs = d_probs ? probs_at(d_probs, off) : a->blockmax;    // blockmax: scratch until step 2 rewrites it
+      if (forward_step(h, asc, nullptr, m, probs, nullptr, st)) return 1;
+      if (d_logp) {
+        ig_logp_kernel<<<(m + 255) / 256, 256, 0, st>>>(probs, 0, m, target, d_logp + static_cast<size_t>(off) * 2);
+        if (check_launch(h, "ig_logp_kernel")) return 1;
+      }
+    }
+    if (attribute_step(h, a, asc, m * steps, target, nullptr, nullptr, st, &ig)) return 1;
+    timer_mark(h, "ig_reduce", st);
+    ig_reduce_kernel<<<dim3((kTok + 255) / 256, m), 256, 0, st>>>(a->gy1, steps, d_attr + static_cast<size_t>(off) * kTok);
+    if (check_launch(h, "ig_reduce_kernel")) return 1;
+    timer_mark(h, "end", st);
+  }
+  return 0;
+}
+
+extern "C" int gnm_attribute_ig_ascii(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, int steps,
+                                      int baseline, float* d_probs, float* d_logp, float* d_attr, void* stream) {
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_ig_ascii: null buffer");
+  return attribute_ig_any(h, a, "gnm_attribute_ig_ascii", d_ascii, nullptr, nullptr, nullptr, n, target, steps, baseline,
+                          d_probs, d_logp, d_attr, stream);
+}
+extern "C" int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, const int64_t* d_win_start,
+                                        const int32_t* d_win_len, int n, int target, int steps, int baseline, float* d_probs,
+                                        float* d_logp, float* d_attr, void* stream) {
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_ig_windows: null buffer");
+  return attribute_ig_any(h, a, "gnm_attribute_ig_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, steps, baseline,
+                          d_probs, d_logp, d_attr, stream);
+}
+
 extern "C" long long gnm_attr_bytes_per_window(void) {
   return static_cast<long long>(kTok) * (3 * kRowBytes + 2 * kC * 4) + 2LL * kPooled * kC * 5 +
          4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + 4);

@@ -299,4 +299,82 @@ layer1_attr_kernel(const uint8_t* __restrict__ ascii, const float* __restrict__ 
   }
 }
 
+// ------------------------------------------------------------------------------------------------ integrated gradients
+// Layer 1 of row r of an integrated-gradients chunk: window r / m at alpha_k (encode.cuh, ig_row).  The gradient of log p_c at
+// x' + alpha (x - x') with respect to the one-hot input is g[t, v] = (1 / s_w) sum_u <g_z1[u], W1[t-u+5, v, :]> at any v, so
+//   zero baseline: out[r][t] = g[t, tok[t]]                   (x - x' = the one-hot row of tok[t])
+//   N baseline:    out[r][t] = g[t, tok[t]] - g[t, 0]         (x - x' = e_tok - e_0; 0 where tok[t] = 0)
+// each dot product in layer1_attr_kernel's order, so g[t, tok[t]] is bitwise what that kernel computes for the row.
+// grid (24, rows), 256 threads, one warp per position, u ascending.  out: [rows][5997] (the workspace's g_y1 rows, free once
+// conv2's backward has consumed them).
+__global__ void __launch_bounds__(256)
+layer1_ig_kernel(const uint8_t* __restrict__ ascii, const float* __restrict__ g_z1, const float* __restrict__ table,
+                 const float* __restrict__ s_w, int m, int baseline, float* __restrict__ out) {
+  __shared__ int16_t s_tok[kAttrSeg];
+  const int r = blockIdx.y, t0 = blockIdx.x * kAttrSeg, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int w = ig_row(r, m).win;
+  {
+    const int t = t0 + threadIdx.x;
+    if (t < kTok) {
+      const uint8_t* s = ascii + static_cast<size_t>(w) * kWindow + t;
+      s_tok[threadIdx.x] = static_cast<int16_t>(kmer_token(base_code(s[0]), base_code(s[1]), base_code(s[2]), base_code(s[3])));
+    }
+  }
+  __syncthreads();
+  const float inv = 1.f / s_w[r];
+  const bool sub = baseline == kIgN;
+  const int i_end = min(kAttrSeg, kTok - t0);
+  for (int i = warp; i < i_end; i += 8) {
+    const int t = t0 + i, tk = s_tok[i];
+    if (sub && tk == 0) {                                        // x - x' = 0 at this position
+      if (lane == 0) out[static_cast<size_t>(r) * kTok + t] = 0.f;
+      continue;
+    }
+    float a = 0.f, a0 = 0.f;
+    const int u_end = min(t + 5, kTok - 1);
+    for (int u = t; u <= u_end; ++u) {
+      const float4 gz = reinterpret_cast<const float4*>(g_z1 + (static_cast<size_t>(r) * kTok + u) * kC)[lane];
+      const float4 wr = __ldg(reinterpret_cast<const float4*>(table + (static_cast<size_t>(t - u + 5) * kVocab + tk) * kC) + lane);
+      a = fmaf(gz.w, wr.w, fmaf(gz.z, wr.z, fmaf(gz.y, wr.y, fmaf(gz.x, wr.x, a))));
+      if (sub) {
+        const float4 w0 = __ldg(reinterpret_cast<const float4*>(table + static_cast<size_t>(t - u + 5) * kVocab * kC) + lane);
+        a0 = fmaf(gz.w, w0.w, fmaf(gz.z, w0.z, fmaf(gz.y, w0.y, fmaf(gz.x, w0.x, a0))));
+      }
+    }
+    a = warp_sum(a);
+    if (sub) a = a * inv - warp_sum(a0) * inv;
+    else a *= inv;
+    if (lane == 0) out[static_cast<size_t>(r) * kTok + t] = a;
+  }
+}
+
+// IG[w][t] = (((g_0 + g_1) + g_2) + ... + g_{m-1}) / m over rows w m + k of layer1_ig_kernel, k ascending, fp32, no atomics.
+// grid (24, windows), 256 threads, one position per thread.
+__global__ void __launch_bounds__(256)
+ig_reduce_kernel(const float* __restrict__ rows, int m, float* __restrict__ out) {
+  const int w = blockIdx.y, t = blockIdx.x * 256 + threadIdx.x;
+  if (t >= kTok) return;
+  const float* g = rows + static_cast<size_t>(w) * m * kTok + t;
+  float a = g[0];
+  for (int k = 1; k < m; ++k) a += g[static_cast<size_t>(k) * kTok];
+  out[static_cast<size_t>(w) * kTok + t] = a / static_cast<float>(m);
+}
+
+// log p_c from a row of fp32 probabilities without cancellation: -log1p(sum_{i != c} p_i) (the sum in ascending i, as the head
+// gradient's) when c is the argmax (p_c >= every p_i), log p_c otherwise; evaluated in fp64 and rounded once to fp32.
+// out[2 i] for i < n, from probs row i, or from row 0 for every i when `broadcast` (the baseline's value in every row).
+__global__ void __launch_bounds__(256)
+ig_logp_kernel(const float* __restrict__ probs, int broadcast, int n, int target, float* __restrict__ out) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  const float* p = probs + (broadcast ? 0 : static_cast<size_t>(i) * 3);
+  float other = 0.f;
+  bool top = true;
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+    if (k != target) { other += p[k]; top = top && p[target] >= p[k]; }
+  out[static_cast<size_t>(i) * 2] = top ? static_cast<float>(-log1p(static_cast<double>(other)))
+                                        : static_cast<float>(log(static_cast<double>(p[target])));
+}
+
 }  // namespace gnm

@@ -100,18 +100,37 @@ constexpr int kEmbThreads = 256;
 constexpr int kTriple = 4096;
 static_assert(kEmbThreads == kEmbSeg, "embed_conv1_kernel computes one position's table codes per thread");
 
-template <bool kFromAscii>
-__global__ void __launch_bounds__(kEmbThreads)
-embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict__ tokens_in,
-                   const float* __restrict__ table,   // [6][257][128]
-                   const float* __restrict__ triple,  // [2][4096][128]: A-table, B-table
-                   const float* __restrict__ bias,    // [128]
-                   uint8_t* __restrict__ y_out,       // [n][5997][768 B] activation rows (hi16 | lo16 | e4m3 pairs)
-                   int n_windows, DeviceStatus* status) {
+// Integrated gradients (attr.cuh, DESIGN.md "Integrated gradients") run layer 1 at inputs on the straight line from a
+// baseline x' to the window x.  Conv1D #1 is linear in its one-hot input, so the pre-activation there is
+//   alpha * S_tok + (1 - alpha) * S_base + b,   S_tok = the (A + B) sum below,
+//   S_base = 0 (kIgZero: all-zero one-hot rows) or sum_{j: t-5+j >= 0} W1[j][0] (kIgN: the all-N window, token 0 everywhere;
+//            summed in the fallback's order, so it is bitwise the all-N window's A + B).
+// computed as fmaf(alpha, S_tok, fmaf(1 - alpha, S_base, b)) (kIgN) or fmaf(alpha, S_tok, b) (kIgZero): at alpha = 1 that is
+// exactly the (A + B) + b of the plain kernel, so the row is bitwise the plain kernel's.
+constexpr int kIgZero = 0, kIgN = 1;
+
+// Row `row` of an interpolated launch: window row / m at alpha_k = (k + 1/2) / m, k = row mod m (midpoint rule); m = 0 is the
+// baseline itself (alpha = 0).
+struct IgRow {
+  int win; float alpha, beta;                // beta = 1 - alpha, both rounded once from exact numerators
+};
+__device__ __forceinline__ IgRow ig_row(int row, int m) {
+  if (m <= 0) return {0, 0.f, 1.f};
+  const int k = row % m;
+  return {row / m, (static_cast<float>(k) + 0.5f) / static_cast<float>(m), (static_cast<float>(m - k) - 0.5f) / static_cast<float>(m)};
+}
+
+// The body of embed_conv1_kernel; kIg (ASCII input only) adds the interpolation of the pre-activation.  win: the window whose
+// bytes / tokens are read, out_row: the output row.
+template <bool kFromAscii, bool kIg>
+__device__ __forceinline__ void embed_conv1_body(const uint8_t* __restrict__ ascii, const uint16_t* __restrict__ tokens_in,
+                                                 const float* __restrict__ table, const float* __restrict__ triple,
+                                                 const float* __restrict__ bias, uint8_t* __restrict__ y_out, int win, int out_row,
+                                                 float alpha, float beta, int baseline, DeviceStatus* status) {
   __shared__ int16_t s_tok[kEmbSeg + 8];    // s_tok[i] = token at position t0 - 5 + i, or -1 (causal pad)
   __shared__ uint8_t s_b[kEmbSeg + 16];
   __shared__ int s_code[kEmbSeg];           // per position: (A code | B code << 16), 0xFFFF in a half = that half needs the 3-row fallback
-  const int w = blockIdx.y;
+  const int w = win;
   const int t0 = blockIdx.x * kEmbSeg;
   if (kFromAscii) {
     const uint8_t* src = ascii + static_cast<size_t>(w) * kWindow;
@@ -173,16 +192,28 @@ embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict
     if (cb != 0xFFFF) B = __ldg(tri4 + (static_cast<size_t>(kTriple) + cb) * (kC / 4) + lane);
     else B = add4(add4(row(3, s_tok[i + 3]), row(4, s_tok[i + 4])), row(5, s_tok[i + 5]));
     float4 a = add4(A, B);
+    if (kIg) {
+      float4 b = b4;
+      if (baseline == kIgN) {                          // S_base: token 0 at every tap inside the window, in the fallback's order
+        const auto r0 = [&](int j) { return row(j, t - 5 + j >= 0 ? 0 : -1); };
+        const float4 sb = add4(add4(add4(r0(0), r0(1)), r0(2)), add4(add4(r0(3), r0(4)), r0(5)));
+        b = make_float4(fmaf(beta, sb.x, b4.x), fmaf(beta, sb.y, b4.y), fmaf(beta, sb.z, b4.z), fmaf(beta, sb.w, b4.w));
+      }
+      a = make_float4(fmaf(alpha, a.x, b.x), fmaf(alpha, a.y, b.y), fmaf(alpha, a.z, b.z), fmaf(alpha, a.w, b.w));
+      a.x = kActScale * lrelu(a.x); a.y = kActScale * lrelu(a.y);
+      a.z = kActScale * lrelu(a.z); a.w = kActScale * lrelu(a.w);
+    } else {
     // Y = 32 * y1; planes: hi16, lo16 (w_v, gather), lo8 / hi8 (conv2 correction passes)
     a.x = kActScale * lrelu(a.x + b4.x); a.y = kActScale * lrelu(a.y + b4.y);
     a.z = kActScale * lrelu(a.z + b4.z); a.w = kActScale * lrelu(a.w + b4.w);
+    }
     amax = fmaxf(amax, fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))));
     __half2 h01, h23, l01, l23;
     split2_f16(a.x, a.y, h01, l01);
     split2_f16(a.z, a.w, h23, l23);
     const float2 fa = __half22float2(h01), fb = __half22float2(h23);
     const float f0 = fa.x, f1 = fa.y, f2 = fb.x, f3 = fb.y;
-    uint8_t* rowp = y_out + (static_cast<size_t>(w) * kTok + t) * kRowBytes;
+    uint8_t* rowp = y_out + (static_cast<size_t>(out_row) * kTok + t) * kRowBytes;
     *reinterpret_cast<uint2*>(rowp + kOffHi16 + lane * 8) =
         make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
     *reinterpret_cast<uint2*>(rowp + kOffLo16 + lane * 8) =
@@ -195,6 +226,26 @@ embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict
             (static_cast<uint32_t>(pack_e4m3x2((a.w - f3) * kLo8Scale, f3 * kHi8Scale)) << 16));
   }
   flag_act_overflow(status, amax, kHi8Limit, 1);
+}
+
+template <bool kFromAscii>
+__global__ void __launch_bounds__(kEmbThreads)
+embed_conv1_kernel(const uint8_t* __restrict__ ascii, const uint16_t* __restrict__ tokens_in,
+                   const float* __restrict__ table,   // [6][257][128]
+                   const float* __restrict__ triple,  // [2][4096][128]: A-table, B-table
+                   const float* __restrict__ bias,    // [128]
+                   uint8_t* __restrict__ y_out,       // [n][5997][768 B] activation rows (hi16 | lo16 | e4m3 pairs)
+                   int n_windows, DeviceStatus* status) {
+  embed_conv1_body<kFromAscii, false>(ascii, tokens_in, table, triple, bias, y_out, blockIdx.y, blockIdx.y, 1.f, 0.f, 0, status);
+}
+
+// Interpolated layer 1 (integrated gradients): grid (24, rows); row r is window r / m of `ascii` at alpha_k (ig_row), so a
+// chunk holds each window's bytes once, not m copies.  m = 0: every row is the baseline x' (alpha = 0).
+__global__ void __launch_bounds__(kEmbThreads)
+embed_conv1_ig_kernel(const uint8_t* __restrict__ ascii, const float* __restrict__ table, const float* __restrict__ triple,
+                      const float* __restrict__ bias, uint8_t* __restrict__ y_out, int m, int baseline, DeviceStatus* status) {
+  const IgRow r = ig_row(blockIdx.y, m);
+  embed_conv1_body<true, true>(ascii, nullptr, table, triple, bias, y_out, r.win, blockIdx.y, r.alpha, r.beta, baseline, status);
 }
 
 }  // namespace gnm

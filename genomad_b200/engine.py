@@ -88,6 +88,10 @@ EXPORTS = {
     "gnm_attribute_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_attribute_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
                                         C.c_void_p, C.c_void_p]),
+    "gnm_attribute_ig_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_fasta_last_error": (C.c_char_p, []),
     "gnm_fasta_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_open_gz": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -161,10 +165,26 @@ class Attributions(NamedTuple):
     length: "object"          # int32 [W]
     offsets: "object"         # int32 [n_contigs + 1], CSR
     attr: "object"            # float32 [W, 5997]: d log p_target / d one-hot token, token t = bases t .. t+3 of the window
+    logp: "object" = None     # integrated gradients only: float32 [W, 2], log p_target(window), log p_target(baseline)
 
 
 CLASSES = ("chromosome", "plasmid", "virus")
 ATTR_MAX_BATCH = 256             # windows per attribution chunk (attribution context, ~21 MB per window)
+IG_BASELINES = ("zero", "N")     # GNM_IG_BASELINE_ZERO, GNM_IG_BASELINE_N
+IG_STEPS = 64                    # default integrated-gradients steps: the smallest m of the fp64 convergence study with every
+                                 # completeness gap below 1 on the unsharpened weights (profiles/integrated_gradients_h100.md)
+
+
+def ig_baseline_index(baseline) -> int:
+    """"zero" / "N" (or 0 / 1) -> GNM_IG_BASELINE_*."""
+    if isinstance(baseline, str):
+        if baseline not in IG_BASELINES:
+            raise ValueError(f"baseline must be one of {IG_BASELINES}, not {baseline!r}")
+        return IG_BASELINES.index(baseline)
+    b = int(baseline)
+    if b not in (0, 1):
+        raise ValueError(f"baseline must be 0 (zero) or 1 (N), not {b}")
+    return b
 
 
 def class_index(target) -> int:
@@ -536,6 +556,65 @@ class Classifier:
         probs, attr = self.attribute_windows(seq, start, length, target)
         rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
         return Attributions(probs, contig, rel, length, woff, attr)
+
+    def _ig_args(self, steps, baseline):
+        steps = int(steps)
+        if steps < 1:
+            raise ValueError(f"steps must be >= 1, not {steps}")
+        return steps, ig_baseline_index(baseline)
+
+    def integrated_gradients_ascii(self, ascii_windows, target, steps: int = IG_STEPS, baseline="zero"):
+        """uint8 cuda [n, 6000], target class -> (probabilities float32 [n, 3], logp float32 [n, 2], attributions float32
+        [n, 5997]) by integrated gradients (gnm_attribute_ig_ascii): attr[i, t] = (1/m) sum_k g_k[t, tok[t]] (baseline "zero",
+        all-zero one-hot rows) or (1/m) sum_k (g_k[t, tok[t]] - g_k[t, 0]) (baseline "N", the all-N window), g_k the input
+        gradient of log p_target at x' + (k + 1/2)/m (x - x'), m = steps.  The attributions add up to about
+        logp[:, 0] - logp[:, 1] = log p_target(x) - log p_target(x').  The probabilities are bitwise those of predict_ascii.
+        steps is capped by the attribution context's max_batch (ATTR_MAX_BATCH)."""
+        t = self._torch
+        a = ascii_windows.contiguous()
+        assert a.dtype == t.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        c = class_index(target)
+        m, b = self._ig_args(steps, baseline)
+        n = a.shape[0]
+        probs = t.empty((n, 3), dtype=t.float32, device=a.device)
+        logp = t.empty((n, 2), dtype=t.float32, device=a.device)
+        attr = t.empty((n, TOKENS), dtype=t.float32, device=a.device)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_ig_ascii(self._h, self._attr_ctx(), a.data_ptr(), n, c, m, b, probs.data_ptr(),
+                                                             logp.data_ptr(), attr.data_ptr(), self._stream()))
+        return probs, logp, attr
+
+    def integrated_gradients_windows(self, seq_u8, win_start, win_len, target, steps: int = IG_STEPS, baseline="zero"):
+        """Planned windows of a sequence buffer (see predict_windows) -> (probabilities [W, 3], logp [W, 2], attributions
+        [W, 5997]) by integrated gradients (see integrated_gradients_ascii)."""
+        t = self._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        c = class_index(target)
+        m, b = self._ig_args(steps, baseline)
+        n = start.numel()
+        probs = t.empty((n, 3), dtype=t.float32, device=seq_u8.device)
+        logp = t.empty((n, 2), dtype=t.float32, device=seq_u8.device)
+        attr = t.empty((n, TOKENS), dtype=t.float32, device=seq_u8.device)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_ig_windows(self._h, self._attr_ctx(), seq_u8.data_ptr(), start.data_ptr(),
+                                                               length.data_ptr(), n, c, m, b, probs.data_ptr(), logp.data_ptr(),
+                                                               attr.data_ptr(), self._stream()))
+        return probs, logp, attr
+
+    def integrated_gradients_contigs(self, seqs, target, steps: int = IG_STEPS, baseline="zero",
+                                     single_window: bool = False) -> "Attributions":
+        """attribute_contigs by integrated gradients: the same windows and record, attr the IG attributions and logp
+        float32 [W, 2] = (log p_target(window), log p_target(baseline))."""
+        t = self._torch
+        seq, offs = self.contig_buffers(seqs)
+        start, length, woff = self.contig_windows(seq, offs, single_window)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        probs, logp, attr = self.integrated_gradients_windows(seq, start, length, target, steps, baseline)
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        return Attributions(probs, contig, rel, length, woff, attr, logp)
 
     # ------------------------------------------------------------------ host-buffer API
     def classify_host(self, ascii_windows: np.ndarray) -> np.ndarray:

@@ -114,7 +114,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     With `attributions` ({"target": class name}), every chunk goes through the attribution calls instead
     (Classifier.attribute_ascii: the same forward step, so bitwise the same probabilities, plus each window's 5,997
     attributions in a device buffer of this rank's shard); they are collected on rank 0 in window order and stored as
-    attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).
+    attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).  With attributions["steps"] >= 1 the
+    calls are the integrated-gradients ones (Classifier.integrated_gradients_ascii, same probabilities), and the rows of
+    log p_target at the window and at the baseline travel to rank 0 the same way, as attributions["logp"] (float32 [n_windows, 2]).
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -141,10 +143,18 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 sync()
     if attributions is not None:
         d_attr = torch.empty((end - start, ATTR_TOKENS), dtype=torch.float32, device=dev)
+        ig_steps = attributions.get("steps") or 0
+        if ig_steps:
+            d_logp = torch.empty((end - start, 2), dtype=torch.float32, device=dev)
 
         def run(win, m, row):                                # probabilities and attributions from the attribution calls
             d_win = torch.from_numpy(win[:m]).to(dev)
-            probs, attr = clf.attribute_ascii(d_win, attributions["target"])
+            if ig_steps:
+                probs, logp, attr = clf.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
+                                                                   attributions["baseline"])
+                d_logp[row: row + m].copy_(logp)
+            else:
+                probs, attr = clf.attribute_ascii(d_win, attributions["target"])
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
             if embeddings:
@@ -176,6 +186,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     if attributions is not None:
         full = gdist.collect_window_probs(d_attr, n, info)
         attributions["attr"] = full.cpu().numpy() if full is not None else None
+        if ig_steps:
+            full = gdist.collect_window_probs(d_logp, n, info)
+            attributions["logp"] = full.cpu().numpy() if full is not None else None
     return out[0] if len(out) == 1 else tuple(out)
 
 
@@ -307,24 +320,76 @@ def attributions_target(value=None):
     return v
 
 
-def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr) -> None:
+ATTR_BASELINES = ("zero", "N")
+IG_METHOD = "integrated_gradients"
+
+
+def attribution_steps(value=None) -> int:
+    """Integrated-gradients steps of the attributions (``--attribution-steps N`` / GENOMAD_B200_ATTRIBUTION_STEPS=N /
+    main(..., attribution_steps=N)): 0 (the default) keeps gradient x input, N >= 1 selects integrated gradients."""
+    if value is None:
+        value = os.environ.get("GENOMAD_B200_ATTRIBUTION_STEPS", "").strip() or 0
+    from .engine import ATTR_MAX_BATCH
+    try:
+        v = int(value)
+    except (TypeError, ValueError):
+        raise ValueError(f"attribution steps must be an integer in [0, {ATTR_MAX_BATCH}], not {value!r}") from None
+    if not 0 <= v <= ATTR_MAX_BATCH:
+        raise ValueError(f"attribution steps must be in [0, {ATTR_MAX_BATCH}], not {value!r}")
+    return v
+
+
+def _check_ig_steps_fit(clf, steps: int) -> None:
+    """A window's `steps` rows share one chunk of the attribution context, which holds min(ATTR_MAX_BATCH, the classifier's
+    windows per step) rows (Classifier._attr_ctx); the step can be smaller than ATTR_MAX_BATCH on a device short of memory
+    (device_step)."""
+    from .engine import ATTR_MAX_BATCH
+    limit = min(ATTR_MAX_BATCH, int(clf.max_batch))
+    if steps > limit:
+        raise ValueError(f"attribution steps must be at most {limit} on this device (the attribution context holds {limit} "
+                         f"rows), not {steps}")
+
+
+def attribution_baseline(value=None) -> str:
+    """Baseline of integrated gradients (``--attribution-baseline {zero,N}`` / GENOMAD_B200_ATTRIBUTION_BASELINE /
+    main(..., attribution_baseline=)): "zero" (all-zero one-hot rows, the default) or "N" (the all-N window)."""
+    if value is None:
+        value = os.environ.get("GENOMAD_B200_ATTRIBUTION_BASELINE", "").strip() or "zero"
+    v = str(value).strip()
+    if v not in ATTR_BASELINES:
+        raise ValueError(f"attribution baseline must be one of {ATTR_BASELINES}, not {value!r}")
+    return v
+
+
+def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr, steps: int = 0,
+                        baseline: str = "zero", logp=None) -> None:
     # np.savez, as for the embeddings: 24 KB of fp32 per window barely compresses
     offsets = np.asarray(offsets, dtype=np.int32)
-    np.savez(path, **{names_key: names,
-                      "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
-                      "window_start": np.asarray(starts, dtype=np.int64),
-                      "window_length": np.asarray(lengths, dtype=np.int32),
-                      "target": np.str_(target),
-                      "attributions": np.asarray(attr, dtype=np.float32).reshape(-1, ATTR_TOKENS)})
+    keys = {names_key: names,
+            "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+            "window_start": np.asarray(starts, dtype=np.int64),
+            "window_length": np.asarray(lengths, dtype=np.int32),
+            "target": np.str_(target),
+            "attributions": np.asarray(attr, dtype=np.float32).reshape(-1, ATTR_TOKENS)}
+    if steps:                                       # integrated gradients; a gradient x input file keeps the keys above only
+        keys.update({"method": np.str_(IG_METHOD), "steps": np.int32(steps), "baseline": np.str_(baseline),
+                     "log_p_target": np.asarray(logp, dtype=np.float32).reshape(-1, 2)})
+    np.savez(path, **keys)
 
 
-def _attributions_current(path: Path, target: str) -> bool:
-    """The attributions file exists and was written for this class."""
+def _attributions_current(path: Path, target: str, steps: int = 0, baseline: str = "zero") -> bool:
+    """The attributions file exists and was written for this class by this method (a file without "method" is gradient x
+    input), with these integrated-gradients steps and baseline."""
     if not path.exists():
         return False
     try:
         with np.load(path) as z:
-            return str(z["target"]) == target
+            if str(z["target"]) != target:
+                return False
+            method = str(z["method"]) if "method" in z.files else "gradient_x_input"
+            if not steps:
+                return method == "gradient_x_input"
+            return method == IG_METHOD and int(z["steps"]) == steps and str(z["baseline"]) == baseline
     except Exception:
         return False
 
@@ -400,8 +465,12 @@ def contig_reduce_mode(default: str = "gather") -> str:
     return mode
 
 
+_attribution_steps, _attribution_baseline = attribution_steps, attribution_baseline
+
+
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
-         write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None):
+         write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
+         attribution_steps=None, attribution_baseline=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -415,6 +484,17 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                            else bool(write_window_scores))
     window_stride = sequence.WINDOW if window_stride is None else int(window_stride)
     attr_target = attributions_target(write_attributions)
+    # both options are validated whether or not they take effect; an option without effect is reported in the log
+    steps_opt, baseline_opt = _attribution_steps(attribution_steps), _attribution_baseline(attribution_baseline)
+    baseline_given = attribution_baseline is not None or bool(os.environ.get("GENOMAD_B200_ATTRIBUTION_BASELINE", "").strip())
+    ig_notes = []
+    if not attr_target and (steps_opt or baseline_given):
+        ig_notes.append("--attribution-steps / --attribution-baseline have no effect without --write-attributions.")
+    elif attr_target and baseline_given and not steps_opt:
+        ig_notes.append("--attribution-baseline has no effect with --attribution-steps 0 (gradient x input).")
+    ig_steps = steps_opt if attr_target else 0
+    ig_baseline = baseline_opt if ig_steps else "zero"
+    attr_method = f", integrated gradients, {ig_steps} steps, baseline {ig_baseline}" if ig_steps else ""
     if not 1 <= window_stride <= sequence.WINDOW:
         raise ValueError(f"window_stride must be in [1, {sequence.WINDOW}], not {window_stride}")
     if is_main:
@@ -445,7 +525,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         descr += ["window classification: tabular format", "window classification: binary format"]
     if attr_target:
         files.append(outputs.nn_classification_attributions_output)
-        descr.append(f"window attributions ({attr_target}): binary format")
+        descr.append(f"window attributions ({attr_target}{attr_method}): binary format")
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -459,10 +539,16 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             descr += ["provirus window classification: tabular format", "provirus window classification: binary format"]
         if attr_target:
             files.append(outputs.provirus_nn_classification_attributions_output)
-            descr.append(f"provirus window attributions ({attr_target}): binary format")
+            descr.append(f"provirus window attributions ({attr_target}{attr_method}): binary format")
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
+    for note in ig_notes:
+        console.log(f"Warning: {note}")
+    ig_clf = None
+    if ig_steps:                     # the steps must fit this device's attribution context: fail before any work
+        ig_clf = _make_classifier(batch_size, info.local_rank)
+        _check_ig_steps_fit(ig_clf, ig_steps)
 
     parsed_input = sequence.ParsedFasta(input_path, single_window, threads)      # one native index pass: check + windows
     last_timings["index_s"] = _time.perf_counter() - t_start
@@ -505,7 +591,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         plan = [(bool(skip and j[4].exists()),
                  bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
                       and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
-                      and (not attr_target or _attributions_current(j[13], attr_target))))
+                      and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -525,11 +611,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     def classifier():
         nonlocal clf_future
+        if ig_clf is not None:
+            return ig_clf
         if clf_future is None:
             clf_future = clf_pool.submit(_make_classifier, batch_size, info.local_rank)
         return clf_future.result()
 
-    if not all(cls_skip for _, cls_skip in plan):
+    if not all(cls_skip for _, cls_skip in plan) and ig_clf is None:
         clf_future = clf_pool.submit(_make_classifier, batch_size, info.local_rank)      # start now, overlap with indexing
 
     # ---- stage 1, every job: "encode" (here: record the window -> sequence map; the windows themselves are streamed to the GPU in
@@ -549,7 +637,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
          win_npz_path, win_tsv_path, attr_path), (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
         names = preds = emb = None
-        attr = {"target": attr_target} if attr_target else None      # the contig pass runs through the attribution calls
+        attr = None                     # the contig pass runs through the attribution calls
+        if attr_target:
+            attr = {"target": attr_target, **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
         win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
@@ -573,7 +663,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
                 if attr is not None:
-                    attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), spans=win[:3])
+                    attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), logp=np.zeros((0, 2), np.float32), spans=win[:3])
             else:
                 t_c = _time.perf_counter()
                 ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
@@ -604,8 +694,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                             f"{win_npz_path.name}.")
             if attr is not None:
                 if is_main:
-                    _write_attributions(attr_path, names_key, names, *attr["spans"], attr_target, attr["attr"])
-                console.log(f"{label} window attributions ({attr_target}) in binary format written to {attr_path.name}.")
+                    _write_attributions(attr_path, names_key, names, *attr["spans"], attr_target, attr["attr"], ig_steps,
+                                        ig_baseline, attr.get("logp"))
+                console.log(f"{label} window attributions ({attr_target}{attr_method}) in binary format written to "
+                            f"{attr_path.name}.")
         if parsed is not None:
             parsed.close()
         if cleanup and is_main and enc_dir.is_dir():

@@ -417,6 +417,46 @@ int gnm_attribute_ascii(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int 
 int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
                           int n, int target, float* d_probs, float* d_attr, void* stream);
 
+/*
+ * Integrated gradients (IG): attributions that add up to the change in log p_c from a baseline input x' to the window x, so that
+ * windows classified confidently as the target (where gradient x input scales as e^-margin and reaches exactly 0) get
+ * attributions too.  With m steps and the midpoint rule alpha_k = (k + 1/2) / m, k = 0..m-1, and g_k the gradient of log p_c
+ * with respect to the one-hot input at x' + alpha_k (x - x'):
+ *
+ *   GNM_IG_BASELINE_ZERO  x' = all-zero one-hot rows (the model's causal padding):   IG[t] = (1/m) sum_k g_k[t, tok[t]]
+ *   GNM_IG_BASELINE_N     x' = the all-N window (token 0 everywhere, a real input):  IG[t] = (1/m) sum_k (g_k[t, tok[t]] - g_k[t, 0]),
+ *                         and 0 where tok[t] = 0
+ *
+ *   sum_t IG[t] -> log p_c(x) - log p_c(x') as m grows (completeness; the gap at a given m is measured in
+ *   profiles/integrated_gradients_h100.md).
+ *
+ * Layer 1 at an interpolated input is lrelu(b1 + alpha S_tok + (1 - alpha) S_base) (Conv1D #1 is linear in its one-hot input);
+ * everything after it is the unchanged model, and each (window, alpha_k) row goes through the gnm_attribute_* backward pass
+ * (routing, LeakyReLU branches, head gradient, s_w: per row).  The mean over k is taken in fp32, k ascending, no atomics: the
+ * result does not depend on the batch, the chunking, fuse_l1 or tail_overlap.  DESIGN.md, "Integrated gradients".
+ *
+ * gnm_attribute_ig_ascii / gnm_attribute_ig_windows: windows as for gnm_attribute_ascii / gnm_attribute_windows (the same
+ *   bytes: no case folding for ASCII rows), in chunks of floor(max_batch / steps) windows of the context.
+ *   steps     1 <= steps <= the context's max_batch.
+ *   baseline  GNM_IG_BASELINE_ZERO or GNM_IG_BASELINE_N.
+ *   d_attr    DEVICE float [n][5997], caller-owned.
+ *   d_probs   DEVICE float [n][3] or NULL: bitwise what gnm_forward_ascii / gnm_forward_windows return.
+ *   d_logp    DEVICE float [n][2] or NULL: log p_c(x), log p_c(x') (the second column is the same in every row), from fp32
+ *             probabilities without cancellation: -log1p(sum_{i != c} p_i) when p_c is the largest, log p_c otherwise,
+ *             evaluated in fp64 and rounded to fp32.
+ *   Cost: per window one forward (when d_probs or d_logp is given) plus `steps` attribution rows, ~1 + 4.2 steps forwards;
+ *   one more one-row forward per call for log p_c(x').  No memory beyond the context's.
+ *   After the call, "route*", "routeq*", "attr_y1", "buf0", "buf1", "h2" of gnm_debug_fetch hold the last chunk's ROWS, row
+ *   w * steps + k = window w at alpha_k.  Asynchronous on `stream`; range overflows are reported as for gnm_attribute_*.
+ */
+#define GNM_IG_BASELINE_ZERO 0
+#define GNM_IG_BASELINE_N    1
+int gnm_attribute_ig_ascii(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, int steps, int baseline,
+                           float* d_probs, float* d_logp, float* d_attr, void* stream);
+int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, const int64_t* d_win_start,
+                             const int32_t* d_win_len, int n, int target, int steps, int baseline, float* d_probs, float* d_logp,
+                             float* d_attr, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

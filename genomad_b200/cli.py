@@ -93,6 +93,24 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
                 write_embeddings=True if write_embeddings else None, **extra)
 
 
+@cli.command(name="embedding-neighbours", context_settings=CONTEXT_SETTINGS)
+@click.argument("query", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("--reference", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
+              help="Embeddings file of the sequences to search (nn-classification --write-embeddings output). Without it, the "
+                   "query sequences are searched against each other, a sequence never being its own neighbour.")
+@click.option("--neighbours", "-k", type=click.IntRange(1, 64), default=10, show_default=True,
+              help="Neighbours per query sequence.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def embedding_neighbours(query, output, reference, neighbours, verbose):
+    """Find the nearest neighbours, in cosine similarity of the encoder embeddings, of every sequence of the QUERY embeddings
+    file (nn-classification --write-embeddings output) and write them to the OUTPUT directory as
+    <prefix>_embedding_neighbours.{tsv,npz}. Not a module of the reference."""
+    from . import embedding_neighbours as module
+    module.main(query, reference, output, neighbours, verbose)
+
+
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)
 @click.argument("input", type=click.Path(path_type=Path, exists=True))
 @click.argument("output", type=click.Path(path_type=Path))

@@ -23,6 +23,7 @@
 #include "wv_gather.cuh"
 #include "contigs.cuh"
 #include "attr.cuh"
+#include "neighbours.cuh"
 
 using namespace gnm;
 
@@ -1683,4 +1684,119 @@ extern "C" int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_
 extern "C" long long gnm_attr_bytes_per_window(void) {
   return static_cast<long long>(kTok) * (3 * kRowBytes + 2 * kC * 4) + 2LL * kPooled * kC * 5 +
          4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + 4);
+}
+
+// ------------------------------------------------------------------------------------------------ embedding neighbours
+// No handle: the search runs on the current device and the caller's stream, and its only memory is the caller's workspace.
+namespace {
+struct NbPlan {
+  int splits = 0, tiles_per_split = 0;
+  size_t q_hi = 0, q_lo = 0, r_hi = 0, r_lo = 0, p_sim = 0, p_idx = 0, bytes = 0;   // byte offsets into the workspace
+};
+}  // namespace
+
+static size_t nb_align(size_t x) { return (x + 255) & ~size_t(255); }
+
+static int nb_check_shape(const char* fn, int64_t n_query, int64_t n_ref, int k) {
+  if (k < 1 || k > kNbMaxK) return fail(std::string(fn) + ": k must be in [1, 64], not " + std::to_string(k));
+  if (n_query < 0 || n_ref < 0) return fail(std::string(fn) + ": negative row count");
+  if (n_query > kNbRowMax || n_ref > kNbRowMax)
+    return fail(std::string(fn) + ": more than 2^30 query or reference rows in one call (the kernels use 32-bit row offsets); "
+                "pass the reference in chunks and merge the lists with gnm_neighbours_merge");
+  return 0;
+}
+
+// Splits: enough CTAs for every SM, and at least kNbMinSplits per query tile when there are that many reference tiles.
+static int nb_plan(int64_t n_query, int64_t n_ref, int k, NbPlan* pl) {
+  int dev = 0, sms = 0;
+  GNM_CUDA(cudaGetDevice(&dev));
+  GNM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int64_t qt = (n_query + kNbBM - 1) / kNbBM, rt = (n_ref + kNbBN - 1) / kNbBN;
+  NbPlan p;
+  if (qt > 0 && rt > 0) {
+    const int64_t want = std::max<int64_t>(kNbMinSplits, (sms + qt - 1) / qt);
+    const int64_t splits = std::min<int64_t>(rt, want);
+    p.tiles_per_split = static_cast<int>((rt + splits - 1) / splits);
+    p.splits = static_cast<int>((rt + p.tiles_per_split - 1) / p.tiles_per_split);   // no empty split
+  }
+  const size_t nq = static_cast<size_t>(n_query), nr = static_cast<size_t>(n_ref);
+  size_t off = 0;
+  p.q_hi = off; off += nb_align(nq * kNbDim * 4);
+  p.q_lo = off; off += nb_align(nq * kNbDim * 4);
+  p.r_hi = off; off += nb_align(nr * kNbDim * 4);
+  p.r_lo = off; off += nb_align(nr * kNbDim * 4);
+  p.p_sim = off; off += nb_align(static_cast<size_t>(p.splits) * nq * k * 4);
+  p.p_idx = off; off += nb_align(static_cast<size_t>(p.splits) * nq * k * 4);
+  p.bytes = off;
+  *pl = p;
+  return 0;
+}
+
+extern "C" size_t gnm_neighbours_workspace_bytes(int64_t n_query, int64_t n_ref, int k) {
+  NbPlan pl;
+  if (nb_check_shape("gnm_neighbours_workspace_bytes", n_query, n_ref, k) || nb_plan(n_query, n_ref, k, &pl)) return 0;
+  return pl.bytes;
+}
+
+extern "C" int gnm_embedding_neighbours(const float* d_query, int64_t n_query, const float* d_ref, int64_t n_ref,
+                                        int64_t ref_index0, int64_t self_index0, int k, float* d_sim, int64_t* d_idx, void* d_work,
+                                        size_t work_bytes, void* stream) {
+  const char* fn = "gnm_embedding_neighbours";
+  if (nb_check_shape(fn, n_query, n_ref, k)) return 1;
+  if (ref_index0 < 0 || ref_index0 > INT64_MAX - n_ref) return fail(std::string(fn) + ": ref_index0 out of range");
+  if (self_index0 < -1) return fail(std::string(fn) + ": self_index0 must be -1 (no self-exclusion) or >= 0");
+  if (n_query == 0) return 0;
+  if (!d_query || !d_sim || !d_idx || (n_ref > 0 && (!d_ref || !d_work))) return fail(std::string(fn) + ": null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_query) | reinterpret_cast<uintptr_t>(d_ref)) % 16)
+    return fail(std::string(fn) + ": d_query and d_ref must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(std::string(fn) + ": d_work must be 256-byte aligned");
+  NbPlan pl;
+  if (nb_plan(n_query, n_ref, k, &pl)) return 1;
+  if (n_ref > 0 && work_bytes < pl.bytes)
+    return fail(std::string(fn) + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(pl.bytes) +
+                " needed (gnm_neighbours_workspace_bytes)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nq = static_cast<int>(n_query), nr = static_cast<int>(n_ref);
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  float* part_sim = nullptr; int32_t* part_idx = nullptr;
+  if (nr > 0) {
+    float* q_hi = reinterpret_cast<float*>(w + pl.q_hi); float* q_lo = reinterpret_cast<float*>(w + pl.q_lo);
+    float* r_hi = reinterpret_cast<float*>(w + pl.r_hi); float* r_lo = reinterpret_cast<float*>(w + pl.r_lo);
+    part_sim = reinterpret_cast<float*>(w + pl.p_sim); part_idx = reinterpret_cast<int32_t*>(w + pl.p_idx);
+    nb_prep_kernel<<<(nq + 7) / 8, 256, 0, st>>>(d_query, nq, q_hi, q_lo);
+    nb_prep_kernel<<<(nr + 7) / 8, 256, 0, st>>>(d_ref, nr, r_hi, r_lo);
+    GNM_CUDA(cudaGetLastError());
+    PFN_encodeTiled enc = nullptr;
+    if (get_encode_fn(&enc)) return 1;
+    CUtensorMap tm[4];
+    if (make_f32_map(enc, &tm[0], q_hi, kNbDim, nq, kNbBM) || make_f32_map(enc, &tm[1], q_lo, kNbDim, nq, kNbBM) ||
+        make_f32_map(enc, &tm[2], r_hi, kNbDim, nr, kNbBN) || make_f32_map(enc, &tm[3], r_lo, kNbDim, nr, kNbBN))
+      return 1;
+    NbSearchParams p;
+    p.part_sim = part_sim; p.part_idx = part_idx;
+    p.n_query = nq; p.n_ref = nr; p.k = k; p.tiles_per_split = pl.tiles_per_split;
+    p.self_off = self_index0 < 0 ? LLONG_MIN : static_cast<long long>(self_index0 - ref_index0);
+    p.status = nullptr;
+    const int smem = nb_smem_bytes(k);
+    GNM_CUDA(cudaFuncSetAttribute(nb_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    dim3 grid(pl.splits, (nq + kNbBM - 1) / kNbBM);
+    nb_search_kernel<<<grid, kNbThreads, smem, st>>>(tm[0], tm[1], tm[2], tm[3], p);
+    GNM_CUDA(cudaGetLastError());
+  }
+  nb_finalize_kernel<<<(nq + 7) / 8, 256, 0, st>>>(part_sim, part_idx, pl.splits, nq, k, static_cast<long long>(ref_index0),
+                                                   d_sim, reinterpret_cast<long long*>(d_idx));
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gnm_neighbours_merge(float* d_sim, int64_t* d_idx, const float* d_sim_b, const int64_t* d_idx_b, int64_t n_query,
+                                    int k, void* stream) {
+  if (nb_check_shape("gnm_neighbours_merge", n_query, 0, k)) return 1;
+  if (n_query == 0) return 0;
+  if (!d_sim || !d_idx || !d_sim_b || !d_idx_b) return fail("gnm_neighbours_merge: null buffer");
+  const int nq = static_cast<int>(n_query);
+  nb_merge_kernel<<<(nq + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      d_sim, reinterpret_cast<long long*>(d_idx), d_sim_b, reinterpret_cast<const long long*>(d_idx_b), nq, k);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
 }

@@ -66,6 +66,12 @@ __device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t da, ui
                : GNM_ACC8(0), GNM_ACC8(8), GNM_ACC8(16), GNM_ACC8(24), GNM_ACC8(32), GNM_ACC8(40), GNM_ACC8(48), GNM_ACC8(56), GNM_ACC8(64), GNM_ACC8(72), GNM_ACC8(80), GNM_ACC8(88), GNM_ACC8(96), GNM_ACC8(104), GNM_ACC8(112), GNM_ACC8(120)
                : "l"(da), "l"(db), "r"(accumulate));
 }
+__device__ __forceinline__ void wgmma_tf32_n192(float (&d)[96], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %98, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95}, %96,%97,p,1,1;\n}"
+               : GNM_ACC8(0), GNM_ACC8(8), GNM_ACC8(16), GNM_ACC8(24), GNM_ACC8(32), GNM_ACC8(40), GNM_ACC8(48), GNM_ACC8(56), GNM_ACC8(64), GNM_ACC8(72), GNM_ACC8(80), GNM_ACC8(88)
+               : "l"(da), "l"(db), "r"(accumulate));
+}
 #undef GNM_ACC8
 
 }  // namespace gnm

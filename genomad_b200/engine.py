@@ -92,6 +92,10 @@ EXPORTS = {
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_attribute_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                            C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_neighbours_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
+    "gnm_embedding_neighbours": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "gnm_neighbours_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
     "gnm_fasta_last_error": (C.c_char_p, []),
     "gnm_fasta_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_open_gz": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -146,6 +150,81 @@ def _check(lib, rc: int):
 
 def _ptr(a: np.ndarray) -> int:
     return a.ctypes.data
+
+
+NEIGHBOURS_MAX_K = 64
+NEIGHBOURS_CHUNK = 1 << 18       # reference rows per gnm_embedding_neighbours call: 1 GB of TF32 halves, whatever the input size
+
+
+def _neighbours_args(t, rows, name):
+    assert rows.dtype == t.float32 and rows.dim() == 2 and rows.shape[1] == EMBED and rows.is_cuda, \
+        f"{name}: float32 cuda tensor [n, {EMBED}] expected"
+    return rows.contiguous()
+
+
+def _neighbours_k(k) -> int:
+    k = int(k)
+    if not 1 <= k <= NEIGHBOURS_MAX_K:
+        raise ValueError(f"k must be in [1, {NEIGHBOURS_MAX_K}], not {k}")
+    return k
+
+
+def embedding_neighbours(query, reference=None, k: int = 10, *, ref_index0: int = 0, self_index0: Optional[int] = None):
+    """The k nearest reference rows of every query row in cosine similarity (gnm_embedding_neighbours, include/gnm.h).
+
+    query float32 cuda [nq, 512]; reference float32 cuda [nr, 512] on the same device, or None for all-vs-all: the query rows
+    are the reference and query i never returns itself.  Returns cuda tensors (sim float32 [nq, k], idx int64 [nq, k]), row q
+    sorted by (similarity descending, index ascending) and padded with (-inf, -1) when fewer than k references qualify.
+    Indices are ref_index0 + reference row; self_index0 (default: ref_index0 for all-vs-all, none otherwise) excludes global
+    index self_index0 + q from query q's list.  The reference is searched NEIGHBOURS_CHUNK rows per call, the lists merged on
+    the device (gnm_neighbours_merge): the result is bitwise that of one call over all rows."""
+    import torch as t
+    k = _neighbours_k(k)
+    q = _neighbours_args(t, query, "query")
+    ref = q if reference is None else _neighbours_args(t, reference, "reference")
+    if ref.device != q.device:
+        raise ValueError("query and reference must be on the same device")
+    self0 = (ref_index0 if reference is None else -1) if self_index0 is None else int(self_index0)
+    lib = load_library()
+    nq, nr = q.shape[0], ref.shape[0]
+    sim = t.empty((nq, k), dtype=t.float32, device=q.device)
+    idx = t.empty((nq, k), dtype=t.int64, device=q.device)
+    with t.cuda.device(q.device):
+        stream = t.cuda.current_stream(q.device).cuda_stream
+        work = t.empty(0, dtype=t.uint8, device=q.device)
+        part = None
+        for a in range(0, max(nr, 1), NEIGHBOURS_CHUNK):
+            b = min(nr, a + NEIGHBOURS_CHUNK)
+            need = int(lib.gnm_neighbours_workspace_bytes(nq, b - a, k))
+            if need == 0 and nq:
+                _check(lib, 1)
+            if need > work.numel():
+                work = t.empty(need, dtype=t.uint8, device=q.device)
+            if a and part is None:
+                part = (t.empty_like(sim), t.empty_like(idx))
+            s_out, i_out = (sim, idx) if a == 0 else part
+            _check(lib, lib.gnm_embedding_neighbours(q.data_ptr(), nq, ref[a:b].data_ptr() if b > a else None, b - a,
+                                                     int(ref_index0) + a, self0, k, s_out.data_ptr(), i_out.data_ptr(),
+                                                     work.data_ptr(), work.numel(), stream))
+            if a:
+                _check(lib, lib.gnm_neighbours_merge(sim.data_ptr(), idx.data_ptr(), s_out.data_ptr(), i_out.data_ptr(), nq, k,
+                                                     stream))
+    return sim, idx
+
+
+def neighbours_merge(sim, idx, sim_b, idx_b):
+    """Merge the neighbour lists (sim_b, idx_b) into (sim, idx) in place (cuda float32 / int64 [nq, k]; gnm_neighbours_merge)."""
+    import torch as t
+    assert sim.dtype == sim_b.dtype == t.float32 and idx.dtype == idx_b.dtype == t.int64 and sim.is_cuda
+    assert sim.shape == idx.shape == sim_b.shape == idx_b.shape and sim.dim() == 2
+    assert sim.is_contiguous() and idx.is_contiguous()
+    sb, ib = sim_b.contiguous(), idx_b.contiguous()
+    k = _neighbours_k(sim.shape[1])
+    lib = load_library()
+    with t.cuda.device(sim.device):
+        _check(lib, lib.gnm_neighbours_merge(sim.data_ptr(), idx.data_ptr(), sb.data_ptr(), ib.data_ptr(), sim.shape[0], k,
+                                             t.cuda.current_stream(sim.device).cuda_stream))
+    return sim, idx
 
 
 class WindowScores(NamedTuple):

@@ -457,6 +457,38 @@ int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, c
                              const int32_t* d_win_len, int n, int target, int steps, int baseline, float* d_probs, float* d_logp,
                              float* d_attr, void* stream);
 
+/*
+ * Embedding neighbours: for each query row, the k reference rows nearest in cosine similarity.  Rows are GNM_EMBED (512) fp32
+ * values (the encoder embeddings of gnm_embed_*), finite, contiguous, row pitch 2 KB.  No handle, no allocation: the calls run on
+ * the current device and `stream`, and use only the caller's workspace.  DESIGN.md, "Embedding neighbours".
+ *
+ *   similarity   s(q, r) = <q / |q|, r / |r|>, |x| the fp32 norm summed in a fixed order; a row of norm 0 becomes the zero row,
+ *                so its similarity with every row is 0.  Computed on the tensor cores as three TF32 products of the split rows
+ *                (hi * hi + lo * hi + hi * lo) in one fp32 accumulator, K ascending: |s - exact| is about 1e-6, and a pair's s
+ *                is bitwise the same whatever call, chunk, tile or offset computes it.
+ *   order        (s descending, global reference index ascending): ties, such as duplicate rows, go to the lower index.
+ *   result       d_sim [n_query][k] float, d_idx [n_query][k] int64 (DEVICE): row q holds query q's k first references under
+ *                that order; global index = ref_index0 + reference row.  When fewer than k references qualify, the list is
+ *                padded with index -1 and similarity -inf.
+ *   self         self_index0 >= 0: query q never returns global index self_index0 + q (all-vs-all: pass the same rows as
+ *                query and reference with self_index0 = ref_index0).  -1: no exclusion.
+ *
+ * gnm_neighbours_workspace_bytes: the bytes of d_work a call with these sizes needs on the current device (0 on invalid
+ *   arguments, see gnm_last_error): the normalised rows of both sets as TF32 halves (4 KB per row) and the partial lists of the
+ *   reference splits (8 k bytes per query and split).
+ * gnm_embedding_neighbours: 1 <= k <= 64; 0 <= n_query, n_ref <= 2^30 (more reference rows: call once per chunk with its
+ *   ref_index0 and merge); d_query, d_ref 16-byte aligned, d_work 256-byte aligned.  n_ref = 0 gives padded lists.
+ * gnm_neighbours_merge: merges the lists (d_sim_b, d_idx_b) into (d_sim, d_idx), in place, under the same order: the result of a
+ *   call over references A followed by a merge of the result over a disjoint set B is bitwise the result of one call over A + B.
+ *   Both inputs must be lists of this form (sorted, padded at the end).
+ */
+size_t gnm_neighbours_workspace_bytes(int64_t n_query, int64_t n_ref, int k);
+int gnm_embedding_neighbours(const float* d_query, int64_t n_query, const float* d_ref, int64_t n_ref, int64_t ref_index0,
+                             int64_t self_index0, int k, float* d_sim, int64_t* d_idx, void* d_work, size_t work_bytes,
+                             void* stream);
+int gnm_neighbours_merge(float* d_sim, int64_t* d_idx, const float* d_sim_b, const int64_t* d_idx_b, int64_t n_query, int k,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

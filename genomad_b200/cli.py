@@ -111,6 +111,23 @@ def embedding_neighbours(query, output, reference, neighbours, verbose):
     module.main(query, reference, output, neighbours, verbose)
 
 
+@cli.command(name="embedding-clusters", context_settings=CONTEXT_SETTINGS)
+@click.argument("input", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("--min-similarity", type=click.FloatRange(0, 1, min_open=True), required=True,
+              help="Cosine similarity a sequence needs with a representative to join its cluster, in (0, 1]. No default: "
+                   "which level separates what in this embedding space has not been measured.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def embedding_clusters(input, output, min_similarity, verbose):
+    """Cluster the sequences of the INPUT embeddings file (nn-classification --write-embeddings output) greedily, in file
+    order, at a cosine similarity threshold of the encoder embeddings, and write each sequence's representative to the OUTPUT
+    directory as <prefix>_embedding_clusters.{tsv,npz}. A representative is the first member of its cluster in file order.
+    Not a module of the reference."""
+    from . import embedding_clusters as module
+    module.main(input, output, min_similarity, verbose)
+
+
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)
 @click.argument("input", type=click.Path(path_type=Path, exists=True))
 @click.argument("output", type=click.Path(path_type=Path))

@@ -24,6 +24,7 @@
 #include "contigs.cuh"
 #include "attr.cuh"
 #include "neighbours.cuh"
+#include "clusters.cuh"
 
 using namespace gnm;
 
@@ -1797,6 +1798,62 @@ extern "C" int gnm_neighbours_merge(float* d_sim, int64_t* d_idx, const float* d
   const int nq = static_cast<int>(n_query);
   nb_merge_kernel<<<(nq + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       d_sim, reinterpret_cast<long long*>(d_idx), d_sim_b, reinterpret_cast<const long long*>(d_idx_b), nq, k);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ embedding clusters
+// Workspace: the block's TF32 halves (nb_prep_kernel), then the threshold mask [n][ceil(n / 32)] words.
+static size_t cl_mask_offset(int64_t n) { return 2 * nb_align(static_cast<size_t>(n) * kNbDim * 4); }
+static int cl_words(int64_t n) { return static_cast<int>((n + 31) / 32); }
+
+extern "C" size_t gnm_cluster_block_workspace_bytes(int64_t n_block) {
+  if (n_block < 0 || n_block > kClMaxBlock) {
+    fail("gnm_cluster_block_workspace_bytes: n_block must be in [0, " + std::to_string(kClMaxBlock) + "], not " +
+         std::to_string(n_block));
+    return 0;
+  }
+  return cl_mask_offset(n_block) + nb_align(static_cast<size_t>(n_block) * cl_words(n_block) * 4);
+}
+
+extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
+                                 int32_t* d_new_reps, int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream) {
+  const char* fn = "gnm_cluster_block";
+  if (n_block < 0 || n_block > kClMaxBlock)
+    return fail(std::string(fn) + ": n_block must be in [0, " + std::to_string(kClMaxBlock) + "], not " + std::to_string(n_block));
+  if (!(min_similarity > 0.f && min_similarity <= 1.f))
+    return fail(std::string(fn) + ": min_similarity must be in (0, 1], not " + std::to_string(min_similarity));
+  if (!d_n_new || (n_block > 0 && (!d_rows || !d_covered || !d_new_reps || !d_work))) return fail(std::string(fn) + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_rows) % 16) return fail(std::string(fn) + ": d_rows must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(std::string(fn) + ": d_work must be 256-byte aligned");
+  const size_t need = gnm_cluster_block_workspace_bytes(n_block);
+  if (work_bytes < need)
+    return fail(std::string(fn) + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(need) +
+                " needed (gnm_cluster_block_workspace_bytes)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int n = static_cast<int>(n_block), words = cl_words(n);
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  float* hi = reinterpret_cast<float*>(w);
+  float* lo = reinterpret_cast<float*>(w + nb_align(static_cast<size_t>(n) * kNbDim * 4));
+  uint32_t* mask = reinterpret_cast<uint32_t*>(w + cl_mask_offset(n));
+  if (n > 0) nb_prep_kernel<<<(n + 7) / 8, 256, 0, st>>>(d_rows, n, hi, lo);
+  GNM_CUDA(cudaGetLastError());
+  const int rt = n > 0 ? nb_mask_tiles((n - 1) / kNbBM * kNbBM, n) : 0;     // the last query tile needs the most
+  if (rt > 0) {
+    PFN_encodeTiled enc = nullptr;
+    if (get_encode_fn(&enc)) return 1;
+    CUtensorMap tm[4];
+    if (make_f32_map(enc, &tm[0], hi, kNbDim, n, kNbBM) || make_f32_map(enc, &tm[1], lo, kNbDim, n, kNbBM) ||
+        make_f32_map(enc, &tm[2], hi, kNbDim, n, kNbBN) || make_f32_map(enc, &tm[3], lo, kNbDim, n, kNbBN))
+      return 1;
+    NbMaskParams p;
+    p.mask = mask; p.n = n; p.words = words; p.tiles_per_split = kClMaskTiles; p.thr = min_similarity; p.status = nullptr;
+    GNM_CUDA(cudaFuncSetAttribute(nb_mask_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kClMaskSmem));
+    dim3 grid((rt + kClMaskTiles - 1) / kClMaskTiles, (n + kNbBM - 1) / kNbBM);
+    nb_mask_kernel<<<grid, kNbThreads, kClMaskSmem, st>>>(tm[0], tm[1], tm[2], tm[3], p);
+    GNM_CUDA(cudaGetLastError());
+  }
+  cl_resolve_kernel<<<1, kClThreads, 0, st>>>(mask, n, words, d_covered, d_new_reps, d_n_new);
   GNM_CUDA(cudaGetLastError());
   return 0;
 }

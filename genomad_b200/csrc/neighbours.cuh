@@ -115,6 +115,63 @@ __device__ __forceinline__ void nb_offer(float v, int col, int rowl, int self_co
   }
 }
 
+// The mainloop shared by nb_search_kernel and nb_mask_kernel (clusters.cuh), so that a pair's similarity has the same bits in
+// both: the same TMA ring, the same wgmma sequence over the same operand bits.  A CTA of kNbThreads: warp 0 lane 0 produces,
+// warpgroups 1 and 2 consume; the ring is smem[0, kNbStages * kNbStageBytes) with barriers full / empty.
+__device__ __forceinline__ void nb_ring_init(const CUtensorMap* tm_q_hi, const CUtensorMap* tm_q_lo, const CUtensorMap* tm_r_hi,
+                                             const CUtensorMap* tm_r_lo, uint64_t* full, uint64_t* empty) {
+  tma_prefetch_desc(tm_q_hi); tma_prefetch_desc(tm_q_lo); tma_prefetch_desc(tm_r_hi); tma_prefetch_desc(tm_r_lo);
+  for (int i = 0; i < kNbStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
+  fence_barrier_init();
+}
+
+// TMA producer: query tile m0 against reference tiles t0 .. t0 + nt - 1, K chunks ascending.
+__device__ __forceinline__ void nb_produce(const CUtensorMap* tm_q_hi, const CUtensorMap* tm_q_lo, const CUtensorMap* tm_r_hi,
+                                           const CUtensorMap* tm_r_lo, uint8_t* smem, uint64_t* full, uint64_t* empty, int m0,
+                                           int t0, int nt, DeviceStatus* status) {
+  const uint64_t pol = l2_policy_evict_last();       // Q is re-read for every reference tile, R by every resident query tile
+  for (int it = 0; it < nt * kNbChunks; ++it) {
+    const int s = it % kNbStages;
+    const uint32_t ph = (it / kNbStages) & 1;
+    mbar_wait(&empty[s], ph ^ 1, status, 700 + s);
+    mbar_arrive_expect_tx(&full[s], kNbStageBytes);
+    uint8_t* st = smem + s * kNbStageBytes;
+    const int k0 = (it % kNbChunks) * kNbBK, r0 = (t0 + it / kNbChunks) * kNbBN;
+    tma_load_2d_hint(st, tm_q_hi, &full[s], k0, m0, pol);
+    tma_load_2d_hint(st + kNbATile, tm_q_lo, &full[s], k0, m0, pol);
+    tma_load_2d_hint(st + 2 * kNbATile, tm_r_hi, &full[s], k0, r0, pol);
+    tma_load_2d_hint(st + 2 * kNbATile + kNbBTile, tm_r_lo, &full[s], k0, r0, pol);
+  }
+}
+
+// Consumer warpgroup g: the tile tt of its run, S = Qhi Rhi + Qlo Rhi + Qhi Rlo per K = 8 step, K chunks ascending, into d
+// (register i holds row 8 ((i >> 1) & 1) + lane / 4 of the warp's 16, column 8 (i >> 2) + 2 (lane % 4) + (i & 1); wgmma.cuh).
+__device__ __forceinline__ void nb_tile_mma(float (&d)[96], uint32_t base, uint64_t* full, uint64_t* empty, int g, int tt,
+                                            DeviceStatus* status) {
+  const int lane = threadIdx.x & 31;
+  for (int c = 0; c < kNbChunks; ++c) {
+    const int it = tt * kNbChunks + c;
+    const int s = it % kNbStages;
+    const uint32_t ph = (it / kNbStages) & 1;
+    mbar_wait(&full[s], ph, status, 710 + s);
+    const uint32_t st = base + s * kNbStageBytes;
+    const uint64_t q_hi = gmma_desc_sw128(st + g * 64 * 128), q_lo = gmma_desc_sw128(st + kNbATile + g * 64 * 128);
+    const uint64_t r_hi = gmma_desc_sw128(st + 2 * kNbATile), r_lo = gmma_desc_sw128(st + 2 * kNbATile + kNbBTile);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kNbBK / 8; ++kk) {                   // K = 8 TF32 = 32 bytes per instruction
+      wgmma_tf32_n192(d, q_hi + kk * 2, r_hi + kk * 2, (c == 0 && kk == 0) ? 0u : 1u);
+      wgmma_tf32_n192(d, q_lo + kk * 2, r_hi + kk * 2, 1u);
+      wgmma_tf32_n192(d, q_hi + kk * 2, r_lo + kk * 2, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);                      // the stage may be refilled
+  }
+  wgmma_fence_regs(d);
+}
+
 __global__ void __launch_bounds__(kNbThreads, 1)
 nb_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constant__ CUtensorMap tm_q_lo,
                  const __grid_constant__ CUtensorMap tm_r_hi, const __grid_constant__ CUtensorMap tm_r_lo, const NbSearchParams p) {
@@ -131,29 +188,13 @@ nb_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_const
   const int t0 = split * p.tiles_per_split;
   const int nt = min(p.tiles_per_split, (p.n_ref + kNbBN - 1) / kNbBN - t0);    // >= 1 by construction of the grid
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_q_hi); tma_prefetch_desc(&tm_q_lo); tma_prefetch_desc(&tm_r_hi); tma_prefetch_desc(&tm_r_lo);
-    for (int i = 0; i < kNbStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
-    fence_barrier_init();
-  }
+  if (warp == 0 && lane == 0) nb_ring_init(&tm_q_hi, &tm_q_lo, &tm_r_hi, &tm_r_lo, full, empty);
   for (int i = threadIdx.x; i < kNbBM * k; i += kNbThreads) { lsim[i] = -CUDART_INF_F; lidx[i] = -1; }
   __syncthreads();
 
   if (warp == 0 && lane == 0) {
     // ===================================================================== TMA producer
-    const uint64_t pol = l2_policy_evict_last();       // Q is re-read for every reference tile, R by every resident query tile
-    for (int it = 0; it < nt * kNbChunks; ++it) {
-      const int s = it % kNbStages;
-      const uint32_t ph = (it / kNbStages) & 1;
-      mbar_wait(&empty[s], ph ^ 1, p.status, 700 + s);
-      mbar_arrive_expect_tx(&full[s], kNbStageBytes);
-      uint8_t* st = smem + s * kNbStageBytes;
-      const int k0 = (it % kNbChunks) * kNbBK, r0 = (t0 + it / kNbChunks) * kNbBN;
-      tma_load_2d_hint(st, &tm_q_hi, &full[s], k0, m0, pol);
-      tma_load_2d_hint(st + kNbATile, &tm_q_lo, &full[s], k0, m0, pol);
-      tma_load_2d_hint(st + 2 * kNbATile, &tm_r_hi, &full[s], k0, r0, pol);
-      tma_load_2d_hint(st + 2 * kNbATile + kNbBTile, &tm_r_lo, &full[s], k0, r0, pol);
-    }
+    nb_produce(&tm_q_hi, &tm_q_lo, &tm_r_hi, &tm_r_lo, smem, full, empty, m0, t0, nt, p.status);
   } else if (warp >= 4) {
     // ===================================================================== MMA + top-k: warpgroup g owns queries 64 g .. 64 g + 63
     const int g = (warp >> 2) - 1, wq = warp & 3;
@@ -169,27 +210,7 @@ nb_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_const
     int wi[2] = {-1, -1}, wp[2] = {k - 1, k - 1};
     float d[96];
     for (int tt = 0; tt < nt; ++tt) {
-      for (int c = 0; c < kNbChunks; ++c) {
-        const int it = tt * kNbChunks + c;
-        const int s = it % kNbStages;
-        const uint32_t ph = (it / kNbStages) & 1;
-        mbar_wait(&full[s], ph, p.status, 710 + s);
-        const uint32_t st = base + s * kNbStageBytes;
-        const uint64_t q_hi = gmma_desc_sw128(st + g * 64 * 128), q_lo = gmma_desc_sw128(st + kNbATile + g * 64 * 128);
-        const uint64_t r_hi = gmma_desc_sw128(st + 2 * kNbATile), r_lo = gmma_desc_sw128(st + 2 * kNbATile + kNbBTile);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < kNbBK / 8; ++kk) {                   // K = 8 TF32 = 32 bytes per instruction
-          wgmma_tf32_n192(d, q_hi + kk * 2, r_hi + kk * 2, (c == 0 && kk == 0) ? 0u : 1u);
-          wgmma_tf32_n192(d, q_lo + kk * 2, r_hi + kk * 2, 1u);
-          wgmma_tf32_n192(d, q_hi + kk * 2, r_lo + kk * 2, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);                      // the stage may be refilled
-      }
-      wgmma_fence_regs(d);
+      nb_tile_mma(d, base, full, empty, g, tt, p.status);
       // ------------------------------------------------------------------- top-k: register i holds row 8 ((i >> 1) & 1) + ...,
       // column 8 (i >> 2) + 2 (lane % 4) + (i & 1) of the tile (wgmma.cuh)
       const int n0 = (t0 + tt) * kNbBN + 2 * (lane & 3);

@@ -83,15 +83,16 @@ def _device(info):
     return torch.device("cuda", info.local_rank) if torch.cuda.is_available() else torch.device("cpu")
 
 
-def search(query: np.ndarray, reference: Optional[np.ndarray], k: int, info) -> Optional[Tuple[np.ndarray, np.ndarray]]:
+def search(query, reference, k: int, info) -> Optional[Tuple[np.ndarray, np.ndarray]]:
     """This rank's reference shard searched on the device, the lists gathered on rank 0 and merged there in rank order.
-    Returns (sim float32 [n, k], idx int64 [n, k]) on rank 0, None on the others.  reference None: all-vs-all."""
+    Returns (sim float32 [n, k], idx int64 [n, k]) on rank 0, None on the others.  reference None: all-vs-all.  query and
+    reference are NumPy arrays, or tensors already on this rank's device (embedding_clusters keeps its rows there)."""
     import torch
     dev = _device(info)
     ref = query if reference is None else reference
     s, e = dist.shard_bounds(ref.shape[0], info.world_size, info.rank)
-    q = torch.from_numpy(query).to(dev)
-    r = torch.from_numpy(ref[s:e]).to(dev)
+    q = torch.as_tensor(query).to(dev)
+    r = torch.as_tensor(ref[s:e]).to(dev)
     sim, idx = engine.embedding_neighbours(q, r, k, ref_index0=s, self_index0=0 if reference is None else -1)
     if info.world_size > 1:
         if not info.is_main:

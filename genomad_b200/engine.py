@@ -96,6 +96,9 @@ EXPORTS = {
     "gnm_embedding_neighbours": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "gnm_neighbours_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                    C.c_void_p]),
     "gnm_fasta_last_error": (C.c_char_p, []),
     "gnm_fasta_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_open_gz": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -225,6 +228,48 @@ def neighbours_merge(sim, idx, sim_b, idx_b):
         _check(lib, lib.gnm_neighbours_merge(sim.data_ptr(), idx.data_ptr(), sb.data_ptr(), ib.data_ptr(), sim.shape[0], k,
                                              t.cuda.current_stream(sim.device).cuda_stream))
     return sim, idx
+
+
+CLUSTER_MAX_BLOCK = 8192         # rows per gnm_cluster_block call: a threshold mask of 8 MB
+
+
+def cluster_threshold(min_similarity) -> float:
+    """The clustering threshold rounded once to fp32 (as a Python float); ValueError outside (0, 1]."""
+    t = float(np.float32(min_similarity))
+    if not 0.0 < t <= 1.0:
+        raise ValueError(f"min_similarity must be in (0, 1], not {min_similarity}")
+    return t
+
+
+def cluster_block(rows, covered, min_similarity):
+    """One block step of greedy clustering (gnm_cluster_block, include/gnm.h).
+
+    rows float32 cuda [n, 512], n <= CLUSTER_MAX_BLOCK: the block's rows in file order; covered uint8 cuda [n]: nonzero where an
+    earlier block's representative has similarity >= min_similarity with the row (embedding_neighbours at k = 1, the row as the
+    query).  Returns the block's new representatives as block-local row indices, int64 cuda, ascending: row j is one iff it is not
+    covered and s(j, i) < min_similarity for every new representative i < j, each comparison bitwise that of the search's
+    similarity.  Waits for the device to read the count."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    n = x.shape[0]
+    if n > CLUSTER_MAX_BLOCK:
+        raise ValueError(f"a block holds at most {CLUSTER_MAX_BLOCK} rows, not {n}")
+    assert covered.dtype == t.uint8 and covered.shape == (n,) and covered.device == x.device, \
+        "covered: uint8 tensor [n] on the rows' device expected"
+    thr = cluster_threshold(min_similarity)
+    cov = covered.contiguous()
+    lib = load_library()
+    with t.cuda.device(x.device):
+        need = int(lib.gnm_cluster_block_workspace_bytes(n))
+        if need == 0 and n:
+            _check(lib, 1)
+        work = t.empty(need, dtype=t.uint8, device=x.device)
+        reps = t.empty(max(n, 1), dtype=t.int32, device=x.device)
+        count = t.empty(1, dtype=t.int32, device=x.device)
+        _check(lib, lib.gnm_cluster_block(x.data_ptr(), n, cov.data_ptr(), thr, reps.data_ptr(), count.data_ptr(),
+                                          work.data_ptr(), need, t.cuda.current_stream(x.device).cuda_stream))
+        m = int(count.item())
+    return reps[:m].long()
 
 
 class WindowScores(NamedTuple):

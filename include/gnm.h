@@ -489,6 +489,33 @@ int gnm_embedding_neighbours(const float* d_query, int64_t n_query, const float*
 int gnm_neighbours_merge(float* d_sim, int64_t* d_idx, const float* d_sim_b, const int64_t* d_idx_b, int64_t n_query, int k,
                          void* stream);
 
+/*
+ * Embedding clusters: one block step of greedy clustering at a cosine threshold t.  Rows are processed in file order, block by
+ * block; row j is a representative iff s(j, i) < t for every representative i < j, where s(a, b) is the similarity
+ * gnm_embedding_neighbours returns for QUERY row a and REFERENCE row b (s is not bitwise symmetric: the row being placed is
+ * always the query, the candidate representative always the reference).  Same rules as the neighbour calls: no handle, no
+ * allocation, the current device and `stream`.  DESIGN.md, "Embedding clusters".
+ *
+ * The caller finds the covered rows of the block, those whose best representative of earlier blocks has s >= t, with
+ * gnm_embedding_neighbours at k = 1 against those representatives; this call decides the rest against the block itself:
+ *   d_rows          DEVICE float [n_block][512], 16-byte aligned: the block's rows in file order.
+ *   d_covered       DEVICE uint8 [n_block]: nonzero = covered by a representative of an earlier block.
+ *   min_similarity  t in (0, 1] (fp32).
+ *   d_new_reps      DEVICE int32 [n_block]: the block's new representatives, block-local rows, ascending; row j is one iff it is
+ *                   not covered and s(j, i) < t for every new representative i < j of the block.
+ *   d_n_new         DEVICE int32 [1]: their count.
+ * Each in-block comparison s(j, i) >= t is computed by the search's own tensor-core mainloop, so it is bitwise the comparison of
+ * the similarity gnm_embedding_neighbours returns for that pair.  A zero row has s = 0 with every row, so it is never covered
+ * and never covers.
+ *
+ * gnm_cluster_block_workspace_bytes: the bytes of d_work (256-byte aligned) a block of n_block rows needs (0 on invalid
+ *   arguments, and for n_block = 0): TF32 halves of the rows (4 KB per row) and the threshold mask (n_block * ceil(n_block / 32)
+ *   words; 8 MB at the largest block).  0 <= n_block <= 8192.
+ */
+size_t gnm_cluster_block_workspace_bytes(int64_t n_block);
+int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity, int32_t* d_new_reps,
+                      int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1775,12 +1775,13 @@ extern "C" int gnm_embedding_neighbours(const float* d_query, int64_t n_query, c
       return 1;
     NbSearchParams p;
     p.part_sim = part_sim; p.part_idx = part_idx;
-    p.n_query = nq; p.n_ref = nr; p.k = k; p.tiles_per_split = pl.tiles_per_split;
+    p.n_query = nq; p.n_ref = nr; p.k = k; p.splits = pl.splits; p.tiles_per_split = pl.tiles_per_split;
     p.self_off = self_index0 < 0 ? LLONG_MIN : static_cast<long long>(self_index0 - ref_index0);
     p.status = nullptr;
     const int smem = nb_smem_bytes(k);
     GNM_CUDA(cudaFuncSetAttribute(nb_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    dim3 grid(pl.splits, (nq + kNbBM - 1) / kNbBM);
+    // one CTA per (query tile, split), split fastest; at most 2^23 query tiles x max(8, #SMs) splits, inside gridDim.x's 2^31 - 1
+    const unsigned grid = static_cast<unsigned>(pl.splits) * static_cast<unsigned>((nq + kNbBM - 1) / kNbBM);
     nb_search_kernel<<<grid, kNbThreads, smem, st>>>(tm[0], tm[1], tm[2], tm[3], p);
     GNM_CUDA(cudaGetLastError());
   }

@@ -1,8 +1,9 @@
 // Nearest neighbours in the encoder's embedding space (gnm_embedding_neighbours, include/gnm.h): for every query row, the k
 // reference rows of highest cosine similarity, under the total order (similarity descending, reference index ascending).
 //
-//   nb_prep_kernel      one warp per 512-wide row: the fp32 norm (each lane sums its 16 squares in order, then a fixed xor
-//                       butterfly), x / norm (a zero norm gives the zero row), and the TF32 halves of split_tf32 (logits_tc.cuh)
+//   nb_prep_kernel      one warp per 512-wide row: the row prescaled by the power of two that brings its max |x| into [1, 2), the
+//                       fp32 norm (each lane sums its 16 squares in order, then a fixed xor butterfly), x / norm (a zero norm
+//                       gives the zero row), and the TF32 halves of split_tf32 (logits_tc.cuh)
 //                       as two row-major [n][512] fp32 matrices that TMA reads as 128-byte-swizzled K-major tiles.
 //   nb_search_kernel    the similarity tile S = Q R^T of 128 queries x 192 references on the tensor cores with the recipe of
 //                       logits_tc_kernel (D = Qhi Rhi + Qlo Rhi + Qhi Rlo per K = 8 step, K chunks of 32 in ascending order, one
@@ -44,6 +45,7 @@ struct NbSearchParams {
   float* part_sim;          // [splits][n_query][k], each list sorted
   int32_t* part_idx;        // reference rows of this call, -1 = empty
   int n_query, n_ref, k;
+  int splits;               // CTA b: split b % splits of query tile b / splits
   int tiles_per_split;      // reference tiles of kNbBN rows per split
   long long self_off;       // query q never returns reference row q + self_off (LLONG_MIN: no exclusion)
   DeviceStatus* status;
@@ -54,16 +56,40 @@ __device__ __forceinline__ bool nb_beats(float as, long long ai, float bs, long 
   return as > bs || (as == bs && ai < bi);
 }
 
+// 2^e as a float, exactly, for e in [-149, 127]
+__device__ __forceinline__ float nb_pow2(int e) {
+  return e >= -126 ? __int_as_float((e + 127) << 23) : __int_as_float(1 << (e + 149));
+}
+
+// Prescale: the row is first multiplied by the power of two 2^-E that brings its max |x| into [1, 2) (one exact factor, or two
+// for a subnormal max, which needs more than 2^127), so the fp32 sum of squares neither overflows (a row with sum x^2 > FLT_MAX
+// would get norm inf and become the zero row) nor loses digits to subnormal squares.  The product is exact whenever the scaled
+// entry is a normal float, so:
+//   * when every partial sum of squares is a normal float (or zero) both before and after the prescale -- e.g. every nonzero
+//     x_i^2 is normal, scaled or not, and sum x^2 is finite -- the halves are bitwise those of the same recipe without it (the
+//     fma, sqrt and division results are those unscaled times exact powers of two, and x / norm is the same quotient);
+//   * x * 2^e gives bitwise the halves of x whenever every nonzero entry of x and of x * 2^e is a normal float (both prescale to
+//     the same row).
 __global__ void __launch_bounds__(256) nb_prep_kernel(const float* __restrict__ x, int n, float* __restrict__ hi,
                                                       float* __restrict__ lo) {
   const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= n) return;
   const float4* src = reinterpret_cast<const float4*>(x + static_cast<size_t>(row) * kNbDim);
   float4 v[4];
-  float ss = 0.f;
+  float mx = 0.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     v[i] = src[lane + 32 * i];
+    mx = fmaxf(mx, fmaxf(fmaxf(fabsf(v[i].x), fabsf(v[i].y)), fmaxf(fabsf(v[i].z), fabsf(v[i].w))));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  const int E = mx > 0.f ? ilogbf(mx) : 0;                                        // mx * 2^-E in [1, 2)
+  const float f0 = E < -127 ? nb_pow2(64) : 1.f, f1 = nb_pow2(E < -127 ? -E - 64 : -E);
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    v[i].x = v[i].x * f0 * f1; v[i].y = v[i].y * f0 * f1; v[i].z = v[i].z * f0 * f1; v[i].w = v[i].w * f0 * f1;
     ss = fmaf(v[i].x, v[i].x, ss); ss = fmaf(v[i].y, v[i].y, ss); ss = fmaf(v[i].z, v[i].z, ss); ss = fmaf(v[i].w, v[i].w, ss);
   }
 #pragma unroll
@@ -184,7 +210,8 @@ nb_search_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_const
   uint64_t* empty = full + kNbStages;                                             // one arrival per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int split = blockIdx.x, m0 = blockIdx.y * kNbBM;
+  // a 1-D grid, split fastest (the order of a (splits, query tiles) grid): gridDim.y would cap the query tiles at 65,535
+  const int split = static_cast<int>(blockIdx.x % p.splits), m0 = static_cast<int>(blockIdx.x / p.splits) * kNbBM;
   const int t0 = split * p.tiles_per_split;
   const int nt = min(p.tiles_per_split, (p.n_ref + kNbBN - 1) / kNbBN - t0);    // >= 1 by construction of the grid
 

@@ -96,6 +96,23 @@ class NNOutputs:
     def provirus_nn_classification_attributions_output(self) -> Path:
         return self._nn("provirus_nn_classification_attributions.npz")
 
+    # ---- opt-in (--both-strands), not a reference output: scores of the forward strand, the reverse strand and their mean
+    @property
+    def nn_classification_strands_output(self) -> Path:
+        return self._nn("nn_classification_strands.tsv")
+
+    @property
+    def nn_classification_strands_npz_output(self) -> Path:
+        return self._nn("nn_classification_strands.npz")
+
+    @property
+    def provirus_nn_classification_strands_output(self) -> Path:
+        return self._nn("provirus_nn_classification_strands.tsv")
+
+    @property
+    def provirus_nn_classification_strands_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_strands.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

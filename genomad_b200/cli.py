@@ -69,9 +69,14 @@ def cli():
 @click.option("--attribution-baseline", type=click.Choice(["zero", "N"]), default=None, show_default="zero",
               help="Baseline of integrated gradients: zero (all-zero one-hot input) or N (a window of N). Not an option of the "
                    "reference.")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Also classify every sequence's reverse complement and write the scores of the forward strand, the reverse "
+                   "strand and their mean to <prefix>_nn_classification_strands.{tsv,npz}; with --write-embeddings the "
+                   "embeddings file also gets embeddings_reverse and embeddings_both_strands. The main outputs are unchanged. "
+                   "About twice the GPU time. Not an option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
                       write_embeddings, write_window_scores, window_stride, write_attributions, attribution_steps,
-                      attribution_baseline):
+                      attribution_baseline, both_strands):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -89,6 +94,8 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["attribution_steps"] = attribution_steps
     if attribution_baseline is not None:
         extra["attribution_baseline"] = attribution_baseline
+    if both_strands:
+        extra["both_strands"] = True
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
 
@@ -101,14 +108,17 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
                    "query sequences are searched against each other, a sequence never being its own neighbour.")
 @click.option("--neighbours", "-k", type=click.IntRange(1, 64), default=10, show_default=True,
               help="Neighbours per query sequence.")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Search the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
+                   "--write-embeddings --both-strands) of every input file, so a sequence and its reverse complement match.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def embedding_neighbours(query, output, reference, neighbours, verbose):
+def embedding_neighbours(query, output, reference, neighbours, both_strands, verbose):
     """Find the nearest neighbours, in cosine similarity of the encoder embeddings, of every sequence of the QUERY embeddings
     file (nn-classification --write-embeddings output) and write them to the OUTPUT directory as
     <prefix>_embedding_neighbours.{tsv,npz}. Not a module of the reference."""
     from . import embedding_neighbours as module
-    module.main(query, reference, output, neighbours, verbose)
+    module.main(query, reference, output, neighbours, verbose, both_strands=both_strands)
 
 
 @cli.command(name="embedding-clusters", context_settings=CONTEXT_SETTINGS)
@@ -117,15 +127,18 @@ def embedding_neighbours(query, output, reference, neighbours, verbose):
 @click.option("--min-similarity", type=click.FloatRange(0, 1, min_open=True), required=True,
               help="Cosine similarity a sequence needs with a representative to join its cluster, in (0, 1]. No default: "
                    "which level separates what in this embedding space has not been measured.")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Cluster the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
+                   "--write-embeddings --both-strands), so a sequence and its reverse complement share a cluster.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def embedding_clusters(input, output, min_similarity, verbose):
+def embedding_clusters(input, output, min_similarity, both_strands, verbose):
     """Cluster the sequences of the INPUT embeddings file (nn-classification --write-embeddings output) greedily, in file
     order, at a cosine similarity threshold of the encoder embeddings, and write each sequence's representative to the OUTPUT
     directory as <prefix>_embedding_clusters.{tsv,npz}. A representative is the first member of its cluster in file order.
     Not a module of the reference."""
     from . import embedding_clusters as module
-    module.main(input, output, min_similarity, verbose)
+    module.main(input, output, min_similarity, verbose, both_strands=both_strands)
 
 
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)

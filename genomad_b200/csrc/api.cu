@@ -1068,8 +1068,8 @@ extern "C" int gnm_encode(gnm_handle* h, const uint8_t* d_ascii, int n, uint16_t
 // d_win_offsets only, so a too-small capacity is reported before anything is written to d_win_start / d_win_len.
 // gnm_contig_windows is the stride-6000 call of the same kernels as gnm_contig_windows_stride.
 static int plan_contig_windows(gnm_handle* h, const char* fn, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
-                               int single_window, int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
-                               int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+                               int single_window, int stride, bool reverse, int64_t* d_win_start, int32_t* d_win_len,
+                               int64_t capacity, int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
   const std::string f(fn);
   if (!h) return fail(f + ": null handle");
   if (n_contigs < 0) return fail(f + ": negative contig count");
@@ -1087,7 +1087,8 @@ static int plan_contig_windows(gnm_handle* h, const char* fn, const uint8_t* d_s
     return 0;
   }
   const int step = single_window ? 0 : stride;         // 0: the first window only
-  contig_plan_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, nullptr, nullptr);
+  if (reverse) contig_plan_rc_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, nullptr, nullptr);
+  else contig_plan_kernel<false><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, nullptr, nullptr);
   if (check_launch(h, "contig_plan_kernel<count>")) return 1;
   contig_scan_kernel<<<1, kScanThreads, 0, st>>>(d_win_offsets, n_contigs);
   if (check_launch(h, "contig_scan_kernel")) return 1;
@@ -1101,45 +1102,68 @@ static int plan_contig_windows(gnm_handle* h, const char* fn, const uint8_t* d_s
     return fail(f + ": the contigs have " + std::to_string(total) + " windows, capacity is " + std::to_string(capacity) +
                 " (n_contigs + total_bytes / " + std::to_string(stride) + " is always enough)");
   if (total == 0) return 0;
-  contig_plan_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, d_win_start, d_win_len);
+  if (reverse)
+    contig_plan_rc_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, d_win_start, d_win_len);
+  else
+    contig_plan_kernel<true><<<n_contigs, kPlanThreads, 0, st>>>(d_seq, d_seq_offsets, step, d_win_offsets, d_win_start, d_win_len);
   return check_launch(h, "contig_plan_kernel<write>");
 }
 
 extern "C" int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
                                   int single_window, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
                                   int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
-  return plan_contig_windows(h, "gnm_contig_windows", d_seq, d_seq_offsets, n_contigs, single_window, kWindow, d_win_start,
-                             d_win_len, capacity, d_win_offsets, h_n_windows, stream);
+  return plan_contig_windows(h, "gnm_contig_windows", d_seq, d_seq_offsets, n_contigs, single_window, kWindow, false,
+                             d_win_start, d_win_len, capacity, d_win_offsets, h_n_windows, stream);
 }
 
 extern "C" int gnm_contig_windows_stride(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
                                          int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
                                          int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
-  return plan_contig_windows(h, "gnm_contig_windows_stride", d_seq, d_seq_offsets, n_contigs, 0, stride, d_win_start,
+  return plan_contig_windows(h, "gnm_contig_windows_stride", d_seq, d_seq_offsets, n_contigs, 0, stride, false, d_win_start,
                              d_win_len, capacity, d_win_offsets, h_n_windows, stream);
 }
 
+extern "C" int gnm_contig_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs,
+                                     int single_window, int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity,
+                                     int32_t* d_win_offsets, int64_t* h_n_windows, void* stream) {
+  return plan_contig_windows(h, "gnm_contig_windows_rc", d_seq, d_seq_offsets, n_contigs, single_window, stride, true,
+                             d_win_start, d_win_len, capacity, d_win_offsets, h_n_windows, stream);
+}
+
 static int launch_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
-                                 uint8_t* d_ascii, cudaStream_t st) {
+                                 uint8_t* d_ascii, cudaStream_t st, bool rc = false) {
+  if (rc) {
+    gather_windows_rc_kernel<<<n, kGatherThreads, 0, st>>>(d_seq, d_win_start, d_win_len, d_ascii);
+    return check_launch(h, "gather_windows_rc_kernel");
+  }
   gather_windows_kernel<<<n, kGatherThreads, 0, st>>>(d_seq, d_win_start, d_win_len, d_ascii);
   return check_launch(h, "gather_windows_kernel");
 }
 
+static int gather_windows(gnm_handle* h, const char* fn, const uint8_t* d_seq, const int64_t* d_win_start,
+                          const int32_t* d_win_len, int n, uint8_t* d_ascii, void* stream, bool rc) {
+  const std::string f(fn);
+  if (!h) return fail(f + ": null handle");
+  if (n < 0) return fail(f + ": negative window count");
+  if (n == 0) return 0;
+  if (!d_seq || !d_win_start || !d_win_len || !d_ascii) return fail(f + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_ascii) % 16) return fail(f + ": d_ascii must be 16-byte aligned");
+  GNM_CUDA(cudaSetDevice(h->device));
+  return launch_gather_windows(h, d_seq, d_win_start, d_win_len, n, d_ascii, static_cast<cudaStream_t>(stream), rc);
+}
 extern "C" int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                                   uint8_t* d_ascii, void* stream) {
-  if (!h) return fail("gnm_gather_windows: null handle");
-  if (n < 0) return fail("gnm_gather_windows: negative window count");
-  if (n == 0) return 0;
-  if (!d_seq || !d_win_start || !d_win_len || !d_ascii) return fail("gnm_gather_windows: null buffer");
-  if (reinterpret_cast<uintptr_t>(d_ascii) % 16) return fail("gnm_gather_windows: d_ascii must be 16-byte aligned");
-  GNM_CUDA(cudaSetDevice(h->device));
-  return launch_gather_windows(h, d_seq, d_win_start, d_win_len, n, d_ascii, static_cast<cudaStream_t>(stream));
+  return gather_windows(h, "gnm_gather_windows", d_seq, d_win_start, d_win_len, n, d_ascii, stream, false);
+}
+extern "C" int gnm_gather_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                     int n, uint8_t* d_ascii, void* stream) {
+  return gather_windows(h, "gnm_gather_windows_rc", d_seq, d_win_start, d_win_len, n, d_ascii, stream, true);
 }
 
 // Steps of max_batch windows: gather into in_stage[step parity], then the unchanged forward step.  The gather runs on the
 // step's main stream, ahead of the layer-1 kernel that reads the stage, so the TailOverlap ordering covers both buffers.
 static int forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
-                           float* d_probs, float* d_embed, void* stream) {
+                           float* d_probs, float* d_embed, void* stream, bool rc = false) {
   if (!h) return fail("gnm_forward_windows: null handle");
   if (n < 0) return fail("gnm_forward_windows: negative window count");
   if (n == 0) return 0;
@@ -1151,8 +1175,8 @@ static int forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d
   for (int i = 0, off = 0; off < n; ++i, off += h->max_batch) {
     const int m = std::min(h->max_batch, n - off);
     uint8_t* stage = h->in_stage[i & 1];
-    timer_mark(h, "gather_windows", st);
-    if (launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, stage, st)) return 1;
+    timer_mark(h, rc ? "gather_windows_rc" : "gather_windows", st);
+    if (launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, stage, st, rc)) return 1;
     if (ov.step(stage, nullptr, m, probs_at(d_probs, off), embed_at(d_embed, off))) return 1;
   }
   return ov.join();
@@ -1165,6 +1189,15 @@ extern "C" int gnm_embed_windows(gnm_handle* h, const uint8_t* d_seq, const int6
                                  int n, float* d_probs, float* d_embed, void* stream) {
   if (!d_embed && n > 0) return fail("gnm_embed_windows: d_embed is null");
   return forward_windows(h, d_seq, d_win_start, d_win_len, n, d_probs, d_embed, stream);
+}
+extern "C" int gnm_forward_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                      int n, float* d_probs, void* stream) {
+  return forward_windows(h, d_seq, d_win_start, d_win_len, n, d_probs, nullptr, stream, true);
+}
+extern "C" int gnm_embed_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len,
+                                    int n, float* d_probs, float* d_embed, void* stream) {
+  if (!d_embed && n > 0) return fail("gnm_embed_windows_rc: d_embed is null");
+  return forward_windows(h, d_seq, d_win_start, d_win_len, n, d_probs, d_embed, stream, true);
 }
 
 static int segment_any(gnm_handle* h, const float* d_probs, const int32_t* d_offsets, int n_contigs, float* d_out,

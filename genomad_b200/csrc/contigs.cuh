@@ -126,10 +126,13 @@ __device__ __forceinline__ int64_t candidate_windows(int64_t L, int64_t step) {
 // a score profile, each candidate's N count re-reads its 6000 bytes, i.e. ~6000 / step reads per byte; 0: --single-window).
 // kWrite = false: counts[c] = kept windows of contig c (-1 if its byte range is reversed).
 // kWrite = true : offsets = the scanned counts; contig c writes its kept windows to win_start / win_len [offsets[c], offsets[c+1]).
-template <bool kWrite>
-__global__ void __launch_bounds__(kPlanThreads)
-contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets, int window_step,
-                   int32_t* __restrict__ offsets, int64_t* __restrict__ win_start, int32_t* __restrict__ win_len) {
+// kReverse: the windows of the contig's reverse complement rc(S) (genomad/sequence.py:41-43).  Candidate k is laid from the
+// stripped end: it is rc(S)[k step, k step + len_k), i.e. the forward segment [L - k step - len_k, L - k step), and
+// win_start / win_len name that segment.  rc maps 'N' to 'N', so the N rule counts the segment's 'N' bytes.
+template <bool kWrite, bool kReverse>
+__device__ __forceinline__ void contig_plan(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets,
+                                            int window_step, int32_t* __restrict__ offsets, int64_t* __restrict__ win_start,
+                                            int32_t* __restrict__ win_len) {
   __shared__ unsigned long long s_best;
   __shared__ int s_keep[kPlanWarps];
   const int c = blockIdx.x;
@@ -153,20 +156,21 @@ contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ 
   const int64_t step = window_step;
   const int64_t n_cand = candidate_windows(L, step);
   auto wlen = [&](int64_t w) { return static_cast<int32_t>(min(static_cast<int64_t>(kWindow), L - w * step)); };
+  auto wbeg = [&](int64_t w) { return kReverse ? first + L - w * step - wlen(w) : first + w * step; };
   if (kWrite && n_kept == n_cand) {                    // nothing dropped by the N rule: window k is candidate k
     for (int64_t w = threadIdx.x; w < n_cand; w += blockDim.x) {
-      win_start[base + w] = first + w * step;
+      win_start[base + w] = wbeg(w);
       win_len[base + w] = wlen(w);
     }
     return;
   }
-  if (kWrite && threadIdx.x == 0) { win_start[base] = first; win_len[base] = wlen(0); }     // the first window is exempt
+  if (kWrite && threadIdx.x == 0) { win_start[base] = wbeg(0); win_len[base] = wlen(0); }     // the first window is exempt
   int64_t kept = 1;                                    // windows kept so far, identical in every thread
   for (int64_t w0 = 1; w0 < n_cand; w0 += kPlanWarps) {   // rounds of one candidate per warp, in order
     const int64_t w = w0 + warp;
     int keep = 0;
     if (w < n_cand) {
-      const int64_t a = first + w * step;
+      const int64_t a = wbeg(w);
       keep = warp_count_N(seq, a, a + wlen(w)) <= kMaxN;
     }
     if (lane == 0) s_keep[warp] = keep;
@@ -175,13 +179,26 @@ contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ 
 #pragma unroll
     for (int i = 0; i < kPlanWarps; ++i) { before += i < warp ? s_keep[i] : 0; total += s_keep[i]; }
     if (kWrite && keep && lane == 0) {
-      win_start[base + kept + before] = first + w * step;
+      win_start[base + kept + before] = wbeg(w);
       win_len[base + kept + before] = wlen(w);
     }
     kept += total;
     __syncthreads();                                   // s_keep is rewritten by the next round
   }
   if (!kWrite && threadIdx.x == 0) offsets[c] = kept > INT32_MAX ? kCountOverflow : static_cast<int32_t>(kept);
+}
+
+template <bool kWrite>
+__global__ void __launch_bounds__(kPlanThreads)
+contig_plan_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets, int window_step,
+                   int32_t* __restrict__ offsets, int64_t* __restrict__ win_start, int32_t* __restrict__ win_len) {
+  contig_plan<kWrite, false>(seq, seq_offsets, window_step, offsets, win_start, win_len);
+}
+template <bool kWrite>
+__global__ void __launch_bounds__(kPlanThreads)
+contig_plan_rc_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ seq_offsets, int window_step,
+                      int32_t* __restrict__ offsets, int64_t* __restrict__ win_start, int32_t* __restrict__ win_len) {
+  contig_plan<kWrite, true>(seq, seq_offsets, window_step, offsets, win_start, win_len);
 }
 
 // offsets[0, n) = per-contig window counts -> exclusive prefix sums in place, offsets[n] = the total, or kPlanOverflow if it
@@ -267,6 +284,54 @@ gather_windows_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict
       x = (x & in) | (0x4e4e4e4eu & ~in);
       const uint32_t lower = __vcmpgeu4(x, 0x61616161u) & __vcmpleu4(x, 0x7a7a7a7au);
       o[k] = x - (lower & 0x20202020u);
+    }
+    *reinterpret_cast<uint4*>(dst + 16 * i) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+// upper(comp(c)) in each byte: comp is Sequence.rc()'s table (ACTGNactgn -> TGACNtgacn, every other byte unchanged), and upper()
+// changes 'a'..'z' only.  Upper-casing first leaves A, C, G, T exactly where comp acts ('N' and 'n' become 'N' either way);
+// then A <-> T is ^ 0x15 and C <-> G is ^ 0x04.
+__device__ __forceinline__ uint32_t rc_upper4(uint32_t x) {
+  const uint32_t lower = __vcmpgeu4(x, 0x61616161u) & __vcmpleu4(x, 0x7a7a7a7au);
+  const uint32_t u = x - (lower & 0x20202020u);
+  const uint32_t at = __vcmpeq4(u, 0x41414141u) | __vcmpeq4(u, 0x54545454u);
+  const uint32_t cg = __vcmpeq4(u, 0x43434343u) | __vcmpeq4(u, 0x47474747u);
+  return u ^ (at & 0x15151515u) ^ (cg & 0x04040404u);
+}
+
+// gather_windows_kernel for the windows of the reverse complement: (start, length) names the window's forward segment seg, and
+// row byte j = upper(comp(seg[len - 1 - j])), 'N' past len.  The staged copy starts 16 bytes into s_w so that a word read
+// backwards from the segment's first byte stays inside the buffer; each output word is the staged word that ends at
+// seg[len - 1 - j], byte-reversed.
+__global__ void __launch_bounds__(kGatherThreads)
+gather_windows_rc_kernel(const uint8_t* __restrict__ seq, const int64_t* __restrict__ win_start,
+                         const int32_t* __restrict__ win_len, uint8_t* __restrict__ out) {
+  __shared__ __align__(16) uint32_t s_w[(kWindow + 48) / 4];
+  const int64_t w = blockIdx.x;
+  const int len = min(max(win_len[w], 0), kWindow);
+  const uint8_t* src = seq + win_start[w];
+  const int shift = static_cast<int>(reinterpret_cast<uintptr_t>(src) & 15);
+  const uint4* v0 = reinterpret_cast<const uint4*>(src - shift);
+  const int nvec = len > 0 ? (shift + len + 15) / 16 : 0;
+  for (int i = threadIdx.x; i < nvec; i += blockDim.x) reinterpret_cast<uint4*>(s_w)[i + 1] = v0[i];
+  __syncthreads();
+  uint8_t* dst = out + w * kWindow;
+  const int last = 16 + shift + len - 4;               // staged byte index of seg[len - 4]
+  for (int i = threadIdx.x; i < kWindow / 16; i += blockDim.x) {
+    uint32_t o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int j = 16 * i + 4 * k;                    // first byte of this word in the row
+      const int e = len - j;
+      uint32_t x = 0x4e4e4e4eu;
+      if (e > 0) {
+        const int p = last - j;                        // >= 13: staged bytes p .. p+3 = seg[len-4-j .. len-1-j]
+        x = __byte_perm(__funnelshift_r(s_w[p >> 2], s_w[(p >> 2) + 1], 8 * (p & 3)), 0, 0x0123);
+        const uint32_t in = e >= 4 ? 0xffffffffu : 0xffffffffu >> (32 - 8 * e);   // bytes before seg's start: 'N'
+        x = rc_upper4((x & in) | (0x4e4e4e4eu & ~in));
+      }
+      o[k] = x;
     }
     *reinterpret_cast<uint4*>(dst + 16 * i) = make_uint4(o[0], o[1], o[2], o[3]);
   }

@@ -122,6 +122,7 @@ struct gnm_fasta_windows {
   const gnm_fasta* f = nullptr;
   int64_t step = kWin;
   int single_window = 0;
+  int reverse = 0;                              // windows of the reverse complement (see reverse_begin)
   int64_t n_windows = 0;
   std::vector<int64_t> first;                   // per kept record: its first window in the list (sorted: window -> record)
   std::vector<int32_t> off_idx, kept_idx;       // per kept record: index into win_off / kept_wins, or -1
@@ -195,36 +196,42 @@ static inline int64_t candidate_windows(int64_t L, int64_t step, int single_wind
   return single_window ? 1 : 1 + (L > kMinTail ? (L - kMinTail) / step : 0);
 }
 
+// Reverse lists: candidate k is window k of rc(S) -- rc(S)[k step, k step + len_k) with len_k = min(6000, L - k step) -- and
+// that is the forward segment [L - k step - len_k, L - k step) of the stripped sequence, read backwards and complemented.
+// reverse_begin is that segment's first position (forward lists: k step).  rc maps 'N' to 'N', so the N rule counts the
+// segment's 'N' bytes.
+static inline int64_t window_len(int64_t L, int64_t step, int64_t k) { return std::min(kWin, L - k * step); }
+static inline int64_t segment_begin(int64_t L, int64_t step, int reverse, int64_t k) {
+  return reverse ? L - k * step - window_len(L, step, k) : k * step;
+}
+
 // One kept record's windows in list p: returns how many are kept; fills *offs (irregular records: file offset of every
 // candidate's first byte) and *keptw (only if the N rule dropped one: the candidate numbers kept).  The N count of candidate w
 // is the running count of 'N' at its end minus the one at its start; both are taken in one walk over the lines, so
 // overlapping windows cost no re-reading.  Only the windows open at one position (<= 6000 / step + 1) keep their start count,
 // in a ring, so the walk needs no memory per candidate; a window is kept or dropped as soon as its end is reached.
-static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, int single_window, std::vector<int64_t>* offs,
-                           std::vector<int32_t>* keptw) {
+// The walk takes the candidates in the order of their forward segments: k = 0, 1, .. for a forward list, k = ncand - 1, .., 0
+// for a reverse one (both starts and ends then ascend, and window j - ring has still ended before window j starts).
+static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, int single_window, int reverse,
+                           std::vector<int64_t>* offs, std::vector<int32_t>* keptw) {
   const int64_t L = R.seq_len;
   if (L == 0) return 0;
   const int64_t ncand = candidate_windows(L, step, single_window);
   if (ncand == 1 && R.stride != 0) return 1;   // one window (exempt from the N rule) of a regular record: nothing to walk
-  auto wend = [&](int64_t w) { return std::min(L, w * step + kWin); };     // end of candidate w, in the stripped sequence
+  auto cand = [&](int64_t j) { return reverse ? ncand - 1 - j : j; };     // walk position -> candidate number
+  auto wbeg = [&](int64_t j) { return segment_begin(L, step, reverse, cand(j)); };
+  auto wend = [&](int64_t j) { return wbeg(j) + window_len(L, step, cand(j)); };   // in the stripped sequence
   const bool need_n = ncand > 1;            // the first window is exempt from the N rule
   const bool need_off = R.stride == 0;
-  // ring of the running 'N' count at the start of the open windows: window w - ring has ended before window w starts
+  // ring of the running 'N' count at the start of the open windows: window j - ring has ended before window j starts
   // (ring * step > 6000 >= any window's length)
   const int64_t ring = kWin / step + 2;
   std::vector<int64_t> n_start(need_n ? static_cast<size_t>(std::min(ring, ncand)) : 0);
   if (need_off) offs->assign(static_cast<size_t>(ncand), -1);
-  int64_t nkept = 1;                        // window 0 is always kept
-  bool dropped = false;
-  auto decide = [&](int64_t w, int64_t n_count) {      // windows 1.. in order
-    if (n_count <= kMaxN) {
-      if (dropped) keptw->push_back(static_cast<int32_t>(w));
-      ++nkept;
-    } else if (!dropped) {                   // first drop: the kept candidates so far are 0 .. w-1
-      dropped = true;
-      keptw->resize(static_cast<size_t>(w));
-      for (int64_t k = 0; k < w; ++k) (*keptw)[static_cast<size_t>(k)] = static_cast<int32_t>(k);
-    }
+  std::vector<int32_t> drops;               // candidates the N rule dropped (rare)
+  auto decide = [&](int64_t j, int64_t n_count) {
+    const int64_t k = cand(j);
+    if (k > 0 && n_count > kMaxN) drops.push_back(static_cast<int32_t>(k));
   };
   const uint8_t* t = f->text;
   const int64_t s0 = R.lead, s1 = R.lead + wend(ncand - 1);
@@ -236,7 +243,7 @@ static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, in
     const int64_t base = ls + s0 - pos;              // file offset of stripped position 0 on this line's terms
     if (a < e) {
       for (;;) {                                     // window starts in [a, e) and ends in (a, e], in order
-        const int64_t qs = ws < ncand ? ws * step : INT64_MAX;
+        const int64_t qs = ws < ncand ? wbeg(ws) : INT64_MAX;
         const int64_t qe = need_n && we < ncand ? wend(we) : INT64_MAX;
         const bool is_start = qs < e && qs <= qe;
         if (!is_start && qe > e) break;
@@ -245,10 +252,10 @@ static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, in
         a = q;
         if (is_start) {
           if (need_n) n_start[static_cast<size_t>(ws % ring)] = cnt;
-          if (need_off) (*offs)[static_cast<size_t>(ws)] = base + q;
+          if (need_off) (*offs)[static_cast<size_t>(cand(ws))] = base + q;
           ++ws;
         } else {
-          if (we > 0) decide(we, cnt - n_start[static_cast<size_t>(we % ring)]);
+          decide(we, cnt - n_start[static_cast<size_t>(we % ring)]);
           ++we;
         }
       }
@@ -256,7 +263,16 @@ static int64_t plan_record(const gnm_fasta* f, const Record& R, int64_t step, in
     }
     pos += n;
   });
-  return nkept;
+  if (!drops.empty()) {                     // the kept candidate numbers, ascending
+    std::sort(drops.begin(), drops.end());
+    keptw->reserve(static_cast<size_t>(ncand) - drops.size());
+    size_t d = 0;
+    for (int64_t k = 0; k < ncand; ++k) {
+      if (d < drops.size() && drops[d] == k) ++d;
+      else keptw->push_back(static_cast<int32_t>(k));
+    }
+  }
+  return ncand - static_cast<int64_t>(drops.size());
 }
 
 // Windows of a stripped record of L nt at `step`, before the N rule (closed form): what a list can hold at most.
@@ -273,7 +289,8 @@ static void build_windows(const gnm_fasta* f, gnm_fasta_windows* p, int threads)
   std::vector<std::vector<int32_t>> keptw(nk);
   std::vector<int64_t> nw(nk);
   parallel_for(static_cast<int64_t>(nk), threads, [&](int64_t i) {
-    nw[i] = plan_record(f, f->recs[static_cast<size_t>(f->kept[i])], p->step, p->single_window, &offs[i], &keptw[i]);
+    nw[i] = plan_record(f, f->recs[static_cast<size_t>(f->kept[i])], p->step, p->single_window, p->reverse, &offs[i],
+                        &keptw[i]);
   });
   p->f = f;
   p->n_windows = 0;
@@ -515,6 +532,19 @@ static inline int64_t regular_offset(const Record& R, int64_t a) {
   return R.body_begin + (a / R.line_len) * R.stride + a % R.line_len;
 }
 
+// upper(comp(c)) for every byte: comp is the reference's Sequence.rc() table (sequence.py:41-43), ACTGNactgn -> TGACNtgacn and
+// every other byte unchanged; upper() changes 'a'..'z' only
+struct RcUpperTable {
+  uint8_t v[256];
+  RcUpperTable() {
+    for (int c = 0; c < 256; ++c) v[c] = static_cast<uint8_t>(c);
+    const char* from = "ACTGNactgn";
+    const char* to = "TGACNtgacn";
+    for (int i = 0; i < 10; ++i) v[static_cast<uint8_t>(from[i])] = static_cast<uint8_t>(to[i]);
+    for (int c = 0; c < 256; ++c) if (v[c] >= 'a' && v[c] <= 'z') v[c] = static_cast<uint8_t>(v[c] - 32);
+  }
+};
+
 // window wdx of list p -> dst[6000]
 static void extract_window(const gnm_fasta_windows* p, int64_t wdx, uint8_t* dst) {
   const gnm_fasta* f = p->f;
@@ -522,11 +552,11 @@ static void extract_window(const gnm_fasta_windows* p, int64_t wdx, uint8_t* dst
   const Record& R = f->recs[static_cast<size_t>(f->kept[ki])];
   int64_t cand = wdx - p->first[ki];
   if (p->kept_idx[ki] >= 0) cand = p->kept_wins[static_cast<size_t>(p->kept_idx[ki])][static_cast<size_t>(cand)];
-  const int64_t n = std::min(kWin, R.seq_len - cand * p->step);
+  const int64_t n = window_len(R.seq_len, p->step, cand);
   const uint8_t* t = f->text;
   int64_t got = 0;
   if (R.stride > 0) {
-    const int64_t a = R.lead + cand * p->step;
+    const int64_t a = R.lead + segment_begin(R.seq_len, p->step, p->reverse, cand);
     int64_t off = regular_offset(R, a), in_line = R.line_len - a % R.line_len;
     while (got < n) {
       const int64_t c = std::min(n - got, in_line);
@@ -549,9 +579,18 @@ static void extract_window(const gnm_fasta_windows* p, int64_t wdx, uint8_t* dst
       i = j + 1;                      // a "\r\n" pair leaves an empty line behind: harmless
     }
   }
-  for (int64_t k = 0; k < n; ++k) {   // ASCII upper(), as bytes.upper()
-    const uint8_t c = dst[k];
-    dst[k] = (c >= 'a' && c <= 'z') ? static_cast<uint8_t>(c - 32) : c;
+  if (p->reverse) {                   // rc, then ASCII upper(): byte j = upper(comp(segment[n - 1 - j]))
+    static const RcUpperTable tab;
+    for (int64_t i = 0, j = n - 1; i <= j; ++i, --j) {
+      const uint8_t c = dst[i];
+      dst[i] = tab.v[dst[j]];
+      dst[j] = tab.v[c];
+    }
+  } else {
+    for (int64_t k = 0; k < n; ++k) {   // ASCII upper(), as bytes.upper()
+      const uint8_t c = dst[k];
+      dst[k] = (c >= 'a' && c <= 'z') ? static_cast<uint8_t>(c - 32) : c;
+    }
   }
   if (n < kWin) std::memset(dst + n, 'N', static_cast<size_t>(kWin - n));
 }
@@ -624,23 +663,37 @@ extern "C" int gnm_fasta_release_before(const gnm_fasta* f, int64_t upto) {
 }
 
 // ------------------------------------------------------------------------------------------------ window lists at any step
-extern "C" int gnm_fasta_windows_plan(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out) {
-  if (!f || !out) { g_fasta_err = "gnm_fasta_windows_plan: null argument"; return 1; }
+static int plan_windows(const char* fn, const gnm_fasta* f, int stride, int single_window, int reverse, int threads,
+                        gnm_fasta_windows** out) {
+  const std::string name(fn);
+  if (!f || !out) { g_fasta_err = name + ": null argument"; return 1; }
   if (stride < 1 || stride > kWin) {
-    g_fasta_err = "gnm_fasta_windows_plan: stride must be in [1, 6000], not " + std::to_string(stride);
+    g_fasta_err = name + ": stride must be in [1, 6000], not " + std::to_string(stride);
     return 1;
   }
   // checked before anything is built: the candidate count has a closed form, and the kept windows are at most that many
   if (candidate_total(f, stride, single_window) > INT32_MAX) {
-    g_fasta_err = "gnm_fasta_windows_plan: more than 2^31-1 windows (before the N rule)";
+    g_fasta_err = name + ": more than 2^31-1 windows (before the N rule)";
     return 1;
   }
   std::unique_ptr<gnm_fasta_windows> p(new gnm_fasta_windows());
   p->step = stride;
   p->single_window = single_window;
+  p->reverse = reverse;
   build_windows(f, p.get(), std::max(1, threads));
   *out = p.release();
   return 0;
+}
+
+extern "C" int gnm_fasta_windows_plan(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out) {
+  return plan_windows("gnm_fasta_windows_plan", f, stride, single_window, 0, threads, out);
+}
+
+// The windows of every kept record's reverse complement: the list gnm_fasta_windows_plan makes from rc(S), with starts and
+// lengths naming each window's forward segment
+extern "C" int gnm_fasta_windows_plan_rc(const gnm_fasta* f, int stride, int single_window, int threads,
+                                         gnm_fasta_windows** out) {
+  return plan_windows("gnm_fasta_windows_plan_rc", f, stride, single_window, 1, threads, out);
 }
 
 extern "C" int gnm_fasta_windows_info(const gnm_fasta_windows* p, int64_t* n_contigs, int64_t* n_windows) {
@@ -663,8 +716,8 @@ static void window_spans(const gnm_fasta_windows* p, int32_t* offsets, int64_t* 
     const std::vector<int32_t>* kw = p->kept_idx[i] >= 0 ? &p->kept_wins[static_cast<size_t>(p->kept_idx[i])] : nullptr;
     for (int64_t w = w0; w < w1; ++w) {
       const int64_t cand = kw ? (*kw)[static_cast<size_t>(w - w0)] : w - w0;
-      if (starts) starts[w] = R.lead + cand * p->step;
-      if (lengths) lengths[w] = static_cast<int32_t>(std::min(kWin, R.seq_len - cand * p->step));
+      if (starts) starts[w] = R.lead + segment_begin(R.seq_len, p->step, p->reverse, cand);
+      if (lengths) lengths[w] = static_cast<int32_t>(window_len(R.seq_len, p->step, cand));
     }
   }
 }

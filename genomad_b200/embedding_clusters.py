@@ -132,10 +132,12 @@ def write_tsv(path, names, rep_index, similarity) -> None:
 
 
 def main(input_npz, output_dir, min_similarity: float, verbose: bool = True, *, block: int = engine.CLUSTER_MAX_BLOCK,
-         rep_chunk: int = engine.NEIGHBOURS_CHUNK):
+         rep_chunk: int = engine.NEIGHBOURS_CHUNK, both_strands: bool = False):
+    """both_strands: cluster the strand-averaged embeddings (EN.BOTH_STRANDS_KEY), so that a sequence and its reverse
+    complement have bitwise the same row."""
     console = utils.HybridConsole(None, verbose)
     thr = engine.cluster_threshold(min_similarity)
-    names, emb = EN.read_embeddings(input_npz)
+    names, emb = EN.read_embeddings(input_npz, EN.BOTH_STRANDS_KEY if both_strands else "embeddings")
     info = dist.init_process_group_if_needed()
     tsv_path, npz_path = output_paths(input_npz, output_dir)
     console.log(f"Clustering {len(names):,} sequences at cosine similarity >= {thr:.6g}.")

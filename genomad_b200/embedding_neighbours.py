@@ -48,8 +48,13 @@ def output_paths(query_npz, output_dir) -> Tuple[Path, Path]:
     return out / f"{prefix}_embedding_neighbours.tsv", out / f"{prefix}_embedding_neighbours.npz"
 
 
-def read_embeddings(path) -> Tuple[np.ndarray, np.ndarray]:
-    """An embeddings NPZ of nn-classification -> (names [n] str, embeddings float32 [n, 512]); every check before any GPU work."""
+BOTH_STRANDS_KEY = "embeddings_both_strands"
+
+
+def read_embeddings(path, key: str = "embeddings") -> Tuple[np.ndarray, np.ndarray]:
+    """An embeddings NPZ of nn-classification -> (names [n] str, embeddings float32 [n, 512]); every check before any GPU work.
+    key: the array to read, "embeddings" (the forward strand) or BOTH_STRANDS_KEY (the mean of both strands' embeddings,
+    which nn-classification --write-embeddings --both-strands adds)."""
     path = Path(path)
     try:
         z = np.load(path, allow_pickle=False)
@@ -57,21 +62,24 @@ def read_embeddings(path) -> Tuple[np.ndarray, np.ndarray]:
     except Exception as e:
         raise EmbeddingsFileError(f"{path}: not a readable NPZ file ({e})") from None
     keys = [k for k in NAME_KEYS if k in files]
-    if len(keys) != 1 or "embeddings" not in files:
+    if key != "embeddings" and key not in files and len(keys) == 1 and "embeddings" in files:
+        raise EmbeddingsFileError(f"{path}: no '{key}' array: nn-classification writes it with --write-embeddings "
+                                  f"--both-strands")
+    if len(keys) != 1 or key not in files:
         raise EmbeddingsFileError(f"{path}: expected 'embeddings' and one of {NAME_KEYS} (nn-classification "
                                   f"--write-embeddings output), found {sorted(files)}")
     try:
-        names, emb = z[keys[0]], z["embeddings"]
+        names, emb = z[keys[0]], z[key]
     except Exception as e:
         raise EmbeddingsFileError(f"{path}: cannot read its arrays ({e})") from None
     if emb.ndim != 2 or emb.shape[1] != engine.EMBED:
-        raise EmbeddingsFileError(f"{path}: 'embeddings' must be [n, {engine.EMBED}], not {list(emb.shape)}")
+        raise EmbeddingsFileError(f"{path}: '{key}' must be [n, {engine.EMBED}], not {list(emb.shape)}")
     if not np.issubdtype(emb.dtype, np.floating):
-        raise EmbeddingsFileError(f"{path}: 'embeddings' must be floating point, not {emb.dtype}")
+        raise EmbeddingsFileError(f"{path}: '{key}' must be floating point, not {emb.dtype}")
     emb = np.ascontiguousarray(emb, dtype=np.float32)
     if not np.isfinite(emb).all():
         bad = int(np.flatnonzero(~np.isfinite(emb).all(axis=1))[0])
-        raise EmbeddingsFileError(f"{path}: 'embeddings' has non-finite values (first in row {bad})")
+        raise EmbeddingsFileError(f"{path}: '{key}' has non-finite values (first in row {bad})")
     if names.ndim != 1 or names.shape[0] != emb.shape[0]:
         raise EmbeddingsFileError(f"{path}: {names.shape[0] if names.ndim == 1 else list(names.shape)} names in "
                                   f"'{keys[0]}' for {emb.shape[0]} embedding rows")
@@ -116,14 +124,17 @@ def write_tsv(path, query_names, reference_names, sim, idx) -> None:
                     fout.write(f"{qn}\t{rank}\t{reference_names[i]}\t{float(s):.6f}\n")
 
 
-def main(query_npz, reference_npz, output_dir, k: int = 10, verbose: bool = True):
+def main(query_npz, reference_npz, output_dir, k: int = 10, verbose: bool = True, *, both_strands: bool = False):
+    """both_strands: search the strand-averaged embeddings (BOTH_STRANDS_KEY) of every input file, so that a sequence and its
+    reverse complement have bitwise the same row."""
     console = utils.HybridConsole(None, verbose)
     k = int(k)
     if not 1 <= k <= engine.NEIGHBOURS_MAX_K:
         raise ValueError(f"k must be in [1, {engine.NEIGHBOURS_MAX_K}], not {k}")
-    qnames, qemb = read_embeddings(query_npz)
+    key = BOTH_STRANDS_KEY if both_strands else "embeddings"
+    qnames, qemb = read_embeddings(query_npz, key)
     if reference_npz is not None:
-        rnames, remb = read_embeddings(reference_npz)
+        rnames, remb = read_embeddings(reference_npz, key)
     else:
         rnames, remb = qnames, None
     info = dist.init_process_group_if_needed()

@@ -68,11 +68,17 @@ EXPORTS = {
                                      C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "gnm_contig_windows_stride": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                             C.c_int64, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
+    "gnm_contig_windows_rc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p]),
     "gnm_gather_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_gather_windows_rc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_forward_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_forward_windows_rc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_embed_tokens": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_embed_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_embed_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_embed_windows_rc": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
     "gnm_embed_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_segment_sum_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int]),
@@ -110,6 +116,7 @@ EXPORTS = {
     "gnm_fasta_export_windows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int]),
     "gnm_fasta_free": (None, [C.c_void_p]),
     "gnm_fasta_windows_plan": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "gnm_fasta_windows_plan_rc": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_windows_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "gnm_fasta_windows_spans": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_fasta_windows_export": (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int]),
@@ -270,6 +277,16 @@ def cluster_block(rows, covered, min_similarity):
                                           work.data_ptr(), need, t.cuda.current_stream(x.device).cuda_stream))
         m = int(count.item())
     return reps[:m].long()
+
+
+def both_strands(forward, reverse):
+    """A contig's strand-averaged scores or embedding: (forward + reverse) * 0.5 in fp32, for float32 numpy arrays or torch
+    tensors of the same shape (the per-contig outputs of the forward and the reverse strand).  fp32 addition commutes, so a
+    contig and its reverse complement get bitwise the same result."""
+    if isinstance(forward, np.ndarray):
+        f, r = np.asarray(forward, np.float32), np.asarray(reverse, np.float32)
+        return (f + r) * np.float32(0.5)
+    return (forward + reverse) * 0.5
 
 
 class WindowScores(NamedTuple):
@@ -463,14 +480,15 @@ class Classifier:
                                                   self._stream()))
         return probs, emb
 
-    def embed_windows(self, seq_u8, win_start, win_len):
+    def embed_windows(self, seq_u8, win_start, win_len, reverse: bool = False):
         """Windows straight from the sequence buffer (see predict_windows) -> (probabilities [W, 3], embeddings [W, 512])."""
         t = self._torch
         start, length = win_start.contiguous(), win_len.contiguous()
         assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
         probs, emb = self._embed_out(start.numel(), seq_u8.device)
-        _check(self.lib, self.lib.gnm_embed_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
-                                                    start.numel(), probs.data_ptr(), emb.data_ptr(), self._stream()))
+        fn = self.lib.gnm_embed_windows_rc if reverse else self.lib.gnm_embed_windows
+        _check(self.lib, fn(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(), start.numel(), probs.data_ptr(),
+                            emb.data_ptr(), self._stream()))
         return probs, emb
 
     def embed_host_into(self, ascii_ptr: int, n: int, probs_ptr: int, d_embed_ptr: int):
@@ -520,11 +538,14 @@ class Classifier:
             seq = t.zeros(16, dtype=t.uint8, device=dev)          # all contigs empty: the library still wants a buffer
         return seq.contiguous(), offs.contiguous()
 
-    def contig_windows(self, seq_u8, seq_offsets_i64, single_window: bool = False, stride: int = WINDOW):
+    def contig_windows(self, seq_u8, seq_offsets_i64, single_window: bool = False, stride: int = WINDOW,
+                       reverse: bool = False):
         """Plan the windows of contigs on the device: uint8 cuda [total_bytes] + int64 cuda offsets [n_contigs + 1] ->
         (win_start int64 [W] absolute byte offsets, win_len int32 [W], win_offsets int32 [n_contigs + 1]).
         stride 6000: the reference's windows (gnm_contig_windows); any other stride in [1, 6000]: a window every `stride` nt of
-        the whole contig (gnm_contig_windows_stride; not with single_window)."""
+        the whole contig (gnm_contig_windows_stride; not with single_window).  reverse: the same windows of each contig's
+        reverse complement (gnm_contig_windows_rc); start / length then name each window's forward segment, laid from the
+        stripped end."""
         t = self._torch
         assert seq_u8.dtype == t.uint8 and seq_offsets_i64.dtype == t.int64 and seq_u8.is_cuda and seq_offsets_i64.is_cuda
         stride = int(stride)
@@ -540,7 +561,11 @@ class Classifier:
         length = t.empty(cap, dtype=t.int32, device=seq.device)
         woff = t.empty(n + 1, dtype=t.int32, device=seq.device)
         nw = C.c_int64()
-        if stride == WINDOW:
+        if reverse:
+            rc = self.lib.gnm_contig_windows_rc(self._h, seq.data_ptr(), offs.data_ptr(), n, int(bool(single_window)), stride,
+                                                start.data_ptr(), length.data_ptr(), cap, woff.data_ptr(), C.byref(nw),
+                                                self._stream())
+        elif stride == WINDOW:
             rc = self.lib.gnm_contig_windows(self._h, seq.data_ptr(), offs.data_ptr(), n, int(bool(single_window)),
                                              start.data_ptr(), length.data_ptr(), cap, woff.data_ptr(), C.byref(nw),
                                              self._stream())
@@ -550,29 +575,33 @@ class Classifier:
         _check(self.lib, rc)
         return start[:nw.value], length[:nw.value], woff
 
-    def gather_windows(self, seq_u8, win_start, win_len):
-        """Kept windows -> uint8 cuda [W, 6000], upper-cased and N-padded (gnm_gather_windows)."""
+    def gather_windows(self, seq_u8, win_start, win_len, reverse: bool = False):
+        """Kept windows -> uint8 cuda [W, 6000], upper-cased and N-padded (gnm_gather_windows).  reverse: each window's
+        segment reverse-complemented first (gnm_gather_windows_rc, for the windows of contig_windows(..., reverse=True))."""
         t = self._torch
         start, length = win_start.contiguous(), win_len.contiguous()
         assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
         out = t.empty((start.numel(), WINDOW), dtype=t.uint8, device=seq_u8.device)
-        _check(self.lib, self.lib.gnm_gather_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
-                                                     start.numel(), out.data_ptr(), self._stream()))
+        fn = self.lib.gnm_gather_windows_rc if reverse else self.lib.gnm_gather_windows
+        _check(self.lib, fn(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(), start.numel(), out.data_ptr(),
+                            self._stream()))
         return out
 
-    def predict_windows(self, seq_u8, win_start, win_len, out=None):
-        """Per-window probabilities float32 [W, 3] straight from the sequence buffer (gnm_forward_windows)."""
+    def predict_windows(self, seq_u8, win_start, win_len, out=None, reverse: bool = False):
+        """Per-window probabilities float32 [W, 3] straight from the sequence buffer (gnm_forward_windows; reverse:
+        gnm_forward_windows_rc, the reverse-complement gather of gather_windows(..., reverse=True))."""
         t = self._torch
         start, length = win_start.contiguous(), win_len.contiguous()
         assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
         if out is None:
             out = t.empty((start.numel(), 3), dtype=t.float32, device=seq_u8.device)
-        _check(self.lib, self.lib.gnm_forward_windows(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(),
-                                                      start.numel(), out.data_ptr(), self._stream()))
+        fn = self.lib.gnm_forward_windows_rc if reverse else self.lib.gnm_forward_windows
+        _check(self.lib, fn(self._h, seq_u8.data_ptr(), start.data_ptr(), length.data_ptr(), start.numel(), out.data_ptr(),
+                            self._stream()))
         return out
 
     def classify_contigs(self, seqs, single_window: bool = False, return_window_probs: bool = False,
-                         return_embeddings: bool = False):
+                         return_embeddings: bool = False, strand: str = "forward"):
         """Contigs in, one score triple per contig out -- what the reference module computes per contig
         (nn_classification.py:65-75, 316-320), with windowing on the GPU.
 
@@ -580,14 +609,21 @@ class Classifier:
         Returns cuda tensors (means float32 [n_contigs, 3], window counts int32 [n_contigs]), then, if asked, the per-window
         probabilities float32 [W, 3], then, if asked, the per-contig mean encoder embeddings float32 [n_contigs, 512]
         (segment_sum_rows / count in fp32).  A contig that is empty after stripping n/N has count 0, mean (0, 0, 0) and a zero
-        embedding; the reference drops such contigs, so drop those rows to mirror its outputs."""
+        embedding; the reference drops such contigs, so drop those rows to mirror its outputs.
+
+        strand "reverse" scores each contig's reverse complement instead (the reference's Sequence.rc(), windowed as the
+        reference windows any contig): bitwise the forward call on the reverse-complemented contigs.  both_strands() combines
+        the two calls' outputs."""
         t = self._torch
+        if strand not in ("forward", "reverse"):
+            raise ValueError(f"strand must be 'forward' or 'reverse', not {strand!r}")
+        rev = strand == "reverse"
         seq, offs = self.contig_buffers(seqs)
-        start, length, woff = self.contig_windows(seq, offs, single_window)
+        start, length, woff = self.contig_windows(seq, offs, single_window, reverse=rev)
         if return_embeddings:
-            probs, emb = self.embed_windows(seq, start, length)
+            probs, emb = self.embed_windows(seq, start, length, reverse=rev)
         else:
-            probs = self.predict_windows(seq, start, length)
+            probs = self.predict_windows(seq, start, length, reverse=rev)
         if probs.numel():
             means = self.segment_mean(probs, woff)
         else:                 # no contig has a window (an empty probs tensor has no buffer to hand to gnm_segment_mean)

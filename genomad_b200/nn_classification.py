@@ -428,10 +428,65 @@ def embeddings_enabled() -> bool:
     return os.environ.get("GENOMAD_B200_EMBEDDINGS", "0") not in ("", "0")
 
 
-def _write_embeddings(path: Path, names_key: str, names, emb) -> None:
+def _write_embeddings(path: Path, names_key: str, names, emb, emb_reverse=None) -> None:
     # np.savez, not savez_compressed: 2 KB of fp32 per contig barely compresses, and zlib would turn writing a large
     # input's embeddings into minutes of work
-    np.savez(path, **{names_key: names, "embeddings": np.asarray(emb, dtype=np.float32)})
+    keys = {names_key: names, "embeddings": np.asarray(emb, dtype=np.float32)}
+    if emb_reverse is not None:                     # --both-strands: "embeddings" keeps its bytes, two keys follow it
+        from .engine import both_strands
+        keys["embeddings_reverse"] = np.asarray(emb_reverse, dtype=np.float32)
+        keys["embeddings_both_strands"] = both_strands(keys["embeddings"], keys["embeddings_reverse"])
+    np.savez(path, **keys)
+
+
+def both_strands_enabled() -> bool:
+    """Opt-in (``--both-strands`` / GENOMAD_B200_BOTH_STRANDS=1): also classify every sequence's reverse complement and write
+    the scores of each strand and their mean (and, with embeddings, the reverse strand's and the mean embeddings)."""
+    return os.environ.get("GENOMAD_B200_BOTH_STRANDS", "0") not in ("", "0")
+
+
+STRANDS = ("forward", "reverse", "both_strands")
+_STRANDS_HEADER = ("seq_name\t" + "\t".join(f"{c}_score_{s}" for s in STRANDS for c in ("chromosome", "plasmid", "virus"))
+                   + "\n")
+
+
+def _write_strands(npz_path: Path, tsv_path: Path, names_key: str, names, forward, reverse) -> None:
+    """<prefix>_nn_classification_strands.{npz,tsv}: float32 [n, 3] per strand and their mean, nine scores per TSV row."""
+    from .engine import both_strands
+    fwd, rev = np.asarray(forward, dtype=np.float32), np.asarray(reverse, dtype=np.float32)
+    both = both_strands(fwd, rev)
+    np.savez_compressed(npz_path, **{names_key: names, "forward": fwd, "reverse": rev, "both_strands": both})
+    with open(tsv_path, "w") as fout:
+        fout.write(_STRANDS_HEADER)
+        for name, a, b, c in zip(names, fwd, rev, both):
+            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in (*a, *b, *c)) + "\n")
+
+
+def _strands_current(npz_path: Path, tsv_path: Path, emb_path: Path, embeddings: bool) -> bool:
+    """Both strand files exist and, with embeddings, the embeddings file holds the reverse strand's keys."""
+    if not (npz_path.exists() and tsv_path.exists()):
+        return False
+    if not embeddings:
+        return True
+    try:
+        with np.load(emb_path) as z:
+            return "embeddings_reverse" in z.files and "embeddings_both_strands" in z.files
+    except Exception:
+        return False
+
+
+def _classify_reverse(clf, parsed, single_window: bool, info, contig_reduce, embeddings: bool):
+    """The reverse strand: the windows of every record's reverse complement (sequence.WindowList, reverse=True) through the
+    forward pass's chunk loop, per-contig reduction, embedding carry chain and multi-GPU routes.  A record keeps its row: it
+    has at least one window on either strand.  Returns (preds, embeddings or None)."""
+    wl = parsed.windows(sequence.WINDOW, single_window, reverse=True)
+    try:
+        offsets = wl.spans()[0]
+        if embeddings:
+            return _classify_parsed(clf, wl, offsets, info, contig_reduce, embeddings=True)
+        return _classify_parsed(clf, wl, offsets, info, contig_reduce), None
+    finally:
+        wl.close()
 
 
 def _encode_stage(console, enc_dir: Path, id_path: Path, names_key, ids_key, what, is_main, parsed, classifier=None):
@@ -470,7 +525,7 @@ _attribution_steps, _attribution_baseline = attribution_steps, attribution_basel
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
          write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
-         attribution_steps=None, attribution_baseline=None):
+         attribution_steps=None, attribution_baseline=None, both_strands=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -479,6 +534,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     is_main = info.is_main
     contig_reduce = contig_reduce or contig_reduce_mode()
     write_embeddings = embeddings_enabled() if write_embeddings is None else bool(write_embeddings)
+    strands = both_strands_enabled() if both_strands is None else bool(both_strands)
     # a stride asks for a profile: it implies the window scores unless they are switched off explicitly
     write_window_scores = ((window_scores_enabled() or window_stride is not None) if write_window_scores is None
                            else bool(write_window_scores))
@@ -526,6 +582,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if attr_target:
         files.append(outputs.nn_classification_attributions_output)
         descr.append(f"window attributions ({attr_target}{attr_method}): binary format")
+    if strands:
+        files += [outputs.nn_classification_strands_output, outputs.nn_classification_strands_npz_output]
+        descr += ["classification of both strands: tabular format", "classification of both strands: binary format"]
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -540,6 +599,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if attr_target:
             files.append(outputs.provirus_nn_classification_attributions_output)
             descr.append(f"provirus window attributions ({attr_target}{attr_method}): binary format")
+        if strands:
+            files += [outputs.provirus_nn_classification_strands_output, outputs.provirus_nn_classification_strands_npz_output]
+            descr += ["provirus classification of both strands: tabular format",
+                      "provirus classification of both strands: binary format"]
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -561,13 +624,15 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     jobs = [("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
              "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
              outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
-             outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output)]
+             outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output,
+             outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
                      outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
                      outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
-                     outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output))
+                     outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output,
+                     outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output))
 
     plan = None
     info_writer = None
@@ -587,11 +652,12 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
         # (with embeddings or window scores requested, a classification whose embeddings file is missing, or whose window
         # scores are missing or were written at another stride, or whose attributions are missing or were written for another
-        # class, is redone: same predictions, bit for bit)
+        # class, or whose strand files are missing, is redone: same predictions, bit for bit)
         plan = [(bool(skip and j[4].exists()),
                  bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
                       and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
-                      and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))))
+                      and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))
+                      and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -635,8 +701,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
-         win_npz_path, win_tsv_path, attr_path), (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
+         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path), (enc_skip, cls_skip), (parsed, index) \
+            in zip(jobs, plan, staged):
         names = preds = emb = None
+        rev_preds = rev_emb = None      # --both-strands: the reverse strand's scores and embeddings
         attr = None                     # the contig pass runs through the attribution calls
         if attr_target:
             attr = {"target": attr_target, **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
@@ -664,6 +732,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                        np.zeros((0, 3), np.float32))
                 if attr is not None:
                     attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), logp=np.zeros((0, 2), np.float32), spans=win[:3])
+                rev_preds, rev_emb = preds, emb
             else:
                 t_c = _time.perf_counter()
                 ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
@@ -676,6 +745,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, **ak)
                 if attr is not None:
                     attr["spans"] = (index.offsets, *parsed.spans()) if is_main else None
+                if strands:
+                    rev_preds, rev_emb = _classify_reverse(classifier(), parsed, single_window, info, contig_reduce,
+                                                           write_embeddings)
                 last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
                 names = index.names
             console.log(f"{'Sequences' if what == 'sequence' else 'Proviruses'} classified.")
@@ -684,8 +756,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             console.log(f"{label} classification in binary format written to {npz_path.name}.")
             if write_embeddings:
                 if is_main:
-                    _write_embeddings(emb_path, names_key, names, emb)
+                    _write_embeddings(emb_path, names_key, names, emb, rev_emb if strands else None)
                 console.log(f"{label} embeddings in binary format written to {emb_path.name}.")
+            if strands:
+                if is_main:
+                    _write_strands(strands_npz_path, strands_tsv_path, names_key, names, preds.astype(np.float32), rev_preds)
+                console.log(f"{label} classification of both strands written to {strands_tsv_path.name} and "
+                            f"{strands_npz_path.name}.")
             if write_window_scores:
                 if is_main:
                     _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,

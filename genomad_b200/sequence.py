@@ -131,6 +131,23 @@ def window_spans(length: int, single_window: bool = False) -> List[Tuple[int, in
     return spans
 
 
+_RC_TABLE = bytes.maketrans(b"ACTGNactgn", b"TGACNtgacn")
+
+
+def reverse_complement(seq: bytes) -> bytes:
+    """The reference's Sequence.rc() (sequence.py:41-43) on bytes: ACTGNactgn -> TGACNtgacn, every other byte (IUPAC codes,
+    U / u, anything else) unchanged, then reversed."""
+    return bytes(seq).translate(_RC_TABLE)[::-1]
+
+
+def rc_spans(length: int, stride: int = WINDOW, single_window: bool = False) -> List[Tuple[int, int]]:
+    """[start, end) in forward coordinates of every candidate window of the reverse complement of a stripped contig of
+    `length` nt, before the N rule: candidate k of rc(S) is rc(S)[k * stride, k * stride + len_k), which is the forward
+    segment [length - k * stride - len_k, length - k * stride)."""
+    spans = profile_spans(length, stride)[:1] if single_window else profile_spans(length, stride)
+    return [(length - e, length - s) for s, e in spans]
+
+
 def profile_spans(length: int, stride: int) -> List[Tuple[int, int]]:
     """[start, end) of every candidate window of a stripped contig of `length` nt at window stride `stride` (1..6000), before
     the N rule: candidate k starts at k * stride and is min(6000, length - k * stride) long; the first is always a candidate,
@@ -281,10 +298,11 @@ class ParsedFasta:
                 raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
         return starts, lengths
 
-    def windows(self, stride: int = WINDOW, single_window: bool = False) -> "WindowList":
+    def windows(self, stride: int = WINDOW, single_window: bool = False, reverse: bool = False) -> "WindowList":
         """The window list at `stride` (1..6000) over this index (native, records on the reader threads).  At stride 6000 with
-        this file's single_window it is the list export_windows() serves."""
-        return WindowList(self, stride, single_window)
+        this file's single_window it is the list export_windows() serves.  reverse: the same list made from every record's
+        reverse complement (reverse_complement()); its export is reverse-complemented, its spans name forward segments."""
+        return WindowList(self, stride, single_window, reverse)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -301,18 +319,20 @@ class ParsedFasta:
 
 class WindowList:
     """
-    Windows every `stride` nt of every kept record of a ParsedFasta (gnm_fasta_windows_*): what the module streams for a
-    score profile.  Same interface as ParsedFasta for the classifier's chunk loop (n_windows, export_windows,
+    Windows every `stride` nt of every kept record of a ParsedFasta (gnm_fasta_windows_*), or of every kept record's reverse
+    complement (reverse=True): what the module streams for a score profile or for the reverse strand.  Same interface as ParsedFasta for the classifier's chunk loop (n_windows, export_windows,
     release_before), plus spans(): the CSR offsets per contig and each window's start (0-based, in the record's sequence
     before stripping) and length (padding excluded).  The ParsedFasta must stay open while the list is used.
     """
 
-    def __init__(self, parsed: ParsedFasta, stride: int, single_window: bool = False):
+    def __init__(self, parsed: ParsedFasta, stride: int, single_window: bool = False, reverse: bool = False):
         import ctypes as C
         self._parsed, self._lib, self._threads = parsed, parsed._lib, parsed._threads
         self.stride = int(stride)
+        self.reverse = bool(reverse)
         self._h = C.c_void_p()
-        rc = self._lib.gnm_fasta_windows_plan(parsed._h, self.stride, int(bool(single_window)), self._threads, C.byref(self._h))
+        plan = self._lib.gnm_fasta_windows_plan_rc if self.reverse else self._lib.gnm_fasta_windows_plan
+        rc = plan(parsed._h, self.stride, int(bool(single_window)), self._threads, C.byref(self._h))
         if rc != 0:
             raise RuntimeError(self._lib.gnm_fasta_last_error().decode())
         nc, nw = C.c_int64(), C.c_int64()

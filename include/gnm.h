@@ -176,6 +176,19 @@ int gnm_classify_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_pro
  *   synchronise `stream` before calling gnm_classify_host on the same handle.
  *
  * Per-contig scores: gnm_segment_mean(h, d_probs, d_win_offsets, n_contigs, d_mean, stream).
+ *
+ * The reverse strand.  rc(S) is the reference's Sequence.rc() (sequence.py:41-43): ACTGNactgn -> TGACNtgacn, every other byte
+ * unchanged, then reversed; stripping n/N commutes with it.
+ * gnm_contig_windows_rc: the windows of every contig's reverse complement, i.e. what gnm_contig_windows (single_window) or
+ *   gnm_contig_windows_stride (stride) plans for rc(S), with the same arguments, capacity rule, failures and messages.
+ *   Candidate k is laid from the stripped end: it covers the forward segment [L - k stride - len_k, L - k stride) of the
+ *   stripped contig, len_k = min(6000, L - k stride), and d_win_start / d_win_len name that segment (so a start is still an
+ *   offset in d_seq).  Its N count is the segment's 'N' count.  single_window: the last <= 6000 nt.  At L = 10000 and stride
+ *   6000 the windows are [4000, 10000) and [0, 4000), not the forward ones in reverse order.
+ * gnm_gather_windows_rc: planned reverse windows -> d_ascii rows, row byte j = upper(comp(seg[len - 1 - j])), 'N' past len:
+ *   the rows gnm_gather_windows gives for rc(S).
+ * gnm_forward_windows_rc / gnm_embed_windows_rc: gnm_forward_windows / gnm_embed_windows with that gather: the same staging and
+ *   the same forward step, so bitwise gnm_forward_ascii / gnm_embed_ascii on gnm_gather_windows_rc's rows.
  */
 int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int single_window,
                        int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
@@ -183,10 +196,17 @@ int gnm_contig_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq
 int gnm_contig_windows_stride(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int stride,
                               int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
                               int64_t* h_n_windows, void* stream);
+int gnm_contig_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_seq_offsets, int n_contigs, int single_window,
+                          int stride, int64_t* d_win_start, int32_t* d_win_len, int64_t capacity, int32_t* d_win_offsets,
+                          int64_t* h_n_windows, void* stream);
 int gnm_gather_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                        uint8_t* d_ascii, void* stream);
+int gnm_gather_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                          uint8_t* d_ascii, void* stream);
 int gnm_forward_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                         float* d_probs, void* stream);
+int gnm_forward_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                           float* d_probs, void* stream);
 
 /* ---- encoder embeddings ------------------------------------------------------------------- */
 
@@ -215,6 +235,8 @@ int gnm_embed_tokens(gnm_handle* h, const uint16_t* d_tokens, int n, float* d_pr
 int gnm_embed_ascii(gnm_handle* h, const uint8_t* d_ascii, int n, float* d_probs, float* d_embed, void* stream);
 int gnm_embed_windows(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
                       float* d_probs, float* d_embed, void* stream);
+int gnm_embed_windows_rc(gnm_handle* h, const uint8_t* d_seq, const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                         float* d_probs, float* d_embed, void* stream);
 int gnm_embed_host(gnm_handle* h, const uint8_t* h_ascii, int n, float* h_probs, float* d_embed);
 int gnm_segment_sum_rows(gnm_handle* h, const float* d_rows, const int32_t* d_offsets, int k, const float* d_carry_in,
                          float* d_sums, float* d_carry_out, void* stream);
@@ -248,6 +270,9 @@ int gnm_segment_sum_rows(gnm_handle* h, const float* d_rows, const int32_t* d_of
  *                      Fails, before anything is built, if the list could have more than 2^31 - 1 windows (its
  *                      candidates before the N rule, a closed form).  Each list releases the pages behind its own
  *                      export cursor (gnm_fasta_windows_release_before), so a second pass over the file stays bounded too.
+ *   gnm_fasta_windows_plan_rc: the list gnm_fasta_windows_plan makes from every kept record's reverse complement rc(S)
+ *                      (gnm_contig_windows_rc's windows); its export reverse-complements and upper-cases, its spans name each
+ *                      window's forward segment.  N counts come from the same one-walk running count.
  *   gnm_fasta_windows_info   : kept records (= contigs) and windows of the list.
  *   gnm_fasta_windows_spans  : offsets int32 [n_contigs + 1] (CSR: the windows of contig c), starts int64 [n_windows] (0-based,
  *                      in the record's sequence BEFORE stripping, i.e. its joined lines), lengths int32 [n_windows] (1..6000,
@@ -268,6 +293,7 @@ int gnm_fasta_release_before(const gnm_fasta* f, int64_t upto);
 void gnm_fasta_free(gnm_fasta* f);
 typedef struct gnm_fasta_windows gnm_fasta_windows;
 int gnm_fasta_windows_plan(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out);
+int gnm_fasta_windows_plan_rc(const gnm_fasta* f, int stride, int single_window, int threads, gnm_fasta_windows** out);
 int gnm_fasta_windows_info(const gnm_fasta_windows* w, int64_t* n_contigs, int64_t* n_windows);
 int gnm_fasta_windows_spans(const gnm_fasta_windows* w, int32_t* offsets, int64_t* starts, int32_t* lengths);
 int gnm_fasta_windows_export(const gnm_fasta_windows* w, int64_t first, int64_t count, uint8_t* dst, int threads);

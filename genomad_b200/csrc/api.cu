@@ -262,6 +262,23 @@ static int pack_conv_weights(const float* Wk, std::vector<uint8_t>& pk, float* o
   return 0;
 }
 
+// Exponent k of the power of two applied to w_v and to the folded patch weights before their fp16 hi / lo split: max |w| * 2^k
+// in [2^13, 2^14), so that the lo halves stay in fp16's normal range.  k is clamped to [-126, 121], where 2^k, 2^-k (the
+// gather's unscale) and 2^-k / 32 (the q epilogues' scale) are normal fp32: every max |w| >= 2^-107 gets its exact k, smaller
+// ones keep k = 121 (their halves still carry the gather's precision while max |w| is a normal fp32 number), and no finite
+// weight overflows the fp16 halves (max |w| < 2^128 needs k >= -114).  False if a weight is not finite: it has no split.
+static constexpr int kSplitExpMin = -126, kSplitExpMax = 121;
+static bool split_exponent(const float* w, size_t n, int* k) {
+  float wmax = 0.f;
+  for (size_t i = 0; i < n; ++i) {
+    if (!std::isfinite(w[i])) return false;
+    wmax = std::max(wmax, std::fabs(w[i]));
+  }
+  *k = 0;
+  if (wmax > 0.f) { int ex; std::frexp(wmax, &ex); *k = std::max(kSplitExpMin, std::min(kSplitExpMax, 14 - ex)); }
+  return true;
+}
+
 // One IGLOO layer's patch set as the gather kernels want it (host only).
 //   * fold the patch weights (Wf = w_mult * w_summer / 32, reference igloo.py:199-204 applied to rows that carry the activation
 //     scale), sort the 8,400 (patch, slot) entries by position and deal them to the kGsSlots entry slots (padding slots:
@@ -269,9 +286,10 @@ static int pack_conv_weights(const float* Wk, std::vector<uint8_t>& pk, float* o
 //   * wv_gather_kernel's view of the same sorted entries: POSITION GROUPS = the entries that sit on one position, at most
 //     kWgGroupMax = 4 per group (the 8 columns of the warp-level mma are 4 entries x (hi, lo); 8,400 entries hit ~4,500 positions),
 //     the first group of every band of kBandRows positions, and the folded weights as that instruction's B fragments: fp16 hi / lo
-//     halves of w * 2^k (k moves the largest weight to [2^13, 2^14) so that the lo halves stay in fp16's normal range; the kernel
-//     multiplies the sums by unscale = 2^-k).  Fragment word order per slot: [K-half][k-step][tig] x {hi b0, hi b1, lo b0, lo b1},
-//     b0 = channels (k0, k0 + 1), b1 = (k0 + 8, k0 + 9), k0 = 64 K-half + 16 k-step + 2 tig.
+//     halves of w * 2^k (k = split_exponent; the kernel multiplies the sums by unscale = 2^-k).  Fragment word order per slot:
+//     [K-half][k-step][tig] x {hi b0, hi b1, lo b0, lo b1}, b0 = channels (k0, k0 + 1), b1 = (k0 + 8, k0 + 9),
+//     k0 = 64 K-half + 16 k-step + 2 tig.
+// Returns false, with o incomplete, if a folded weight is not finite.
 struct PatchPack {
   std::vector<float> ent_w;              // [kGsSlots][128]
   std::vector<int32_t> ent_pos, slot_of; // [kGsSlots], [8400]
@@ -280,7 +298,7 @@ struct PatchPack {
   std::vector<uint32_t> frag;            // [kGsSlots][128]
   float unscale = 1.f;
 };
-static void pack_patches(const int32_t* patches, const float* w_mult, const float* w_summer, PatchPack& o) {
+static bool pack_patches(const int32_t* patches, const float* w_mult, const float* w_summer, PatchPack& o) {
   std::vector<int> order(static_cast<size_t>(kPatches) * kPatchLen);
   for (size_t i = 0; i < order.size(); ++i) order[i] = static_cast<int>(i);
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return patches[a] < patches[b]; });
@@ -296,10 +314,8 @@ static void pack_patches(const int32_t* patches, const float* w_mult, const floa
     for (int c = 0; c < kC; ++c)
       ent_w[slot * kC + c] = (w_mult[static_cast<size_t>(e) * kC + c] * w_summer[k * kC + c]) * (1.f / kActScale);
   }
-  float wmax = 0.f;
-  for (float v : ent_w) wmax = std::max(wmax, std::fabs(v));
-  int k2 = 0;
-  if (wmax > 0.f && std::isfinite(wmax)) { int ex; std::frexp(wmax, &ex); k2 = std::max(-24, std::min(40, 14 - ex)); }   // wmax * 2^k2 in [2^13, 2^14)
+  int k2;
+  if (!split_exponent(ent_w.data(), ent_w.size(), &k2)) return false;
   const float wscale = std::ldexp(1.f, k2);
   o.unscale = std::ldexp(1.f, -k2);
   o.groups.clear();
@@ -336,6 +352,7 @@ static void pack_patches(const int32_t* patches, const float* w_mult, const floa
           uint32_t* f = &o.frag[(((e * 2 + kh) * 4 + ks) * 4 + tig) * 4];
           f[0] = h2(hi[0], hi[1]); f[1] = h2(hi[2], hi[3]); f[2] = h2(lo[0], lo[1]); f[3] = h2(lo[2], lo[3]);
         }
+  return true;
 }
 // Test hook (host only): the packing above for one IGLOO layer, into caller-owned buffers; see include/gnm.h.
 extern "C" int gnm_pack_patches(const int32_t* patches, const float* w_mult, const float* w_summer, int32_t* slot_of, int32_t* ent_pos,
@@ -347,7 +364,8 @@ extern "C" int gnm_pack_patches(const int32_t* patches, const float* w_mult, con
   for (int i = 0; i < kPatches * kPatchLen; ++i)
     if (patches[i] < 0 || patches[i] >= kTok) return fail("gnm_pack_patches: patch index out of range");
   PatchPack pk;
-  pack_patches(patches, w_mult, w_summer, pk);
+  if (!pack_patches(patches, w_mult, w_summer, pk))
+    return fail("gnm_pack_patches: folded patch weights w_mult * w_summer / 32 not finite: no fp16 operand split carries them");
   const int real_groups = pk.band_gstart[kNumBands];
   if (groups && *n_groups < real_groups) return fail("gnm_pack_patches: groups buffer too small");
   if (slot_of) std::memcpy(slot_of, pk.slot_of.data(), pk.slot_of.size() * sizeof(int32_t));
@@ -416,12 +434,12 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
       if (dev_upload(h, &h->conv_w32[L], convw[L], static_cast<size_t>(kTaps) * kC * kC)) return 1;
     }
     for (int s = 0; s < 2; ++s) {                          // w_v: (K-half, weight hi/lo) of the fp16 split of w_v * 2^e
-      // e moves max |w_v| to [2^13, 2^14) (as for the patch weights): unscaled, the lo halves of small weights (|w| < 0.125)
-      // fall into fp16's subnormal range and the Ahi * Wlo pass stops correcting.  The q epilogues multiply by 2^-e / 32.
-      float wmax = 0.f;
-      for (int i = 0; i < kC * kC; ++i) wmax = std::max(wmax, std::fabs(w->igloo[s].w_v[i]));
-      int e = 0;
-      if (wmax > 0.f && std::isfinite(wmax)) { int ex; std::frexp(wmax, &ex); e = std::max(-24, std::min(40, 14 - ex)); }
+      // e moves max |w_v| to [2^13, 2^14) (split_exponent, as for the patch weights): unscaled, the lo halves of small weights
+      // (|w| < 0.125) fall into fp16's subnormal range and the Ahi * Wlo pass stops correcting.  The q epilogues multiply by
+      // 2^-e / 32.
+      int e;
+      if (!split_exponent(w->igloo[s].w_v, static_cast<size_t>(kC) * kC, &e))
+        return fail("gnm_create: IGLOO layer " + std::to_string(s) + ": w_v not finite: no fp16 operand split carries it");
       h->wv_out_scale[s] = std::ldexp(1.f / kActScale, -e);
       std::vector<uint8_t> pk;
       for (int kh = 0; kh < 2; ++kh)
@@ -435,7 +453,9 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
   for (int s = 0; s < 2; ++s) {
     const gnm_igloo_weights& g = w->igloo[s];
     PatchPack pk;
-    pack_patches(g.patches, g.w_mult, g.w_summer, pk);
+    if (!pack_patches(g.patches, g.w_mult, g.w_summer, pk))
+      return fail("gnm_create: IGLOO layer " + std::to_string(s) +
+                  ": folded patch weights w_mult * w_summer / 32 not finite: no fp16 operand split carries them");
     h->gather_unscale[s] = pk.unscale;
     h->band_groups[s].resize(kNumBands);
     for (int b = 0; b < kNumBands; ++b) h->band_groups[s][b] = pk.band_gstart[b + 1] - pk.band_gstart[b];

@@ -80,7 +80,8 @@ const char* gnm_version(void);
 /*
  * Create a classifier on CUDA device `device`.  Copies and re-packs the weights (fp16 hi/lo
  * operand splits, folded patch weights, batch-norm scale/shift) and allocates a workspace able
- * to process `max_batch` windows per internal step.  Synchronous.
+ * to process `max_batch` windows per internal step.  Synchronous.  Fails, naming the IGLOO layer, if its w_v or its folded
+ * patch weights w_mult * w_summer / 32 are not all finite (no fp16 operand split carries them); any finite ones are accepted.
  * Replaces create_classifier() + load_weights() (nn_classification.py:309-310).
  */
 int gnm_create(int device, const gnm_weights* weights, int max_batch, gnm_handle** out);
@@ -371,8 +372,8 @@ int gnm_get_option(gnm_handle* h, const char* name, int* value);
  *   frag [slots][128] words   the folded weights * 2^k as mma.m16n8k16 B fragments: per slot [K-half 2][k-step 4][tig 4] x
  *                             {hi b0, hi b1, lo b0, lo b1}, each word two fp16: b0 = channels (k0, k0 + 1), b1 = (k0 + 8, k0 + 9),
  *                             k0 = 64 K-half + 16 k-step + 2 tig; hi = fp16(w 2^k), lo = fp16(w 2^k - hi)
- *   unscale                   2^-k
- * Any output pointer may be NULL.
+ *   unscale                   2^-k, k = 14 - (exponent of max |w|) clamped to [-126, 121]: max |w| 2^k in [2^13, 2^14)
+ * Any output pointer may be NULL.  Fails if a folded weight is not finite (as gnm_create does).
  */
 int gnm_pack_patches(const int32_t* patches, const float* w_mult, const float* w_summer, int32_t* slot_of, int32_t* ent_pos,
                      float* ent_w, int32_t* groups, int* n_groups, int32_t* band_first_group, uint32_t* frag, float* unscale,

@@ -125,7 +125,7 @@ struct gnm_handle {
   std::vector<void*> allocs;
   const uint8_t* attr_route[2] = {nullptr, nullptr};   // routing / maxima of the last attribution chunk (gnm_debug_fetch "route*", "routeq*")
   const float* attr_rq[2] = {nullptr, nullptr};
-  const uint8_t* attr_y1 = nullptr;                    // the attribution pass's layer-1 copy (gnm_debug_fetch "attr_y1")
+  const gnm_attr* attr_last = nullptr;                 // the context of the last attribution chunk (gnm_debug_fetch "attr_*")
   int attr_mb = 0;                                     // max_batch of the context those buffers belong to
 };
 
@@ -1013,8 +1013,8 @@ static int check_device_status(gnm_handle* h) {
     h->status->act_overflow = 0;
     for (int i = 0; i < 4; ++i) h->status->ov_stage[i] = 0;
     if (stage == 0)
-      return fail("gradient range exceeded in conv3's backward pass of an attribution call: |g_z2| * s_w > 3.5 saturates the "
-                  "e4m3 correction plane -- the attributions of that step are not within their precision bar");
+      return fail("gradient range exceeded in the backward pass of an attribution call: a gradient is not finite, or its "
+                  "per-window scale cannot bring it under 3.5 -- the attributions of that step are not within their precision bar");
     return fail(std::string("activation range exceeded in ") + (stage == 1 ? "layer 1" : stage == 2 ? "conv2" : "conv3") +
                 ": |y| > 3.5 saturates the e4m3 correction plane (|y| > 2047 overflows fp16) -- these weights are outside the "
                 "range the split-operand tensor-core recipe supports (common.cuh); results of that step are not within 1e-4");
@@ -1369,6 +1369,8 @@ extern "C" int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int
   return 0;
 }
 
+static int attr_debug_fetch(gnm_handle* h, const gnm_attr* a, const std::string& k, int n, float* d_dst, cudaStream_t st);
+
 extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream) {
   if (!h || !which || !d_dst) return fail("null argument");
   if (n < 1 || n > h->max_batch) return fail("gnm_debug_fetch: n out of range");
@@ -1377,7 +1379,7 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
   const std::string k(which);
   const float* src = nullptr;
   size_t count = 0;
-  if ((k.rfind("route", 0) == 0 || k == "attr_y1") && n > h->attr_mb)        // the last attribution context's buffers
+  if ((k.rfind("route", 0) == 0 || k.rfind("attr_", 0) == 0) && n > h->attr_mb)   // the last attribution context's buffers
     return fail("gnm_debug_fetch: n exceeds the max_batch of the last attribution call's context (" + std::to_string(h->attr_mb) + ")");
   if (k == "buf0" || k == "buf1") {
     const size_t rows = static_cast<size_t>(n) * kTok;
@@ -1395,15 +1397,13 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
     if (!r) return fail("gnm_debug_fetch: no attribution call has run on this handle");
     GNM_CUDA(cudaMemcpyAsync(d_dst, r, static_cast<size_t>(n) * kPooled * kC, cudaMemcpyDeviceToDevice, st));
     return 0;
-  } else if (k == "attr_y1") {
-    if (!h->attr_y1) return fail("gnm_debug_fetch: no attribution call has run on this handle");
-    const size_t rows = static_cast<size_t>(n) * kTok;
-    join_rows_kernel<<<static_cast<unsigned>((rows * kC + 255) / 256), 256, 0, st>>>(h->attr_y1, d_dst, rows, 0);
-    return check_launch(h, "join_rows_kernel");
   } else if (k == "routeq0" || k == "routeq1") {
     src = h->attr_rq[k == "routeq1"];
     if (!src) return fail("gnm_debug_fetch: no attribution call has run on this handle");
     count = static_cast<size_t>(n) * kPooled * kC;
+  } else if (k.rfind("attr_", 0) == 0) {
+    if (!h->attr_last) return fail("gnm_debug_fetch: no attribution call has run on this handle");
+    return attr_debug_fetch(h, h->attr_last, k, n, d_dst, st);
   }
   else return fail("gnm_debug_fetch: unknown buffer " + k);
   GNM_CUDA(cudaMemcpyAsync(d_dst, src, count * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1413,17 +1413,18 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
 // ------------------------------------------------------------------------------------------------ attributions (attr.cuh)
 // Workspace of the attribution pass, separate from the handle so that plain handles keep their memory.  Per window:
 // y1 copy, g_z3 and g_z2 operand rows (3 x 4.6 MB), fp32 g_y1 / g_z rows (2 x 3.1 MB), routing + routed maxima (2 x 0.48 MB):
-// ~21 MB (kAttrBytesPerWindow).
+// ~21 MB (gnm_attr_bytes_per_window).
 struct gnm_attr {
   gnm_handle* h = nullptr;
   int max_batch = 0;
   uint8_t* y1 = nullptr;                                // layer 1 re-run: the forward's y1 (ybuf[0] is overwritten by conv3)
   uint8_t* gz3 = nullptr; uint8_t* gz2 = nullptr;       // conv operand rows of s_w g_z3, s_w g_z2, time-reversed
-  float* f32a = nullptr;                                // fp32 rows: g_z3 (before packing), then g_z1 (conv2 backward output)
+  float* f32a = nullptr;                                // fp32 rows: g_z3, then s_w g_z2 (each before packing), then s_w g_z1
   float* gy1 = nullptr;                                 // fp32 rows: IGLOO#0's part of g_y1
   uint8_t* route[2] = {nullptr, nullptr}; float* rq[2] = {nullptr, nullptr};
   float* g_out = nullptr; float* alpha = nullptr; float* g_logit = nullptr; float* g_mpi = nullptr;
   float* blockmax = nullptr; float* s_w = nullptr; float* probs = nullptr;
+  float* unitmax = nullptr; float* s2 = nullptr;        // conv3 backward: max |s_w g_z2| per unit and warp; its power of two
   uint8_t* wpackT[2] = {nullptr, nullptr};              // W2^T, W3^T packed like the forward's conv weights
   float out_scaleT[2] = {1.f, 1.f};
   float* wvT[2] = {nullptr, nullptr}; float* wqkT[2] = {nullptr, nullptr};
@@ -1456,7 +1457,8 @@ extern "C" int gnm_attr_destroy(gnm_attr* a) {
   cudaDeviceSynchronize();
   for (int s = 0; s < 2; ++s)
     if (a->h->attr_route[s] == a->route[s]) {
-      a->h->attr_route[s] = nullptr; a->h->attr_rq[s] = nullptr; a->h->attr_y1 = nullptr; a->h->attr_mb = 0;
+      a->h->attr_route[s] = nullptr; a->h->attr_rq[s] = nullptr; a->h->attr_last = nullptr;
+      a->h->attr_mb = 0;
     }
   for (void* p : a->allocs) cudaFree(p);
   delete a;
@@ -1491,6 +1493,8 @@ extern "C" int gnm_attr_create(gnm_handle* h, int max_batch, gnm_attr** out) {
   ATTR_ALLOC(a->g_mpi, mb * kPatches * sizeof(float));
   ATTR_ALLOC(a->blockmax, mb * kAttrPosBlocks * sizeof(float));
   ATTR_ALLOC(a->s_w, mb * sizeof(float));
+  ATTR_ALLOC(a->unitmax, mb * kUnitsPerWin * 8 * sizeof(float));
+  ATTR_ALLOC(a->s2, mb * sizeof(float));
   ATTR_ALLOC(a->probs, mb * 3 * sizeof(float));
 #undef ATTR_ALLOC
   // ---- weights, derived from the handle's device copies
@@ -1550,16 +1554,16 @@ static int launch_route(gnm_handle* h, gnm_attr* a, int s, const CUtensorMap& tm
   conv_t_attr_kernel<kConvRoute><<<std::min(h->num_sms, p.n_tiles), kConvThreads, kConvTSmem, st>>>(tm, h->tm_w_half[2 + s], p, x);
   return check_launch(h, "conv_t_attr_kernel<route>");
 }
-// backward of conv layer L (0 = conv2, 1 = conv3) over time-reversed gradient rows
+// backward of conv layer L (0 = conv2, 1 = conv3) over time-reversed gradient rows into fp32 rows
 static int launch_conv_bwd(gnm_handle* h, gnm_attr* a, int L, const CUtensorMap& tm_in, const uint8_t* mask_rows,
-                           const float* add_rows, uint8_t* rows_out, float* f32_out, int n, cudaStream_t st) {
+                           const float* add_rows, const float* s_in, float* f32_out, float* unit_max, int n, cudaStream_t st) {
   ConvTcParams p;
   p.status = h->status; p.experiment = 0; p.dbg = nullptr;
-  p.bias = nullptr; p.y_out = rows_out; p.q_out = nullptr;
+  p.bias = nullptr; p.y_out = nullptr; p.q_out = nullptr;
   p.out_scale = a->out_scaleT[L]; p.out_fp8 = 1;
   p.n_tiles = n * kUnitsPerWin;
   ConvAttrExt x = {};
-  x.mask_rows = mask_rows; x.add_rows = add_rows; x.s_w = a->s_w; x.f32_out = f32_out;
+  x.mask_rows = mask_rows; x.add_rows = add_rows; x.s_w = a->s_w; x.s_in = s_in; x.f32_out = f32_out; x.unit_max = unit_max;
   conv_t_attr_kernel<kConvBwd><<<std::min(h->num_sms, p.n_tiles), kConvThreads, kConvTSmem, st>>>(tm_in, a->tm_wT[L], p, x);
   return check_launch(h, "conv_t_attr_kernel<bwd>");
 }
@@ -1609,12 +1613,14 @@ static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, in
   attr_pack_kernel<<<sgrid, 256, 0, st>>>(a->f32a, a->blockmax, a->s_w, a->gz3);
   if (check_launch(h, "attr_pack_kernel")) return 1;
   timer_mark(h, "attr_conv3_bwd", st);
-  if (launch_conv_bwd(h, a, 1, a->tm_gz3, h->ybuf[1], nullptr, a->gz2, nullptr, n, st)) return 1;   // mask y2 -> s_w g_z2
+  if (launch_conv_bwd(h, a, 1, a->tm_gz3, h->ybuf[1], nullptr, nullptr, a->f32a, a->unitmax, n, st)) return 1;   // mask y2 -> s_w g_z2
+  attr_pack_gz2_kernel<<<sgrid, 256, 0, st>>>(a->f32a, a->unitmax, a->s2, a->gz2, h->status);      // s2 s_w g_z2
+  if (check_launch(h, "attr_pack_gz2_kernel")) return 1;
   timer_mark(h, "attr_igloo0", st);
   if (launch_logits(h, 0, n, st)) return 1;                                  // IGLOO#0's logits (the tail overwrote them)
   if (launch_igloo_bwd(h, a, 0, n, st)) return 1;                            // -> fp32 g_y1 (IGLOO#0 part)
   timer_mark(h, "attr_conv2_bwd", st);
-  if (launch_conv_bwd(h, a, 0, a->tm_gz2, a->y1, a->gy1, nullptr, a->f32a, n, st)) return 1;        // + s_w g_y1, mask y1 -> s_w g_z1
+  if (launch_conv_bwd(h, a, 0, a->tm_gz2, a->y1, a->gy1, a->s2, a->f32a, nullptr, n, st)) return 1;   // / s2, + s_w g_y1, mask y1 -> s_w g_z1
   timer_mark(h, "attr_layer1_attr", st);
   if (ig) {
     layer1_ig_kernel<<<sgrid, 256, 0, st>>>(d_ascii, a->f32a, h->conv1_table, a->s_w, ig->m, ig->baseline, a->gy1);
@@ -1625,8 +1631,34 @@ static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, in
   }
   timer_mark(h, "end", st);
   for (int s = 0; s < 2; ++s) { h->attr_route[s] = a->route[s]; h->attr_rq[s] = a->rq[s]; }
-  h->attr_y1 = a->y1;
+  h->attr_last = a;
   h->attr_mb = a->max_batch;
+  return 0;
+}
+
+// gnm_debug_fetch's "attr_*" buffers of the last attribution chunk (include/gnm.h); n <= the context's max_batch (checked)
+static int attr_debug_fetch(gnm_handle* h, const gnm_attr* a, const std::string& k, int n, float* d_dst, cudaStream_t st) {
+  const size_t rows = static_cast<size_t>(n) * kTok;
+  const float* src = nullptr;
+  size_t count = 0;
+  if (k == "attr_gz3" || k == "attr_gz2") {                // operand rows, time-reversed: joined, back in position order
+    const uint8_t* r = k == "attr_gz3" ? a->gz3 : a->gz2;
+    join_rows_kernel<<<static_cast<unsigned>((rows * kC + 255) / 256), 256, 0, st>>>(r, d_dst, rows, 1);
+    if (check_launch(h, "join_rows_kernel")) return 1;
+    reverse_rows_kernel<<<static_cast<unsigned>((rows * kC / 2 + 255) / 256), 256, 0, st>>>(d_dst, n);
+    return check_launch(h, "reverse_rows_kernel");
+  }
+  if (k == "attr_g_out") { src = a->g_out; count = static_cast<size_t>(n) * 256; }
+  else if (k == "attr_s_w") { src = a->s_w; count = n; }
+  else if (k == "attr_s2") { src = a->s2; count = n; }
+  else if (k == "attr_gy1") { src = a->gy1; count = rows * kC; }
+  else if (k == "attr_gz1") { src = a->f32a; count = rows * kC; }
+  else if (k == "attr_y1") {
+    join_rows_kernel<<<static_cast<unsigned>((rows * kC + 255) / 256), 256, 0, st>>>(a->y1, d_dst, rows, 0);
+    return check_launch(h, "join_rows_kernel");
+  }
+  else return fail("gnm_debug_fetch: unknown buffer " + k);
+  GNM_CUDA(cudaMemcpyAsync(d_dst, src, count * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
@@ -1737,7 +1769,7 @@ extern "C" int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_
 
 extern "C" long long gnm_attr_bytes_per_window(void) {
   return static_cast<long long>(kTok) * (3 * kRowBytes + 2 * kC * 4) + 2LL * kPooled * kC * 5 +
-         4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + 4);
+         4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + kUnitsPerWin * 8 + 5);
 }
 
 // ------------------------------------------------------------------------------------------------ embedding neighbours

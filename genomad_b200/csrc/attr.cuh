@@ -14,9 +14,11 @@
 //   convs    g_z = g_y * lrelu'(y);  g_yprev[s] = sum_j g_z[s+5-j] W[j]^T  (conv_t_attr_kernel<kConvBwd>, rows reversed)
 //   layer 1  attr[t] = sum_{u=t}^{min(t+5,5996)} <g_z1[u], W1[t-u+5, tok[t], :]>
 // From g_z3 on, the gradient is carried times a per-window power of two s_w (max |g_z3| s_w in [0.25, 0.5)) so that the conv
-// operand formats (common.cuh) see values in their range; layer 1 divides it out.
+// operand formats (common.cuh) see values in their range; layer 1 divides it out.  conv3's backward output gets a power of two
+// of its own, s2 (max |s_w g_z2| s2 in [1, 2)), for the operand rows conv2's backward pass reads; that pass divides it out.
 #pragma once
 #include "common.cuh"
+#include "conv_t.cuh"
 #include "encode.cuh"
 #include "igloo.cuh"
 
@@ -224,26 +226,32 @@ attr_igloo_backward_kernel(const IglooBwdParams P) {
   }
 }
 
-// s_w = 2^k with max |g_z3| * s_w in [0.25, 0.5) (1 for an all-zero gradient)
-__device__ __forceinline__ float attr_scale_of(float gmax) {
+// 2^k with gmax * 2^k in [2^(top-1), 2^top) (1 for an all-zero gradient)
+__device__ __forceinline__ float attr_scale_of(float gmax, int top) {
   if (!(gmax > 0.f) || !isfinite(gmax)) return 1.f;
   int e;
   frexpf(gmax, &e);                                              // gmax = m 2^e, m in [0.5, 1)
-  return ldexpf(1.f, max(-120, min(120, -e - 1)));
+  return ldexpf(1.f, max(-120, min(120, top - e)));
 }
 
-// fp32 g_z3 rows (natural order) -> conv operand rows (hi16 | - | e4m3 pairs) of s_w * g_z3 at row 5996 - t, the input of
-// conv3's backward pass.  grid (24, n), 256 threads, one warp per position; block 0 also stores s_w.
-__global__ void __launch_bounds__(256)
-attr_pack_kernel(const float* __restrict__ g, const float* __restrict__ blockmax, float* __restrict__ s_w_out,
-                 uint8_t* __restrict__ rows_out) {
+// fp32 gradient rows (natural order) -> conv operand rows (hi16 | - | e4m3 pairs) of s * g at row 5996 - t, the input of a
+// conv's backward pass, with s the per-window power of two that puts max |g| s in [2^(kTop-1), 2^kTop).  s depends only on the
+// window's maximum (kNb block maxima of |g| per window), so s times the rows is the same bits for any gradient scale.
+// grid (24, n), 256 threads, one warp per position; block 0 also stores s.  With `status`, a window whose scaled maximum lies
+// above the hi8 plane's range (a gradient that is not finite) raises act_overflow, stage 0.
+template <int kNb, int kTop>
+__device__ __forceinline__ void attr_pack_body(const float* __restrict__ g, const float* __restrict__ blockmax,
+                                               float* __restrict__ s_out, uint8_t* __restrict__ rows_out, DeviceStatus* status) {
   __shared__ float s_sw;
   const int w = blockIdx.y, t0 = blockIdx.x * kAttrSeg, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     float m = 0.f;
-    for (int i = 0; i < kAttrPosBlocks; ++i) m = fmaxf(m, blockmax[static_cast<size_t>(w) * kAttrPosBlocks + i]);
-    s_sw = attr_scale_of(m);
-    if (blockIdx.x == 0) s_w_out[w] = s_sw;
+    for (int i = 0; i < kNb; ++i) m = fmaxf(m, blockmax[static_cast<size_t>(w) * kNb + i]);
+    s_sw = attr_scale_of(m, kTop);
+    if (blockIdx.x == 0) {
+      s_out[w] = s_sw;
+      if (status && !(m * s_sw <= kHi8Limit / kActScale)) { status->act_overflow = 1; status->ov_stage[0] = 1; }
+    }
   }
   __syncthreads();
   const float sc = kActScale * s_sw;
@@ -265,6 +273,34 @@ attr_pack_kernel(const float* __restrict__ g, const float* __restrict__ blockmax
         static_cast<uint32_t>(pack_e4m3x2((a.z - fb.x) * kLo8Scale, fb.x * kHi8Scale)) |
             (static_cast<uint32_t>(pack_e4m3x2((a.w - fb.y) * kLo8Scale, fb.y * kHi8Scale)) << 16));
   }
+}
+
+// g_z3 (IGLOO#1's block maxima) -> s_w g_z3 rows, max |s_w g_z3| in [0.25, 0.5): the input of conv3's backward pass.  A
+// gradient that is not finite reaches conv3's backward output and is reported by the g_z2 pack below.
+__global__ void __launch_bounds__(256)
+attr_pack_kernel(const float* __restrict__ g, const float* __restrict__ blockmax, float* __restrict__ s_w_out,
+                 uint8_t* __restrict__ rows_out) {
+  attr_pack_body<kAttrPosBlocks, -1>(g, blockmax, s_w_out, rows_out, nullptr);
+}
+
+// s_w g_z2 (conv3's backward output and its unit maxima) -> s2 s_w g_z2 rows, max in [1, 2): the input of conv2's backward pass
+__global__ void __launch_bounds__(256)
+attr_pack_gz2_kernel(const float* __restrict__ g, const float* __restrict__ unit_max, float* __restrict__ s2_out,
+                     uint8_t* __restrict__ rows_out, DeviceStatus* status) {
+  attr_pack_body<kUnitsPerWin * 8, 1>(g, unit_max, s2_out, rows_out, status);
+}
+
+// fp32 rows [n][5997][128] reversed in place within each window (gnm_debug_fetch of the time-reversed operand rows)
+__global__ void reverse_rows_kernel(float* __restrict__ rows, int n) {
+  const size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t half = static_cast<size_t>(kTok / 2) * kC;
+  if (i >= static_cast<size_t>(n) * half) return;
+  const size_t w = i / half, rc = i - w * half, r = rc / kC, c = rc - r * kC;
+  float* a = rows + (w * kTok + r) * kC + c;
+  float* b = rows + (w * kTok + (kTok - 1 - r)) * kC + c;
+  const float t = *a;
+  *a = *b;
+  *b = t;
 }
 
 // ------------------------------------------------------------------------------------------------ layer 1

@@ -114,14 +114,16 @@ template <bool kWvMode> __device__ __forceinline__ constexpr int region_src(int 
 // Epilogue modes of the kernel body.  kConvFwd / kConvWv are the forward's conv_t_kernel<false> / <true>.  The attribution
 // pass (attr.cuh) adds two: kConvRoute is the w_v pass with an epilogue that also stores WHERE each pooled maximum sits, and
 // kConvBwd is the conv pass run over time-reversed gradient rows against W[j]^T (no bias; lrelu' of the forward activation at the
-// mirrored row; optional fp32 rows added first; fp32 or operand-format output).  MMA loop, producers and rings are shared.
+// mirrored row; optional fp32 rows added first; fp32 output).  MMA loop, producers and rings are shared.
 constexpr int kConvFwd = 0, kConvWv = 1, kConvRoute = 2, kConvBwd = 3;
 struct ConvAttrExt {
   uint8_t* route_out;         // kConvRoute: [n][749][128] row (0..7) of each pooled maximum, the first one on ties
   const uint8_t* mask_rows;   // kConvBwd: forward activation rows [n][5997][768 B]; the sign of hi16 at row 5996 - r gives lrelu'
   const float* add_rows;      // kConvBwd: fp32 rows [n][5997][128] (natural order) added as s_w * add before the mask, or nullptr
   const float* s_w;           // kConvBwd: [n] per-window gradient scale (with add_rows)
-  float* f32_out;             // kConvBwd: fp32 rows [n][5997][128] at the mirrored (natural) row, or nullptr: operand rows p.y_out
+  const float* s_in;          // kConvBwd: [n] per-window power of two the input rows carry on top of s_w, divided out, or nullptr
+  float* f32_out;             // kConvBwd: fp32 rows [n][5997][128] at the mirrored (natural) row
+  float* unit_max;            // kConvBwd: [n][24][8] max |output| per unit and consumer warp, or nullptr
 };
 
 template <int kMode>
@@ -320,9 +322,12 @@ __device__ __forceinline__ void conv_t_body(const CUtensorMap* tm_act_p, const C
             qrow[ch0 + 8] = m1 * oscale;
           }
         }
-      } else if (kMode == kConvBwd && x.f32_out) {
-        // backward pass into fp32 rows: accumulator row r is the gradient at position 5996 - r; plain 4-byte stores
+      } else if constexpr (kMode == kConvBwd) {
+        // backward pass into fp32 rows: accumulator row r is the gradient at position 5996 - r; plain 4-byte stores.  The input
+        // scale s_in is a power of two, so dividing it out is exact; the unit maxima are order-free (deterministic)
         const float sw = x.add_rows ? x.s_w[w] : 0.f;
+        const float inv = x.s_in ? 1.f / x.s_in[w] : 1.f;
+        float umax = 0.f;
 #pragma unroll
         for (int j = 0; j < 32; ++j)
 #pragma unroll
@@ -334,11 +339,19 @@ __device__ __forceinline__ void conv_t_body(const CUtensorMap* tm_act_p, const C
                 const int ch = ch0 + 8 * h;
                 const size_t row = static_cast<size_t>(w) * kTok + (kTok - 1 - pos);
                 float v = d[4 * j + 2 * h + e] * oscale;
+                if (x.s_in) v *= inv;
                 if (x.add_rows) v = fmaf(sw, x.add_rows[row * kC + ch], v);
                 const __half m = *reinterpret_cast<const __half*>(x.mask_rows + row * kRowBytes + kOffHi16 + 2 * ch);
-                x.f32_out[row * kC + ch] = __hgt(m, __float2half(0.f)) ? v : v * kLeaky;
+                v = __hgt(m, __float2half(0.f)) ? v : v * kLeaky;
+                x.f32_out[row * kC + ch] = v;
+                umax = fmaxf(umax, fabsf(v));
               }
             }
+        if (x.unit_max) {
+#pragma unroll
+          for (int off = 16; off > 0; off >>= 1) umax = fmaxf(umax, __shfl_xor_sync(0xffffffffu, umax, off));
+          if (lane == 0) x.unit_max[static_cast<size_t>(unit) * 8 + g * 4 + wq] = umax;
+        }
       } else {
         // Column group j of the accumulator is this warp's 16 channels x 8 positions 8 j .. 8 j + 7.  Per output plane that is
         // 8 rows x 32 contiguous bytes, both planes 512 B: one 16-byte store per lane.  Both planes are b16 per (channel,
@@ -361,18 +374,8 @@ __device__ __forceinline__ void conv_t_body(const CUtensorMap* tm_act_p, const C
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const float bias = h ? bias1 : bias0;
-            float y0, y1;
-            if constexpr (kMode == kConvBwd) {
-              // gradient rows, time-reversed in and out: lrelu' of the forward activation at the mirrored position
-              y0 = y1 = 0.f;
-              const int pos = t0 + 8 * j + 2 * (lane & 3);
-              const __half* mrow = reinterpret_cast<const __half*>(x.mask_rows + (static_cast<size_t>(w) * kTok + (kTok - 1 - pos)) * kRowBytes + kOffHi16) + ch0 + 8 * h;
-              if (pos < kTok) y0 = kActScale * d[4 * j + 2 * h] * oscale * (__hgt(mrow[0], __float2half(0.f)) ? 1.f : kLeaky);
-              if (pos + 1 < kTok) y1 = kActScale * d[4 * j + 2 * h + 1] * oscale * (__hgt(mrow[-kRowBytes / 2], __float2half(0.f)) ? 1.f : kLeaky);
-            } else {
-              y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
-              y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
-            }
+            const float y0 = kActScale * lrelu(fmaf(d[4 * j + 2 * h], oscale, bias));
+            const float y1 = kActScale * lrelu(fmaf(d[4 * j + 2 * h + 1], oscale, bias));
             amax = fmaxf(amax, fmaxf(fabsf(y0), fabsf(y1)));
             if (p.out_fp8) {
               const __half2 hh = __floats2half2_rn(y0, y1);
@@ -398,8 +401,7 @@ __device__ __forceinline__ void conv_t_body(const CUtensorMap* tm_act_p, const C
       }
       t_epi += clock64() - tq;
     }
-    if constexpr (kMode == kConvBwd) { if (!x.f32_out) flag_act_overflow(p.status, amax, kHi8Limit, 0); }
-    else if (!kWvMode) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
+    if constexpr (!kWvMode && kMode != kConvBwd) flag_act_overflow(p.status, amax, p.out_fp8 ? kHi8Limit : kF16Limit, p.out_fp8 ? 2 : 3);
     if (p.dbg && wq == 0 && lane == 0) {     // include/gnm.h, "conv_dbg"
       long long* dd = p.dbg + blockIdx.x * 8;
       if (g == 0) { dd[0] = clock64() - t_begin; dd[1] = t_mma; dd[2] = w_a; dd[3] = w_w; dd[4] = it; dd[6] = t_epi; }

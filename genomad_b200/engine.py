@@ -810,7 +810,9 @@ class Classifier:
         shapes = {"buf0": (n, TOKENS, 128), "buf1": (n, TOKENS, 128), "q0": (n, 749, 128), "q1": (n, 749, 128),
                   "mpi0": (n, 2100), "mpi1": (n, 2100), "h0": (n, 256), "h1": (n, 512), "h2": (n, 512), "logits": (n, 752),
                   "conv_dbg": (self.get_option("num_sms"), 16), "routeq0": (n, 749, 128), "routeq1": (n, 749, 128),
-                  "route0": (n, 749, 128), "route1": (n, 749, 128), "attr_y1": (n, TOKENS, 128)}
+                  "route0": (n, 749, 128), "route1": (n, 749, 128), "attr_y1": (n, TOKENS, 128), "attr_g_out": (n, 256),
+                  "attr_s_w": (n,), "attr_s2": (n,), "attr_gz3": (n, TOKENS, 128), "attr_gz2": (n, TOKENS, 128),
+                  "attr_gy1": (n, TOKENS, 128), "attr_gz1": (n, TOKENS, 128)}
         dtype = t.uint8 if which in ("route0", "route1") else t.float32
         out = t.empty(shapes[which], dtype=dtype, device=self._dev())
         _check(self.lib, self.lib.gnm_debug_fetch(self._h, which.encode(), n, out.data_ptr(), self._stream()))

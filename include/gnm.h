@@ -407,7 +407,12 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  * [n][749][128], the row 0..7 inside each max-pool window of the pooled maximum (first row on ties) -- n * 749 * 128 BYTES are
  * written to d_dst; "routeq0","routeq1" [n][749][128] = the maxima the routing pass found (bitwise "q0","q1"); "attr_y1"
  * [n][5997][128] = its layer-1 copy (y1, bitwise what the forward's layer 1 wrote).  An attribution
- * call re-runs IGLOO#0's logits, so "logits" then holds the first IGLOO kernel's.
+ * call re-runs IGLOO#0's logits, so "logits" then holds the first IGLOO kernel's.  The backward pass's intermediates, same
+ * conditions, positions in natural order: "attr_g_out" [n][256] = d log p_c / d h0 (unscaled); "attr_s_w" [n] = the per-window
+ * power of two s_w; "attr_s2" [n] = the power of two of conv3's backward output (max |s_w g_z2| s2 in [1, 2)); "attr_gz3",
+ * "attr_gz2" [n][5997][128] = s_w g_z3 and s2 s_w g_z2 as the next conv reads them (the joined hi16 + lo8 of the operand rows);
+ * "attr_gy1" [n][5997][128] = IGLOO#0's part of g_y1 (fp32, unscaled); "attr_gz1" [n][5997][128] = s_w g_z1 (fp32).  After an
+ * integrated-gradients call they hold the last chunk's rows, except "attr_gy1", which then holds the layer-1 IG rows.
  */
 int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void* stream);
 
@@ -432,8 +437,10 @@ int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d_dst, void*
  *   in order (no tail overlap), then the backward pass over what that step left on the device.
  *   d_attr  DEVICE float [n][5997], caller-owned.
  *   d_probs DEVICE float [n][3] or NULL; when given, bitwise what gnm_forward_ascii / gnm_forward_windows return.
- *   Asynchronous on `stream`; a gradient range overflow (|g| * s_w beyond the conv operand format) is reported by the next call
- *   or gnm_check_status, like act_overflow.  Fails with conv_impl = 1: the fp32 validation kernels have no backward pass.
+ *   Asynchronous on `stream`.  The gradient rows the two backward convs read carry per-window powers of two (s_w, s2) that put
+ *   their maxima in the operand format's range whatever the weights' scale; only a gradient that is not finite is reported, as
+ *   a gradient range overflow by the next call or gnm_check_status, like act_overflow.  Fails with conv_impl = 1: the fp32
+ *   validation kernels have no backward pass.
  */
 typedef struct gnm_attr gnm_attr;
 int gnm_attr_create(gnm_handle* h, int max_batch, gnm_attr** out);

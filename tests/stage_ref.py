@@ -50,6 +50,16 @@ BARS: Dict[str, tuple] = {
                                      # step gives 3.6e-6 for the logits' 352-product split-K partials (tests/test_stage_recipes.py)
     "attention": (1e-5, 5e-5),       # softmax over 749 logits + weighted sum of q, fp32 (h0[:128] also carries logits0's error)
     "probs": (2e-6, 1e-5),           # Dense(3) + softmax, fp32; absolute error of the probabilities
+    # attribution backward pass (tests/attr_stage_ref.py); the bars come from tests/test_attr_stage_recipes_cpu.py, which emulates
+    # each stage and a mutant of each.  conv_bwd_tc: the conv recipe over gradient rows whose per-window scale puts the maximum
+    # in [1, 2): entries more than ~2^7 below it keep a normal lo8 no longer, so the per-output max is wider than conv_tc's
+    "conv_bwd_tc": (4e-5, 4e-4),     # conv3 / conv2 backward on tensor cores, operand-row output (conv3) or fp32 rows (conv2)
+    "attr_head": (1e-5, 1e-5),       # g_out: Dense(3), Dense(512) and Dense(512) backward, fp32
+    "attr_igloo": (1e-5, 5e-5),      # g_y / g_z3: softmax, g_alpha, the g_mpi sgemm, value and patch paths, fp32
+    "attr_layer1": (1e-5, 1e-5),     # attr: 6 table rows x 128 channels per position, fp32
+    "attr_gz3_rows": (1e-4, 2e-3),   # IGLOO#1 + pack: s_w g_z3 stored as hi16 + lo8, max in [0.25, 0.5) (the max bar is
+                                     # wider than the emulation's 2x for the 1.1e-3 the H100 measures; only the rms bar
+                                     # separates the recipe from its mutant, rows without lo8)
 }
 
 

@@ -21,6 +21,8 @@ KERNELS = {   # mangled name: register cap
     "_ZN3gnm26attr_igloo_backward_kernelILb0EEEvNS_14IglooBwdParamsE": 64,
     "_ZN3gnm26attr_igloo_backward_kernelILb1EEEvNS_14IglooBwdParamsE": 64,
     "_ZN3gnm16attr_pack_kernelEPKfS1_PfPh": 64,
+    "_ZN3gnm20attr_pack_gz2_kernelEPKfS1_PfPhPNS_12DeviceStatusE": 64,
+    "_ZN3gnm19reverse_rows_kernelEPfi": 64,
     "_ZN3gnm18layer1_attr_kernelEPKhPKfS3_S3_Pf": 64,
 }
 

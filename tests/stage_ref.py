@@ -165,19 +165,29 @@ def head_softmax(h2: torch.Tensor, w) -> Ref:
 
 
 # ------------------------------------------------------------------------------------------ metrics
-def position_regions(n: int, pooled: bool = False, windows: Optional[list] = None) -> Dict[str, tuple]:
+def position_regions(n: int, pooled: bool = False, windows: Optional[list] = None, tile: Optional[int] = None) -> Dict[str, tuple]:
     """Index sets (window slice or indices, position slice) where kernels tend to go wrong: the causal zero fill (positions 0-5),
     the last, partial 256-position conv unit (5888-5996), the last 24-position IGLOO band (5976-5996), and the windows on both
     sides of the 8-window groups of the fused IGLOO kernel (8k - 1, 8k, 8k + 1).  pooled: the same regions in max-pool groups.
     windows: the batch indices of the rows actually compared (a sample of an n-window batch); the window regions then index
-    into that sample."""
+    into that sample.  tile: also the windows on both sides of every `tile`-row M tile edge of the tail GEMMs (tile k - 1,
+    tile k, tile k + 1) and, when the last M tile is partial, the windows of that tile."""
     f = (lambda a, b: slice(a // POOL, min(N_POOL, (b + POOL) // POOL))) if pooled else (lambda a, b: slice(a, b + 1))
-    edges = {i for k in range(8, n + 1, 8) for i in (k - 1, k, k + 1) if i < n}
-    edge = sorted(edges) if windows is None else [r for r, i in enumerate(windows) if i in edges]
+
+    def rows(edges):
+        return sorted(edges) if windows is None else [r for r, i in enumerate(windows) if i in edges]
+    edge = rows({i for k in range(8, n + 1, 8) for i in (k - 1, k, k + 1) if i < n})
     regions = {"all": (slice(None), slice(None)), "pos 0-5": (slice(None), f(0, 5)),
                "pos 5888-5996": (slice(None), f(5888, 5996)), "pos 5976-5996": (slice(None), f(5976, 5996))}
     if edge:
         regions["win 8k+-1"] = (edge, slice(None))
+    if tile:
+        t_edge = rows({i for k in range(tile, n, tile) for i in (k - 1, k, k + 1) if i < n})
+        if t_edge:
+            regions[f"win {tile}k+-1"] = (t_edge, slice(None))
+        last = rows(set(range(n // tile * tile, n)))
+        if n % tile and last:
+            regions["win last tile"] = (last, slice(None))
     return regions
 
 

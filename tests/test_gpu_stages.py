@@ -72,34 +72,38 @@ def _fetch(w, a, max_batch, opts, stops=(2, 3, 0)):
     return got
 
 
-def _check(label, w, a, got, conv_impl=0, tokens=None, regions=None):
+def _check(label, w, a, got, conv_impl=0, tokens=None, regions=None, rows=None):
     """Every stage present in `got` against its bar; prints one table row per stage, returns the misses.  tokens: layer 1's
     input when it is not the tokenization of the windows `a`; regions: (positions, pooled positions) region sets of
-    R.position_regions when `got` holds a sample of a larger batch."""
+    R.position_regions when `got` holds a sample of a larger batch; rows: window regions (R.position_regions' "win ..."
+    entries) for the stages with one row per window (mpi, logits1, h0, h1, h2, probs).  `got` may hold the tail alone (q0, mpi0,
+    q1, mpi1 and the tail buffers, no activations): the tail stages are then checked on their own inputs."""
     n = len(a)
     reg, preg = regions or (R.position_regions(n), R.position_regions(n, pooled=True))
+    rows = rows or {}
     conv_bar = "conv_fp32" if conv_impl else "conv_tc"
     checks = []
     if "y1" in got:
         checks += [("y1", "y1", got["y1"], R.conv1(T.tokenize_windows(a) if tokens is None else tokens, w), reg),
                    ("y2 (conv2)", conv_bar, got["y2"], R.conv(got["y1"], w["c2w"], w["c2b"]), reg),
                    ("q0 (w_v#0)", "wv", got["q0"], R.wv_pool(got["y1"], w["ig0_w_v"]), preg),
-                   ("mpi0", "gather", got["mpi0"], R.gather(got["y1"], w, 0), {})]
+                   ("mpi0", "gather", got["mpi0"], R.gather(got["y1"], w, 0), rows)]
     if "y3" in got:
         checks += [("y3 (conv3)", conv_bar, got["y3"], R.conv(got["y2_3"], w["c3w"], w["c3b"]), reg)]
         if "y2" in got:
             assert torch.equal(got["y2"], got["y2_3"]), "conv2 is not deterministic across steps"
-    if "q1" in got:
+    if "q1" in got and "y3" in got:
         assert torch.equal(got["y3"], got["y3_0"]), "conv3 is not deterministic across steps"
-        logits0 = got["mpi0"] @ torch.as_tensor(w["ig0_w_qk"], dtype=R.D)        # not fetchable: fp64 from the kernel's mpi0
         checks += [("q1 (w_v#1)", "wv", got["q1"], R.wv_pool(got["y3"], w["ig1_w_v"]), preg),
-                   ("mpi1", "gather", got["mpi1"], R.gather(got["y3"], w, 1), {}),
-                   ("logits1", "tf32x3", got["logits"], R.matmul(got["mpi1"], w["ig1_w_qk"]), {}),
-                   ("h0[:128]", "attention", got["h0"][:, :128], R.attention(logits0, got["q0"]), {}),
-                   ("h0[128:]", "attention", got["h0"][:, 128:], R.attention(got["logits"], got["q1"]), {}),
-                   ("h1 (dense0)", "tf32x3", got["h1"], R.dense_bn_relu(got["h0"], w, 0), {}),
-                   ("h2 (dense1)", "tf32x3", got["h2"], R.dense_bn_relu(got["h1"], w, 1), {}),
-                   ("probs", "probs", got["probs"], R.head_softmax(got["h2"], w), {})]
+                   ("mpi1", "gather", got["mpi1"], R.gather(got["y3"], w, 1), rows)]
+    if "h1" in got:
+        logits0 = got["mpi0"] @ torch.as_tensor(w["ig0_w_qk"], dtype=R.D)        # not fetchable: fp64 from the kernel's mpi0
+        checks += [("logits1", "tf32x3", got["logits"], R.matmul(got["mpi1"], w["ig1_w_qk"]), rows),
+                   ("h0[:128]", "attention", got["h0"][:, :128], R.attention(logits0, got["q0"]), rows),
+                   ("h0[128:]", "attention", got["h0"][:, 128:], R.attention(got["logits"], got["q1"]), rows),
+                   ("h1 (dense0)", "tf32x3", got["h1"], R.dense_bn_relu(got["h0"], w, 0), rows),
+                   ("h2 (dense1)", "tf32x3", got["h2"], R.dense_bn_relu(got["h1"], w, 1), rows),
+                   ("probs", "probs", got["probs"], R.head_softmax(got["h2"], w), rows)]
     bad = []
     for stage, key, g, ref, regions in checks:
         if float(ref.s_abs.max()) < 1e-20:

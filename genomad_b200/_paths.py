@@ -113,6 +113,23 @@ class NNOutputs:
     def provirus_nn_classification_strands_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification_strands.npz")
 
+    # ---- opt-in (--head), not a reference output: scores of a user-trained classifier head
+    @property
+    def nn_classification_head_output(self) -> Path:
+        return self._nn("nn_classification_head.tsv")
+
+    @property
+    def nn_classification_head_npz_output(self) -> Path:
+        return self._nn("nn_classification_head.npz")
+
+    @property
+    def provirus_nn_classification_head_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head.tsv")
+
+    @property
+    def provirus_nn_classification_head_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

@@ -74,9 +74,14 @@ def cli():
                    "strand and their mean to <prefix>_nn_classification_strands.{tsv,npz}; with --write-embeddings the "
                    "embeddings file also gets embeddings_reverse and embeddings_both_strands. The main outputs are unchanged. "
                    "About twice the GPU time. Not an option of the reference.")
+@click.option("--head", "head", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
+              help="Also score every sequence with this classifier head (a train-head output, <prefix>_head.npz) and write "
+                   "the scores of its classes to <prefix>_nn_classification_head.{tsv,npz}. The head must have been trained "
+                   "on this encoder (checked before any work). It scores the forward strand only, also with --both-strands. "
+                   "The main outputs are unchanged. Not an option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
                       write_embeddings, write_window_scores, window_stride, write_attributions, attribution_steps,
-                      attribution_baseline, both_strands):
+                      attribution_baseline, both_strands, head):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -96,8 +101,40 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["attribution_baseline"] = attribution_baseline
     if both_strands:
         extra["both_strands"] = True
+    if head is not None:
+        extra["head"] = head
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
+
+
+@cli.command(name="train-head", context_settings=CONTEXT_SETTINGS)
+@click.argument("input", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("labels", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("--epochs", type=click.IntRange(1), default=10, show_default=True, help="Passes over the training windows.")
+@click.option("--batch-size", type=click.IntRange(1, 65536), default=256, show_default=True, help="Windows per training step.")
+@click.option("--learning-rate", type=click.FloatRange(0, min_open=True), default=1e-3, show_default=True,
+              help="Adam learning rate.")
+@click.option("--validation-fraction", type=click.FloatRange(0, 1, max_open=True), default=0.1, show_default=True,
+              help="Share of each class's sequences held out for validation (split by sequence, never by window).")
+@click.option("--class-weight", type=click.Choice(["balanced", "none"]), default="balanced", show_default=True,
+              help="balanced: class c weighs N / (C * N_c) in the loss, over the training windows; none: 1.")
+@click.option("--seed", type=click.IntRange(0), default=0, show_default=True,
+              help="Seed of the initialisation, split, order and dropout (>= 0).")
+@click.option("--threads", "-t", type=int, default=get_n_available_cpus(), show_default=True,
+              help="Number of threads to use.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def train_head(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, threads,
+               verbose):
+    """Train a classifier head for your own classes on the frozen encoder. LABELS is a TSV with the header
+    seq_name<TAB>class and one row per labelled sequence of the INPUT FASTA (seq_name as nn-classification writes it).
+    Writes <prefix>_head.npz (the epoch with the lowest validation loss), <prefix>_head_training.tsv and
+    <prefix>_head_training.log to OUTPUT; score sequences with it by nn-classification --head. One GPU. Not a module of
+    the reference."""
+    from . import train_head as module
+    module.main(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, threads,
+                verbose)
 
 
 @cli.command(name="embedding-neighbours", context_settings=CONTEXT_SETTINGS)

@@ -25,6 +25,7 @@
 #include "attr.cuh"
 #include "neighbours.cuh"
 #include "clusters.cuh"
+#include "head.cuh"
 
 using namespace gnm;
 
@@ -130,15 +131,15 @@ struct gnm_handle {
 };
 
 // ------------------------------------------------------------------------------------------------
-template <class T>
-static int dev_upload(gnm_handle* h, T** dst, const T* src, size_t count) {
+template <class O, class T>     // O: any owner with an `allocs` list (the handle, a head, a trainer)
+static int dev_upload(O* h, T** dst, const T* src, size_t count) {
   GNM_CUDA(cudaMalloc(reinterpret_cast<void**>(dst), count * sizeof(T)));
   h->allocs.push_back(*dst);
   GNM_CUDA(cudaMemcpy(*dst, src, count * sizeof(T), cudaMemcpyHostToDevice));
   return 0;
 }
-template <class T>
-static int dev_alloc(gnm_handle* h, T** dst, size_t count) {
+template <class O, class T>
+static int dev_alloc(O* h, T** dst, size_t count) {
   GNM_CUDA(cudaMalloc(reinterpret_cast<void**>(dst), count * sizeof(T)));
   h->allocs.push_back(*dst);
   return 0;
@@ -379,6 +380,24 @@ extern "C" int gnm_pack_patches(const int32_t* patches, const float* w_mult, con
   return 0;
 }
 
+// keras BN inference form  x * inv + (beta - mean * inv),  inv = gamma * rsqrt(var + eps)
+static void fold_bn(const gnm_bn_weights& b, std::vector<float>& sc, std::vector<float>& sh) {
+  sc.resize(kHidden); sh.resize(kHidden);
+  for (int i = 0; i < kHidden; ++i) {
+    const float inv = b.gamma[i] * (1.0f / std::sqrt(b.moving_variance[i] + 1e-3f));
+    sc[i] = inv;
+    sh[i] = b.beta[i] - b.moving_mean[i] * inv;
+  }
+}
+
+// W [K in][512 out] -> W^T [512][K] as two TF32 halves: the K-major B operand of logits_tc_kernel
+static void split_dense_t(const float* w, int K, std::vector<float>& thi, std::vector<float>& tlo) {
+  thi.resize(static_cast<size_t>(kHidden) * K); tlo.resize(thi.size());
+  for (int k = 0; k < K; ++k)
+    for (int n = 0; n < kHidden; ++n)
+      split_tf32(w[static_cast<size_t>(k) * kHidden + n], thi[static_cast<size_t>(n) * K + k], tlo[static_cast<size_t>(n) * K + k]);
+}
+
 // ------------------------------------------------------------------------------------------------
 extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_handle** out) {
   if (!w || !out) return fail("gnm_create: null argument");
@@ -483,12 +502,8 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
   // ---- head: keras BN inference form  x * inv + (beta - mean * inv),  inv = gamma * rsqrt(var + eps)
   {
     auto bn = [&](const gnm_bn_weights& b, float** scale, float** shift) -> int {
-      std::vector<float> sc(kHidden), sh(kHidden);
-      for (int i = 0; i < kHidden; ++i) {
-        const float inv = b.gamma[i] * (1.0f / std::sqrt(b.moving_variance[i] + 1e-3f));
-        sc[i] = inv;
-        sh[i] = b.beta[i] - b.moving_mean[i] * inv;
-      }
+      std::vector<float> sc, sh;
+      fold_bn(b, sc, sh);
       if (dev_upload(h, scale, sc.data(), kHidden)) return 1;
       return dev_upload(h, shift, sh.data(), kHidden);
     };
@@ -501,10 +516,8 @@ extern "C" int gnm_create(int device, const gnm_weights* w, int max_batch, gnm_h
     const float* dw[2] = {w->dense0_kernel, w->dense1_kernel};
     const int dk[2] = {256, kHidden};
     for (int L = 0; L < 2; ++L) {                          // W^T [512 out][K in] as two TF32 halves: the K-major B operand
-      std::vector<float> thi(static_cast<size_t>(kHidden) * dk[L]), tlo(thi.size());
-      for (int k = 0; k < dk[L]; ++k)
-        for (int n = 0; n < kHidden; ++n)
-          split_tf32(dw[L][static_cast<size_t>(k) * kHidden + n], thi[static_cast<size_t>(n) * dk[L] + k], tlo[static_cast<size_t>(n) * dk[L] + k]);
+      std::vector<float> thi, tlo;
+      split_dense_t(dw[L], dk[L], thi, tlo);
       if (dev_upload(h, &h->dwT_hi[L], thi.data(), thi.size())) return 1;
       if (dev_upload(h, &h->dwT_lo[L], tlo.data(), tlo.size())) return 1;
     }
@@ -623,7 +636,8 @@ extern "C" int gnm_destroy(gnm_handle* h) {
 }
 
 // ------------------------------------------------------------------------------------------------
-static int check_launch(gnm_handle* h, const char* what) {
+template <class O>
+static int check_launch(O* h, const char* what) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(std::string(what) + " launch failed: " + cudaGetErrorString(e));
   h->launches++;
@@ -778,7 +792,8 @@ static int launch_gather(gnm_handle* h, int s, int buf, int n, cudaStream_t st) 
   return check_launch(h, "patch_finish_kernel");
 }
 
-static int launch_sgemm(gnm_handle* h, const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N,
+template <class O>     // O: the handle, or a head trainer (anything that counts its launches)
+static int launch_sgemm(O* h, const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N,
                         int K, const float* bias, const float* scale, const float* shift, int relu, cudaStream_t st) {
   const int nb = (N + kGemmBN - 1) / kGemmBN;
   if (M >= 64) {                                           // 32-row tiles only for tiny batches (measured slower otherwise)
@@ -825,22 +840,26 @@ static int launch_logits(gnm_handle* h, int s, int n, cudaStream_t st) {
 // 128 CTAs run at batch 1024; the split-K partials go through logits_part (6 x 752 floats per window >= 8 x 512).
 constexpr int kHeadSplits = 8;
 static_assert(kHeadSplits * kHidden <= kLgSplits * kLogitsLd, "logits_part is too small for the head's split-K partials");
-static int launch_dense_tc(gnm_handle* h, int layer, int n, float* out, float* out_hi, float* out_lo, float* emit, cudaStream_t st) {
-  const int K = layer == 0 ? 256 : kHidden;
+static int launch_dense_tc_maps(gnm_handle* h, const CUtensorMap* tm_a, const CUtensorMap* tm_b, int K, int n, const float* bias,
+                                const float* scale, const float* shift, float* out, float* out_hi, float* out_lo, float* emit,
+                                cudaStream_t st) {
   LogitsTcParams p;
   p.part = h->logits_part; p.ldc = kHidden; p.n_rows = n; p.n_cols = kHidden; p.status = h->status;
   p.chunks_total = K / kLgBK;
   p.chunks_per_split = (p.chunks_total + kHeadSplits - 1) / kHeadSplits;
   const int splits = (p.chunks_total + p.chunks_per_split - 1) / p.chunks_per_split;
   dim3 grid(kHidden / kLgBN, (n + kLgBM - 1) / kLgBM, splits);
-  logits_tc_kernel<<<grid, kLgThreads, kLgSmem, st>>>(h->tm_hd_a[layer][0], h->tm_hd_a[layer][1], h->tm_hd_b[layer][0],
-                                                      h->tm_hd_b[layer][1], p);
+  logits_tc_kernel<<<grid, kLgThreads, kLgSmem, st>>>(tm_a[0], tm_a[1], tm_b[0], tm_b[1], p);
   if (check_launch(h, "logits_tc_kernel(dense)")) return 1;
   const size_t total = static_cast<size_t>(n) * kHidden;
   splitk_reduce_epi_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-      h->logits_part, out, out_hi, out_lo, emit, n, kHidden, splits, layer == 0 ? h->d0b : h->d1b,
-      layer == 0 ? h->bn0_scale : h->bn1_scale, layer == 0 ? h->bn0_shift : h->bn1_shift, 1);
+      h->logits_part, out, out_hi, out_lo, emit, n, kHidden, splits, bias, scale, shift, 1);
   return check_launch(h, "splitk_reduce_epi_kernel");
+}
+static int launch_dense_tc(gnm_handle* h, int layer, int n, float* out, float* out_hi, float* out_lo, float* emit, cudaStream_t st) {
+  return launch_dense_tc_maps(h, h->tm_hd_a[layer], h->tm_hd_b[layer], layer == 0 ? 256 : kHidden, n, layer == 0 ? h->d0b : h->d1b,
+                              layer == 0 ? h->bn0_scale : h->bn1_scale, layer == 0 ? h->bn0_shift : h->bn1_shift, out, out_hi,
+                              out_lo, emit, st);
 }
 
 // the buffer set the next step's main part writes and its tail reads (kernel arguments are captured at launch, so switching the
@@ -1941,5 +1960,265 @@ extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uin
   }
   cl_resolve_kernel<<<1, kClThreads, 0, st>>>(mask, n, words, d_covered, d_new_reps, d_n_new);
   GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ classifier heads (head.cuh)
+struct gnm_head {
+  int C = 0;
+  std::vector<void*> allocs;
+  float *d1w = nullptr, *d1b = nullptr, *scale = nullptr, *shift = nullptr, *dwT_hi = nullptr, *dwT_lo = nullptr;
+  float *d2w = nullptr, *d2b = nullptr;
+  CUtensorMap tm_b[2];
+};
+
+extern "C" int gnm_head_destroy(gnm_head* hd) {
+  if (!hd) return 0;
+  for (void* p : hd->allocs) cudaFree(p);
+  delete hd;
+  return 0;
+}
+
+static int head_check_weights(const char* fn, const gnm_head_weights* w) {
+  if (!w->dense1_kernel || !w->dense1_bias || !w->bn1.gamma || !w->bn1.beta || !w->bn1.moving_mean || !w->bn1.moving_variance ||
+      !w->dense2_kernel || !w->dense2_bias)
+    return fail(std::string(fn) + ": null weight pointer");
+  if (w->n_classes < 2 || w->n_classes > kHeadMaxClasses)
+    return fail(std::string(fn) + ": n_classes must be in [2, " + std::to_string(kHeadMaxClasses) + "], not " +
+                std::to_string(w->n_classes));
+  return 0;
+}
+
+extern "C" int gnm_head_create(gnm_handle* h, const gnm_head_weights* w, gnm_head** out) {
+  if (!h || !w || !out) return fail("gnm_head_create: null argument");
+  if (head_check_weights("gnm_head_create", w)) return 1;
+  GNM_CUDA(cudaSetDevice(h->device));
+  gnm_head* hd = new gnm_head();
+  hd->C = w->n_classes;
+  *out = hd;   // so the caller can gnm_head_destroy() after a partial failure
+  std::vector<float> sc, sh, thi, tlo;
+  fold_bn(w->bn1, sc, sh);
+  split_dense_t(w->dense1_kernel, kHidden, thi, tlo);
+  if (dev_upload(hd, &hd->d1w, w->dense1_kernel, static_cast<size_t>(kHidden) * kHidden)) return 1;
+  if (dev_upload(hd, &hd->d1b, w->dense1_bias, kHidden)) return 1;
+  if (dev_upload(hd, &hd->scale, sc.data(), kHidden)) return 1;
+  if (dev_upload(hd, &hd->shift, sh.data(), kHidden)) return 1;
+  if (dev_upload(hd, &hd->dwT_hi, thi.data(), thi.size())) return 1;
+  if (dev_upload(hd, &hd->dwT_lo, tlo.data(), tlo.size())) return 1;
+  if (dev_upload(hd, &hd->d2w, w->dense2_kernel, static_cast<size_t>(kHidden) * hd->C)) return 1;
+  if (dev_upload(hd, &hd->d2b, w->dense2_bias, hd->C)) return 1;
+  PFN_encodeTiled enc = nullptr;
+  if (get_encode_fn(&enc)) return 1;
+  if (make_f32_map(enc, &hd->tm_b[0], hd->dwT_hi, kHidden, kHidden, kLgBN)) return 1;
+  if (make_f32_map(enc, &hd->tm_b[1], hd->dwT_lo, kHidden, kHidden, kLgBN)) return 1;
+  return 0;
+}
+
+// Steps of max_batch rows on the handle's head workspace (hA_hi[1] / hA_lo[1], logits_part, h2), in stream order.
+extern "C" int gnm_head_forward(gnm_handle* h, const gnm_head* hd, const float* d_embed, int n, float* d_probs, void* stream) {
+  if (!h || !hd) return fail("gnm_head_forward: null handle");
+  if (n < 0) return fail("gnm_head_forward: negative row count");
+  if (n == 0) return 0;
+  if (!d_embed || !d_probs) return fail("gnm_head_forward: null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int off = 0; off < n; off += h->max_batch) {
+    const int m = std::min(h->max_batch, n - off);
+    const float* x = d_embed + static_cast<size_t>(off) * kHidden;
+    if (h->conv_impl == 0) {
+      const size_t total = static_cast<size_t>(m) * kHidden;
+      head_split_tf32_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(x, h->hA_hi[1], h->hA_lo[1], total);
+      if (check_launch(h, "head_split_tf32_kernel")) return 1;
+      if (launch_dense_tc_maps(h, h->tm_hd_a[1], hd->tm_b, kHidden, m, hd->d1b, hd->scale, hd->shift, h->h2, nullptr, nullptr,
+                               nullptr, st)) return 1;
+    } else {
+      if (launch_sgemm(h, x, kHidden, hd->d1w, kHidden, h->h2, kHidden, m, kHidden, kHidden, hd->d1b, hd->scale, hd->shift, 1,
+                       st)) return 1;
+    }
+    head_softmax_kernel<<<(m * 32 + 255) / 256, 256, 0, st>>>(h->h2, hd->d2w, hd->d2b, d_probs + static_cast<size_t>(off) * hd->C,
+                                                             m, hd->C);
+    if (check_launch(h, "head_softmax_kernel")) return 1;
+  }
+  return 0;
+}
+
+static int head_segment_any(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs, float* d_out,
+                            void* stream, bool mean) {
+  if (!h) return fail("null handle");
+  if (C < 1 || C > kHeadMaxClasses) return fail("gnm_head_segment: width must be in [1, 32]");
+  if (n_contigs < 0) return fail("negative contig count");
+  if (n_contigs == 0) return 0;
+  if (!d_probs || !d_offsets || !d_out) return fail("null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int grid = (n_contigs + 127) / 128;
+  if (mean) head_segment_reduce_kernel<true><<<grid, 128, 0, st>>>(d_probs, d_offsets, n_contigs, C, d_out);
+  else head_segment_reduce_kernel<false><<<grid, 128, 0, st>>>(d_probs, d_offsets, n_contigs, C, d_out);
+  return check_launch(h, "head_segment_reduce_kernel");
+}
+extern "C" int gnm_head_segment_mean(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs,
+                                     float* d_mean, void* stream) {
+  return head_segment_any(h, d_probs, C, d_offsets, n_contigs, d_mean, stream, true);
+}
+extern "C" int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs,
+                                    float* d_sum, void* stream) {
+  return head_segment_any(h, d_probs, C, d_offsets, n_contigs, d_sum, stream, false);
+}
+
+// ---- training
+// Flat parameter layout (gnm.h): W1 [512][512], b1, gamma, beta [512], W2 [512][C], b2 [C]; gradients, Adam m and v alike.
+static size_t head_param_count(int C) { return static_cast<size_t>(kHidden) * kHidden + 3 * kHidden + static_cast<size_t>(kHidden) * C + C; }
+
+struct gnm_head_train {
+  int device = 0, C = 0, max_batch = 0, last_b = 0;
+  long long launches = 0;
+  uint32_t key = 0;
+  long long step = 0;
+  float lr = 1e-3f;
+  size_t n_par = 0;
+  std::vector<void*> allocs;
+  float *P = nullptr, *G = nullptr, *M = nullptr, *V = nullptr, *mov_mean = nullptr, *mov_var = nullptr;
+  float *Xb = nullptr, *XbT = nullptr, *z1 = nullptr, *hb = nullptr, *hT = nullptr, *logits = nullptr, *dz2 = nullptr;
+  float *row_loss = nullptr, *W2T = nullptr, *dH = nullptr, *dz1 = nullptr, *stats = nullptr;
+  uint8_t* mask = nullptr;
+  int* bad = nullptr;                           // mapped host flag: kHeadBadIndex | kHeadBadLabel (head.cuh)
+  float* par(float* base, int which) const {   // 0 W1, 1 b1, 2 gamma, 3 beta, 4 W2, 5 b2
+    const size_t o[6] = {0, static_cast<size_t>(kHidden) * kHidden, static_cast<size_t>(kHidden) * kHidden + kHidden,
+                         static_cast<size_t>(kHidden) * kHidden + 2 * kHidden, static_cast<size_t>(kHidden) * kHidden + 3 * kHidden,
+                         static_cast<size_t>(kHidden) * kHidden + 3 * kHidden + static_cast<size_t>(kHidden) * C};
+    return base + o[which];
+  }
+};
+
+extern "C" int gnm_head_train_destroy(gnm_head_train* tr) {
+  if (!tr) return 0;
+  cudaSetDevice(tr->device);
+  cudaDeviceSynchronize();
+  for (void* p : tr->allocs) cudaFree(p);
+  if (tr->bad) cudaFreeHost(tr->bad);
+  delete tr;
+  return 0;
+}
+
+extern "C" int gnm_head_train_create(int device, const gnm_head_weights* init, int max_batch, uint64_t seed, float learning_rate,
+                                     gnm_head_train** out) {
+  if (!init || !out) return fail("gnm_head_train_create: null argument");
+  if (head_check_weights("gnm_head_train_create", init)) return 1;
+  if (max_batch < 1 || max_batch > 65536) return fail("gnm_head_train_create: max_batch must be in [1, 65536]");
+  if (!(learning_rate > 0.f) || !std::isfinite(learning_rate)) return fail("gnm_head_train_create: learning_rate must be > 0");
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("gnm_head_train_create: no CUDA device available");
+  if (device < 0 || device >= ndev) return fail("gnm_head_train_create: bad device index");
+  GNM_CUDA(cudaSetDevice(device));
+  gnm_head_train* tr = new gnm_head_train();
+  *out = tr;
+  tr->device = device; tr->C = init->n_classes; tr->max_batch = max_batch; tr->key = head_key(seed); tr->lr = learning_rate;
+  tr->n_par = head_param_count(tr->C);
+  const size_t mb = static_cast<size_t>(max_batch), C = static_cast<size_t>(tr->C);
+  for (float** p : {&tr->P, &tr->G, &tr->M, &tr->V})
+    if (dev_alloc(tr, p, tr->n_par)) return 1;
+  GNM_CUDA(cudaMemset(tr->M, 0, tr->n_par * sizeof(float)));
+  GNM_CUDA(cudaMemset(tr->V, 0, tr->n_par * sizeof(float)));
+  GNM_CUDA(cudaMemset(tr->G, 0, tr->n_par * sizeof(float)));
+  const float* src[6] = {init->dense1_kernel, init->dense1_bias, init->bn1.gamma, init->bn1.beta, init->dense2_kernel, init->dense2_bias};
+  const size_t cnt[6] = {static_cast<size_t>(kHidden) * kHidden, kHidden, kHidden, kHidden, kHidden * C, C};
+  for (int i = 0; i < 6; ++i) GNM_CUDA(cudaMemcpy(tr->par(tr->P, i), src[i], cnt[i] * sizeof(float), cudaMemcpyHostToDevice));
+  if (dev_upload(tr, &tr->mov_mean, init->bn1.moving_mean, kHidden)) return 1;
+  if (dev_upload(tr, &tr->mov_var, init->bn1.moving_variance, kHidden)) return 1;
+  for (float** p : {&tr->Xb, &tr->XbT, &tr->z1, &tr->hb, &tr->hT, &tr->dH, &tr->dz1})
+    if (dev_alloc(tr, p, mb * kHidden)) return 1;
+  if (dev_alloc(tr, &tr->logits, mb * C)) return 1;
+  if (dev_alloc(tr, &tr->dz2, mb * C)) return 1;
+  if (dev_alloc(tr, &tr->row_loss, mb)) return 1;
+  if (dev_alloc(tr, &tr->W2T, kHidden * C)) return 1;
+  if (dev_alloc(tr, &tr->stats, 3 * kHidden)) return 1;
+  if (dev_alloc(tr, &tr->mask, mb * kHidden)) return 1;
+  GNM_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&tr->bad), sizeof(int), cudaHostAllocMapped));
+  *tr->bad = 0;
+  return 0;
+}
+
+// Inputs an earlier step found out of range (see kHeadBadIndex); the flag is read without waiting, so a step sees the flags of
+// the steps that have completed, and gnm_head_train_read, which waits, sees them all.
+static int head_train_status(const gnm_head_train* tr, const char* fn) {
+  const int b = *reinterpret_cast<volatile int*>(tr->bad);
+  if (b & kHeadBadIndex) return fail(std::string(fn) + ": a step was given a batch index outside [0, n_rows)");
+  if (b & kHeadBadLabel) return fail(std::string(fn) + ": a step was given a label outside [0, C)");
+  return 0;
+}
+
+extern "C" int gnm_head_train_step(gnm_head_train* tr, const float* d_X, int64_t n_rows, const int64_t* d_idx,
+                                   const int32_t* d_labels, const float* d_class_weights, int B, float* d_loss, void* stream) {
+  if (!tr) return fail("gnm_head_train_step: null trainer");
+  if (n_rows < 1) return fail("gnm_head_train_step: n_rows must be >= 1");
+  if (head_train_status(tr, "gnm_head_train_step")) return 1;
+  if (B < 1 || B > tr->max_batch) return fail("gnm_head_train_step: B must be in [1, max_batch = " + std::to_string(tr->max_batch) + "]");
+  if (!d_X || !d_idx || !d_labels || !d_class_weights || !d_loss) return fail("gnm_head_train_step: null buffer");
+  GNM_CUDA(cudaSetDevice(tr->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int C = tr->C;
+  const size_t rows = static_cast<size_t>(B) * kHidden;
+  const unsigned g_rows = static_cast<unsigned>((rows + 255) / 256);
+  const int col_grid = kHidden / kHeadColBlock, col_threads = kHeadColBlock * kHeadRowGroups;
+  float *W1 = tr->par(tr->P, 0), *b1 = tr->par(tr->P, 1), *gamma = tr->par(tr->P, 2), *beta = tr->par(tr->P, 3);
+  float *W2 = tr->par(tr->P, 4), *b2 = tr->par(tr->P, 5);
+  head_gather_kernel<<<g_rows, 256, 0, st>>>(d_X, n_rows, d_idx, B, tr->Xb, tr->XbT, tr->bad);
+  if (check_launch(tr, "head_gather_kernel")) return 1;
+  if (launch_sgemm(tr, tr->Xb, kHidden, W1, kHidden, tr->z1, kHidden, B, kHidden, kHidden, b1, nullptr, nullptr, 0, st)) return 1;   // z1 = x W1 + b1
+  head_bn_forward_kernel<<<col_grid, col_threads, 0, st>>>(tr->z1, B, gamma, beta, tr->mov_mean, tr->mov_var, tr->key,
+                                                          static_cast<uint32_t>(tr->step), tr->hb, tr->hT, tr->mask, tr->stats);
+  if (check_launch(tr, "head_bn_forward_kernel")) return 1;
+  if (launch_sgemm(tr, tr->hb, kHidden, W2, C, tr->logits, C, B, C, kHidden, b2, nullptr, nullptr, 0, st)) return 1;              // h W2 + b2
+  head_softmax_xent_kernel<<<(B * 32 + 255) / 256, 256, 0, st>>>(tr->logits, n_rows, d_idx, d_labels, d_class_weights, B, C,
+                                                                 tr->dz2, tr->row_loss, tr->bad);
+  if (check_launch(tr, "head_softmax_xent_kernel")) return 1;
+  head_loss_db2_kernel<<<1, 64, 0, st>>>(tr->row_loss, tr->dz2, B, C, d_loss, tr->par(tr->G, 5));
+  if (check_launch(tr, "head_loss_db2_kernel")) return 1;
+  if (launch_sgemm(tr, tr->hT, B, tr->dz2, C, tr->par(tr->G, 4), C, kHidden, C, B, nullptr, nullptr, nullptr, 0, st)) return 1;    // dW2 = h^T dZ2
+  head_transpose_w2_kernel<<<(kHidden * C + 255) / 256, 256, 0, st>>>(W2, C, tr->W2T);
+  if (check_launch(tr, "head_transpose_w2_kernel")) return 1;
+  if (launch_sgemm(tr, tr->dz2, C, tr->W2T, kHidden, tr->dH, kHidden, B, kHidden, C, nullptr, nullptr, nullptr, 0, st)) return 1;  // dH = dZ2 W2^T
+  head_bn_backward_kernel<<<col_grid, col_threads, 0, st>>>(tr->z1, tr->dH, tr->mask, B, gamma, beta, tr->stats, tr->dz1,
+                                                           tr->par(tr->G, 1), tr->par(tr->G, 2), tr->par(tr->G, 3));
+  if (check_launch(tr, "head_bn_backward_kernel")) return 1;
+  if (launch_sgemm(tr, tr->XbT, B, tr->dz1, kHidden, tr->G, kHidden, kHidden, kHidden, B, nullptr, nullptr, nullptr, 0, st)) return 1;  // dW1 = x^T dZ1
+  const double t = static_cast<double>(tr->step + 1);
+  const float alpha = static_cast<float>(tr->lr * std::sqrt(1.0 - std::pow(0.999, t)) / (1.0 - std::pow(0.9, t)));
+  head_adam_kernel<<<static_cast<unsigned>((tr->n_par + 255) / 256), 256, 0, st>>>(tr->P, tr->G, tr->M, tr->V, tr->n_par, alpha,
+                                                                                    static_cast<float>(1.0 - 0.9),
+                                                                                    static_cast<float>(1.0 - 0.999), 1e-7f);
+  if (check_launch(tr, "head_adam_kernel")) return 1;
+  tr->step++;
+  tr->last_b = B;
+  return 0;
+}
+
+extern "C" int gnm_head_train_read(gnm_head_train* tr, float* h_params, float* h_moving_mean, float* h_moving_variance,
+                                   long long* h_step, void* stream) {
+  if (!tr) return fail("gnm_head_train_read: null trainer");
+  GNM_CUDA(cudaSetDevice(tr->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (h_params) GNM_CUDA(cudaMemcpyAsync(h_params, tr->P, tr->n_par * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_moving_mean) GNM_CUDA(cudaMemcpyAsync(h_moving_mean, tr->mov_mean, kHidden * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_moving_variance) GNM_CUDA(cudaMemcpyAsync(h_moving_variance, tr->mov_var, kHidden * sizeof(float), cudaMemcpyDeviceToHost, st));
+  GNM_CUDA(cudaStreamSynchronize(st));
+  if (h_step) *h_step = tr->step;
+  return head_train_status(tr, "gnm_head_train_read");
+}
+
+extern "C" int gnm_head_train_fetch(gnm_head_train* tr, const char* which, void* h_dst, void* stream) {
+  if (!tr || !which || !h_dst) return fail("gnm_head_train_fetch: null argument");
+  if (!tr->last_b) return fail("gnm_head_train_fetch: no step has run on this trainer");
+  GNM_CUDA(cudaSetDevice(tr->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const std::string k(which);
+  const void* src = nullptr;
+  size_t bytes = 0;
+  if (k == "grad") { src = tr->G; bytes = tr->n_par * sizeof(float); }
+  else if (k == "mask") { src = tr->mask; bytes = static_cast<size_t>(tr->last_b) * kHidden; }
+  else if (k == "batch_stats") { src = tr->stats; bytes = 3 * kHidden * sizeof(float); }
+  else return fail("gnm_head_train_fetch: unknown buffer " + k);
+  GNM_CUDA(cudaMemcpyAsync(h_dst, src, bytes, cudaMemcpyDeviceToHost, st));
+  GNM_CUDA(cudaStreamSynchronize(st));
   return 0;
 }

@@ -91,15 +91,16 @@ def local_offsets(offsets: np.ndarray, start: int, end: int) -> np.ndarray:
 
 
 def gather_window_probs(local_probs, n_total: int, world_size: int, group=None):
-    """all_gather of contiguous shards of unequal length -> [n_total, 3] in global window order."""
+    """all_gather of contiguous shards of unequal length [W_local, width] -> [n_total, width] in global window order."""
     import torch
     import torch.distributed as dist
     if world_size == 1:
         return local_probs
     max_len = -(-n_total // world_size)
-    buf = torch.zeros((max_len, 3), dtype=local_probs.dtype, device=local_probs.device)
+    width = local_probs.shape[1]
+    buf = torch.zeros((max_len, width), dtype=local_probs.dtype, device=local_probs.device)
     buf[: local_probs.shape[0]] = local_probs
-    out = torch.empty((world_size * max_len, 3), dtype=local_probs.dtype, device=local_probs.device)
+    out = torch.empty((world_size * max_len, width), dtype=local_probs.dtype, device=local_probs.device)
     dist.all_gather_into_tensor(out, buf, group=group)
     parts = []
     for r in range(world_size):
@@ -133,7 +134,7 @@ def collect_window_probs(local_probs, n_total: int, info: "DistInfo", send=None,
 
 
 def allreduce_partials(partials, world_size: int, group=None):
-    """[n_contigs, 4] per-rank (sum p0, sum p1, sum p2, count) -> global; then mean = sums / count."""
+    """[n_contigs, C + 1] per-rank (sum p0, ..., sum p_{C-1}, count) -> global; then mean = sums / count."""
     import torch.distributed as dist
     if world_size > 1:
         dist.all_reduce(partials, op=dist.ReduceOp.SUM, group=group)
@@ -141,8 +142,9 @@ def allreduce_partials(partials, world_size: int, group=None):
 
 
 def finish_mean(partials):
-    cnt = partials[:, 3:4].clamp(min=1)
-    return partials[:, :3] / cnt
+    """[n_contigs, C + 1] (sums, count) -> [n_contigs, C] means."""
+    cnt = partials[:, -1:].clamp(min=1)
+    return partials[:, :-1] / cnt
 
 
 # ------------------------------------------------------------------------------------------------ per-contig embeddings

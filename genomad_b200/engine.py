@@ -51,6 +51,11 @@ class _Weights(C.Structure):
                 ("dense2_kernel", C.c_void_p), ("dense2_bias", C.c_void_p)]
 
 
+class _HeadW(C.Structure):
+    _fields_ = [("n_classes", C.c_int), ("dense1_kernel", C.c_void_p), ("dense1_bias", C.c_void_p), ("bn1", _BnW),
+                ("dense2_kernel", C.c_void_p), ("dense2_bias", C.c_void_p)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "gnm_last_error": (C.c_char_p, []),
@@ -105,6 +110,17 @@ EXPORTS = {
     "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]),
+    "gnm_head_create": (C.c_int, [C.c_void_p, C.POINTER(_HeadW), C.POINTER(C.c_void_p)]),
+    "gnm_head_destroy": (C.c_int, [C.c_void_p]),
+    "gnm_head_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_head_segment_mean": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_head_segment_sum": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_head_train_create": (C.c_int, [C.c_int, C.POINTER(_HeadW), C.c_int, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)]),
+    "gnm_head_train_destroy": (C.c_int, [C.c_void_p]),
+    "gnm_head_train_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                      C.c_void_p, C.c_void_p]),
+    "gnm_head_train_read": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong), C.c_void_p]),
+    "gnm_head_train_fetch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p]),
     "gnm_fasta_last_error": (C.c_char_p, []),
     "gnm_fasta_open": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     "gnm_fasta_open_gz": (C.c_int, [C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
@@ -817,3 +833,161 @@ class Classifier:
         out = t.empty(shapes[which], dtype=dtype, device=self._dev())
         _check(self.lib, self.lib.gnm_debug_fetch(self._h, which.encode(), n, out.data_ptr(), self._stream()))
         return out
+
+
+# ------------------------------------------------------------------------------------------------ classifier heads
+def head_param_count(C: int) -> int:
+    """Floats of a head's flat parameter buffer: W1, b1, gamma, beta, W2, b2 (gnm_head_train_read)."""
+    return EMBED * EMBED + 3 * EMBED + EMBED * C + C
+
+
+class Head:
+    """A C-class head (weights.HeadFile, or a dict with arrays / class_names) on a Classifier's device and workspace: encoder
+    embeddings -> class probabilities (gnm_head_forward), per-contig means and sums (gnm_head_segment_*).  Follows the
+    classifier's conv_impl; the shipped head at C = 3 gives bitwise the classifier's own probabilities."""
+
+    def __init__(self, clf: "Classifier", head):
+        self.clf, self.lib = clf, clf.lib
+        self.class_names = tuple(head.class_names)
+        self._a = {k: np.ascontiguousarray(head.arrays[k], dtype=np.float32) for k in _weights.HEAD_KEYS}
+        self.n_classes = int(self._a["d2b"].shape[0])
+        hw = _weights.head_c_struct(self._a, _HeadW, _BnW)
+        self._hd = C.c_void_p()
+        with clf._torch.cuda.device(clf.device):
+            rc = self.lib.gnm_head_create(clf._h, C.byref(hw), C.byref(self._hd))
+        if rc != 0:
+            msg = self.lib.gnm_last_error().decode(errors="replace")
+            self.close()
+            raise GnmError(msg)
+
+    def close(self):
+        if getattr(self, "_hd", None):
+            self.lib.gnm_head_destroy(self._hd)
+            self._hd = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def predict(self, embeddings, out=None):
+        """float32 cuda [n, 512] -> float32 [n, C] probabilities (into `out` when given)."""
+        t = self.clf._torch
+        x = embeddings.contiguous()
+        assert x.dtype == t.float32 and x.dim() == 2 and x.shape[1] == EMBED and x.is_cuda
+        if out is None:
+            out = t.empty((x.shape[0], self.n_classes), dtype=t.float32, device=x.device)
+        assert out.shape == (x.shape[0], self.n_classes) and out.is_contiguous() and out.dtype == t.float32
+        if x.shape[0]:
+            _check(self.lib, self.lib.gnm_head_forward(self.clf._h, self._hd, x.data_ptr(), x.shape[0], out.data_ptr(),
+                                                       self.clf._stream()))
+        return out
+
+    def _segment(self, fn, probs, offsets, width):
+        t = self.clf._torch
+        assert probs.dtype == t.float32 and offsets.dtype == t.int32 and probs.is_cuda and offsets.is_cuda
+        C_ = probs.shape[1]
+        n = offsets.numel() - 1
+        out = t.zeros((n, width(C_)), dtype=t.float32, device=probs.device)
+        if n and probs.numel():
+            _check(self.lib, fn(self.clf._h, probs.contiguous().data_ptr(), C_, offsets.contiguous().data_ptr(), n,
+                                out.data_ptr(), self.clf._stream()))
+        return out
+
+    def segment_mean(self, probs, offsets):
+        """probs float32 cuda [W, C], offsets int32 cuda [n + 1] -> float32 [n, C]: fp32 running mean in window order."""
+        return self._segment(self.lib.gnm_head_segment_mean, probs, offsets, lambda c: c)
+
+    def segment_sum(self, probs, offsets):
+        """-> float32 [n, C + 1] = (sums, window count): the cross-GPU partial."""
+        return self._segment(self.lib.gnm_head_segment_sum, probs, offsets, lambda c: c + 1)
+
+
+class HeadTrainer:
+    """Training of a C-class head on cached embeddings (gnm_head_train_*; semantics in include/gnm.h).  `init` maps the
+    short names of weights.HEAD_KEYS to the initial arrays (weights.initial_head)."""
+
+    def __init__(self, init: Dict[str, np.ndarray], device: int = 0, max_batch: int = 1024, seed: int = 0,
+                 learning_rate: float = 1e-3):
+        import torch
+        self._torch = torch
+        self.lib = load_library()
+        self.device, self.max_batch = int(device), int(max_batch)
+        self._a = {k: np.ascontiguousarray(init[k], dtype=np.float32) for k in _weights.HEAD_KEYS}
+        self.n_classes = int(self._a["d2b"].shape[0])
+        hw = _weights.head_c_struct(self._a, _HeadW, _BnW)
+        self._tr = C.c_void_p()
+        with torch.cuda.device(self.device):
+            rc = self.lib.gnm_head_train_create(self.device, C.byref(hw), self.max_batch, int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                                float(learning_rate), C.byref(self._tr))
+        if rc != 0:
+            msg = self.lib.gnm_last_error().decode(errors="replace")
+            self.close()
+            raise GnmError(msg)
+
+    def close(self):
+        if getattr(self, "_tr", None):
+            self.lib.gnm_head_train_destroy(self._tr)
+            self._tr = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _stream(self) -> int:
+        return self._torch.cuda.current_stream(self.device).cuda_stream
+
+    def step(self, X, idx, labels, class_weights, loss=None):
+        """One step on rows idx (int64 cuda [B]) of X (float32 cuda [N, 512]); labels int32 cuda [N]; class_weights float32
+        cuda [C].  Returns the batch loss, float32 cuda [1] (`loss` when given).  Asynchronous: an index outside [0, N) or a
+        label outside [0, C) is caught on the device, and the next step or weights() raises GnmError."""
+        t = self._torch
+        assert X.dtype == t.float32 and X.dim() == 2 and X.shape[1] == EMBED and X.is_contiguous()
+        assert idx.dtype == t.int64 and labels.dtype == t.int32 and class_weights.dtype == t.float32
+        assert class_weights.numel() == self.n_classes and labels.numel() == X.shape[0]
+        if loss is None:
+            loss = t.empty(1, dtype=t.float32, device=X.device)
+        with t.cuda.device(self.device):
+            _check(self.lib, self.lib.gnm_head_train_step(self._tr, X.data_ptr(), X.shape[0], idx.contiguous().data_ptr(),
+                                                          labels.contiguous().data_ptr(), class_weights.contiguous().data_ptr(),
+                                                          idx.numel(), loss.data_ptr(), self._stream()))
+        self._last_b = idx.numel()
+        return loss
+
+    def weights(self) -> Dict[str, np.ndarray]:
+        """The current parameters and moving statistics as arrays for weights.save_head (waits for the device)."""
+        C_ = self.n_classes
+        flat = np.empty(head_param_count(C_), np.float32)
+        mm, mv = np.empty(EMBED, np.float32), np.empty(EMBED, np.float32)
+        step = C.c_longlong()
+        with self._torch.cuda.device(self.device):
+            _check(self.lib, self.lib.gnm_head_train_read(self._tr, _ptr(flat), _ptr(mm), _ptr(mv), C.byref(step),
+                                                          self._stream()))
+        self.steps = step.value
+        return {**_unflatten_head(flat, C_), "bn1m": mm, "bn1v": mv}
+
+    def fetch(self, which: str):
+        """Test hook: the last step's "grad" (dict of gradients by short name), "mask" (uint8 [B, 512]) or "batch_stats"
+        (float32 [3, 512]: mu, 1 / sqrt(var + 1e-3), var)."""
+        if which == "grad":
+            out = np.empty(head_param_count(self.n_classes), np.float32)
+        elif which == "mask":
+            out = np.empty((getattr(self, "_last_b", 0), EMBED), np.uint8)
+        else:
+            out = np.empty((3, EMBED), np.float32)
+        with self._torch.cuda.device(self.device):
+            _check(self.lib, self.lib.gnm_head_train_fetch(self._tr, which.encode(), _ptr(out), self._stream()))
+        return _unflatten_head(out, self.n_classes) if which == "grad" else out
+
+
+def _unflatten_head(flat: np.ndarray, C_: int) -> Dict[str, np.ndarray]:
+    E = EMBED
+    parts, o = {}, 0
+    for k, shape in (("d1w", (E, E)), ("d1b", (E,)), ("bn1g", (E,)), ("bn1b", (E,)), ("d2w", (E, C_)), ("d2b", (C_,))):
+        n = int(np.prod(shape))
+        parts[k] = flat[o: o + n].reshape(shape).copy()
+        o += n
+    return parts

@@ -91,7 +91,8 @@ def _device(clf):
 
 
 def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather",
-                     embeddings: bool = False, window_probs: bool = False, attributions: "dict | None" = None):
+                     embeddings: bool = False, window_probs: bool = False, attributions: "dict | None" = None,
+                     head: "dict | None" = None, window_embeddings=None):
     """
     Indexed FASTA -> float32 [n_contigs, 3] per-contig mean (identical on all ranks).
 
@@ -117,6 +118,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).  With attributions["steps"] >= 1 the
     calls are the integrated-gradients ones (Classifier.integrated_gradients_ascii, same probabilities), and the rows of
     log p_target at the window and at the baseline travel to rank 0 the same way, as attributions["logp"] (float32 [n_windows, 2]).
+
+    With `head` ({"head": engine.Head}), every chunk takes the embedding route and the head scores each window's embedding on
+    the device into a buffer of this rank's shard; they are reduced per contig by the routes of the class scores (gather or
+    allreduce, any width) and stored as head["preds"] (float32 [n_contigs, C], identical on all ranks).  With
+    `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -133,10 +139,23 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
 
     def run(win, m, row):                                    # one chunk: windows win[:m] are rows [row, row + m) of the shard
         clf.classify_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12)
+    scorer = head["head"] if head is not None else None
+    if scorer is not None:
+        d_head = torch.empty((end - start, scorer.n_classes), dtype=torch.float32, device=dev)
     if embeddings:
         shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
+    if embeddings or scorer is not None or window_embeddings is not None:
         d_emb = torch.empty((min(chunk, max(1, end - start)), 512), dtype=torch.float32, device=dev)
-        if attributions is None:
+        if attributions is None and (scorer is not None or window_embeddings is not None):
+            def run(win, m, row):                            # the worker owns d_emb: one chunk at a time
+                e = window_embeddings[row: row + m] if window_embeddings is not None else d_emb[:m]
+                clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, e.data_ptr())
+                if scorer is not None:
+                    scorer.predict(e, out=d_head[row: row + m])
+                if embeddings:
+                    shard.add(e)
+                sync()
+        elif attributions is None:
             def run(win, m, row):                            # the worker owns d_emb: one chunk at a time
                 clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, d_emb.data_ptr())
                 shard.add(d_emb[:m])
@@ -157,8 +176,12 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 probs, attr = clf.attribute_ascii(d_win, attributions["target"])
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
-            if embeddings:
-                shard.add(clf.embed_ascii(d_win)[1])
+            if embeddings or scorer is not None:
+                e = clf.embed_ascii(d_win)[1]
+                if embeddings:
+                    shard.add(e)
+                if scorer is not None:
+                    scorer.predict(e, out=d_head[row: row + m])
             sync()
     futures = []
     with ThreadPoolExecutor(max_workers=1) as gpu:
@@ -180,6 +203,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
             lo, means = shard.finish(info)
             emb = gdist.gather_contig_means(lo, means, len(offsets) - 1, info)
             out.append(emb.cpu().numpy() if emb is not None else None)
+        if scorer is not None:
+            head["preds"] = _reduce_rows(scorer.segment_mean, scorer.segment_sum, d_head, offsets, start, end, n, info,
+                                         contig_reduce)
     if window_probs:
         full = gdist.collect_window_probs(local_t, n, info)
         out.append(full.cpu().numpy() if full is not None else None)
@@ -189,20 +215,28 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
         if ig_steps:
             full = gdist.collect_window_probs(d_logp, n, info)
             attributions["logp"] = full.cpu().numpy() if full is not None else None
+    if not out:
+        return None
     return out[0] if len(out) == 1 else tuple(out)
 
 
 def _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce) -> np.ndarray:
     """This rank's per-window probabilities (device) -> float32 [n_contigs, 3] per-contig means, identical on all ranks."""
+    return _reduce_rows(lambda p, o: clf.segment_mean(p, o), lambda p, o: clf.segment_sum(p, o), local_t, offsets, start, end,
+                        n, info, contig_reduce)
+
+
+def _reduce_rows(segment_mean, segment_sum, local_t, offsets, start, end, n, info, contig_reduce) -> np.ndarray:
+    """_reduce_probs for rows of any width C, given the segment mean ([W, C] -> [k, C]) and sum ([W, C] -> [k, C + 1])."""
     import torch
     dev = local_t.device
     if contig_reduce == "allreduce" and info.world_size > 1:
         loc_off = torch.from_numpy(gdist.local_offsets(offsets, start, end)).to(dev)
-        partials = gdist.allreduce_partials(clf.segment_sum(local_t, loc_off), info.world_size)
+        partials = gdist.allreduce_partials(segment_sum(local_t, loc_off), info.world_size)
         return gdist.finish_mean(partials).cpu().numpy()
     probs = gdist.gather_window_probs(local_t, n, info.world_size)
     off_t = torch.from_numpy(offsets.astype(np.int32)).to(dev)
-    return clf.segment_mean(probs, off_t).cpu().numpy()
+    return segment_mean(probs, off_t).cpu().numpy()
 
 
 def _classify_windows(clf, windows: np.ndarray, offsets: np.ndarray, info: gdist.DistInfo,
@@ -277,12 +311,14 @@ def _window_scores_current(npz_path: Path, tsv_path: Path, stride: int) -> bool:
 
 
 def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, embeddings: bool,
-                         attributions=None):
+                         attributions=None, head=None):
     """Per-contig scores (+ embeddings) and the per-window scores at `stride`: (preds, emb or None, offsets, starts, lengths,
     probs); the window arrays are None off rank 0.  At stride 6000 without --single-window the profile windows are the
     contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list."""
     emb = None
     ak = {"attributions": attributions} if attributions is not None else {}      # option off: the call of before
+    if head is not None:
+        ak["head"] = head
     if stride == sequence.WINDOW and not single_window:
         res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True, **ak)
         preds, probs = res[0], res[-1]
@@ -392,6 +428,42 @@ def _attributions_current(path: Path, target: str, steps: int = 0, baseline: str
             return method == IG_METHOD and int(z["steps"]) == steps and str(z["baseline"]) == baseline
     except Exception:
         return False
+
+
+def _write_head(npz_path: Path, tsv_path: Path, names_key: str, names, preds, class_names, head_sha: str) -> None:
+    """<prefix>_nn_classification_head.{npz,tsv}: the head's per-sequence scores, float32 [n, C], one column per class."""
+    preds = np.asarray(preds, dtype=np.float32).reshape(len(names), len(class_names))
+    np.savez_compressed(npz_path, **{names_key: names, "predictions": preds, "class_names": np.array(class_names),
+                                     "head_sha256": np.str_(head_sha)})
+    with open(tsv_path, "w") as fout:
+        fout.write("seq_name\t" + "\t".join(f"{c}_score" for c in class_names) + "\n")
+        for name, row in zip(names, preds):
+            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in row) + "\n")
+
+
+def _head_current(npz_path: Path, tsv_path: Path, head_sha: str) -> bool:
+    """Both head files exist and were written for the head file with this sha256."""
+    if not (npz_path.exists() and tsv_path.exists()):
+        return False
+    try:
+        with np.load(npz_path) as z:
+            return str(z["head_sha256"]) == head_sha
+    except Exception:
+        return False
+
+
+def _load_head_file(path):
+    """(weights.HeadFile, sha256 of the file) of a --head file, checked against the shipped encoder (ValueError otherwise)."""
+    import hashlib
+    from . import weights as _w
+    head = _w.load_head(path, _w.load_weights())
+    return head, hashlib.sha256(Path(path).read_bytes()).hexdigest()
+
+
+def _make_head(clf, head_file):
+    """Factory (patched in CPU tests): the head on the classifier's device."""
+    from .engine import Head
+    return Head(clf, head_file)
 
 
 def tfrecords_enabled() -> bool:
@@ -525,7 +597,7 @@ _attribution_steps, _attribution_baseline = attribution_steps, attribution_basel
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
          write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
-         attribution_steps=None, attribution_baseline=None, both_strands=None):
+         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -585,6 +657,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if strands:
         files += [outputs.nn_classification_strands_output, outputs.nn_classification_strands_npz_output]
         descr += ["classification of both strands: tabular format", "classification of both strands: binary format"]
+    if head is not None:
+        files += [outputs.nn_classification_head_output, outputs.nn_classification_head_npz_output]
+        descr += ["classification by the --head classifier: tabular format",
+                  "classification by the --head classifier: binary format"]
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -603,11 +679,22 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             files += [outputs.provirus_nn_classification_strands_output, outputs.provirus_nn_classification_strands_npz_output]
             descr += ["provirus classification of both strands: tabular format",
                       "provirus classification of both strands: binary format"]
+        if head is not None:
+            files += [outputs.provirus_nn_classification_head_output, outputs.provirus_nn_classification_head_npz_output]
+            descr += ["provirus classification by the --head classifier: tabular format",
+                      "provirus classification by the --head classifier: binary format"]
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
     for note in ig_notes:
         console.log(f"Warning: {note}")
+    head_file = head_sha = None
+    if head is not None:             # a head for another encoder (or a malformed file) is refused before any work
+        try:
+            head_file, head_sha = _load_head_file(head)
+        except (OSError, ValueError, KeyError) as e:
+            console.error(f"{head} is not a usable head file: {e}")
+            sys.exit(1)
     ig_clf = None
     if ig_steps:                     # the steps must fit this device's attribution context: fail before any work
         ig_clf = _make_classifier(batch_size, info.local_rank)
@@ -625,14 +712,16 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
              outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
              outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output,
-             outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output)]
+             outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output,
+             outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
                      outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
                      outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
                      outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output,
-                     outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output))
+                     outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output,
+                     outputs.provirus_nn_classification_head_npz_output, outputs.provirus_nn_classification_head_output))
 
     plan = None
     info_writer = None
@@ -657,7 +746,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                  bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
                       and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
                       and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))
-                      and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))))
+                      and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))
+                      and (head_file is None or _head_current(j[16], j[17], head_sha))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -683,6 +773,14 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             clf_future = clf_pool.submit(_make_classifier, batch_size, info.local_rank)
         return clf_future.result()
 
+    scorer = None
+
+    def head_scorer():
+        nonlocal scorer
+        if scorer is None:
+            scorer = _make_head(classifier(), head_file)
+        return scorer
+
     if not all(cls_skip for _, cls_skip in plan) and ig_clf is None:
         clf_future = clf_pool.submit(_make_classifier, batch_size, info.local_rank)      # start now, overlap with indexing
 
@@ -701,7 +799,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
-         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path), (enc_skip, cls_skip), (parsed, index) \
+         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path), \
+            (enc_skip, cls_skip), (parsed, index) \
             in zip(jobs, plan, staged):
         names = preds = emb = None
         rev_preds = rev_emb = None      # --both-strands: the reverse strand's scores and embeddings
@@ -709,6 +808,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if attr_target:
             attr = {"target": attr_target, **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
         win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
+        hd = None                       # --head: the chunk loop also scores every window with the head (forward strand)
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
         if cls_skip:
@@ -727,6 +827,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                         info_writer.join()                    # the reference has written the JSON by this point
                     sys.exit(1)
                 names, preds = index.names, np.zeros((len(index.names), 3), np.float32)
+                if head_file is not None:
+                    hd = {"preds": np.zeros((len(index.names), len(head_file.class_names)), np.float32)}
                 emb = np.zeros((len(index.names), 512), np.float32)
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
@@ -736,6 +838,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             else:
                 t_c = _time.perf_counter()
                 ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
+                if head_file is not None:
+                    hd = {"head": head_scorer()}
+                    ak["head"] = hd
                 if write_window_scores:
                     preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
                                                             contig_reduce, write_embeddings, **ak)
@@ -763,6 +868,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     _write_strands(strands_npz_path, strands_tsv_path, names_key, names, preds.astype(np.float32), rev_preds)
                 console.log(f"{label} classification of both strands written to {strands_tsv_path.name} and "
                             f"{strands_npz_path.name}.")
+            if hd is not None:
+                if is_main:
+                    _write_head(head_npz_path, head_tsv_path, names_key, names, hd["preds"], head_file.class_names, head_sha)
+                console.log(f"{label} classification by the head written to {head_tsv_path.name} and {head_npz_path.name}.")
             if write_window_scores:
                 if is_main:
                     _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,

@@ -15,8 +15,10 @@ Layer order in the file (root attr ``layer_names`` / group ``model`` attr ``weig
 from __future__ import annotations
 
 import ctypes as C
+import hashlib
+import re
 from pathlib import Path
-from typing import Dict
+from typing import Dict, NamedTuple, Tuple
 
 import numpy as np
 
@@ -112,3 +114,133 @@ def to_c_struct(w: Dict[str, np.ndarray], Weights, IglooW, BnW):
     cw.bn1 = BnW(ptr("bn1g"), ptr("bn1b"), ptr("bn1m"), ptr("bn1v"))
     cw.dense2_kernel, cw.dense2_bias = ptr("d2w"), ptr("d2b")
     return cw
+
+
+# ------------------------------------------------------------------------------------------------ classifier heads
+# A head file (.npz) holds the layers the reference trains on the frozen encoder (create_classifier, model.py:34-45) under the
+# shipped file's names and layouts, with C classes instead of 3, plus `class_names` (C strings) and `encoder_sha256` (the
+# encoder it was trained on).  INTEGRATION.md, "Head files".
+HEAD_KEYS = ("d1w", "d1b", "bn1g", "bn1b", "bn1m", "bn1v", "d2w", "d2b")
+HEAD_MIN_CLASSES, HEAD_MAX_CLASSES = 2, 32
+SHIPPED_CLASSES = ("chromosome", "plasmid", "virus")
+_CLASS_NAME = re.compile(r"[A-Za-z0-9_.-]+")
+
+
+class HeadFile(NamedTuple):
+    arrays: Dict[str, np.ndarray]   # short names of HEAD_KEYS -> float32 arrays; d2w [512, C], d2b [C]
+    class_names: Tuple[str, ...]
+    encoder_sha256: str
+
+
+def encoder_sha256(weights: Dict[str, np.ndarray]) -> str:
+    """sha256 over the encoder arrays (every KEYS entry that is not a head layer), in KEYS order, as raw little-endian bytes."""
+    h = hashlib.sha256()
+    for short in KEYS:
+        if short in HEAD_KEYS:
+            continue
+        a = np.asarray(weights[short])
+        h.update(np.ascontiguousarray(a, dtype=a.dtype.newbyteorder("<")).tobytes())
+    return h.hexdigest()
+
+
+def check_class_names(names) -> Tuple[str, ...]:
+    """C unique names matching [A-Za-z0-9_.-]+ with 2 <= C <= 32 (ValueError otherwise)."""
+    names = tuple(str(x) for x in names)
+    if not HEAD_MIN_CLASSES <= len(names) <= HEAD_MAX_CLASSES:
+        raise ValueError(f"class_names: {len(names)} classes, a head has {HEAD_MIN_CLASSES} to {HEAD_MAX_CLASSES}")
+    bad = [x for x in names if not _CLASS_NAME.fullmatch(x)]
+    if bad:
+        raise ValueError(f"class_names: {bad[0]!r} does not match [A-Za-z0-9_.-]+")
+    dup = sorted({x for x in names if names.count(x) > 1})
+    if dup:
+        raise ValueError(f"class_names: {dup[0]!r} appears more than once")
+    return names
+
+
+def _check_head_arrays(arrays, C: int) -> Dict[str, np.ndarray]:
+    out = {}
+    for short in HEAD_KEYS:
+        path, shape = KEYS[short]
+        if short == "d2w":
+            shape = (512, C)
+        elif short == "d2b":
+            shape = (C,)
+        if short not in arrays:
+            raise ValueError(f"{path} missing")
+        a = np.asarray(arrays[short])
+        if a.dtype != np.float32:
+            raise ValueError(f"{path}: dtype {a.dtype}, expected float32")
+        if tuple(a.shape) != shape:
+            raise ValueError(f"{path}: shape {a.shape}, expected {shape}")
+        if not np.isfinite(a).all():
+            raise ValueError(f"{path}: not all finite")
+        out[short] = np.ascontiguousarray(a)
+    return out
+
+
+def load_head(path, weights: Dict[str, np.ndarray]) -> HeadFile:
+    """Read and validate a head file against the encoder `weights` (load_weights()); ValueError naming the offending key."""
+    with np.load(Path(path), allow_pickle=False) as z:
+        files = set(z.files)
+        for key in ("class_names", "encoder_sha256"):
+            if key not in files:
+                raise ValueError(f"{key} missing")
+        names = z["class_names"]
+        if names.ndim != 1 or names.dtype.kind != "U":
+            raise ValueError(f"class_names: expected a 1-D array of strings, not {names.dtype} {names.shape}")
+        names = check_class_names(names.tolist())
+        sha = z["encoder_sha256"]
+        if sha.dtype.kind != "U" or sha.ndim != 0:
+            raise ValueError("encoder_sha256: expected one string")
+        sha = str(sha)
+        arrays = _check_head_arrays({s: z[KEYS[s][0]] for s in HEAD_KEYS if KEYS[s][0] in files}, len(names))
+    if sha != encoder_sha256(weights):
+        raise ValueError("encoder_sha256: the head was trained on another encoder than the one loaded")
+    return HeadFile(arrays, names, sha)
+
+
+def save_head(path, arrays: Dict[str, np.ndarray], class_names, weights: Dict[str, np.ndarray]) -> None:
+    """Write a head file.  The zip members carry a fixed timestamp, so equal heads give byte-identical files."""
+    import zipfile
+    names = check_class_names(class_names)
+    arrays = _check_head_arrays(arrays, len(names))
+    members = [(KEYS[s][0], arrays[s]) for s in HEAD_KEYS]
+    members += [("class_names", np.array(names, dtype=f"<U{max(len(x) for x in names)}")),
+                ("encoder_sha256", np.array(encoder_sha256(weights)))]
+    with zipfile.ZipFile(Path(path), "w", compression=zipfile.ZIP_STORED) as zf:
+        for name, a in members:
+            with zf.open(zipfile.ZipInfo(name + ".npy", date_time=(1980, 1, 1, 0, 0, 0)), "w", force_zip64=True) as f:
+                np.lib.format.write_array(f, np.asarray(a), allow_pickle=False)
+
+
+def shipped_head(weights: Dict[str, np.ndarray]) -> HeadFile:
+    """The shipped classifier's own head (chromosome, plasmid, virus) as a head: the reference point of the head path."""
+    return HeadFile({s: np.ascontiguousarray(weights[s], dtype=np.float32) for s in HEAD_KEYS}, SHIPPED_CLASSES,
+                    encoder_sha256(weights))
+
+
+def initial_head(C: int, seed: int) -> Dict[str, np.ndarray]:
+    """Keras defaults for a new head, drawn with numpy.random.default_rng(seed): Glorot-uniform dense_1 then dense_2 kernels,
+    zero biases, gamma 1, beta 0, moving mean 0, moving variance 1."""
+    rng = np.random.default_rng(seed)
+
+    def glorot(fan_in, fan_out):
+        lim = np.sqrt(6.0 / (fan_in + fan_out))
+        return rng.uniform(-lim, lim, (fan_in, fan_out)).astype(np.float32)
+    d1w = glorot(512, 512)
+    d2w = glorot(512, C)
+    z, o = np.zeros(512, np.float32), np.ones(512, np.float32)
+    return {"d1w": d1w, "d1b": z.copy(), "bn1g": o.copy(), "bn1b": z.copy(), "bn1m": z.copy(), "bn1v": o.copy(),
+            "d2w": d2w, "d2b": np.zeros(C, np.float32)}
+
+
+def head_c_struct(arrays: Dict[str, np.ndarray], HeadW, BnW):
+    """Fill the ctypes mirror of ``gnm_head_weights`` (include/gnm.h) with host pointers into ``arrays``."""
+    def ptr(k):
+        return arrays[k].ctypes.data_as(C.c_void_p)
+    hw = HeadW()
+    hw.n_classes = int(arrays["d2b"].shape[0])
+    hw.dense1_kernel, hw.dense1_bias = ptr("d1w"), ptr("d1b")
+    hw.bn1 = BnW(ptr("bn1g"), ptr("bn1b"), ptr("bn1m"), ptr("bn1v"))
+    hw.dense2_kernel, hw.dense2_bias = ptr("d2w"), ptr("d2b")
+    return hw

@@ -550,6 +550,81 @@ size_t gnm_cluster_block_workspace_bytes(int64_t n_block);
 int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity, int32_t* d_new_reps,
                       int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream);
 
+/*
+ * Classifier heads: the layers the reference trains on the frozen encoder (create_classifier, model.py:34-45), with C classes
+ * instead of 3.  DESIGN.md, "Classifier heads".  Host pointers, Keras layouts; 2 <= n_classes <= 32.
+ */
+typedef struct gnm_head_weights {
+  int n_classes;               /* C */
+  const float* dense1_kernel;  /* [512][512] */
+  const float* dense1_bias;    /* [512] */
+  gnm_bn_weights bn1;          /* batch_normalization_1 (epsilon 1e-3) */
+  const float* dense2_kernel;  /* [512][C] */
+  const float* dense2_bias;    /* [C] */
+} gnm_head_weights;
+typedef struct gnm_head gnm_head;
+typedef struct gnm_head_train gnm_head_train;
+
+/*
+ * Upload a head for inference on handle h's device.  BN is folded into scale and shift and dense_1 split into TF32 halves with
+ * the host code gnm_create uses for the shipped head.  Synchronous.
+ */
+int gnm_head_create(gnm_handle* h, const gnm_head_weights* w, gnm_head** out);
+int gnm_head_destroy(gnm_head* head);
+
+/*
+ * Encoder embeddings DEVICE float [n][512] (gnm_embed_*) -> probabilities DEVICE float [n][C].  Steps of max_batch rows on the
+ * handle's head workspace, in `stream` order (so not concurrently with other calls on h), following h's conv_impl: 0 splits
+ * the rows into TF32 halves (the bits the forward pass writes for its dense_1) and runs the forward pass's 3 x TF32 dense_1
+ * GEMM + BN + ReLU; 1 runs the FFMA dense_1 kernel.  Both end in a C-class softmax with dense3's k order, shuffle tree and
+ * max / exp / sum / multiply sequence, so the shipped head at C = 3 gives bitwise the probabilities of gnm_forward_*.
+ */
+int gnm_head_forward(gnm_handle* h, const gnm_head* head, const float* d_embed, int n, float* d_probs, void* stream);
+
+/*
+ * gnm_segment_mean / gnm_segment_sum for rows of C columns (1 <= C <= 32): float [n_contigs][C] means, or [n_contigs][C + 1]
+ * = (sums, count).  One fp32 running sum per column in window order, so C = 3 gives the bits of gnm_segment_*.
+ */
+int gnm_head_segment_mean(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs, float* d_mean,
+                          void* stream);
+int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs, float* d_sum,
+                         void* stream);
+
+/*
+ * Head training on cached embeddings (no encoder gradients).  Semantics, Keras 3 defaults with the reference's stack:
+ *   training forward  z1 = x W1 + b1;  mu, var = batch mean and biased batch variance of z1 (per column);
+ *                     y = gamma (z1 - mu) / sqrt(var + 1e-3) + beta;  h = relu(y) * keep / 0.8;  logits = h W2 + b2
+ *   dropout           keep(seed, step, row, col) = mix32(mix32(mix32(K(seed) ^ step) + row) + col) >= ceil(0.2 * 2^32),
+ *                     mix32 = lowbias32, K(seed) = (seed * 0x9E3779B1 + 0x7F4A7C15) mod 2^32 (genomad_b200/synth.py),
+ *                     step = the 0-based global step, row = the position in the batch; arithmetic mod 2^32
+ *   loss              sum_i w[y_i] * (-log softmax(logits_i)[y_i]) / B  (log-softmax from the logits, max-shifted)
+ *   Adam              t = step + 1; m += (g - m)(1 - 0.9); v += (g^2 - v)(1 - 0.999);
+ *                     p -= (m * lr sqrt(1 - 0.999^t) / (1 - 0.9^t)) / (sqrt(v) + 1e-7), over W1, b1, gamma, beta, W2, b2; no decay
+ *   moving stats      mean = 0.99 mean + 0.01 mu;  var = 0.99 var + 0.01 var_batch (biased)
+ * Every reduction (over the batch or over k) runs in a fixed order without atomics: a run is bitwise reproducible for a seed
+ * on one device model.
+ *
+ * gnm_head_train_create: `init` holds the initial parameters and moving statistics (the caller draws them); seed keys the
+ *   dropout; max_batch in [1, 65536] bounds B.  Adam moments start at zero.  Synchronous.
+ * gnm_head_train_step: one step on the batch rows d_idx (DEVICE int64 [B], indices into d_X) of d_X (DEVICE float
+ *   [n_rows][512], the embeddings of the whole training set); d_labels DEVICE int32 [n_rows] (label of each row of d_X, in
+ *   [0, C)); d_class_weights DEVICE float [C]; 1 <= B <= max_batch.  Writes the batch loss to d_loss (DEVICE float [1]).
+ *   Asynchronous on `stream`.  An index outside [0, n_rows) or a label outside [0, C) is not read: the step flags it (and uses
+ *   row 0 / class 0), and the next gnm_head_train_step or gnm_head_train_read fails naming which; the trainer is then spent.
+ * gnm_head_train_read: waits for `stream` and copies the parameters to HOST buffers (any may be NULL): h_params float
+ *   [512*512 + 3*512 + 512*C + C] flat = W1, b1, gamma, beta, W2, b2; moving mean and variance [512]; the step count.
+ * gnm_head_train_fetch (tests): HOST copy of the last step's "grad" (float, flat like h_params), "mask" (uint8 [B][512], 1 =
+ *   kept) or "batch_stats" (float [3][512] = mu, 1 / sqrt(var + 1e-3), var).  Waits for `stream`.
+ */
+int gnm_head_train_create(int device, const gnm_head_weights* init, int max_batch, uint64_t seed, float learning_rate,
+                          gnm_head_train** out);
+int gnm_head_train_destroy(gnm_head_train* tr);
+int gnm_head_train_step(gnm_head_train* tr, const float* d_X, int64_t n_rows, const int64_t* d_idx, const int32_t* d_labels,
+                        const float* d_class_weights, int B, float* d_loss, void* stream);
+int gnm_head_train_read(gnm_head_train* tr, float* h_params, float* h_moving_mean, float* h_moving_variance, long long* h_step,
+                        void* stream);
+int gnm_head_train_fetch(gnm_head_train* tr, const char* which, void* h_dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

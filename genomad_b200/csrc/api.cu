@@ -99,7 +99,11 @@ struct gnm_handle {
   int32_t* cta_split = nullptr;                      // [num_sms + 1] device: unit range per CTA of the current launch
   std::vector<int32_t> split_host[2];                // host copy of the last split per IGLOO kernel (source of the async upload)
   int split_groups[2] = {-1, -1}, split_grid[2] = {-1, -1};
-  float wv_cost_base = 1.f, wv_cost_group = 0.1f;    // unit cost model of wv_split: base + per position group of the busiest warp
+  // Unit cost model of wv_split: base + per position group of the busiest gather warp.  Fitted by least squares to the per-CTA
+  // cycle counters of a batch-1024 launch (tools/ab_stages.py --wvg-fit: CTA cycles = a x units + b x summed busiest-warp groups,
+  // 132 CTAs, 8 launches averaged; wv_cost_group = b / a).  H100, shipped patch sets: a = 7,912 and b = 254 cycles, so 0.032.
+  // With the folded weights read per unit the same fit gave 0.164; keeping them in registers made a group ~4x cheaper.
+  float wv_cost_base = 1.f, wv_cost_group = 0.032f;
   int mb_pad = 0;                                    // max_batch rounded up to a multiple of 8 (window groups of wv_gather_kernel)
   CUtensorMap tm_band[2];                            // activations, box = 128 B x 8 windows x 24 positions (make_band_map)
   float* logits = nullptr; float* logits_part = nullptr; float* h0 = nullptr; float* h1 = nullptr; float* h2 = nullptr;

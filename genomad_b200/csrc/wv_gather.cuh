@@ -10,7 +10,8 @@
 // (192 activation rows; 250 bands x ceil(n/8) window groups).  Units are numbered band-major and every CTA owns a contiguous
 // range of them, so a CTA stays on one band (at most three) for the whole launch while the grid as a whole sweeps the windows
 // front to back.  That is what makes the gather cheap here: the ~34 (patch, slot) entries whose position falls into the CTA's
-// band use the same 17 KB of folded weights for every unit (L1 / L2 resident), instead of every window re-reading all 4.3 MB.
+// band use the same 17 KB of folded weights for every unit (read once per band into the gather warps' registers), instead of
+// every window re-reading all 4.3 MB.
 //
 // Slab.  The four regions of a unit (hi16 / lo16 plane x channel half) are ONE 3-D TMA box each, from a tensor map that lists
 // the window axis BEFORE the position axis (api.cu make_band_map): the box {128 B, 8 windows, 24 positions} lands as
@@ -29,10 +30,13 @@
 //   * patch gather: warp-level mma.sync.m16n8k16 on the slab rows.  Entries are grouped by position (<= 4 per group;
 //     8,400 entries hit ~4,500 positions).  For one group and one channel half, A[16 x 64] = the position's 8 windows' hi16 rows
 //     (rows 0-7) and lo16 rows (rows 8-15), read by 4 ldmatrix.x4; B[64 x 8] = the fp16 hi / lo halves of the group's folded
-//     weights (host-packed in fragment order, scaled by a power of two so the lo halves stay normal; L1 / L2 resident); the sum of
-//     the four D entries of (window, entry) is (hi + lo) . (w_hi + w_lo) with fp32 accumulation -- the fp32-equivalent dot product.
-//     7 gather warps take <= 4 groups each; pass 0 (channels 0-63) waits in registers, pass 1 adds channels 64-127 and writes
-//     part_t[slot][window] (8 lanes = 32 contiguous bytes).  A region goes back to the producer when the 8 MMA warps and all 7
+//     weights (host-packed in fragment order, scaled by a power of two so the lo halves stay normal); the sum of the four D
+//     entries of (window, entry) is (hi + lo) . (w_hi + w_lo) with fp32 accumulation -- the fp32-equivalent dot product.
+//     7 gather warps take <= 4 groups each.  On a band change a warp loads the B fragments of its groups for both channel
+//     halves into 64 registers, where they stay for all of the band's units (weights stationary), so a unit's gather is only
+//     ldmatrix + mma.sync: two groups' ldmatrix, then their mma.  Pass 0 (channels 0-63) waits in registers, pass 1 adds
+//     channels 64-127 and writes part_t[slot][window] (8 lanes = 32 contiguous bytes).  Bands with more than 28 groups take a
+//     generic path that reads the weights per unit.  A region goes back to the producer when the 8 MMA warps and all 7
 //     gather warps have arrived (count 15).  patch_finish_t_kernel adds a patch's four slots in fixed order k = 0..3 plus the bias.
 //
 // Warp roles (512 threads, 1 CTA per SM, 128 registers per thread):  warps 0..7: two MMA + epilogue warpgroups |
@@ -236,40 +240,43 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
   } else {
     // ===================================================================== patch gather
     const int gw = warp - kWgMmaWarps;                         // 0..kWgWarps - 1
-    const float gscale = p.gather_unscale;
     // Gather lane roles.  ldmatrix: lanes 8i..8i+7 address matrix i = (plane i & 1: 0 hi16 / 1 lo16, 16-byte chunk i >> 1 of the
     // k-step), row lane & 7 = window.  The A fragment then holds rows 0..7 = the 8 windows' hi16 halves and rows 8..15 = their
     // lo16 halves; mma: gid = lane >> 2 = window (A / D row) = entry (B column), tig = lane & 3.
     const int lm_plane = (lane >> 3) & 1, lm_chunk = lane >> 4, lm_win = lane & 7;
     const int gid = lane >> 2, tig = lane & 3;
     const uint32_t slab = smem_u32(s_a);
-    int it = 0;
     uint32_t phases = 0;
     int b0 = 0;
-    long long c_wait_full = 0, c_gather = 0, tq = 0;
-    const long long t_begin = clock64();
+    uint32_t c_wait_full = 0, c_gather = 0;                 // 32-bit cycle counters: the resident weights leave few registers
+    const uint32_t t_begin = clock();
     int cur_band = -1, g_first = 0, g_cnt = 0, n_mine = 0;
-    int my_e0[kWgGroupCap] = {}, my_meta[kWgGroupCap] = {};             // this warp's position groups of the band, fast path
+    int my_grp[kWgGroupCap] = {};          // this warp's position groups of the band, fast path: first entry slot << 11 | grp[].y
+    static_assert((kWgGroupMax << 8) < (1 << 11) && kGsSlots < (1 << 20), "my_grp packing: grp[].y below bit 11, slot above it");
     bool fast = true;
     // One position group x one K-half: D[16 x 8] = A[16 x 64] * B[64 x 8] as 4 independent k-steps.  B's
     // columns are (entry 0 hi, entry 0 lo, entry 1 hi, ...): the fp16 hi / lo halves of up to 4 entries' folded weights.
-    // load_group reads a group's fragments, mma_group returns entry tig of window gid: (hi16 row + lo16 row) x (hi-weight
-    // column + lo-weight column).  Split in two so that the fast path can issue a second group's reads before the first
-    // group's mma: the reads and the mma (which queues behind the wgmma stream on the tensor pipe) are latency, not throughput.
-    struct GroupFrag { uint2 b[4]; uint32_t a[4][4]; };
-    auto load_group = [&](int e0, int meta, int kh, uint32_t hi_base, uint32_t lo_base, GroupFrag& f) {
-      const int row = meta & 31, ne = meta >> 8;
+    // load_b reads a group's weight fragments (columns past the group's entries are zero, so they add exact zeros), load_a its
+    // rows of the unit, and mma_group returns entry tig of window gid: (hi16 row + lo16 row) x (hi-weight column + lo-weight
+    // column).  The reads and the mma (which queues behind the wgmma stream on the tensor pipe) are latency, not throughput, so
+    // the fast path reads two groups' rows before either group's mma.
+    auto load_b = [&](int e0, int meta, int kh, uint2 (&b)[4]) {
+      const int ne = meta >> 8;
       const uint2* wf = reinterpret_cast<const uint2*>(p.wfrag) + ((static_cast<size_t>(e0 + (gid >> 1)) * 2 + kh) * 16 + tig) * 2 + (gid & 1);
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) f.b[ks] = ((gid >> 1) < ne && !(p.experiment & 1024)) ? ldg_frag(wf + ks * 8) : make_uint2(0u, 0u);
-      const uint32_t rb = (lm_plane ? lo_base : hi_base) + row * (kBandWins * 128) + lm_win * 128;
+      for (int ks = 0; ks < 4; ++ks) b[ks] = ((gid >> 1) < ne && !(p.experiment & 1024)) ? ldg_frag(wf + ks * 8) : make_uint2(0u, 0u);
+    };
+    auto load_a = [&](int meta, uint32_t hi_base, uint32_t lo_base, uint32_t (&a)[4][4]) {
+      // 128-byte swizzle: chunk j = 2 ks + lm_chunk of the row sits at (j ^ (row & 7)) << 4, i.e. at (ks << 5) ^ ((lm_chunk ^ lm_win)
+      // << 4) inside a 128-byte row whose address has those bits clear
+      const uint32_t rb = (lm_plane ? lo_base : hi_base) + (meta & 31) * (kBandWins * 128) + lm_win * 128 + ((lm_chunk ^ lm_win) << 4);
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
-        if (p.experiment & 2048) { f.a[ks][0] = f.a[ks][1] = f.a[ks][2] = f.a[ks][3] = rb; continue; }
-        ldsm_x4(rb + (((ks * 2 + lm_chunk) ^ lm_win) << 4), f.a[ks]);     // 128-byte swizzle: chunk j -> j ^ (row & 7)
+        if (p.experiment & 2048) { a[ks][0] = a[ks][1] = a[ks][2] = a[ks][3] = rb; continue; }
+        ldsm_x4(rb ^ (ks << 5), a[ks]);
       }
     };
-    auto mma_group = [&](const GroupFrag& f) -> float {
+    auto mma_group = [&](const uint32_t (&a)[4][4], const uint2 (&b)[4]) -> float {
       // four independent accumulators: the warp-level mma shares the tensor pipe with the wgmma stream, so no mma of a group
       // depends on another one
       float d[4][4];
@@ -277,17 +284,20 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
       for (int ks = 0; ks < 4; ++ks) d[ks][0] = d[ks][1] = d[ks][2] = d[ks][3] = 0.f;
       if (p.experiment & 256) {                              // timing experiment: rows and weights are read, no arithmetic
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) asm volatile("" :: "r"(f.a[ks][0] | f.a[ks][1] | f.a[ks][2] | f.a[ks][3] | f.b[ks].x | f.b[ks].y));
+        for (int ks = 0; ks < 4; ++ks) asm volatile("" :: "r"(a[ks][0] | a[ks][1] | a[ks][2] | a[ks][3] | b[ks].x | b[ks].y));
       } else {
 #pragma unroll
-        for (int ks = 0; ks < 4; ++ks) mma_16816(d[ks], f.a[ks], f.b[ks].x, f.b[ks].y);
+        for (int ks = 0; ks < 4; ++ks) mma_16816(d[ks], a[ks], b[ks].x, b[ks].y);
       }
       float v = 0.f;
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) v += (d[ks][0] + d[ks][2]) + (d[ks][1] + d[ks][3]);      // fixed order
-      return v * gscale;
+      return v * p.gather_unscale;
     };
-    for (int unit = u_begin; unit < u_end; ++unit, ++it) {
+    // Weights stationary: the fast path's B fragments depend only on (band, group, K-half, k-step, lane), so they are read once
+    // per band (a CTA stays on a band for ~groups consecutive units) and stay in these 64 registers for all of its units.
+    uint2 wb[kWgGroupCap][2][4];
+    for (int unit = u_begin; unit < u_end; ++unit) {
       const int band = unit / p.groups;
       const int w0 = (unit - band * p.groups) * kBandWins;
       if (band != cur_band) {                                  // this warp's position groups of the band: gw, gw + 7, ...
@@ -299,51 +309,59 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
 #pragma unroll
         for (int i = 0; i < kWgGroupCap; ++i) {
           const int gi = gw + i * kWgWarps;
-          if (fast && gi < g_cnt) { const int2 m = p.grp[g_first + gi]; my_e0[i] = m.x; my_meta[i] = m.y; n_mine = i + 1; }
+          if (fast && gi < g_cnt) {
+            const int2 m = p.grp[g_first + gi]; my_grp[i] = m.x << 11 | m.y; n_mine = i + 1;
+            load_b(m.x, m.y, 0, wb[i][0]);
+            load_b(m.x, m.y, 1, wb[i][1]);
+          }
         }
       }
       // ---------------- gather: this warp's position groups x the unit's 8 windows, one K-half per pass (the MMAs' order, so a
-      // K-half's two regions go back to the producer while the other K-half is still in use)
+      // K-half's two regions go back to the producer while the other K-half is still in use).  Unrolled, so that wb is indexed
+      // by constants and stays in registers.
       float c0[kWgGroupCap];                                   // pass-0 halves of the fast path
-#pragma unroll 1
+#pragma unroll
       for (int kh = 0; kh < 2; ++kh) {
         int bh = b0 + 2 * kh; if (bh >= kWgBufs) bh -= kWgBufs;               // buffer of this K-half's hi16 region
         int bl = b0 + 2 * kh + 1; if (bl >= kWgBufs) bl -= kWgBufs;           // ... and of its lo16 region
         const uint32_t ph_h = (phases >> bh) & 1, ph_l = (phases >> bl) & 1;
         phases ^= (1u << bh) | (1u << bl);
         const uint32_t hi_base = slab + bh * kWgRegion, lo_base = slab + bl * kWgRegion;
-        if (p.dbg) tq = clock64();
+        if (p.dbg) c_wait_full -= clock();
         mbar_wait(&a_full[bh], ph_h, p.status, 550 + bh);          // hi16 K-half kh
         mbar_wait(&a_full[bl], ph_l, p.status, 560 + bl);          // lo16 K-half kh
-        if (p.dbg) { const long long t = clock64(); c_wait_full += t - tq; tq = t; }
+        if (p.dbg) { const uint32_t t = clock(); c_wait_full += t; c_gather -= t; }
         if (fast) {
           auto finish = [&](int i, float v) {
             if (kh == 0) c0[i] = v;
-            else if (tig < (my_meta[i] >> 8) && !(p.experiment & 64))           // 8 lanes (gid = window) write 32 contiguous bytes
-              p.part_t[static_cast<size_t>(my_e0[i] + tig) * p.n_pad + w0 + gid] = c0[i] + v;
+            else if (tig < ((my_grp[i] >> 8) & 7) && !(p.experiment & 64))      // 8 lanes (gid = window) write 32 contiguous bytes
+              p.part_t[static_cast<size_t>((my_grp[i] >> 11) + tig) * p.n_pad + w0 + gid] = c0[i] + v;
           };
 #pragma unroll
-          for (int i = 0; i < kWgGroupCap; i += 2)             // two groups at a time: both groups' reads before either mma
+          for (int i = 0; i < kWgGroupCap; i += 2)             // two groups at a time: both groups' ldmatrix before either mma
             if (i < n_mine) {
-              GroupFrag f0, f1;
-              load_group(my_e0[i], my_meta[i], kh, hi_base, lo_base, f0);
+              uint32_t a0[4][4], a1[4][4];
+              load_a(my_grp[i], hi_base, lo_base, a0);
               if (i + 1 < n_mine) {
-                load_group(my_e0[i + 1], my_meta[i + 1], kh, hi_base, lo_base, f1);
-                finish(i, mma_group(f0));
-                finish(i + 1, mma_group(f1));
+                load_a(my_grp[i + 1], hi_base, lo_base, a1);
+                finish(i, mma_group(a0, wb[i][kh]));
+                finish(i + 1, mma_group(a1, wb[i + 1][kh]));
               } else {
-                finish(i, mma_group(f0));
+                finish(i, mma_group(a0, wb[i][kh]));
               }
             }
         } else {
           // generic path (a band with more than 28 position groups: only patch sets that put more than 4 entries on many
-          // positions): pass-0 halves are parked in part_t itself (the same thread reads them back in pass 1)
+          // positions): weights are read per unit, pass-0 halves are parked in part_t itself (the same thread reads them back
+          // in pass 1)
 #pragma unroll 1
           for (int gi = gw; gi < g_cnt; gi += kWgWarps) {
             const int2 m = p.grp[g_first + gi];
-            GroupFrag f;
-            load_group(m.x, m.y, kh, hi_base, lo_base, f);
-            const float v = mma_group(f);
+            uint2 b[4];
+            uint32_t a[4][4];
+            load_b(m.x, m.y, kh, b);
+            load_a(m.y, hi_base, lo_base, a);
+            const float v = mma_group(a, b);
             if (tig < (m.y >> 8)) {
               float* gp = p.part_t + static_cast<size_t>(m.x + tig) * p.n_pad + w0 + gid;
               *gp = kh == 0 ? v : *gp + v;
@@ -352,13 +370,13 @@ wv_gather_kernel(const __grid_constant__ CUtensorMap tm_band, const __grid_const
         }
         __syncwarp();
         if (lane == 0) { mbar_arrive(&a_empty[bh]); mbar_arrive(&a_empty[bl]); }           // this warp is done with the K-half's regions
-        if (p.dbg) c_gather += clock64() - tq;
+        if (p.dbg) c_gather += clock();
       }
       b0 += 4; if (b0 >= kWgBufs) b0 -= kWgBufs;
     }
     if (p.dbg && warp == kWgMmaWarps && lane == 0) {
       long long* d = p.dbg + blockIdx.x * 8;
-      d[0] = clock64() - t_begin; d[1] = c_wait_full; d[2] = c_gather; d[5] = it;
+      d[0] = static_cast<uint32_t>(clock()) - t_begin; d[1] = c_wait_full; d[2] = c_gather; d[5] = u_end - u_begin;
     }
   }
 }

@@ -27,6 +27,7 @@ def main():
     ap.add_argument("--steps-per-call", type=int, default=1, help="internal steps per API call (> 1 exercises the tail overlap)")
     ap.add_argument("--wvg-cycles", action="store_true", help="print the fused IGLOO kernel's per-CTA cycle breakdown (conv_experiment bit 512)")
     ap.add_argument("--wvg-exp", type=int, nargs="*", default=[0], help="timing-experiment bits to add to the cycle-counter runs (32 = no gather, 256 = gather reads only)")
+    ap.add_argument("--wvg-fit", action="store_true", help="fit wv_split's unit cost model (wv_cost_base, wv_cost_group) to the per-CTA cycle counters")
     args = ap.parse_args()
     B = args.batch
     clf = engine.Classifier(None, device=0, max_batch=B)
@@ -83,6 +84,9 @@ def main():
         clf.set_option("fuse_gather", 1)
         for bits in args.wvg_exp:
             wvg_cycles(clf, pool, bits)
+    if args.wvg_fit:
+        clf.set_option("fuse_gather", 1)
+        wvg_fit(clf, pool)
 
 
 def wvg_cycles(clf, pool, bits=0):
@@ -97,6 +101,39 @@ def wvg_cycles(clf, pool, bits=0):
     print(f"wv_gather_kernel (IGLOO#1) cycle breakdown, experiment bits {bits}, mean over CTAs (first gather warp, first MMA warpgroup, producer):")
     for i, nm in enumerate(names):
         print(f"   {nm:42s} {d[:, i].mean():12.0f}   per unit {d[:, i].mean() / units:9.0f}   (min {d[:, i].min():.0f}, max {d[:, i].max():.0f})")
+
+
+def wvg_fit(clf, pool, reps=8):
+    """Least-squares fit of a CTA's cycles to wv_split's cost model, cycles = a * units + b * (sum over its units of the groups of
+    the band's busiest gather warp), over the CTAs of one IGLOO#1 launch; wv_cost_group = b / a with wv_cost_base = 1.  A CTA's
+    units are a contiguous band-major range, so the counters' unit counts give every CTA's range."""
+    import numpy as np
+    sys.path.insert(0, str(ROOT / "tests"))
+    from test_host_cpu import _pack_patches
+    from oracle import igloo_model as M
+    w = M.load_npz_weights(ROOT / "genomad_b200" / "data" / "nn_classifier.npz")
+    o = _pack_patches(w["ig1_random_patches"].reshape(2100, 4), w["ig1_w_mult"].reshape(2100, 4, 128), w["ig1_w_summer"].reshape(512))
+    per_warp = (np.diff(o["band_first"]) + 6) // 7                     # groups of the busiest of the 7 gather warps, per band
+    clf.set_option("conv_experiment", 512)
+    d = 0
+    for i in range(reps):                                             # back-to-back launches, counters averaged
+        clf.predict_ascii(pool[i % len(pool)]); torch.cuda.synchronize()
+        d = d + clf.debug_fetch("conv_dbg", 1).cpu().view(torch.int64).numpy().astype(float) / reps
+    clf.set_option("conv_experiment", 0)
+    n_units = pool[0].shape[0] // 8 * len(per_warp)
+    units = np.rint(d[:, 5]).astype(np.int64)
+    d = d[units > 0]
+    start = np.concatenate([[0], np.cumsum(units)])[:-1][units > 0]
+    units = units[units > 0]
+    assert start[-1] + units[-1] == n_units, "the counters do not cover every unit"
+    groups = n_units // len(per_warp)
+    gsum = np.array([per_warp[np.arange(s, s + u) // groups].sum() for s, u in zip(start, units)], float)
+    x = np.stack([units, gsum], 1).astype(float)
+    (a, b), *_ = np.linalg.lstsq(x, d[:, 0], rcond=None)
+    resid = d[:, 0] - x @ np.array([a, b])
+    print(f"wv_split cost fit over {len(units)} CTAs: cycles = {a:.0f} x units + {b:.0f} x busiest-warp groups "
+          f"(rms residual {np.sqrt(np.mean(resid ** 2)):.0f} of a mean {d[:, 0].mean():.0f}); "
+          f"wv_cost_group / wv_cost_base = {b / a:.3f}")
 
 
 if __name__ == "__main__":

@@ -130,6 +130,15 @@ class NNOutputs:
     def provirus_nn_classification_head_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification_head.npz")
 
+    # ---- opt-in (--write-head-attributions), not a reference output: per-token input gradients of one of the head's classes
+    @property
+    def nn_classification_head_attributions_output(self) -> Path:
+        return self._nn("nn_classification_head_attributions.npz")
+
+    @property
+    def provirus_nn_classification_head_attributions_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_attributions.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

@@ -64,8 +64,8 @@ def cli():
                    "instead, attributions that add up to the change in log-probability from a baseline to the window, also for "
                    "windows classified with near certainty (where gradient x input is ~0). About 1 + 4.2 N times the "
                    "classification's GPU time; the file adds log_p_target (window, baseline). At most 256, and at most the windows per GPU "
-                   "step of the device (checked before any work). Without --write-attributions it has no effect (a warning is "
-                   "logged). Not an option of the reference.")
+                   "step of the device (checked before any work). Also applies to --write-head-attributions. Without either "
+                   "option it has no effect (a warning is logged). Not an option of the reference.")
 @click.option("--attribution-baseline", type=click.Choice(["zero", "N"]), default=None, show_default="zero",
               help="Baseline of integrated gradients: zero (all-zero one-hot input) or N (a window of N). Not an option of the "
                    "reference.")
@@ -79,9 +79,14 @@ def cli():
                    "the scores of its classes to <prefix>_nn_classification_head.{tsv,npz}. The head must have been trained "
                    "on this encoder (checked before any work). It scores the forward strand only, also with --both-strands. "
                    "The main outputs are unchanged. Not an option of the reference.")
+@click.option("--write-head-attributions", "write_head_attributions", metavar="CLASS", default=None,
+              help="With --head: also write, for every window, the attributions of this class of the head (one of its "
+                   "class names) to <prefix>_nn_classification_head_attributions.npz, as --write-attributions does for the "
+                   "shipped classes; --attribution-steps and --attribution-baseline apply to it. Cannot be combined with "
+                   "--write-attributions. Not an option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
                       write_embeddings, write_window_scores, window_stride, write_attributions, attribution_steps,
-                      attribution_baseline, both_strands, head):
+                      attribution_baseline, both_strands, head, write_head_attributions):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -103,6 +108,8 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["both_strands"] = True
     if head is not None:
         extra["head"] = head
+    if write_head_attributions is not None:
+        extra["write_head_attributions"] = write_head_attributions
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
 

@@ -1433,6 +1433,25 @@ extern "C" int gnm_debug_fetch(gnm_handle* h, const char* which, int n, float* d
   return 0;
 }
 
+// A classifier head (gnm_head_create): its dense_1 with BN folded into scale / shift, dense_1 as TF32 halves for the tensor
+// cores, dense_2.
+struct gnm_head {
+  int C = 0;
+  std::vector<void*> allocs;
+  float *d1w = nullptr, *d1b = nullptr, *scale = nullptr, *shift = nullptr, *dwT_hi = nullptr, *dwT_lo = nullptr;
+  float *d2w = nullptr, *d2b = nullptr;
+  CUtensorMap tm_b[2];
+};
+
+// The head on the tensor cores from the TF32 halves of its input in hA_hi[1] / hA_lo[1] (dense layer 0's epilogue leaves h1's
+// there; gnm_head_forward splits the embeddings into them): dense_1 + BN + ReLU -> h2, then the C-class softmax -> d_probs.
+static int head_forward_tc(gnm_handle* h, const gnm_head* hd, int n, float* d_probs, cudaStream_t st) {
+  if (launch_dense_tc_maps(h, h->tm_hd_a[1], hd->tm_b, kHidden, n, hd->d1b, hd->scale, hd->shift, h->h2, nullptr, nullptr, nullptr,
+                           st)) return 1;
+  head_softmax_kernel<<<(n * 32 + 255) / 256, 256, 0, st>>>(h->h2, hd->d2w, hd->d2b, d_probs, n, hd->C);
+  return check_launch(h, "head_softmax_kernel");
+}
+
 // ------------------------------------------------------------------------------------------------ attributions (attr.cuh)
 // Workspace of the attribution pass, separate from the handle so that plain handles keep their memory.  Per window:
 // y1 copy, g_z3 and g_z2 operand rows (3 x 4.6 MB), fp32 g_y1 / g_z rows (2 x 3.1 MB), routing + routed maxima (2 x 0.48 MB):
@@ -1610,10 +1629,20 @@ static int launch_igloo_bwd(gnm_handle* h, gnm_attr* a, int s, int n, cudaStream
 // (ybuf[0] = y3, ybuf[1] = y2, q / logits of IGLOO#1, h1, h2).  With `ig`, the n rows are interpolated inputs (forward_main)
 // and the layer-1 result of row r, g[t, tok[t]] (minus g[t, 0] for the N baseline), goes to the g_y1 rows as [n][5997]
 // (layer1_ig_kernel); d_attr is not used.
+// With a head `hd`, the gradient is that of the head's log p_c: after the forward step, the head runs on the h1 halves that
+// dense layer 0's epilogue left in hA_hi[1] / hA_lo[1] (head_forward_tc, as gnm_head_forward after its split).  Its hidden rows
+// replace the shipped ones in h2 and its probabilities [n][C] go to d_head_probs, or else to blockmax (376 B per window >= 128):
+// both are read by attr_head_backward_kernel, and blockmax is rewritten only after it, by IGLOO#1's backward.
 static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs, float* d_attr,
-                          cudaStream_t st, const L1Interp* ig = nullptr) {
+                          cudaStream_t st, const L1Interp* ig = nullptr, const gnm_head* hd = nullptr,
+                          float* d_head_probs = nullptr) {
   float* probs = d_probs ? d_probs : a->probs;
   if (forward_step(h, d_ascii, nullptr, n, probs, nullptr, st, ig)) return 1;
+  float* head_probs = d_head_probs ? d_head_probs : a->blockmax;
+  if (hd) {
+    timer_mark(h, "attr_head_fwd", st);
+    if (head_forward_tc(h, hd, n, head_probs, st)) return 1;
+  }
   dim3 egrid((kTok + kEmbSeg - 1) / kEmbSeg, n), sgrid((kTok + kAttrSeg - 1) / kAttrSeg, n);
   timer_mark(h, "attr_layer1", st);
   if (ig) {
@@ -1629,7 +1658,12 @@ static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, in
   timer_mark(h, "attr_route0", st);
   if (launch_route(h, a, 0, a->tm_y1, n, st)) return 1;                      // y1
   timer_mark(h, "attr_head", st);
-  attr_head_backward_kernel<<<n, 256, 0, st>>>(probs, h->h1, h->h2, h->d2w, h->d1w, h->bn1_scale, h->d0w, h->bn0_scale, target, a->g_out);
+  if (hd)
+    attr_head_backward_kernel<<<n, 256, 0, st>>>(head_probs, h->h1, h->h2, hd->d2w, hd->d1w, hd->scale, h->d0w, h->bn0_scale,
+                                                 attr_classes(target, hd->C), a->g_out);
+  else
+    attr_head_backward_kernel<<<n, 256, 0, st>>>(probs, h->h1, h->h2, h->d2w, h->d1w, h->bn1_scale, h->d0w, h->bn0_scale,
+                                                 attr_classes(target, 3), a->g_out);
   if (check_launch(h, "attr_head_backward_kernel")) return 1;
   timer_mark(h, "attr_igloo1", st);
   if (launch_igloo_bwd(h, a, 1, n, st)) return 1;                            // -> fp32 g_z3, block maxima
@@ -1685,14 +1719,24 @@ static int attr_debug_fetch(gnm_handle* h, const gnm_attr* a, const std::string&
   return 0;
 }
 
+// the target check of the attribution calls: the shipped classes, or [0, C) of a head
+static int check_target(const std::string& f, const gnm_head* hd, int target) {
+  if (!hd) {
+    if (target < 0 || target > 2) return fail(f + ": target must be 0 (chromosome), 1 (plasmid) or 2 (virus)");
+  } else if (target < 0 || target >= hd->C) {
+    return fail(f + ": target must be a class of the head, in [0, " + std::to_string(hd->C) + "), not " + std::to_string(target));
+  }
+  return 0;
+}
+
 static int attribute_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
                          const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, float* d_probs, float* d_attr,
-                         void* stream) {
+                         void* stream, const gnm_head* hd = nullptr, float* d_head_probs = nullptr) {
   const std::string f(fn);
   if (!h || !a) return fail(f + ": null handle or attribution context");
   if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
   if (n < 0) return fail(f + ": negative window count");
-  if (target < 0 || target > 2) return fail(f + ": target must be 0 (chromosome), 1 (plasmid) or 2 (virus)");
+  if (check_target(f, hd, target)) return 1;
   if (h->conv_impl != 0)
     return fail(f + ": attributions need the tensor-core path (conv_impl = 0); the fp32 validation kernels have no backward pass");
   if (h->debug_stop != 0) return fail(f + ": debug_stop must be 0");
@@ -1705,7 +1749,9 @@ static int attribute_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8
     const int m = std::min(a->max_batch, n - off);
     const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
     if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
-    if (attribute_step(h, a, asc, m, target, probs_at(d_probs, off), d_attr + static_cast<size_t>(off) * kTok, st)) return 1;
+    float* head_probs = d_head_probs ? d_head_probs + static_cast<size_t>(off) * hd->C : nullptr;
+    if (attribute_step(h, a, asc, m, target, probs_at(d_probs, off), d_attr + static_cast<size_t>(off) * kTok, st, nullptr, hd,
+                       head_probs)) return 1;
   }
   return 0;
 }
@@ -1729,12 +1775,13 @@ extern "C" int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* 
 // d_logp is given), so the debug buffers still hold the last chunk's rows afterwards.
 static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
                             const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps, int baseline,
-                            float* d_probs, float* d_logp, float* d_attr, void* stream) {
+                            float* d_probs, float* d_logp, float* d_attr, void* stream, const gnm_head* hd = nullptr,
+                            float* d_head_probs = nullptr) {
   const std::string f(fn);
   if (!h || !a) return fail(f + ": null handle or attribution context");
   if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
   if (n < 0) return fail(f + ": negative window count");
-  if (target < 0 || target > 2) return fail(f + ": target must be 0 (chromosome), 1 (plasmid) or 2 (virus)");
+  if (check_target(f, hd, target)) return 1;
   if (steps < 1 || steps > a->max_batch)
     return fail(f + ": steps must be in [1, the attribution context's max_batch = " + std::to_string(a->max_batch) + "]");
   if (baseline != GNM_IG_BASELINE_ZERO && baseline != GNM_IG_BASELINE_N)
@@ -1748,10 +1795,12 @@ static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const ui
   if (check_device_status(h)) return 1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int per = a->max_batch / steps;                         // windows per chunk
+  const int C = hd ? hd->C : 3;
   if (d_logp) {                                                 // log p_c(x'), into column 1 of every window
     const L1Interp base = {0, baseline};
     if (forward_step(h, d_ascii ? d_ascii : h->in_stage[0], nullptr, 1, a->probs, nullptr, st, &base)) return 1;
-    ig_logp_kernel<<<(n + 255) / 256, 256, 0, st>>>(a->probs, 1, n, target, d_logp + 1);
+    if (hd && head_forward_tc(h, hd, 1, a->blockmax, st)) return 1;    // the head's p(x'): blockmax, read right below
+    ig_logp_kernel<<<(n + 255) / 256, 256, 0, st>>>(hd ? a->blockmax : a->probs, 1, n, attr_classes(target, C), d_logp + 1);
     if (check_launch(h, "ig_logp_kernel")) return 1;
   }
   const L1Interp ig = {steps, baseline};
@@ -1759,15 +1808,28 @@ static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const ui
     const int m = std::min(per, n - off);
     const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
     if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
-    if (d_probs || d_logp) {
+    if (hd && (d_probs || d_logp || d_head_probs)) {
+      // the windows' own forward and head: shipped probabilities to d_probs or the context's probs rows, the head's to
+      // d_head_probs or blockmax (scratch until step 2 rewrites it), log p_c(x) from the head's
+      float* probs = d_probs ? probs_at(d_probs, off) : a->probs;
+      float* head_probs = d_head_probs ? d_head_probs + static_cast<size_t>(off) * C : a->blockmax;
+      if (forward_step(h, asc, nullptr, m, probs, nullptr, st)) return 1;
+      if (head_forward_tc(h, hd, m, head_probs, st)) return 1;
+      if (d_logp) {
+        ig_logp_kernel<<<(m + 255) / 256, 256, 0, st>>>(head_probs, 0, m, attr_classes(target, C),
+                                                         d_logp + static_cast<size_t>(off) * 2);
+        if (check_launch(h, "ig_logp_kernel")) return 1;
+      }
+    } else if (!hd && (d_probs || d_logp)) {
       float* probs = d_probs ? probs_at(d_probs, off) : a->blockmax;    // blockmax: scratch until step 2 rewrites it
       if (forward_step(h, asc, nullptr, m, probs, nullptr, st)) return 1;
       if (d_logp) {
-        ig_logp_kernel<<<(m + 255) / 256, 256, 0, st>>>(probs, 0, m, target, d_logp + static_cast<size_t>(off) * 2);
+        ig_logp_kernel<<<(m + 255) / 256, 256, 0, st>>>(probs, 0, m, attr_classes(target, 3),
+                                                         d_logp + static_cast<size_t>(off) * 2);
         if (check_launch(h, "ig_logp_kernel")) return 1;
       }
     }
-    if (attribute_step(h, a, asc, m * steps, target, nullptr, nullptr, st, &ig)) return 1;
+    if (attribute_step(h, a, asc, m * steps, target, nullptr, nullptr, st, &ig, hd)) return 1;
     timer_mark(h, "ig_reduce", st);
     ig_reduce_kernel<<<dim3((kTok + 255) / 256, m), 256, 0, st>>>(a->gy1, steps, d_attr + static_cast<size_t>(off) * kTok);
     if (check_launch(h, "ig_reduce_kernel")) return 1;
@@ -1788,6 +1850,40 @@ extern "C" int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_
   if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_ig_windows: null buffer");
   return attribute_ig_any(h, a, "gnm_attribute_ig_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, steps, baseline,
                           d_probs, d_logp, d_attr, stream);
+}
+
+// ---- through a classifier head: the same passes for the head's log p_c (attribute_step); d_probs keeps the shipped classes
+extern "C" int gnm_attribute_head_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                        int target, float* d_probs, float* d_head_probs, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_head_ascii: null head");
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_head_ascii: null buffer");
+  return attribute_any(h, a, "gnm_attribute_head_ascii", d_ascii, nullptr, nullptr, nullptr, n, target, d_probs, d_attr, stream,
+                       head, d_head_probs);
+}
+extern "C" int gnm_attribute_head_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                          const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, float* d_probs,
+                                          float* d_head_probs, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_head_windows: null head");
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_head_windows: null buffer");
+  return attribute_any(h, a, "gnm_attribute_head_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, d_probs, d_attr,
+                       stream, head, d_head_probs);
+}
+extern "C" int gnm_attribute_head_ig_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                           int target, int steps, int baseline, float* d_probs, float* d_head_probs, float* d_logp,
+                                           float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_head_ig_ascii: null head");
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_head_ig_ascii: null buffer");
+  return attribute_ig_any(h, a, "gnm_attribute_head_ig_ascii", d_ascii, nullptr, nullptr, nullptr, n, target, steps, baseline,
+                          d_probs, d_logp, d_attr, stream, head, d_head_probs);
+}
+extern "C" int gnm_attribute_head_ig_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                             const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps,
+                                             int baseline, float* d_probs, float* d_head_probs, float* d_logp, float* d_attr,
+                                             void* stream) {
+  if (!head) return fail("gnm_attribute_head_ig_windows: null head");
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_head_ig_windows: null buffer");
+  return attribute_ig_any(h, a, "gnm_attribute_head_ig_windows", nullptr, d_seq, d_win_start, d_win_len, n, target, steps,
+                          baseline, d_probs, d_logp, d_attr, stream, head, d_head_probs);
 }
 
 extern "C" long long gnm_attr_bytes_per_window(void) {
@@ -1968,13 +2064,6 @@ extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uin
 }
 
 // ------------------------------------------------------------------------------------------------ classifier heads (head.cuh)
-struct gnm_head {
-  int C = 0;
-  std::vector<void*> allocs;
-  float *d1w = nullptr, *d1b = nullptr, *scale = nullptr, *shift = nullptr, *dwT_hi = nullptr, *dwT_lo = nullptr;
-  float *d2w = nullptr, *d2b = nullptr;
-  CUtensorMap tm_b[2];
-};
 
 extern "C" int gnm_head_destroy(gnm_head* hd) {
   if (!hd) return 0;
@@ -2033,15 +2122,14 @@ extern "C" int gnm_head_forward(gnm_handle* h, const gnm_head* hd, const float* 
       const size_t total = static_cast<size_t>(m) * kHidden;
       head_split_tf32_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(x, h->hA_hi[1], h->hA_lo[1], total);
       if (check_launch(h, "head_split_tf32_kernel")) return 1;
-      if (launch_dense_tc_maps(h, h->tm_hd_a[1], hd->tm_b, kHidden, m, hd->d1b, hd->scale, hd->shift, h->h2, nullptr, nullptr,
-                               nullptr, st)) return 1;
+      if (head_forward_tc(h, hd, m, d_probs + static_cast<size_t>(off) * hd->C, st)) return 1;
     } else {
       if (launch_sgemm(h, x, kHidden, hd->d1w, kHidden, h->h2, kHidden, m, kHidden, kHidden, hd->d1b, hd->scale, hd->shift, 1,
                        st)) return 1;
+      head_softmax_kernel<<<(m * 32 + 255) / 256, 256, 0, st>>>(h->h2, hd->d2w, hd->d2b, d_probs + static_cast<size_t>(off) * hd->C,
+                                                               m, hd->C);
+      if (check_launch(h, "head_softmax_kernel")) return 1;
     }
-    head_softmax_kernel<<<(m * 32 + 255) / 256, 256, 0, st>>>(h->h2, hd->d2w, hd->d2b, d_probs + static_cast<size_t>(off) * hd->C,
-                                                             m, hd->C);
-    if (check_launch(h, "head_softmax_kernel")) return 1;
   }
   return 0;
 }

@@ -5,8 +5,9 @@
 // depend on its batch, its chunk or the GPU count.
 //
 // Backward, per window (DESIGN.md, "Attributions"):
-//   head     g_logits = e_c - p, as -p_i and, for the target, the sum of the other two p_i (never 1 - p_c, which cancels
-//            when p_c is near 1); back through Dense(3), BN1 + ReLU, Dense(512), BN0 + ReLU, Dense(512)  -> g_out0, g_out1
+//   head     g_logits = e_c - p, as -p_i and, for the target, the sum of the other p_i (never 1 - p_c, which cancels
+//            when p_c is near 1); back through Dense(C), BN1 + ReLU, Dense(512), BN0 + ReLU, Dense(512)  -> g_out0, g_out1
+//            (C = 3 and the shipped tail, or a trained head's last three layers)
 //   IGLOO k  out = alpha^T q, alpha = softmax(mpi w_qk), q = maxpool8(y w_v)
 //            g_q[p,c] = alpha[p] g_out[c];  g_alpha[p] = sum_c g_out[c] q[p,c];  g_logit = alpha (g_alpha - <alpha, g_alpha>)
 //            g_mpi = w_qk g_logit (sgemm_epi_kernel);  g_y[t] = sum over the (p,c) routed to t of g_q[p,c] w_v[:,c]
@@ -20,6 +21,7 @@
 #include "common.cuh"
 #include "conv_t.cuh"
 #include "encode.cuh"
+#include "head.cuh"
 #include "igloo.cuh"
 
 namespace gnm {
@@ -36,33 +38,45 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // ------------------------------------------------------------------------------------------------ head
-// One window per CTA, 256 threads.  g_out[w][0..255] = d log p_c / d h0 (h0 = [out0 | out1]), unscaled.
+// The class arguments of the head-gradient and log p kernels, target c and class count C, travel in one int, tc = c | C << 8:
+// the kernels keep the parameter lists (and symbols) they had when C was always 3.
+__host__ __device__ constexpr int attr_classes(int target, int C) { return target | (C << 8); }
+__device__ __forceinline__ int attr_target_of(int tc) { return tc & 0xff; }
+__device__ __forceinline__ int attr_count_of(int tc) { return tc >> 8; }
+
+// One window per CTA, 256 threads.  g_out[w][0..255] = d log p_c / d h0 (h0 = [out0 | out1]), unscaled, through a C-class head
+// (2 <= C <= 32): the shipped tail at C = 3 (d2w, d1w, bn1_scale, h2 the handle's) or a trained head (gnm_head's d2w, d1w and
+// folded BN scale, h2 its hidden rows).  Dense(512) #0 and its BN are the encoder's in both cases.
 __global__ void __launch_bounds__(256)
-attr_head_backward_kernel(const float* __restrict__ probs,      // [n][3]
+attr_head_backward_kernel(const float* __restrict__ probs,      // [n][C]
                           const float* __restrict__ h1, const float* __restrict__ h2,   // [n][512] (post-ReLU)
-                          const float* __restrict__ d2w,        // [512][3]
+                          const float* __restrict__ d2w,        // [512][C]
                           const float* __restrict__ d1w,        // [512][512]
                           const float* __restrict__ bn1_scale,  // [512]
                           const float* __restrict__ d0w,        // [256][512]
                           const float* __restrict__ bn0_scale,  // [512]
-                          int target, float* __restrict__ g_out) {
-  __shared__ float s_a1[kHidden], s_a0[kHidden];
+                          int tc,                               // attr_classes(target, C)
+                          float* __restrict__ g_out) {
+  __shared__ float s_a1[kHidden], s_a0[kHidden], s_gl[kHeadMaxClasses];
   const int w = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // g_logits = e_c - p with the target's component as the sum of the other two probabilities (ascending i), not 1 - p_c:
+  const int target = attr_target_of(tc), C = attr_count_of(tc);
+  // g_logits = e_c - p with the target's component as the sum of the other probabilities (ascending i), not 1 - p_c:
   // values just below 1 are 2^-24 apart, so 1 - p_c cancels for a window classified confidently as the target and is
   // exactly 0 once p_c rounds to 1.0f (log-odds margin ~17.3), while the off-target p_i keep their relative precision
-  float gl[3], other = 0.f;
-#pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    const float p = probs[static_cast<size_t>(w) * 3 + i];
-    gl[i] = -p;
-    if (i != target) other += p;
+  if (tid == 0) {
+    float other = 0.f;
+    for (int i = 0; i < C; ++i) {
+      const float p = probs[static_cast<size_t>(w) * C + i];
+      s_gl[i] = -p;
+      if (i != target) other += p;
+    }
+    s_gl[target] = other;
   }
-#pragma unroll
-  for (int i = 0; i < 3; ++i)
-    if (i == target) gl[i] = other;
-  for (int k = tid; k < kHidden; k += 256) {
-    const float g = fmaf(gl[2], d2w[k * 3 + 2], fmaf(gl[1], d2w[k * 3 + 1], gl[0] * d2w[k * 3]));
+  __syncthreads();
+  for (int k = tid; k < kHidden; k += 256) {                    // gl[0] w[k][0], then one fmaf per class, ascending
+    const float* wk = d2w + static_cast<size_t>(k) * C;
+    float g = s_gl[0] * wk[0];
+    for (int i = 1; i < C; ++i) g = fmaf(s_gl[i], wk[i], g);
     s_a1[k] = h2[static_cast<size_t>(w) * kHidden + k] > 0.f ? g * bn1_scale[k] : 0.f;
   }
   __syncthreads();
@@ -396,18 +410,19 @@ ig_reduce_kernel(const float* __restrict__ rows, int m, float* __restrict__ out)
   out[static_cast<size_t>(w) * kTok + t] = a / static_cast<float>(m);
 }
 
-// log p_c from a row of fp32 probabilities without cancellation: -log1p(sum_{i != c} p_i) (the sum in ascending i, as the head
-// gradient's) when c is the argmax (p_c >= every p_i), log p_c otherwise; evaluated in fp64 and rounded once to fp32.
+// log p_c from a row of C fp32 probabilities without cancellation: -log1p(sum_{i != c} p_i) (the sum in ascending i, as the
+// head gradient's) when c is the argmax (p_c >= every p_i), log p_c otherwise; evaluated in fp64 and rounded once to fp32.
 // out[2 i] for i < n, from probs row i, or from row 0 for every i when `broadcast` (the baseline's value in every row).
 __global__ void __launch_bounds__(256)
-ig_logp_kernel(const float* __restrict__ probs, int broadcast, int n, int target, float* __restrict__ out) {
+ig_logp_kernel(const float* __restrict__ probs, int broadcast, int n, int tc /* attr_classes(target, C) */,
+               float* __restrict__ out) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n) return;
-  const float* p = probs + (broadcast ? 0 : static_cast<size_t>(i) * 3);
+  const int target = attr_target_of(tc), C = attr_count_of(tc);
+  const float* p = probs + (broadcast ? 0 : static_cast<size_t>(i) * C);
   float other = 0.f;
   bool top = true;
-#pragma unroll
-  for (int k = 0; k < 3; ++k)
+  for (int k = 0; k < C; ++k)
     if (k != target) { other += p[k]; top = top && p[target] >= p[k]; }
   out[static_cast<size_t>(i) * 2] = top ? static_cast<float>(-log1p(static_cast<double>(other)))
                                         : static_cast<float>(log(static_cast<double>(p[target])));

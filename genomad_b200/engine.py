@@ -103,6 +103,15 @@ EXPORTS = {
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     "gnm_attribute_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                            C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_head_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_head_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_head_ig_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_head_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p]),
     "gnm_neighbours_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
     "gnm_embedding_neighbours": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -323,6 +332,7 @@ class Attributions(NamedTuple):
     offsets: "object"         # int32 [n_contigs + 1], CSR
     attr: "object"            # float32 [W, 5997]: d log p_target / d one-hot token, token t = bases t .. t+3 of the window
     logp: "object" = None     # integrated gradients only: float32 [W, 2], log p_target(window), log p_target(baseline)
+    head_probs: "object" = None   # Head.attribute_contigs / integrated_gradients_contigs: float32 [W, C], the head's scores
 
 
 CLASSES = ("chromosome", "plasmid", "virus")
@@ -883,6 +893,114 @@ class Head:
             _check(self.lib, self.lib.gnm_head_forward(self.clf._h, self._hd, x.data_ptr(), x.shape[0], out.data_ptr(),
                                                        self.clf._stream()))
         return out
+
+    # ------------------------------------------------------------------ attributions of the head's classes
+    def class_index(self, target) -> int:
+        """An index in [0, C) or one of class_names -> class index."""
+        if isinstance(target, str):
+            if target not in self.class_names:
+                raise ValueError(f"target must be one of the head's classes {self.class_names}, not {target!r}")
+            return self.class_names.index(target)
+        t = int(target)
+        if not 0 <= t < self.n_classes:
+            raise ValueError(f"target must be in [0, {self.n_classes}), not {t}")
+        return t
+
+    def _attr_out(self, n, device, ig):
+        t = self.clf._torch
+        probs = t.empty((n, 3), dtype=t.float32, device=device)
+        head_probs = t.empty((n, self.n_classes), dtype=t.float32, device=device)
+        logp = t.empty((n, 2), dtype=t.float32, device=device) if ig else None
+        attr = t.empty((n, TOKENS), dtype=t.float32, device=device)
+        return probs, head_probs, logp, attr
+
+    def attribute_ascii(self, ascii_windows, target):
+        """uint8 cuda [n, 6000], a class of the head (index or name) -> (probabilities float32 [n, 3], head probabilities
+        [n, C], attributions [n, 5997]): attr[i, t] = d log p_target / d x[t, tok[t]] for the head's p (gnm_attribute_head_ascii),
+        through the classifier's attribution context.  The probabilities are bitwise those of Classifier.predict_ascii, the head
+        probabilities those of predict(embed_ascii(...))."""
+        clf = self.clf
+        a = ascii_windows.contiguous()
+        assert a.dtype == clf._torch.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        c = self.class_index(target)
+        probs, head_probs, _, attr = self._attr_out(a.shape[0], a.device, False)
+        if a.shape[0]:
+            _check(self.lib, self.lib.gnm_attribute_head_ascii(clf._h, clf._attr_ctx(), self._hd, a.data_ptr(), a.shape[0], c,
+                                                               probs.data_ptr(), head_probs.data_ptr(), attr.data_ptr(),
+                                                               clf._stream()))
+        return probs, head_probs, attr
+
+    def attribute_windows(self, seq_u8, win_start, win_len, target):
+        """Planned windows of a sequence buffer (see Classifier.predict_windows) -> (probabilities [W, 3], head probabilities
+        [W, C], attributions [W, 5997])."""
+        clf, t = self.clf, self.clf._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        c = self.class_index(target)
+        n = start.numel()
+        probs, head_probs, _, attr = self._attr_out(n, seq_u8.device, False)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_head_windows(clf._h, clf._attr_ctx(), self._hd, seq_u8.data_ptr(),
+                                                                 start.data_ptr(), length.data_ptr(), n, c, probs.data_ptr(),
+                                                                 head_probs.data_ptr(), attr.data_ptr(), clf._stream()))
+        return probs, head_probs, attr
+
+    def _contig_record(self, seqs, single_window, attr_fn):
+        clf, t = self.clf, self.clf._torch
+        seq, offs = clf.contig_buffers(seqs)
+        start, length, woff = clf.contig_windows(seq, offs, single_window)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        out = attr_fn(seq, start, length)
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        probs, head_probs, attr = out[0], out[1], out[-1]
+        logp = out[2] if len(out) == 4 else None
+        return Attributions(probs, contig, rel, length, woff, attr, logp, head_probs)
+
+    def attribute_contigs(self, seqs, target, single_window: bool = False) -> "Attributions":
+        """Classifier.attribute_contigs for a class of the head: the same windows and record, with head_probs [W, C]."""
+        return self._contig_record(seqs, single_window, lambda s, b, l: self.attribute_windows(s, b, l, target))
+
+    def integrated_gradients_ascii(self, ascii_windows, target, steps: int = IG_STEPS, baseline="zero"):
+        """uint8 cuda [n, 6000], a class of the head -> (probabilities [n, 3], head probabilities [n, C], logp [n, 2],
+        attributions [n, 5997]) by integrated gradients of the head's log p_target (gnm_attribute_head_ig_ascii; the rule of
+        Classifier.integrated_gradients_ascii)."""
+        clf = self.clf
+        a = ascii_windows.contiguous()
+        assert a.dtype == clf._torch.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        c = self.class_index(target)
+        m, b = clf._ig_args(steps, baseline)
+        n = a.shape[0]
+        probs, head_probs, logp, attr = self._attr_out(n, a.device, True)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_head_ig_ascii(clf._h, clf._attr_ctx(), self._hd, a.data_ptr(), n, c, m, b,
+                                                                  probs.data_ptr(), head_probs.data_ptr(), logp.data_ptr(),
+                                                                  attr.data_ptr(), clf._stream()))
+        return probs, head_probs, logp, attr
+
+    def integrated_gradients_windows(self, seq_u8, win_start, win_len, target, steps: int = IG_STEPS, baseline="zero"):
+        """Planned windows of a sequence buffer -> (probabilities [W, 3], head probabilities [W, C], logp [W, 2], attributions
+        [W, 5997]) by integrated gradients (see integrated_gradients_ascii)."""
+        clf, t = self.clf, self.clf._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        c = self.class_index(target)
+        m, b = clf._ig_args(steps, baseline)
+        n = start.numel()
+        probs, head_probs, logp, attr = self._attr_out(n, seq_u8.device, True)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_head_ig_windows(clf._h, clf._attr_ctx(), self._hd, seq_u8.data_ptr(),
+                                                                    start.data_ptr(), length.data_ptr(), n, c, m, b,
+                                                                    probs.data_ptr(), head_probs.data_ptr(), logp.data_ptr(),
+                                                                    attr.data_ptr(), clf._stream()))
+        return probs, head_probs, logp, attr
+
+    def integrated_gradients_contigs(self, seqs, target, steps: int = IG_STEPS, baseline="zero",
+                                     single_window: bool = False) -> "Attributions":
+        """attribute_contigs by integrated gradients, with logp [W, 2] of the head's class."""
+        return self._contig_record(seqs, single_window,
+                                   lambda s, b, l: self.integrated_gradients_windows(s, b, l, target, steps, baseline))
 
     def _segment(self, fn, probs, offsets, width):
         t = self.clf._torch

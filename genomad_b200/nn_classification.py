@@ -118,6 +118,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).  With attributions["steps"] >= 1 the
     calls are the integrated-gradients ones (Classifier.integrated_gradients_ascii, same probabilities), and the rows of
     log p_target at the window and at the baseline travel to rank 0 the same way, as attributions["logp"] (float32 [n_windows, 2]).
+    With attributions["head"] true, the target is a class of the `head` and the calls are the head's (Head.attribute_ascii /
+    integrated_gradients_ascii): one call gives the probabilities, the head's scores of the windows (bitwise Head.predict of
+    their embeddings) and the attributions of the head's log p_target, so the chunk takes no other route.
 
     With `head` ({"head": engine.Head}), every chunk takes the embedding route and the head scores each window's embedding on
     the device into a buffer of this rank's shard; they are reduced per contig by the routes of the class scores (gather or
@@ -166,9 +169,20 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
         if ig_steps:
             d_logp = torch.empty((end - start, 2), dtype=torch.float32, device=dev)
 
+        head_route = bool(attributions.get("head"))
+        assert not head_route or scorer is not None
+
         def run(win, m, row):                                # probabilities and attributions from the attribution calls
             d_win = torch.from_numpy(win[:m]).to(dev)
-            if ig_steps:
+            if head_route:                                   # the head's scores come out of the same call
+                if ig_steps:
+                    probs, head_probs, logp, attr = scorer.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
+                                                                                      attributions["baseline"])
+                    d_logp[row: row + m].copy_(logp)
+                else:
+                    probs, head_probs, attr = scorer.attribute_ascii(d_win, attributions["target"])
+                d_head[row: row + m].copy_(head_probs)
+            elif ig_steps:
                 probs, logp, attr = clf.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
                                                                    attributions["baseline"])
                 d_logp[row: row + m].copy_(logp)
@@ -176,11 +190,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 probs, attr = clf.attribute_ascii(d_win, attributions["target"])
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
-            if embeddings or scorer is not None:
+            if embeddings or (scorer is not None and not head_route):
                 e = clf.embed_ascii(d_win)[1]
                 if embeddings:
                     shard.add(e)
-                if scorer is not None:
+                if scorer is not None and not head_route:
                     scorer.predict(e, out=d_head[row: row + m])
             sync()
     futures = []
@@ -397,8 +411,19 @@ def attribution_baseline(value=None) -> str:
     return v
 
 
+def head_attributions_target(value=None):
+    """The class of the --head classifier whose attributions are written (``--write-head-attributions CLASS`` /
+    GENOMAD_B200_HEAD_ATTRIBUTIONS=CLASS / main(..., write_head_attributions=CLASS)), or None; it is checked against the head
+    file's class names once that is loaded.  value None: the environment decides; False / "" / "0": off."""
+    if value is None:
+        value = os.environ.get("GENOMAD_B200_HEAD_ATTRIBUTIONS", "")
+    if value is False or value is None or str(value).strip() in ("", "0"):
+        return None
+    return str(value).strip()
+
+
 def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr, steps: int = 0,
-                        baseline: str = "zero", logp=None) -> None:
+                        baseline: str = "zero", logp=None, extra=None) -> None:
     # np.savez, as for the embeddings: 24 KB of fp32 per window barely compresses
     offsets = np.asarray(offsets, dtype=np.int32)
     keys = {names_key: names,
@@ -410,6 +435,7 @@ def _write_attributions(path: Path, names_key: str, names, offsets, starts, leng
     if steps:                                       # integrated gradients; a gradient x input file keeps the keys above only
         keys.update({"method": np.str_(IG_METHOD), "steps": np.int32(steps), "baseline": np.str_(baseline),
                      "log_p_target": np.asarray(logp, dtype=np.float32).reshape(-1, 2)})
+    keys.update(extra or {})                        # the head attributions file: head_sha256, class_names
     np.savez(path, **keys)
 
 
@@ -426,6 +452,17 @@ def _attributions_current(path: Path, target: str, steps: int = 0, baseline: str
             if not steps:
                 return method == "gradient_x_input"
             return method == IG_METHOD and int(z["steps"]) == steps and str(z["baseline"]) == baseline
+    except Exception:
+        return False
+
+
+def _head_attributions_current(path: Path, target: str, head_sha: str, steps: int = 0, baseline: str = "zero") -> bool:
+    """The head attributions file is current for this class, method, steps and baseline, and was written for this head."""
+    if not _attributions_current(path, target, steps, baseline):
+        return False
+    try:
+        with np.load(path) as z:
+            return str(z["head_sha256"]) == head_sha
     except Exception:
         return False
 
@@ -597,7 +634,7 @@ _attribution_steps, _attribution_baseline = attribution_steps, attribution_basel
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
          write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
-         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None):
+         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None, write_head_attributions=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -612,15 +649,23 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                            else bool(write_window_scores))
     window_stride = sequence.WINDOW if window_stride is None else int(window_stride)
     attr_target = attributions_target(write_attributions)
+    head_attr_target = head_attributions_target(write_head_attributions)
+    if head_attr_target is not None and head is None:
+        raise ValueError("--write-head-attributions needs --head: it names a class of the head file")
+    if head_attr_target is not None and attr_target:
+        raise ValueError("--write-head-attributions and --write-attributions cannot be combined in one run: the contig pass "
+                         "runs through one kind of attribution call")
+    any_attr = bool(attr_target or head_attr_target)
     # both options are validated whether or not they take effect; an option without effect is reported in the log
     steps_opt, baseline_opt = _attribution_steps(attribution_steps), _attribution_baseline(attribution_baseline)
     baseline_given = attribution_baseline is not None or bool(os.environ.get("GENOMAD_B200_ATTRIBUTION_BASELINE", "").strip())
     ig_notes = []
-    if not attr_target and (steps_opt or baseline_given):
-        ig_notes.append("--attribution-steps / --attribution-baseline have no effect without --write-attributions.")
-    elif attr_target and baseline_given and not steps_opt:
+    if not any_attr and (steps_opt or baseline_given):
+        ig_notes.append("--attribution-steps / --attribution-baseline have no effect without --write-attributions or "
+                        "--write-head-attributions.")
+    elif any_attr and baseline_given and not steps_opt:
         ig_notes.append("--attribution-baseline has no effect with --attribution-steps 0 (gradient x input).")
-    ig_steps = steps_opt if attr_target else 0
+    ig_steps = steps_opt if any_attr else 0
     ig_baseline = baseline_opt if ig_steps else "zero"
     attr_method = f", integrated gradients, {ig_steps} steps, baseline {ig_baseline}" if ig_steps else ""
     if not 1 <= window_stride <= sequence.WINDOW:
@@ -661,6 +706,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         files += [outputs.nn_classification_head_output, outputs.nn_classification_head_npz_output]
         descr += ["classification by the --head classifier: tabular format",
                   "classification by the --head classifier: binary format"]
+    if head_attr_target:
+        files.append(outputs.nn_classification_head_attributions_output)
+        descr.append(f"window attributions of the --head classifier ({head_attr_target}{attr_method}): binary format")
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -683,6 +731,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             files += [outputs.provirus_nn_classification_head_output, outputs.provirus_nn_classification_head_npz_output]
             descr += ["provirus classification by the --head classifier: tabular format",
                       "provirus classification by the --head classifier: binary format"]
+        if head_attr_target:
+            files.append(outputs.provirus_nn_classification_head_attributions_output)
+            descr.append(f"provirus window attributions of the --head classifier ({head_attr_target}{attr_method}): "
+                         "binary format")
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -694,6 +746,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             head_file, head_sha = _load_head_file(head)
         except (OSError, ValueError, KeyError) as e:
             console.error(f"{head} is not a usable head file: {e}")
+            sys.exit(1)
+        if head_attr_target is not None and head_attr_target not in head_file.class_names:
+            console.error(f"--write-head-attributions {head_attr_target}: not a class of {head} "
+                          f"({', '.join(head_file.class_names)})")
             sys.exit(1)
     ig_clf = None
     if ig_steps:                     # the steps must fit this device's attribution context: fail before any work
@@ -713,7 +769,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
              outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output,
              outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output,
-             outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output)]
+             outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output,
+             outputs.nn_classification_head_attributions_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
@@ -721,7 +778,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                      outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
                      outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output,
                      outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output,
-                     outputs.provirus_nn_classification_head_npz_output, outputs.provirus_nn_classification_head_output))
+                     outputs.provirus_nn_classification_head_npz_output, outputs.provirus_nn_classification_head_output,
+                     outputs.provirus_nn_classification_head_attributions_output))
 
     plan = None
     info_writer = None
@@ -747,7 +805,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                       and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
                       and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))
                       and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))
-                      and (head_file is None or _head_current(j[16], j[17], head_sha))))
+                      and (head_file is None or _head_current(j[16], j[17], head_sha))
+                      and (not head_attr_target
+                           or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -799,7 +859,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
-         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path), \
+         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path,
+         head_attr_path), \
             (enc_skip, cls_skip), (parsed, index) \
             in zip(jobs, plan, staged):
         names = preds = emb = None
@@ -807,6 +868,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         attr = None                     # the contig pass runs through the attribution calls
         if attr_target:
             attr = {"target": attr_target, **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
+        elif head_attr_target:          # the same, through the head's attribution calls
+            attr = {"target": head_attr_target, "head": True,
+                    **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
         win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
         hd = None                       # --head: the chunk loop also scores every window with the head (forward strand)
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
@@ -878,7 +942,15 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                                          threads or 1)
                 console.log(f"{label} window scores (stride {window_stride}) written to {win_tsv_path.name} and "
                             f"{win_npz_path.name}.")
-            if attr is not None:
+            if attr is not None and head_attr_target:
+                if is_main:
+                    _write_attributions(head_attr_path, names_key, names, *attr["spans"], head_attr_target, attr["attr"],
+                                        ig_steps, ig_baseline, attr.get("logp"),
+                                        extra={"head_sha256": np.str_(head_sha),
+                                               "class_names": np.array(head_file.class_names)})
+                console.log(f"{label} window attributions of the head ({head_attr_target}{attr_method}) in binary format "
+                            f"written to {head_attr_path.name}.")
+            elif attr is not None:
                 if is_main:
                     _write_attributions(attr_path, names_key, names, *attr["spans"], attr_target, attr["attr"], ig_steps,
                                         ig_baseline, attr.get("logp"))

@@ -492,6 +492,45 @@ int gnm_attribute_ig_windows(gnm_handle* h, gnm_attr* a, const uint8_t* d_seq, c
                              float* d_attr, void* stream);
 
 /*
+ * Head attributions: the same attributions and integrated gradients for a class of a trained head (gnm_head_create, below),
+ * so that a sequence scored as one of the user's classes can be explained.  For a head with C classes, a target c in [0, C)
+ * and the head's inference-mode forward on the window's encoder output h1 (dense layer 0's output, gnm_embed_*):
+ *
+ *     z = h1 W1 + b1;  a = scale * z + shift (BN folded as gnm_head_create folds it);  hh = relu(a);
+ *     logits = hh W2 + b2;  p = softmax(logits) (the sequence of gnm_head_forward)
+ *     attr[t] = d log p_c / d x[t, tok[t]]
+ *
+ * at the window's own input, with the routing rule (first row on ties) and LeakyReLU branches of gnm_attribute_*.  The head
+ * gradient keeps the shipped rule for all C classes: g_i = -p_i for i != c and g_c = sum_{i != c} p_i in ascending i, never
+ * 1 - p_c.  IG uses the same midpoint rule and baselines, and log p_c(x), log p_c(x') the same no-cancellation form, over the
+ * head's C probabilities.  A head with the shipped tail's own weights (C = 3) gives bitwise the attributions of gnm_attribute_*.
+ *
+ * gnm_attribute_head_ascii / _windows, gnm_attribute_head_ig_ascii / _ig_windows: arguments as gnm_attribute_* and
+ *   gnm_attribute_ig_*, plus
+ *   head          a head created on h (gnm_head_create).
+ *   target        in [0, C); any other value is refused.
+ *   d_probs       DEVICE float [n][3] or NULL: the shipped probabilities, bitwise those of gnm_forward_*.
+ *   d_head_probs  DEVICE float [n][C] or NULL: the head's probabilities, bitwise those of gnm_head_forward on the gnm_embed_*
+ *                 output of the same windows.
+ *   d_logp        (IG) DEVICE float [n][2] or NULL: log p_c(x), log p_c(x') of the head's class.
+ *   Per chunk, one dense_1 GEMM on the tensor cores and one softmax more than gnm_attribute_*; no memory beyond the context's
+ *   (the head's hidden rows use the handle's h2, its probabilities the context's scratch).  Refused under conv_impl = 1 or a
+ *   debug_stop, as gnm_attribute_*.  Asynchronous on `stream`.
+ */
+typedef struct gnm_head gnm_head;
+int gnm_attribute_head_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n, int target,
+                             float* d_probs, float* d_head_probs, float* d_attr, void* stream);
+int gnm_attribute_head_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq, const int64_t* d_win_start,
+                               const int32_t* d_win_len, int n, int target, float* d_probs, float* d_head_probs, float* d_attr,
+                               void* stream);
+int gnm_attribute_head_ig_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n, int target,
+                                int steps, int baseline, float* d_probs, float* d_head_probs, float* d_logp, float* d_attr,
+                                void* stream);
+int gnm_attribute_head_ig_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                  const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps, int baseline,
+                                  float* d_probs, float* d_head_probs, float* d_logp, float* d_attr, void* stream);
+
+/*
  * Embedding neighbours: for each query row, the k reference rows nearest in cosine similarity.  Rows are GNM_EMBED (512) fp32
  * values (the encoder embeddings of gnm_embed_*), finite, contiguous, row pitch 2 KB.  No handle, no allocation: the calls run on
  * the current device and `stream`, and use only the caller's workspace.  DESIGN.md, "Embedding neighbours".
@@ -562,8 +601,7 @@ typedef struct gnm_head_weights {
   const float* dense2_kernel;  /* [512][C] */
   const float* dense2_bias;    /* [C] */
 } gnm_head_weights;
-typedef struct gnm_head gnm_head;
-typedef struct gnm_head_train gnm_head_train;
+typedef struct gnm_head_train gnm_head_train;   /* gnm_head: declared with the head attributions */
 
 /*
  * Upload a head for inference on handle h's device.  BN is folded into scale and shift and dense_1 split into TF32 halves with

@@ -2307,6 +2307,8 @@ extern "C" int gnm_head_train_fetch(gnm_head_train* tr, const char* which, void*
   const void* src = nullptr;
   size_t bytes = 0;
   if (k == "grad") { src = tr->G; bytes = tr->n_par * sizeof(float); }
+  else if (k == "adam_m") { src = tr->M; bytes = tr->n_par * sizeof(float); }
+  else if (k == "adam_v") { src = tr->V; bytes = tr->n_par * sizeof(float); }
   else if (k == "mask") { src = tr->mask; bytes = static_cast<size_t>(tr->last_b) * kHidden; }
   else if (k == "batch_stats") { src = tr->stats; bytes = 3 * kHidden * sizeof(float); }
   else return fail("gnm_head_train_fetch: unknown buffer " + k);

@@ -178,7 +178,10 @@ head_bn_forward_kernel(const float* __restrict__ z, int B, const float* __restri
 }
 
 // Softmax, class-weighted cross-entropy and dZ2 = w_y (p - onehot(y)) / B of one row per warp (lane c = class c); the row's
-// loss w_y * (-log softmax(logits)_y) goes to row_loss[r].  log softmax_y = (l_y - max) - log(sum exp(l - max)).
+// loss w_y * (-log softmax(logits)_y) goes to row_loss[r].  With e_c = exp(l_c - max) and a the lowest lane holding the max
+// (e_a = 1), both are taken from sums that leave a term out, so neither cancels once the row is classified confidently
+// (values just below 1.0f are 2^-24 apart, so 1 - p_y and log(s) would keep only a few bits):
+//   s = 1 + sum_{c != a} e_c;  dZ2_y = -w (sum_{c != y} e_c) / s / B;  loss = w ((max - l_y) + log1p(sum_{c != a} e_c)).
 __global__ void __launch_bounds__(256)
 head_softmax_xent_kernel(const float* __restrict__ logits, int64_t n_rows, const int64_t* __restrict__ idx,
                          const int32_t* __restrict__ labels, const float* __restrict__ class_w, int B, int C,
@@ -191,19 +194,24 @@ head_softmax_xent_kernel(const float* __restrict__ logits, int64_t n_rows, const
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
   const float e = lane < C ? expf(l - m) : 0.f;
-  float s = e;
-#pragma unroll
-  for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+  const int a = __ffs(__ballot_sync(0xffffffffu, lane < C && l == m)) - 1;
   const int64_t row = idx[r];
   int y = (row >= 0 && row < n_rows) ? labels[row] : 0;       // a bad index is flagged by head_gather_kernel
   if (y < 0 || y >= C) {
     if (lane == 0) *bad |= kHeadBadLabel;
     y = 0;
   }
+  float sa = lane == a ? 0.f : e, sy = lane == y ? 0.f : e;   // sums over c != a and over c != y
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    sa += __shfl_xor_sync(0xffffffffu, sa, off);
+    sy += __shfl_xor_sync(0xffffffffu, sy, off);
+  }
+  const float s = 1.f + sa;
   const float w = class_w[y];
-  if (lane < C) dz2[static_cast<size_t>(r) * C + lane] = w * (e / s - (lane == y ? 1.f : 0.f)) / static_cast<float>(B);
+  if (lane < C) dz2[static_cast<size_t>(r) * C + lane] = w * (lane == y ? -(sy / s) : e / s) / static_cast<float>(B);
   const float ly = __shfl_sync(0xffffffffu, l, y);
-  if (lane == 0) row_loss[r] = w * -((ly - m) - logf(s));
+  if (lane == 0) row_loss[r] = w * ((m - ly) + log1pf(sa));
 }
 
 // One CTA of 64 threads: loss = sum_r row_loss[r] / B, db2[c] = sum_r dZ2[r][c], in row order (fp64).

@@ -1088,9 +1088,10 @@ class HeadTrainer:
         return {**_unflatten_head(flat, C_), "bn1m": mm, "bn1v": mv}
 
     def fetch(self, which: str):
-        """Test hook: the last step's "grad" (dict of gradients by short name), "mask" (uint8 [B, 512]) or "batch_stats"
-        (float32 [3, 512]: mu, 1 / sqrt(var + 1e-3), var)."""
-        if which == "grad":
+        """Test hook: the last step's "grad", "adam_m" or "adam_v" (dicts by short name: the gradients, the Adam moments after
+        the step), "mask" (uint8 [B, 512]) or "batch_stats" (float32 [3, 512]: mu, 1 / sqrt(var + 1e-3), var)."""
+        flat = which in ("grad", "adam_m", "adam_v")
+        if flat:
             out = np.empty(head_param_count(self.n_classes), np.float32)
         elif which == "mask":
             out = np.empty((getattr(self, "_last_b", 0), EMBED), np.uint8)
@@ -1098,7 +1099,7 @@ class HeadTrainer:
             out = np.empty((3, EMBED), np.float32)
         with self._torch.cuda.device(self.device):
             _check(self.lib, self.lib.gnm_head_train_fetch(self._tr, which.encode(), _ptr(out), self._stream()))
-        return _unflatten_head(out, self.n_classes) if which == "grad" else out
+        return _unflatten_head(out, self.n_classes) if flat else out
 
 
 def _unflatten_head(flat: np.ndarray, C_: int) -> Dict[str, np.ndarray]:

@@ -635,7 +635,9 @@ int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32
  *   dropout           keep(seed, step, row, col) = mix32(mix32(mix32(K(seed) ^ step) + row) + col) >= ceil(0.2 * 2^32),
  *                     mix32 = lowbias32, K(seed) = (seed * 0x9E3779B1 + 0x7F4A7C15) mod 2^32 (genomad_b200/synth.py),
  *                     step = the 0-based global step, row = the position in the batch; arithmetic mod 2^32
- *   loss              sum_i w[y_i] * (-log softmax(logits_i)[y_i]) / B  (log-softmax from the logits, max-shifted)
+ *   loss              sum_i w[y_i] * (-log softmax(logits_i)[y_i]) / B  (log-softmax from the logits, max-shifted:
+ *                     -log softmax_y = (max - l_y) + log1p(sum_{c != a} exp(l_c - max)), a the lowest class at the max; the
+ *                     gradient's target component is -sum_{c != y} p_c, never p_y - 1, so neither cancels when p_y is near 1)
  *   Adam              t = step + 1; m += (g - m)(1 - 0.9); v += (g^2 - v)(1 - 0.999);
  *                     p -= (m * lr sqrt(1 - 0.999^t) / (1 - 0.9^t)) / (sqrt(v) + 1e-7), over W1, b1, gamma, beta, W2, b2; no decay
  *   moving stats      mean = 0.99 mean + 0.01 mu;  var = 0.99 var + 0.01 var_batch (biased)
@@ -651,8 +653,9 @@ int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32
  *   row 0 / class 0), and the next gnm_head_train_step or gnm_head_train_read fails naming which; the trainer is then spent.
  * gnm_head_train_read: waits for `stream` and copies the parameters to HOST buffers (any may be NULL): h_params float
  *   [512*512 + 3*512 + 512*C + C] flat = W1, b1, gamma, beta, W2, b2; moving mean and variance [512]; the step count.
- * gnm_head_train_fetch (tests): HOST copy of the last step's "grad" (float, flat like h_params), "mask" (uint8 [B][512], 1 =
- *   kept) or "batch_stats" (float [3][512] = mu, 1 / sqrt(var + 1e-3), var).  Waits for `stream`.
+ * gnm_head_train_fetch (tests): HOST copy of the last step's "grad" (float, flat like h_params), "adam_m" and "adam_v" (the
+ *   Adam moments after the step, float, flat like h_params), "mask" (uint8 [B][512], 1 = kept) or "batch_stats" (float [3][512]
+ *   = mu, 1 / sqrt(var + 1e-3), var).  Waits for `stream`.
  */
 int gnm_head_train_create(int device, const gnm_head_weights* init, int max_batch, uint64_t seed, float learning_rate,
                           gnm_head_train** out);

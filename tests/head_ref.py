@@ -39,6 +39,64 @@ def softmax(l):
     return e / e.sum(1, keepdims=True)
 
 
+def xent(logits, labels):
+    """Per row -log softmax(logits)[y] and its gradient softmax(logits) - onehot(y) in fp64, each to full relative precision:
+    the loss is (max - l_y) + log1p(sum_{c != a} e^(l_c - max)), a the argmax, and the target component -sum_{c != y} p_c.
+    p_y - 1 and log(sum e^(l - max)) would cancel once the margin reaches about 37, where p_y == 1.0 in fp64."""
+    l = np.asarray(logits, np.float64)
+    r, y = np.arange(len(l)), np.asarray(labels)
+    m = l.max(1)
+    e = np.exp(l - m[:, None])
+    cls = np.arange(l.shape[1])[None, :]
+    s = e.sum(1)
+    g = e / s[:, None]
+    g[r, y] = -np.where(cls == y[:, None], 0.0, e).sum(1) / s
+    nll = (m - l[r, y]) + np.log1p(np.where(cls == l.argmax(1)[:, None], 0.0, e).sum(1))
+    return nll, g
+
+
+def _butterfly(v):
+    """The xor-shuffle sum of 32 float32 lanes (lanes past the row's classes hold 0), as every lane of the warp ends it."""
+    lanes = np.zeros((v.shape[0], 32), np.float32)
+    lanes[:, :v.shape[1]] = v
+    for off in (16, 8, 4, 2, 1):
+        lanes = lanes + lanes[:, np.arange(32) ^ off]
+    return lanes[:, 0]
+
+
+def xent_fp32(logits32, labels, cw, B: int):
+    """(row loss, dZ2) in float32 in head_softmax_xent_kernel's order: m = max, e = exp(l - m), a = the lowest class at m,
+    sa / sy = butterfly sums of e without class a / class y, s = 1 + sa; dZ2 = w (e / s) / B off the label and
+    w (-(sy / s)) / B at it; loss = w ((m - l_y) + log1p(sa)).  NumPy's float32 exp and log1p stand in for expf and log1pf."""
+    l = np.asarray(logits32, np.float32)
+    r, y = np.arange(len(l)), np.asarray(labels)
+    cls = np.arange(l.shape[1])[None, :]
+    m = l.max(1)
+    e = np.exp(l - m[:, None])
+    a = (l == m[:, None]).argmax(1)
+    sa = _butterfly(np.where(cls == a[:, None], np.float32(0), e))
+    sy = _butterfly(np.where(cls == y[:, None], np.float32(0), e))
+    s = np.float32(1) + sa
+    w = np.asarray(cw, np.float32)[y]
+    q = e / s[:, None]
+    q[r, y] = -(sy / s)
+    return w * ((m - l[r, y]) + np.log1p(sa)), w[:, None] * q / np.float32(B)
+
+
+def xent_fp32_cancelling(logits32, labels, cw, B: int):
+    """The same from the formula the kernel used before: dZ2 = w (e / s - onehot(y)) / B, loss = w -((l_y - m) - log(s)) with
+    s the butterfly sum of every e.  Both cancel once p_y is near 1."""
+    l = np.asarray(logits32, np.float32)
+    r, y = np.arange(len(l)), np.asarray(labels)
+    m = l.max(1)
+    e = np.exp(l - m[:, None])
+    s = _butterfly(e)
+    w = np.asarray(cw, np.float32)[y]
+    q = e / s[:, None]
+    q[r, y] -= np.float32(1)
+    return w * -((l[r, y] - m) - np.log(s)), w[:, None] * q / np.float32(B)
+
+
 def infer(a, X) -> np.ndarray:
     """Head in inference mode: float64 probabilities [n, C]."""
     f = {k: np.asarray(v, np.float64) for k, v in a.items()}
@@ -60,21 +118,17 @@ def forward(p, X, labels, cw, mask):
     y = f["bn1g"] * xh + f["bn1b"]
     h = np.maximum(y, 0) * mask / KEEP
     logits = h @ f["d2w"] + f["d2b"]
-    m = logits.max(1, keepdims=True)
-    lse = np.log(np.exp(logits - m).sum(1, keepdims=True))
-    logp = logits - m - lse
+    nll, g_logits = xent(logits, labels)
     w = np.asarray(cw, np.float64)[labels]
-    loss = float((w * -logp[np.arange(B), labels]).sum() / B)
-    return loss, dict(X=X, z=z, mu=mu, var=var, inv=inv, xh=xh, y=y, h=h, logp=logp, w=w, labels=labels, mask=mask, f=f)
+    loss = float((w * nll).sum() / B)
+    return loss, dict(X=X, z=z, mu=mu, var=var, inv=inv, xh=xh, y=y, h=h, logits=logits, nll=nll, g_logits=g_logits, w=w,
+                      labels=labels, mask=mask, f=f)
 
 
 def backward(c):
     """Gradients of the loss with respect to d1w, d1b, bn1g, bn1b, d2w, d2b."""
     B = c["X"].shape[0]
-    p = np.exp(c["logp"])
-    onehot = np.zeros_like(p)
-    onehot[np.arange(B), c["labels"]] = 1.0
-    dz2 = c["w"][:, None] * (p - onehot) / B
+    dz2 = c["w"][:, None] * c["g_logits"] / B
     g = {"d2w": c["h"].T @ dz2, "d2b": dz2.sum(0)}
     dh = dz2 @ c["f"]["d2w"].T
     dy = dh * c["mask"] / KEEP * (c["y"] > 0)

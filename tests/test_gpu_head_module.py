@@ -64,19 +64,55 @@ def test_shipped_head_through_nn_classification_is_bitwise(torch, tmp_path):
     assert np.array_equal(z["predictions"].view(np.uint32), main.view(np.uint32))
 
 
-def test_train_head_learns_composition_classes(torch, tmp_path):
-    from genomad_b200 import nn_classification as nnc, train_head
+def _print_margins(head_arrays, X, labels):
+    """How confidently the written head classifies its training windows: the log-odds margin of the labelled class,
+    mu = l_y - max_{c != y} l_c, from fp64 inference-mode logits.  Past mu ~ 9 a float32 p_y - 1 keeps only a few bits."""
+    f = {k: np.asarray(v, np.float64) for k, v in head_arrays.items()}
+    z = X.astype(np.float64) @ f["d1w"] + f["d1b"]
+    h = np.maximum((z - f["bn1m"]) / np.sqrt(f["bn1v"] + 1e-3) * f["bn1g"] + f["bn1b"], 0)
+    lg = h @ f["d2w"] + f["d2b"]
+    r = np.arange(len(lg))
+    mu = lg[r, labels] - np.where(np.arange(lg.shape[1])[None, :] == labels[:, None], -np.inf, lg).max(1)
+    edges = [-np.inf, 0, 9, 12, 17, 40, np.inf]
+    counts = np.histogram(mu, edges)[0]
+    print(f"training-window margins under the written head ({len(mu)} windows): median {np.median(mu):.1f}, "
+          f"p10 {np.quantile(mu, 0.1):.1f}, p90 {np.quantile(mu, 0.9):.1f}, max {mu.max():.1f}; "
+          + ", ".join(f"[{lo:g}, {hi:g}): {n}" for lo, hi, n in zip(edges[:-1], edges[1:], counts)))
+
+
+def test_train_head_learns_composition_classes(torch, tmp_path, monkeypatch):
+    from genomad_b200 import nn_classification as nnc, train_head, weights as W
     train_fa, test_fa = tmp_path / "train.fna", tmp_path / "test.fna"
     write_set(train_fa, 1, 60)
     truth = write_set(test_fa, 2, 20)
+    seen = {}
+    make = train_head._make_trainer
+
+    def spy(*args, **kwargs):            # records the training matrix, labels and batch rows of the first run
+        tr = make(*args, **kwargs)
+        step = tr.step
+
+        def recorded(X, idx, labels, cw, loss=None):
+            seen.setdefault("X", X)
+            seen.setdefault("labels", labels)
+            seen.setdefault("idx", []).append(idx.clone())
+            return step(X, idx, labels, cw, loss=loss)
+        tr.step = recorded
+        return tr
     runs = []
     for k in range(2):
         out = tmp_path / f"head{k}"
-        train_head.main(train_fa, str(train_fa) + ".labels.tsv", out, epochs=10, batch_size=256, seed=3, verbose=False)
+        with monkeypatch.context() as m:
+            if k == 0:
+                m.setattr(train_head, "_make_trainer", spy)
+            train_head.main(train_fa, str(train_fa) + ".labels.tsv", out, epochs=10, batch_size=256, seed=3, verbose=False)
         runs.append((out / "train_head.npz").read_bytes())
     assert runs[0] == runs[1], "two train-head runs wrote different head files"
     tsv = (tmp_path / "head0" / "train_head_training.tsv").read_text().splitlines()
     print("\n".join(tsv))
+    rows = torch.unique(torch.cat(seen["idx"])).cpu().numpy()
+    best = W.load_head(tmp_path / "head0" / "train_head.npz", W.load_weights())
+    _print_margins(best.arrays, seen["X"].cpu().numpy()[rows], seen["labels"].cpu().numpy()[rows])
     nnc.main(test_fa, tmp_path / "scored", False, 128, False, 2, False, False, head=tmp_path / "head0" / "train_head.npz")
     z = np.load(tmp_path / "scored" / "test_nn_classification" / "test_nn_classification_head.npz")
     names, preds, cls = z["contig_names"], z["predictions"], list(z["class_names"])

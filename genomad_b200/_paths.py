@@ -130,6 +130,40 @@ class NNOutputs:
     def provirus_nn_classification_head_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification_head.npz")
 
+    # ---- opt-in (--head with --both-strands), not a reference output: the head's scores of each strand and their mean
+    @property
+    def nn_classification_head_strands_output(self) -> Path:
+        return self._nn("nn_classification_head_strands.tsv")
+
+    @property
+    def nn_classification_head_strands_npz_output(self) -> Path:
+        return self._nn("nn_classification_head_strands.npz")
+
+    @property
+    def provirus_nn_classification_head_strands_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_strands.tsv")
+
+    @property
+    def provirus_nn_classification_head_strands_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_strands.npz")
+
+    # ---- opt-in (--head with --write-window-scores), not a reference output: the head's scores of every window
+    @property
+    def nn_classification_head_windows_output(self) -> Path:
+        return self._nn("nn_classification_head_windows.tsv")
+
+    @property
+    def nn_classification_head_windows_npz_output(self) -> Path:
+        return self._nn("nn_classification_head_windows.npz")
+
+    @property
+    def provirus_nn_classification_head_windows_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_windows.tsv")
+
+    @property
+    def provirus_nn_classification_head_windows_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_windows.npz")
+
     # ---- opt-in (--write-head-attributions), not a reference output: per-token input gradients of one of the head's classes
     @property
     def nn_classification_head_attributions_output(self) -> Path:

@@ -49,7 +49,9 @@ def cli():
 @click.option("--write-window-scores", is_flag=True, default=False, show_default=True,
               help="Also write the class scores of every window, with its coordinates in the sequence, to "
                    "<prefix>_nn_classification_windows.{tsv,npz}: where along a sequence the chromosome, plasmid and virus "
-                   "signal lies. Not an option of the reference.")
+                   "signal lies. With --head, the head's scores of the same windows also go to "
+                   "<prefix>_nn_classification_head_windows.{tsv,npz}; every other file is unchanged. Not an option of the "
+                   "reference.")
 @click.option("--window-stride", type=click.IntRange(1, 6000), default=None, show_default="6000",
               help="Write the window scores (implies --write-window-scores) for a 6,000-base window every N bases (overlapping "
                    "windows when N < 6000), a finer score profile. Sequence scores always use the reference's windows. Not an "
@@ -72,13 +74,16 @@ def cli():
 @click.option("--both-strands", is_flag=True, default=False, show_default=True,
               help="Also classify every sequence's reverse complement and write the scores of the forward strand, the reverse "
                    "strand and their mean to <prefix>_nn_classification_strands.{tsv,npz}; with --write-embeddings the "
-                   "embeddings file also gets embeddings_reverse and embeddings_both_strands. The main outputs are unchanged. "
-                   "About twice the GPU time. Not an option of the reference.")
+                   "embeddings file also gets embeddings_reverse and embeddings_both_strands. With --head, the head's scores "
+                   "of both strands and their mean also go to <prefix>_nn_classification_head_strands.{tsv,npz}. The main "
+                   "outputs are unchanged. About twice the GPU time. Not an option of the reference.")
 @click.option("--head", "head", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
               help="Also score every sequence with this classifier head (a train-head output, <prefix>_head.npz) and write "
                    "the scores of its classes to <prefix>_nn_classification_head.{tsv,npz}. The head must have been trained "
-                   "on this encoder (checked before any work). It scores the forward strand only, also with --both-strands. "
-                   "The main outputs are unchanged. Not an option of the reference.")
+                   "on this encoder (checked before any work). That file holds the forward strand's scores; with "
+                   "--both-strands the head also scores the reverse strand (<prefix>_nn_classification_head_strands.{tsv,npz}) "
+                   "and with --write-window-scores every window (<prefix>_nn_classification_head_windows.{tsv,npz}). The main "
+                   "outputs are unchanged. Not an option of the reference.")
 @click.option("--write-head-attributions", "write_head_attributions", metavar="CLASS", default=None,
               help="With --head: also write, for every window, the attributions of this class of the head (one of its "
                    "class names) to <prefix>_nn_classification_head_attributions.npz, as --write-attributions does for the "
@@ -128,20 +133,25 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
               help="balanced: class c weighs N / (C * N_c) in the loss, over the training windows; none: 1.")
 @click.option("--seed", type=click.IntRange(0), default=0, show_default=True,
               help="Seed of the initialisation, split, order and dropout (>= 0).")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Also train on the windows of every labelled sequence's reverse complement, so the head scores a sequence "
+                   "alike on either strand; the validation sequence accuracy then uses the strand-averaged scores that "
+                   "nn-classification --head --both-strands writes. About twice the embedding time and time per epoch.")
 @click.option("--threads", "-t", type=int, default=get_n_available_cpus(), show_default=True,
               help="Number of threads to use.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def train_head(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, threads,
-               verbose):
+def train_head(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, both_strands,
+               threads, verbose):
     """Train a classifier head for your own classes on the frozen encoder. LABELS is a TSV with the header
     seq_name<TAB>class and one row per labelled sequence of the INPUT FASTA (seq_name as nn-classification writes it).
     Writes <prefix>_head.npz (the epoch with the lowest validation loss), <prefix>_head_training.tsv and
     <prefix>_head_training.log to OUTPUT; score sequences with it by nn-classification --head. One GPU. Not a module of
     the reference."""
     from . import train_head as module
+    extra = {"both_strands": True} if both_strands else {}
     module.main(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, threads,
-                verbose)
+                verbose, **extra)
 
 
 @cli.command(name="embedding-neighbours", context_settings=CONTEXT_SETTINGS)

@@ -1,9 +1,10 @@
 // Per-window score table of nn-classification --write-window-scores (host code, part of libgnm.so).
 //
 // One line per window: "<seq_name>\t<start>\t<end>\t<chromosome>\t<plasmid>\t<virus>\n", start 1-based and end inclusive (the
-// convention of geNomad's provirus table).  Scores carry the digits Python's f"{float(x):.4f}" gives, which is what the
-// contig table uses: the float32 value, exactly, rounded half to even at the fourth decimal.  That rounding is done here in
-// integer arithmetic (no printf, so no locale and no libc rounding mode is involved).  A table can have hundreds of millions
+// convention of geNomad's provirus table); a classifier head's table (gnm_write_window_tsv_cols) has one score column per
+// class.  Scores carry the digits Python's f"{float(x):.4f}" gives, which is what the contig table uses: the float32 value,
+// exactly, rounded half to even at the fourth decimal.  That rounding is done here in integer arithmetic (no printf, so no
+// locale and no libc rounding mode is involved).  A table can have hundreds of millions
 // of rows: blocks of rows are formatted on `threads` threads and written in order.
 #include <algorithm>
 #include <atomic>
@@ -72,10 +73,12 @@ extern "C" int gnm_format_scores(const float* x, int64_t n, char* out, int64_t* 
   return 0;
 }
 
-extern "C" int gnm_write_window_tsv(const char* path, const char* header, const char* names, const int64_t* name_offsets,
-                                    int64_t n_contigs, const int32_t* win_offsets, const int64_t* starts,
-                                    const int32_t* lengths, const float* probs, int threads) {
+extern "C" int gnm_write_window_tsv_cols(const char* path, const char* header, const char* names,
+                                         const int64_t* name_offsets, int64_t n_contigs, const int32_t* win_offsets,
+                                         const int64_t* starts, const int32_t* lengths, const float* probs, int n_cols,
+                                         int threads) {
   if (!path || !header || !name_offsets || !win_offsets || n_contigs < 0) { g_tsv_err = "gnm_write_window_tsv: null argument"; return 1; }
+  if (n_cols < 1 || n_cols > 32) { g_tsv_err = "gnm_write_window_tsv: n_cols must be in [1, 32]"; return 1; }
   const int64_t n = win_offsets[n_contigs];
   if (n < 0 || (n > 0 && (!names || !starts || !lengths || !probs))) { g_tsv_err = "gnm_write_window_tsv: null argument"; return 1; }
   for (int64_t c = 0; c < n_contigs; ++c)
@@ -89,21 +92,22 @@ extern "C" int gnm_write_window_tsv(const char* path, const char* header, const 
   constexpr int64_t kRows = 1 << 16;                      // rows per block
   threads = std::max(1, threads);
   const int64_t n_blocks = (n + kRows - 1) / kRows;
+  // a row is at most nl + row_max bytes: name, 3 tabs + two 20-character coordinates, n_cols x (tab + <= 45-character score +
+  // snprintf's terminator), newline
+  const size_t row_max = 44 + 47 * static_cast<size_t>(n_cols);
   std::vector<std::string> buf(static_cast<size_t>(threads));
   for (int64_t b0 = 0; ok && b0 < n_blocks; b0 += threads) {
     const int nb = static_cast<int>(std::min<int64_t>(threads, n_blocks - b0));
     auto work = [&](int t) {
       const int64_t lo = (b0 + t) * kRows, hi = std::min(n, lo + kRows);
       std::string& s = buf[static_cast<size_t>(t)];
-      s.resize(static_cast<size_t>(hi - lo) * 200);         // grown below for long names
+      s.resize(static_cast<size_t>(hi - lo) * (152 + 16 * static_cast<size_t>(n_cols)));   // grown below for long rows
       size_t at = 0;
       int64_t c = std::upper_bound(win_offsets, win_offsets + n_contigs + 1, static_cast<int32_t>(lo)) - win_offsets - 1;
       for (int64_t w = lo; w < hi; ++w) {
         while (win_offsets[c + 1] <= w) ++c;
         const size_t nl = static_cast<size_t>(name_offsets[c + 1] - name_offsets[c]);
-        // a row is at most nl + 190 bytes: name, 3 tabs + two 20-character coordinates, 3 x (tab + <= 45-character score +
-        // snprintf's terminator), newline
-        if (s.size() < at + nl + 256) s.resize((at + nl + 256) * 2);
+        if (s.size() < at + nl + row_max + 64) s.resize((at + nl + row_max + 64) * 2);
         char* p = &s[at];
         std::memcpy(p, names + name_offsets[c], nl);
         p += nl;
@@ -111,7 +115,7 @@ extern "C" int gnm_write_window_tsv(const char* path, const char* header, const 
         p = std::to_chars(p, p + 24, starts[w] + 1).ptr;
         *p++ = '\t';
         p = std::to_chars(p, p + 24, starts[w] + lengths[w]).ptr;
-        for (int k = 0; k < 3; ++k) { *p++ = '\t'; p += format_score(probs[3 * w + k], p); }
+        for (int k = 0; k < n_cols; ++k) { *p++ = '\t'; p += format_score(probs[static_cast<int64_t>(n_cols) * w + k], p); }
         *p++ = '\n';
         at = static_cast<size_t>(p - s.data());
       }
@@ -126,4 +130,11 @@ extern "C" int gnm_write_window_tsv(const char* path, const char* header, const 
   if (std::fclose(fh) != 0) ok = false;
   if (!ok) { g_tsv_err = std::string("gnm_write_window_tsv: write to ") + path + " failed"; return 1; }
   return 0;
+}
+
+extern "C" int gnm_write_window_tsv(const char* path, const char* header, const char* names, const int64_t* name_offsets,
+                                    int64_t n_contigs, const int32_t* win_offsets, const int64_t* starts,
+                                    const int32_t* lengths, const float* probs, int threads) {
+  return gnm_write_window_tsv_cols(path, header, names, name_offsets, n_contigs, win_offsets, starts, lengths, probs, 3,
+                                   threads);
 }

@@ -151,6 +151,8 @@ EXPORTS = {
     "gnm_tsv_last_error": (C.c_char_p, []),
     "gnm_write_window_tsv": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_void_p, C.c_int]),
+    "gnm_write_window_tsv_cols": (C.c_int, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "gnm_format_scores": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_int64)]),
     "gnm_tfrecord_last_error": (C.c_char_p, []),
     "gnm_tfrecord_write": (C.c_int, [C.c_char_p, C.c_void_p, C.c_int64, C.c_int]),
@@ -315,8 +317,8 @@ def both_strands(forward, reverse):
 
 
 class WindowScores(NamedTuple):
-    """Result of Classifier.window_scores (cuda tensors)."""
-    probs: "object"           # float32 [W, 3] (chromosome, plasmid, virus)
+    """Result of Classifier.window_scores and Head.window_scores (cuda tensors)."""
+    probs: "object"           # float32 [W, 3] (chromosome, plasmid, virus); Head.window_scores: [W, C]
     contig: "object"          # int32 [W], index of the window's contig
     start: "object"           # int64 [W], first byte in the contig (0-based, before stripping n/N)
     length: "object"          # int32 [W], bytes of sequence (1..6000; the rest of the window is 'N' padding)
@@ -893,6 +895,41 @@ class Head:
             _check(self.lib, self.lib.gnm_head_forward(self.clf._h, self._hd, x.data_ptr(), x.shape[0], out.data_ptr(),
                                                        self.clf._stream()))
         return out
+
+    # ------------------------------------------------------------------ contigs in memory
+    def classify_contigs(self, seqs, single_window: bool = False, strand: str = "forward"):
+        """Classifier.classify_contigs for the head's classes: contigs in, cuda tensors (means float32 [n_contigs, C], window
+        counts int32 [n_contigs]) out.  The windows are planned on the device (Classifier.contig_windows), embedded
+        (Classifier.embed_windows), scored by predict and averaged per contig by segment_mean; a contig without a window has
+        count 0 and mean 0.  strand "reverse" scores each contig's reverse complement: bitwise the forward call on the
+        reverse-complemented contigs, and both_strands() combines the two calls' means."""
+        clf = self.clf
+        if strand not in ("forward", "reverse"):
+            raise ValueError(f"strand must be 'forward' or 'reverse', not {strand!r}")
+        rev = strand == "reverse"
+        seq, offs = clf.contig_buffers(seqs)
+        start, length, woff = clf.contig_windows(seq, offs, single_window, reverse=rev)
+        probs = self._window_probs(seq, start, length, rev)
+        return self.segment_mean(probs, woff), woff[1:] - woff[:-1]
+
+    def window_scores(self, seqs, stride: int = WINDOW) -> "WindowScores":
+        """Classifier.window_scores for the head's classes: WindowScores with probs float32 [W, C], the head's scores of every
+        window (a window every `stride` nt), and the same contig, start, length and offsets as Classifier.window_scores."""
+        clf, t = self.clf, self.clf._torch
+        seq, offs = clf.contig_buffers(seqs)
+        start, length, woff = clf.contig_windows(seq, offs, stride=stride)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        probs = self._window_probs(seq, start, length, False)
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        return WindowScores(probs, contig, rel, length, woff)
+
+    def _window_probs(self, seq, start, length, reverse):
+        t = self.clf._torch
+        if not start.numel():
+            return t.zeros((0, self.n_classes), dtype=t.float32, device=seq.device)
+        return self.predict(self.clf.embed_windows(seq, start, length, reverse=reverse)[1])
 
     # ------------------------------------------------------------------ attributions of the head's classes
     def class_index(self, target) -> int:

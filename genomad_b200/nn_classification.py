@@ -124,8 +124,10 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
 
     With `head` ({"head": engine.Head}), every chunk takes the embedding route and the head scores each window's embedding on
     the device into a buffer of this rank's shard; they are reduced per contig by the routes of the class scores (gather or
-    allreduce, any width) and stored as head["preds"] (float32 [n_contigs, C], identical on all ranks).  With
-    `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
+    allreduce, any width) and stored as head["preds"] (float32 [n_contigs, C], identical on all ranks).  With head["windows"]
+    true, those rows are also collected on rank 0 in window order, as the class scores are with `window_probs`, and stored as
+    head["window_preds"] (float32 [n_windows, C] on rank 0, None on the other ranks); with offsets None only that is done.
+    With `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -223,6 +225,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     if window_probs:
         full = gdist.collect_window_probs(local_t, n, info)
         out.append(full.cpu().numpy() if full is not None else None)
+    if scorer is not None and head.get("windows"):
+        full = gdist.collect_window_probs(d_head, n, info)
+        head["window_preds"] = full.cpu().numpy() if full is not None else None
     if attributions is not None:
         full = gdist.collect_window_probs(d_attr, n, info)
         attributions["attr"] = full.cpu().numpy() if full is not None else None
@@ -279,10 +284,11 @@ def window_scores_enabled() -> bool:
     return os.environ.get("GENOMAD_B200_WINDOW_SCORES", "0") not in ("", "0")
 
 
-def _write_window_tsv(path: Path, names, offsets, starts, lengths, probs, threads: int = 1) -> None:
+def _write_window_tsv(path: Path, names, offsets, starts, lengths, probs, threads: int = 1, header: str = _WINDOW_HEADER,
+                      n_cols: int = 3) -> None:
     """One row per window: name, 1-based start, inclusive end (in the record's sequence before stripping n/N), and the three
-    scores with the digits of f"{x:.4f}" -- formatted natively on `threads` threads (gnm_write_window_tsv): a profile can
-    have hundreds of millions of rows."""
+    scores (a head's table: its n_cols) with the digits of f"{x:.4f}" -- formatted natively on `threads` threads
+    (gnm_write_window_tsv[_cols]): a profile can have hundreds of millions of rows."""
     from . import engine
     lib = engine.load_library()
     blobs = [str(x).encode() for x in names]
@@ -294,9 +300,15 @@ def _write_window_tsv(path: Path, names, offsets, starts, lengths, probs, thread
     lengths = np.ascontiguousarray(lengths, dtype=np.int32)
     probs = np.ascontiguousarray(probs, dtype=np.float32)
     assert len(offsets) == len(blobs) + 1 and len(starts) == len(lengths) == len(probs) == offsets[-1]
-    rc = lib.gnm_write_window_tsv(str(path).encode(), _WINDOW_HEADER.encode(), blob, name_off.ctypes.data, len(blobs),
-                                  offsets.ctypes.data, starts.ctypes.data, lengths.ctypes.data, probs.ctypes.data,
-                                  max(1, int(threads)))
+    if n_cols == 3:
+        rc = lib.gnm_write_window_tsv(str(path).encode(), header.encode(), blob, name_off.ctypes.data, len(blobs),
+                                      offsets.ctypes.data, starts.ctypes.data, lengths.ctypes.data, probs.ctypes.data,
+                                      max(1, int(threads)))
+    else:
+        assert probs.size == len(starts) * n_cols
+        rc = lib.gnm_write_window_tsv_cols(str(path).encode(), header.encode(), blob, name_off.ctypes.data, len(blobs),
+                                           offsets.ctypes.data, starts.ctypes.data, lengths.ctypes.data, probs.ctypes.data,
+                                           int(n_cols), max(1, int(threads)))
     if rc != 0:
         raise RuntimeError(lib.gnm_tsv_last_error().decode())
 
@@ -311,6 +323,25 @@ def _write_window_scores(npz_path: Path, tsv_path: Path, names_key: str, names, 
                           "predictions": np.asarray(probs, dtype=np.float32).reshape(-1, 3),
                           "window_stride": np.int32(stride)})
     _write_window_tsv(tsv_path, names, offsets, starts, lengths, probs, threads)
+
+
+def _write_head_windows(npz_path: Path, tsv_path: Path, names_key: str, names, offsets, starts, lengths, preds, stride: int,
+                        class_names, head_sha: str, threads: int) -> None:
+    """<prefix>_nn_classification_head_windows.{npz,tsv}: the window-score files' windows and keys, with the head's scores
+    float32 [W, C] as predictions, plus class_names and head_sha256."""
+    C = len(class_names)
+    offsets = np.asarray(offsets, dtype=np.int32)
+    preds = np.asarray(preds, dtype=np.float32).reshape(-1, C)
+    np.savez(npz_path, **{names_key: names,
+                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+                          "window_start": np.asarray(starts, dtype=np.int64),
+                          "window_length": np.asarray(lengths, dtype=np.int32),
+                          "predictions": preds,
+                          "window_stride": np.int32(stride),
+                          "class_names": np.array(class_names),
+                          "head_sha256": np.str_(head_sha)})
+    header = "seq_name\tstart\tend\t" + "\t".join(f"{c}_score" for c in class_names) + "\n"
+    _write_window_tsv(tsv_path, names, offsets, starts, lengths, preds, threads, header=header, n_cols=C)
 
 
 def _window_scores_current(npz_path: Path, tsv_path: Path, stride: int) -> bool:
@@ -328,11 +359,14 @@ def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, i
                          attributions=None, head=None):
     """Per-contig scores (+ embeddings) and the per-window scores at `stride`: (preds, emb or None, offsets, starts, lengths,
     probs); the window arrays are None off rank 0.  At stride 6000 without --single-window the profile windows are the
-    contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list."""
+    contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list.
+    With `head`, the head's scores of the same windows are stored as head["window_preds"] (rank 0): the contig pass's own
+    rows, or the second pass's, which then takes the embedding route with the head (the same probabilities, bitwise)."""
     emb = None
     ak = {"attributions": attributions} if attributions is not None else {}      # option off: the call of before
     if head is not None:
         ak["head"] = head
+        head["windows"] = stride == sequence.WINDOW and not single_window
     if stride == sequence.WINDOW and not single_window:
         res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True, **ak)
         preds, probs = res[0], res[-1]
@@ -346,7 +380,12 @@ def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, i
         preds = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, **ak)
     wl = parsed.windows(stride)
     try:
-        probs = _classify_parsed(clf, wl, None, info, window_probs=True)
+        if head is not None:
+            profile = {"head": head["head"], "windows": True}
+            probs = _classify_parsed(clf, wl, None, info, window_probs=True, head=profile)
+            head["window_preds"] = profile["window_preds"]
+        else:
+            probs = _classify_parsed(clf, wl, None, info, window_probs=True)
         offsets, starts, lengths = wl.spans() if info.is_main else (None, None, None)
     finally:
         wl.close()
@@ -478,6 +517,34 @@ def _write_head(npz_path: Path, tsv_path: Path, names_key: str, names, preds, cl
             fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in row) + "\n")
 
 
+def _write_head_strands(npz_path: Path, tsv_path: Path, names_key: str, names, forward, reverse, class_names,
+                        head_sha: str) -> None:
+    """<prefix>_nn_classification_head_strands.{npz,tsv}: the head's float32 [n, C] per strand and their mean, laid out as the
+    strand files are (strand outermost, class innermost), plus class_names and head_sha256."""
+    from .engine import both_strands
+    C = len(class_names)
+    fwd = np.asarray(forward, dtype=np.float32).reshape(len(names), C)
+    rev = np.asarray(reverse, dtype=np.float32).reshape(len(names), C)
+    both = both_strands(fwd, rev)
+    np.savez_compressed(npz_path, **{names_key: names, "forward": fwd, "reverse": rev, "both_strands": both,
+                                     "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)})
+    with open(tsv_path, "w") as fout:
+        fout.write("seq_name\t" + "\t".join(f"{c}_score_{s}" for s in STRANDS for c in class_names) + "\n")
+        for name, a, b, c in zip(names, fwd, rev, both):
+            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in (*a, *b, *c)) + "\n")
+
+
+def _head_windows_current(npz_path: Path, tsv_path: Path, head_sha: str, stride: int) -> bool:
+    """Both head window files exist and were written for this head at this stride."""
+    if not _head_current(npz_path, tsv_path, head_sha):
+        return False
+    try:
+        with np.load(npz_path) as z:
+            return int(z["window_stride"]) == stride
+    except Exception:
+        return False
+
+
 def _head_current(npz_path: Path, tsv_path: Path, head_sha: str) -> bool:
     """Both head files exist and were written for the head file with this sha256."""
     if not (npz_path.exists() and tsv_path.exists()):
@@ -584,16 +651,25 @@ def _strands_current(npz_path: Path, tsv_path: Path, emb_path: Path, embeddings:
         return False
 
 
-def _classify_reverse(clf, parsed, single_window: bool, info, contig_reduce, embeddings: bool):
+def _classify_reverse(clf, parsed, single_window: bool, info, contig_reduce, embeddings: bool, head=None):
     """The reverse strand: the windows of every record's reverse complement (sequence.WindowList, reverse=True) through the
     forward pass's chunk loop, per-contig reduction, embedding carry chain and multi-GPU routes.  A record keeps its row: it
-    has at least one window on either strand.  Returns (preds, embeddings or None)."""
+    has at least one window on either strand.  Returns (preds, embeddings or None).  With `head` ({"head": engine.Head}), the
+    list takes the embedding route with the head, as the forward pass does, and the head's per-contig means of the reverse
+    windows are stored as head["reverse_preds"] (float32 [n_contigs, C], identical on all ranks)."""
     wl = parsed.windows(sequence.WINDOW, single_window, reverse=True)
+    hk = {}
+    if head is not None:
+        hk["head"] = rev_head = {"head": head["head"]}
     try:
         offsets = wl.spans()[0]
         if embeddings:
-            return _classify_parsed(clf, wl, offsets, info, contig_reduce, embeddings=True)
-        return _classify_parsed(clf, wl, offsets, info, contig_reduce), None
+            res = _classify_parsed(clf, wl, offsets, info, contig_reduce, embeddings=True, **hk)
+        else:
+            res = _classify_parsed(clf, wl, offsets, info, contig_reduce, **hk), None
+        if head is not None:
+            head["reverse_preds"] = rev_head["preds"]
+        return res
     finally:
         wl.close()
 
@@ -706,6 +782,14 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         files += [outputs.nn_classification_head_output, outputs.nn_classification_head_npz_output]
         descr += ["classification by the --head classifier: tabular format",
                   "classification by the --head classifier: binary format"]
+    if head is not None and strands:
+        files += [outputs.nn_classification_head_strands_output, outputs.nn_classification_head_strands_npz_output]
+        descr += ["classification of both strands by the --head classifier: tabular format",
+                  "classification of both strands by the --head classifier: binary format"]
+    if head is not None and write_window_scores:
+        files += [outputs.nn_classification_head_windows_output, outputs.nn_classification_head_windows_npz_output]
+        descr += ["window classification by the --head classifier: tabular format",
+                  "window classification by the --head classifier: binary format"]
     if head_attr_target:
         files.append(outputs.nn_classification_head_attributions_output)
         descr.append(f"window attributions of the --head classifier ({head_attr_target}{attr_method}): binary format")
@@ -731,6 +815,16 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             files += [outputs.provirus_nn_classification_head_output, outputs.provirus_nn_classification_head_npz_output]
             descr += ["provirus classification by the --head classifier: tabular format",
                       "provirus classification by the --head classifier: binary format"]
+        if head is not None and strands:
+            files += [outputs.provirus_nn_classification_head_strands_output,
+                      outputs.provirus_nn_classification_head_strands_npz_output]
+            descr += ["provirus classification of both strands by the --head classifier: tabular format",
+                      "provirus classification of both strands by the --head classifier: binary format"]
+        if head is not None and write_window_scores:
+            files += [outputs.provirus_nn_classification_head_windows_output,
+                      outputs.provirus_nn_classification_head_windows_npz_output]
+            descr += ["provirus window classification by the --head classifier: tabular format",
+                      "provirus window classification by the --head classifier: binary format"]
         if head_attr_target:
             files.append(outputs.provirus_nn_classification_head_attributions_output)
             descr.append(f"provirus window attributions of the --head classifier ({head_attr_target}{attr_method}): "
@@ -770,7 +864,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output,
              outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output,
              outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output,
-             outputs.nn_classification_head_attributions_output)]
+             outputs.nn_classification_head_attributions_output,
+             outputs.nn_classification_head_strands_npz_output, outputs.nn_classification_head_strands_output,
+             outputs.nn_classification_head_windows_npz_output, outputs.nn_classification_head_windows_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
@@ -779,7 +875,11 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                      outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output,
                      outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output,
                      outputs.provirus_nn_classification_head_npz_output, outputs.provirus_nn_classification_head_output,
-                     outputs.provirus_nn_classification_head_attributions_output))
+                     outputs.provirus_nn_classification_head_attributions_output,
+                     outputs.provirus_nn_classification_head_strands_npz_output,
+                     outputs.provirus_nn_classification_head_strands_output,
+                     outputs.provirus_nn_classification_head_windows_npz_output,
+                     outputs.provirus_nn_classification_head_windows_output))
 
     plan = None
     info_writer = None
@@ -799,13 +899,17 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
         # (with embeddings or window scores requested, a classification whose embeddings file is missing, or whose window
         # scores are missing or were written at another stride, or whose attributions are missing or were written for another
-        # class, or whose strand files are missing, is redone: same predictions, bit for bit)
+        # class, or whose strand files are missing, or whose head files are missing or were written for another head or
+        # stride, is redone: same predictions, bit for bit)
         plan = [(bool(skip and j[4].exists()),
                  bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
                       and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
                       and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))
                       and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))
                       and (head_file is None or _head_current(j[16], j[17], head_sha))
+                      and (head_file is None or not strands or _head_current(j[19], j[20], head_sha))
+                      and (head_file is None or not write_window_scores
+                           or _head_windows_current(j[21], j[22], head_sha, window_stride))
                       and (not head_attr_target
                            or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))))
                 for j in jobs]
@@ -860,7 +964,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
          win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path,
-         head_attr_path), \
+         head_attr_path, head_strands_npz_path, head_strands_tsv_path, head_win_npz_path, head_win_tsv_path), \
             (enc_skip, cls_skip), (parsed, index) \
             in zip(jobs, plan, staged):
         names = preds = emb = None
@@ -872,7 +976,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             attr = {"target": head_attr_target, "head": True,
                     **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
         win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
-        hd = None                       # --head: the chunk loop also scores every window with the head (forward strand)
+        hd = None                       # --head: the chunk loop also scores every window with the head
         label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
         # ---- classify
         if cls_skip:
@@ -892,7 +996,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     sys.exit(1)
                 names, preds = index.names, np.zeros((len(index.names), 3), np.float32)
                 if head_file is not None:
-                    hd = {"preds": np.zeros((len(index.names), len(head_file.class_names)), np.float32)}
+                    C = len(head_file.class_names)
+                    hd = {"preds": np.zeros((len(index.names), C), np.float32), "window_preds": np.zeros((0, C), np.float32)}
+                    hd["reverse_preds"] = hd["preds"]
                 emb = np.zeros((len(index.names), 512), np.float32)
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
@@ -916,7 +1022,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     attr["spans"] = (index.offsets, *parsed.spans()) if is_main else None
                 if strands:
                     rev_preds, rev_emb = _classify_reverse(classifier(), parsed, single_window, info, contig_reduce,
-                                                           write_embeddings)
+                                                           write_embeddings, head=hd)
                 last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
                 names = index.names
             console.log(f"{'Sequences' if what == 'sequence' else 'Proviruses'} classified.")
@@ -936,12 +1042,24 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                 if is_main:
                     _write_head(head_npz_path, head_tsv_path, names_key, names, hd["preds"], head_file.class_names, head_sha)
                 console.log(f"{label} classification by the head written to {head_tsv_path.name} and {head_npz_path.name}.")
+                if strands:
+                    if is_main:
+                        _write_head_strands(head_strands_npz_path, head_strands_tsv_path, names_key, names, hd["preds"],
+                                            hd["reverse_preds"], head_file.class_names, head_sha)
+                    console.log(f"{label} classification of both strands by the head written to "
+                                f"{head_strands_tsv_path.name} and {head_strands_npz_path.name}.")
             if write_window_scores:
                 if is_main:
                     _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,
                                          threads or 1)
                 console.log(f"{label} window scores (stride {window_stride}) written to {win_tsv_path.name} and "
                             f"{win_npz_path.name}.")
+                if hd is not None:
+                    if is_main:
+                        _write_head_windows(head_win_npz_path, head_win_tsv_path, names_key, names, *win[:3],
+                                            hd["window_preds"], window_stride, head_file.class_names, head_sha, threads or 1)
+                    console.log(f"{label} window scores of the head (stride {window_stride}) written to "
+                                f"{head_win_tsv_path.name} and {head_win_npz_path.name}.")
             if attr is not None and head_attr_target:
                 if is_main:
                     _write_attributions(head_attr_path, names_key, names, *attr["spans"], head_attr_target, attr["attr"],

@@ -9,6 +9,11 @@ head is then trained on that matrix (engine.HeadTrainer, include/gnm.h for the e
 inference mode: Keras' fit would also run the encoder's SpatialDropout layers, here the embeddings are computed once and cached,
 which is what makes training cheap.  The head of the epoch with the lowest validation loss is written as
 <prefix>_head.npz, for ``nn-classification --head``.
+
+With ``--both-strands`` the windows of the same records' reverse complements (nn-classification --both-strands' reverse list)
+are embedded too, into rows after the forward ones, and take the same labels: the head then learns from both strands, the
+split stays by sequence (both strands of a sequence on the same side), and a validation sequence is scored by the mean of its
+two strands' scores, as ``nn-classification --head --both-strands`` reports it.
 """
 from __future__ import annotations
 
@@ -182,9 +187,10 @@ def _make_head(clf, head_file):
 
 def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int = 256, learning_rate: float = 1e-3,
          validation_fraction: float = 0.1, class_weight: str = "balanced", seed: int = 0, threads=None,
-         verbose: bool = True) -> None:
+         verbose: bool = True, both_strands: bool = False) -> None:
     import torch
     from . import nn_classification as nnc
+    from .engine import both_strands as both_strands_mean
     input_path, output_path = Path(input_path), Path(output_path)
     info = gdist.dist_info_from_env()
     if info.world_size > 1:
@@ -210,6 +216,7 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
         sys.exit(1)
     C = len(class_names)
     parsed = sequence.ParsedFasta(input_path, False, threads)
+    rev_list = None
     try:
         if not parsed.check():
             console.error(f"{input_path} is either empty or contains multiple entries with the same identifier.")
@@ -238,22 +245,34 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
             console.error(f"class(es) without a sequence that has a window: {_listed(missing)}")
             sys.exit(1)
         val_seq = split_sequences(seq_class, C, validation_fraction, seed)
-        # rows of X: the windows of the used records only, in file order
-        source = RecordWindows(parsed, offsets, used)
-        local = np.zeros(len(used) + 1, np.int64)
-        np.cumsum(counts[used], out=local[1:])
-        rows = [np.arange(local[i], local[i + 1]) for i in range(len(used))]
-        train_rows = np.concatenate([rows[i] for i in np.nonzero(~val_seq)[0]]).astype(np.int64)
-        val_idx = np.nonzero(val_seq)[0]
-        val_rows = (np.concatenate([rows[i] for i in val_idx]) if len(val_idx) else np.zeros(0)).astype(np.int64)
-        win_class = np.repeat(seq_class, counts[used]).astype(np.int32)
+        # rows of X: the windows of the used records only, in file order; with both strands, then the same records' reverse
+        # windows in file order (a record can have another number of windows on that strand: the N rule)
+        strand_lists = [(RecordWindows(parsed, offsets, used), counts[used])]
+        if both_strands:
+            rev_list = parsed.windows(sequence.WINDOW, False, reverse=True)
+            rev_offsets = np.asarray(rev_list.spans()[0], np.int64)
+            strand_lists.append((RecordWindows(rev_list, rev_offsets, used), np.diff(rev_offsets)[used]))
+        rows, base = [], 0                          # rows[k][i]: the rows of X of strand k of used record i
+        for _, n_win in strand_lists:
+            local = np.zeros(len(used) + 1, np.int64)
+            np.cumsum(n_win, out=local[1:])
+            rows.append([base + np.arange(local[i], local[i + 1]) for i in range(len(used))])
+            base += int(local[-1])
+        train_idx, val_idx = np.nonzero(~val_seq)[0], np.nonzero(val_seq)[0]
+        train_rows = np.concatenate([r[i] for r in rows for i in train_idx]).astype(np.int64)
+        val_rows = (np.concatenate([r[i] for r in rows for i in val_idx]) if len(val_idx) else np.zeros(0)).astype(np.int64)
+        win_class = np.concatenate([np.repeat(seq_class, n_win) for _, n_win in strand_lists]).astype(np.int32)
         cw = class_weights(win_class[train_rows], C, class_weight)
         console.log(f"{C} classes ({', '.join(class_names)}); {len(used)} sequences: {int((~val_seq).sum())} for training "
                     f"({len(train_rows)} windows), {len(val_idx)} for validation ({len(val_rows)} windows); class weights "
                     + ", ".join(f"{x:.6g}" for x in cw) + ".")
+        if both_strands:
+            console.log("Training on both strands: every sequence's forward windows "
+                        f"({strand_lists[0][0].n_windows} in all) and the windows of its reverse complement "
+                        f"({strand_lists[1][0].n_windows}); validation sequences are scored by the mean of their two strands.")
 
         clf = _make_classifier(0)
-        W = source.n_windows
+        W = sum(src.n_windows for src, _ in strand_lists)
         if W * EMBED_BYTES > 0.9 * _free_bytes(clf):
             console.error(f"the embeddings of {W} windows ({W * EMBED_BYTES / 2**30:.1f} GiB) do not fit in the GPU's free "
                           "memory; train on fewer sequences")
@@ -261,8 +280,13 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
         dev = torch.device("cuda", clf.device) if torch.cuda.is_available() else torch.device("cpu")
         X = torch.empty((W, 512), dtype=torch.float32, device=dev)
         console.log(f"Computing the encoder embeddings of {W} windows.")
-        nnc._classify_parsed(clf, source, None, info, window_embeddings=X)
+        row = 0
+        for src, _ in strand_lists:
+            nnc._classify_parsed(clf, src, None, info, window_embeddings=X[row: row + src.n_windows])
+            row += src.n_windows
     finally:
+        if rev_list is not None:
+            rev_list.close()
         parsed.close()
 
     enc_w = _weights.load_weights()
@@ -271,9 +295,13 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
     labels_d = torch.from_numpy(win_class).to(dev)
     cw_d = torch.from_numpy(cw).to(dev)
     Xv = X[torch.from_numpy(val_rows).to(dev)] if len(val_rows) else None
-    v_off = np.zeros(len(val_idx) + 1, np.int32)
-    np.cumsum([len(rows[i]) for i in val_idx], out=v_off[1:])
-    v_off_d = torch.from_numpy(v_off).to(dev)
+    # validation rows are strand by strand; v_off[k] delimits strand k's windows of each validation sequence
+    v_off, at = [], 0
+    for r in rows:
+        o = np.zeros(len(val_idx) + 1, np.int32)
+        np.cumsum([len(r[i]) for i in val_idx], out=o[1:])
+        v_off.append((at, torch.from_numpy(o).to(dev)))
+        at += int(o[-1])
     N = len(train_rows)
     steps = -(-N // batch_size)
     sizes = torch.tensor([min(batch_size, N - s * batch_size) for s in range(steps)], dtype=torch.float64)
@@ -291,7 +319,8 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
             if Xv is not None:
                 head = _make_head(clf, _weights.HeadFile(arrays, class_names, enc_sha))
                 probs = head.predict(Xv)
-                seq_probs = head.segment_mean(probs, v_off_d).cpu().numpy()
+                means = [head.segment_mean(probs[a: a + int(o[-1])], o) for a, o in v_off]
+                seq_probs = (means[0] if len(means) == 1 else both_strands_mean(*means)).cpu().numpy()
                 metrics = validation_metrics(probs.cpu().numpy(), win_class[val_rows], seq_probs, seq_class[val_idx], cw)
                 head.close()
             tsv.write(f"{epoch}\t{train_loss:.6f}\t{metrics[0]:.6f}\t{metrics[1]:.6f}\t{metrics[2]:.6f}\n")

@@ -311,12 +311,17 @@ int gnm_fasta_spans(const gnm_fasta* f, int64_t* starts, int32_t* lengths);
  *   win_offsets int32 [n_contigs + 1] (CSR); probs float [win_offsets[n_contigs]][3].  Scores carry exactly the digits of
  *   Python's f"{float(x):.4f}" (the float value rounded half to even at the fourth decimal; no locale).  Rows are formatted on
  *   `threads` threads and written in order.
+ * gnm_write_window_tsv_cols: the same table with n_cols scores per row (1 <= n_cols <= 32; probs float
+ *   [win_offsets[n_contigs]][n_cols]): the per-window scores of a C-class head.  gnm_write_window_tsv is its n_cols = 3 case.
  * gnm_format_scores: the same score formatting, one value per line into out (<= 49 bytes per value); *out_len = bytes written.
  */
 const char* gnm_tsv_last_error(void);
 int gnm_write_window_tsv(const char* path, const char* header, const char* names, const int64_t* name_offsets, int64_t n_contigs,
                          const int32_t* win_offsets, const int64_t* starts, const int32_t* lengths, const float* probs,
                          int threads);
+int gnm_write_window_tsv_cols(const char* path, const char* header, const char* names, const int64_t* name_offsets,
+                              int64_t n_contigs, const int32_t* win_offsets, const int64_t* starts, const int32_t* lengths,
+                              const float* probs, int n_cols, int threads);
 int gnm_format_scores(const float* x, int64_t n, char* out, int64_t* out_len);
 
 /* ---- TFRecord files of tokenised windows (host side, no GPU involved; off by default) ------ */

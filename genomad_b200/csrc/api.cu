@@ -2079,6 +2079,18 @@ static int head_check_weights(const char* fn, const gnm_head_weights* w) {
   if (w->n_classes < 2 || w->n_classes > kHeadMaxClasses)
     return fail(std::string(fn) + ": n_classes must be in [2, " + std::to_string(kHeadMaxClasses) + "], not " +
                 std::to_string(w->n_classes));
+  const size_t C = static_cast<size_t>(w->n_classes), H = kHidden;
+  const struct { const char* name; const float* p; size_t n; } arrays[] = {
+      {"dense1_kernel", w->dense1_kernel, H * H}, {"dense1_bias", w->dense1_bias, H}, {"bn1.gamma", w->bn1.gamma, H},
+      {"bn1.beta", w->bn1.beta, H}, {"bn1.moving_mean", w->bn1.moving_mean, H}, {"bn1.moving_variance", w->bn1.moving_variance, H},
+      {"dense2_kernel", w->dense2_kernel, H * C}, {"dense2_bias", w->dense2_bias, C}};
+  for (const auto& a : arrays)
+    for (size_t i = 0; i < a.n; ++i)
+      if (!std::isfinite(a.p[i])) return fail(std::string(fn) + ": " + a.name + " not finite at index " + std::to_string(i));
+  // fold_bn's 1 / sqrt(var + 1e-3f) is NaN or infinite unless var + 1e-3f > 0 (in fp32, as fold_bn computes it)
+  for (size_t i = 0; i < H; ++i)
+    if (!(w->bn1.moving_variance[i] + 1e-3f > 0.f))
+      return fail(std::string(fn) + ": bn1.moving_variance + 1e-3 is not > 0 at unit " + std::to_string(i));
   return 0;
 }
 

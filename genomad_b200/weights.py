@@ -174,6 +174,9 @@ def _check_head_arrays(arrays, C: int) -> Dict[str, np.ndarray]:
             raise ValueError(f"{path}: shape {a.shape}, expected {shape}")
         if not np.isfinite(a).all():
             raise ValueError(f"{path}: not all finite")
+        if short == "bn1v" and not (a + np.float32(1e-3) > 0).all():
+            # inference folds 1 / sqrt(var + 1e-3) into the BN scale: NaN or infinite otherwise
+            raise ValueError(f"{path}: moving variance + 1e-3 must be > 0 (unit {int(np.flatnonzero(~(a + np.float32(1e-3) > 0))[0])})")
         out[short] = np.ascontiguousarray(a)
     return out
 

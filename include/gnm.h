@@ -610,7 +610,9 @@ typedef struct gnm_head_train gnm_head_train;   /* gnm_head: declared with the h
 
 /*
  * Upload a head for inference on handle h's device.  BN is folded into scale and shift and dense_1 split into TF32 halves with
- * the host code gnm_create uses for the shipped head.  Synchronous.
+ * the host code gnm_create uses for the shipped head.  Refuses (naming the array and index) an array that is not finite, and a
+ * moving variance with var + 1e-3 <= 0 in fp32, where the folded scale 1 / sqrt(var + 1e-3) would be NaN or infinite;
+ * gnm_head_train_create refuses the same.  Synchronous.
  */
 int gnm_head_create(gnm_handle* h, const gnm_head_weights* w, gnm_head** out);
 int gnm_head_destroy(gnm_head* head);

@@ -195,6 +195,24 @@ def embedding_clusters(input, output, min_similarity, both_strands, verbose):
     module.main(input, output, min_similarity, verbose, both_strands=both_strands)
 
 
+@cli.command(name="window-regions", context_settings=CONTEXT_SETTINGS)
+@click.argument("windows", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("--mean-region-length", type=click.FloatRange(12000), required=True,
+              help="Mean length, in bases, of a region of one class (>= 12,000): sets the switch rate between classes per "
+                   "stride to stride / L. No default: no region length has been measured to suit this model.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def window_regions(windows, output, mean_region_length, verbose):
+    """Call class regions along each sequence of the WINDOWS file (nn-classification --write-window-scores output,
+    <prefix>_nn_classification_windows.npz, a head's <prefix>_nn_classification_head_windows.npz, or their provirus_ twins)
+    by an HMM decode of its window-score profile, and write them with coordinates and posterior confidence to the OUTPUT
+    directory as <prefix>_nn_classification[_head]_regions.{tsv,npz}. Runs in one process on one GPU (not a torchrun job).
+    Not a module of the reference."""
+    from . import window_regions as module
+    module.main(windows, output, mean_region_length, verbose)
+
+
 @cli.command(name="aggregated-classification", context_settings=CONTEXT_SETTINGS)
 @click.argument("input", type=click.Path(path_type=Path, exists=True))
 @click.argument("output", type=click.Path(path_type=Path))

@@ -26,6 +26,7 @@
 #include "neighbours.cuh"
 #include "clusters.cuh"
 #include "head.cuh"
+#include "regions.cuh"
 
 using namespace gnm;
 
@@ -2059,6 +2060,63 @@ extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uin
     GNM_CUDA(cudaGetLastError());
   }
   cl_resolve_kernel<<<1, kClThreads, 0, st>>>(mask, n, words, d_covered, d_new_reps, d_n_new);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ window regions (regions.cuh)
+// Workspace: gamma (alpha-hat during the forward pass) fp64 [W][C], then the traceback data uint32 [W] and uint16 [W].
+static size_t wr_mask_offset(int64_t n, int C) { return nb_align(static_cast<size_t>(n) * C * 8); }
+static size_t wr_idx_offset(int64_t n, int C) { return wr_mask_offset(n, C) + nb_align(static_cast<size_t>(n) * 4); }
+
+extern "C" size_t gnm_window_regions_workspace_bytes(int64_t n_windows, int C) {
+  if (n_windows < 0 || n_windows > INT32_MAX || C < 2 || C > kWrMaxClasses) {
+    fail("gnm_window_regions_workspace_bytes: need 0 <= n_windows < 2^31 and 2 <= C <= 32, not n_windows = " +
+         std::to_string(n_windows) + ", C = " + std::to_string(C));
+    return 0;
+  }
+  return wr_idx_offset(n_windows, C) + nb_align(static_cast<size_t>(n_windows) * 2);
+}
+
+extern "C" int gnm_window_regions(const float* d_scores, int64_t n_windows, int C, const int32_t* d_offsets, int n_seqs,
+                                  const int64_t* d_start, const int32_t* d_length, int stride, double mean_region_length,
+                                  float* d_posterior, int32_t* d_state, uint8_t* d_region_first, int64_t* d_region_start,
+                                  int64_t* d_region_end, int32_t* d_region_windows, float* d_region_posterior,
+                                  float* d_region_scores, void* d_work, size_t work_bytes, void* stream) {
+  const char* fn = "gnm_window_regions";
+  if (C < 2 || C > kWrMaxClasses) return fail(std::string(fn) + ": C must be in [2, 32], not " + std::to_string(C));
+  if (stride < 1 || stride > kWindow) return fail(std::string(fn) + ": stride must be in [1, 6000], not " + std::to_string(stride));
+  if (!(mean_region_length >= 12000.0))
+    return fail(std::string(fn) + ": mean_region_length must be >= 12000, not " + std::to_string(mean_region_length));
+  if (n_windows < 0 || n_windows > INT32_MAX || n_seqs < 0)
+    return fail(std::string(fn) + ": need 0 <= n_windows < 2^31 and n_seqs >= 0, not " + std::to_string(n_windows) + ", " +
+                std::to_string(n_seqs));
+  if (n_seqs == 0 || n_windows == 0) return 0;
+  if (!d_offsets) return fail(std::string(fn) + ": null buffer");
+  if (n_windows > 0 && (!d_scores || !d_start || !d_length || !d_posterior || !d_state || !d_region_first || !d_region_start ||
+                        !d_region_end || !d_region_windows || !d_region_posterior || !d_region_scores || !d_work))
+    return fail(std::string(fn) + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(std::string(fn) + ": d_work must be 256-byte aligned");
+  const size_t need = gnm_window_regions_workspace_bytes(n_windows, C);
+  if (work_bytes < need)
+    return fail(std::string(fn) + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(need) +
+                " needed (gnm_window_regions_workspace_bytes)");
+  WrParams p;
+  p.scores = d_scores; p.offsets = d_offsets; p.start = d_start; p.length = d_length;
+  p.n_seqs = n_seqs; p.C = C; p.stride = stride;
+  const double rho = stride / mean_region_length;
+  p.tau = stride / 6000.0;
+  p.log1p_mq = std::log1p(-rho * C / (C - 1));
+  p.inv_c = 1.0 / C;
+  p.log_c = std::log(static_cast<double>(C));
+  p.posterior = d_posterior; p.state = d_state; p.first = d_region_first; p.r_start = d_region_start; p.r_end = d_region_end;
+  p.r_windows = d_region_windows; p.r_posterior = d_region_posterior; p.r_scores = d_region_scores;
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  p.gam = reinterpret_cast<double*>(w);
+  p.bp_mask = reinterpret_cast<uint32_t*>(w + wr_mask_offset(n_windows, C));
+  p.bp_idx = reinterpret_cast<uint16_t*>(w + wr_idx_offset(n_windows, C));
+  GNM_CUDA(cudaFuncSetAttribute(wr_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWrSmem));
+  wr_decode_kernel<<<(n_seqs + kWrWarps - 1) / kWrWarps, kWrWarps * 32, kWrSmem, static_cast<cudaStream_t>(stream)>>>(p);
   GNM_CUDA(cudaGetLastError());
   return 0;
 }

@@ -119,6 +119,10 @@ EXPORTS = {
     "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]),
+    "gnm_window_regions_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "gnm_window_regions": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                     C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "gnm_head_create": (C.c_int, [C.c_void_p, C.POINTER(_HeadW), C.POINTER(C.c_void_p)]),
     "gnm_head_destroy": (C.c_int, [C.c_void_p]),
     "gnm_head_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
@@ -323,6 +327,108 @@ class WindowScores(NamedTuple):
     start: "object"           # int64 [W], first byte in the contig (0-based, before stripping n/N)
     length: "object"          # int32 [W], bytes of sequence (1..6000; the rest of the window is 'N' padding)
     offsets: "object"         # int32 [n_contigs + 1], CSR: the windows of contig c are [offsets[c], offsets[c+1])
+
+
+class WindowRegions(NamedTuple):
+    """Result of window_regions (cuda tensors); R regions in window order."""
+    posterior: "object"          # float32 [W, C], forward-backward posterior of every class at every window
+    state: "object"              # int32 [W], the Viterbi path
+    region_contig: "object"      # int32 [R]
+    region_start: "object"       # int64 [R], 0-based, in the contig's bytes as given (before stripping n/N)
+    region_end: "object"         # int64 [R], exclusive
+    region_class: "object"       # int32 [R]
+    region_windows: "object"     # int32 [R]
+    region_posterior: "object"   # float32 [R], mean posterior of the region's class over its windows
+    region_scores: "object"      # float32 [R, C], mean window score of every class
+
+
+REGIONS_MIN_LENGTH = 12000       # mean region length L >= 2 * 6000, so the switch rate s / L is at most 0.5 at every stride
+REGIONS_WORK_BYTES = 1 << 30     # workspace per gnm_window_regions call; a call takes whole sequences (at least one)
+
+
+def regions_mean_length(mean_region_length) -> float:
+    """L as a float; ValueError below REGIONS_MIN_LENGTH or not finite."""
+    L = float(mean_region_length)
+    if not (np.isfinite(L) and L >= REGIONS_MIN_LENGTH):
+        raise ValueError(f"mean_region_length must be a finite number >= {REGIONS_MIN_LENGTH}, not {mean_region_length}")
+    return L
+
+
+def window_regions(ws: "WindowScores", stride: int, mean_region_length, *, work_bytes: int = REGIONS_WORK_BYTES) -> "WindowRegions":
+    """Class regions along each sequence from its window-score profile (gnm_window_regions, include/gnm.h; DESIGN.md, "Window
+    regions"): the Viterbi path and forward-backward posteriors of a C-state HMM over the windows, and the maximal runs of the
+    path as regions.
+
+    ws: Classifier.window_scores or Head.window_scores output as it is (C = ws.probs.shape[1], 2..32); stride: the stride it
+    was computed at (1..6000); mean_region_length: L >= 12000 bases.  The windows are checked on the device first (finite
+    scores; within a sequence, starts increasing by positive multiples of the stride) and decoded in calls of whole sequences
+    whose workspace fits work_bytes (a longer sequence gets a call of its own).  A sequence's results depend only on its own
+    windows, so they are bitwise the same whatever the chunking or the other sequences."""
+    import torch as t
+    stride = int(stride)
+    if not 1 <= stride <= WINDOW:
+        raise ValueError(f"stride must be in [1, {WINDOW}], not {stride}")
+    L = regions_mean_length(mean_region_length)
+    probs, contig, start, length, offsets = ws
+    if probs.dim() != 2 or not 2 <= probs.shape[1] <= 32:
+        raise ValueError(f"scores must be [W, C] with 2 <= C <= 32, not {list(probs.shape)}")
+    W, C_ = probs.shape
+    dev = probs.device
+    assert probs.is_cuda and probs.dtype == t.float32, "probs: float32 cuda tensor expected"
+    assert contig.shape == (W,) and start.shape == (W,) and length.shape == (W,), "contig, start, length: [W] expected"
+    probs = probs.contiguous()
+    contig = contig.to(device=dev, dtype=t.int32).contiguous()
+    start = start.to(device=dev, dtype=t.int64).contiguous()
+    length = length.to(device=dev, dtype=t.int32).contiguous()
+    offsets = offsets.to(device=dev, dtype=t.int32).contiguous()
+    offs = offsets.cpu().numpy().astype(np.int64)
+    if offs.ndim != 1 or offs.size < 1 or offs[0] != 0 or offs[-1] != W or (np.diff(offs) < 0).any():
+        raise ValueError(f"offsets must be a non-decreasing CSR from 0 to {W}")
+    if W:
+        same = contig[1:] == contig[:-1]
+        d = start[1:] - start[:-1]
+        bad = t.stack([~t.isfinite(probs).all(), (same & ((d <= 0) | (d % stride != 0))).any(), (length < 1).any(),
+                       (contig != t.repeat_interleave(t.arange(offs.size - 1, dtype=t.int32, device=dev),
+                                                      offsets[1:] - offsets[:-1], output_size=W)).any()]).cpu().numpy()
+        for flag, msg in zip(bad, ("scores are not all finite",
+                                   f"window starts do not increase by positive multiples of the stride {stride} within a sequence",
+                                   "a window length is < 1", "contig does not match offsets")):
+            if flag:
+                raise ValueError(msg)
+    posterior = t.empty((W, C_), dtype=t.float32, device=dev)
+    state = t.empty(W, dtype=t.int32, device=dev)
+    first = t.zeros(W, dtype=t.uint8, device=dev)
+    r_start = t.empty(W, dtype=t.int64, device=dev)
+    r_end = t.empty(W, dtype=t.int64, device=dev)
+    r_windows = t.empty(W, dtype=t.int32, device=dev)
+    r_post = t.empty(W, dtype=t.float32, device=dev)
+    r_scores = t.empty((W, C_), dtype=t.float32, device=dev)
+    lib = load_library()
+    max_windows = max(1, (int(work_bytes) - 768) // (8 * C_ + 6))      # gnm_window_regions_workspace_bytes, include/gnm.h
+    with t.cuda.device(dev):
+        stream = t.cuda.current_stream(dev).cuda_stream
+        work = t.empty(0, dtype=t.uint8, device=dev)
+        n_seqs, a = offs.size - 1, 0
+        while a < n_seqs:
+            # the longest run of whole sequences from a whose windows fit, at least one sequence
+            b = max(a + 1, int(np.searchsorted(offs, offs[a] + max_windows, side="right")) - 1)
+            b = min(b, n_seqs)
+            w0, nw = int(offs[a]), int(offs[b] - offs[a])
+            if nw:
+                need = int(lib.gnm_window_regions_workspace_bytes(nw, C_))
+                if need == 0:
+                    _check(lib, 1)
+                if need > work.numel():
+                    work = t.empty(need, dtype=t.uint8, device=dev)
+                _check(lib, lib.gnm_window_regions(
+                    probs[w0:].data_ptr(), nw, C_, offsets[a:].data_ptr(), b - a, start[w0:].data_ptr(),
+                    length[w0:].data_ptr(), stride, L, posterior[w0:].data_ptr(), state[w0:].data_ptr(), first[w0:].data_ptr(),
+                    r_start[w0:].data_ptr(), r_end[w0:].data_ptr(), r_windows[w0:].data_ptr(), r_post[w0:].data_ptr(),
+                    r_scores[w0:].data_ptr(), work.data_ptr(), work.numel(), stream))
+            a = b
+    rows = t.nonzero(first).flatten()
+    return WindowRegions(posterior, state, contig[rows], r_start[rows], r_end[rows], state[rows], r_windows[rows], r_post[rows],
+                         r_scores[rows])
 
 
 class Attributions(NamedTuple):

@@ -595,6 +595,44 @@ int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_cov
                       int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream);
 
 /*
+ * Window regions: an HMM decode of each sequence's window-score profile (nn-classification --write-window-scores, or a head's)
+ * into class regions.  No handle, no allocation: the current device and `stream`, the caller's workspace.  Asynchronous.
+ * DESIGN.md, "Window regions" states the model; in short, for sequence windows w = 0..n-1 with scores p_w in R^C, starts a_w,
+ * lengths l_w, stride s and mean region length L:
+ *   states      one per class, uniform start;  emission eps_w(k) = (s / 6000) ln max(p_w(k), 1e-30)
+ *   transition  rho = s / L, lambda = 1 - rho C / (C - 1), g_w = (a_w - a_{w-1}) / s;  stay T_g = 1/C + (1 - 1/C) lambda^g,
+ *               move to a given other class (1 - T_g) / (C - 1)
+ *   outputs     forward-backward posteriors gamma_w(k) and the Viterbi path (ties: stay, then the lowest class; the final state
+ *               the lowest class); a region is a maximal run of equal path states, from a_0 or the floor of the midpoint of the
+ *               neighbouring window centres c = a + floor(l / 2), to the next such midpoint or a_{n-1} + l_{n-1}.
+ * All recursions run in fp64.  A sequence's results depend only on its own windows: bitwise the same in any call or order.
+ *
+ *   d_scores       DEVICE float [n_windows][C], finite (not checked: the caller validates)
+ *   d_offsets      DEVICE int32 [n_seqs + 1], non-decreasing: sequence i has the rows [d_offsets[i], d_offsets[i+1]) - d_offsets[0]
+ *                  of every per-window buffer, so a call can take any run of whole sequences of a larger CSR
+ *   d_start        DEVICE int64 [n_windows]: 0-based first base; within a sequence increasing by positive multiples of `stride`
+ *                  (not checked: a violation gives wrong results, never an out-of-bounds access)
+ *   d_length       DEVICE int32 [n_windows]: bases of sequence in the window, >= 1
+ *   d_posterior    DEVICE float [n_windows][C]: gamma;  d_state DEVICE int32 [n_windows]: the Viterbi path
+ *   d_region_first DEVICE uint8 [n_windows]: 1 at the first window of each region, 0 elsewhere.  At those rows only:
+ *                  d_region_start / d_region_end DEVICE int64 (0-based, end exclusive), d_region_windows DEVICE int32 (window
+ *                  count), d_region_posterior DEVICE float (mean gamma of the region's class, an fp64 sum in window order),
+ *                  d_region_scores DEVICE float [n_windows][C] (mean score of every class, fp64 sums in window order); the
+ *                  region's class is d_state at that row.  Compacting the flagged rows in order gives the region table.
+ *   2 <= C <= 32, 1 <= stride <= 6000, mean_region_length >= 12000 (so rho <= 0.5), 0 <= n_windows < 2^31; any other value or a
+ *   null buffer (when n_windows > 0) fails without launching.
+ *
+ * gnm_window_regions_workspace_bytes: the bytes of d_work (256-byte aligned) a call with n_windows windows of C classes needs
+ *   (0 on invalid arguments): 8 C + 6 bytes per window, each part rounded up to 256 bytes.
+ */
+size_t gnm_window_regions_workspace_bytes(int64_t n_windows, int C);
+int gnm_window_regions(const float* d_scores, int64_t n_windows, int C, const int32_t* d_offsets, int n_seqs,
+                       const int64_t* d_start, const int32_t* d_length, int stride, double mean_region_length, float* d_posterior,
+                       int32_t* d_state, uint8_t* d_region_first, int64_t* d_region_start, int64_t* d_region_end,
+                       int32_t* d_region_windows, float* d_region_posterior, float* d_region_scores, void* d_work,
+                       size_t work_bytes, void* stream);
+
+/*
  * Classifier heads: the layers the reference trains on the frozen encoder (create_classifier, model.py:34-45), with C classes
  * instead of 3.  DESIGN.md, "Classifier heads".  Host pointers, Keras layouts; 2 <= n_classes <= 32.
  */

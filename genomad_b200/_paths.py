@@ -164,6 +164,23 @@ class NNOutputs:
     def provirus_nn_classification_head_windows_npz_output(self) -> Path:
         return self._nn("provirus_nn_classification_head_windows.npz")
 
+    # ---- opt-in (--head with a head that carries a novelty model), not a reference output: distance to the head's classes
+    @property
+    def nn_classification_head_novelty_output(self) -> Path:
+        return self._nn("nn_classification_head_novelty.tsv")
+
+    @property
+    def nn_classification_head_novelty_npz_output(self) -> Path:
+        return self._nn("nn_classification_head_novelty.npz")
+
+    @property
+    def provirus_nn_classification_head_novelty_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_novelty.tsv")
+
+    @property
+    def provirus_nn_classification_head_novelty_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_novelty.npz")
+
     # ---- opt-in (--write-head-attributions), not a reference output: per-token input gradients of one of the head's classes
     @property
     def nn_classification_head_attributions_output(self) -> Path:

@@ -137,12 +137,16 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
               help="Also train on the windows of every labelled sequence's reverse complement, so the head scores a sequence "
                    "alike on either strand; the validation sequence accuracy then uses the strand-averaged scores that "
                    "nn-classification --head --both-strands writes. About twice the embedding time and time per epoch.")
+@click.option("--novelty", is_flag=True, default=False, show_default=True,
+              help="Also fit a novelty model (one Gaussian per class with a shared covariance, on the training windows' "
+                   "embeddings) and calibrate it on the validation sequences, so nn-classification --head flags sequences "
+                   "far from every class (<prefix>_nn_classification_head_novelty.{tsv,npz}). Needs a validation fraction > 0.")
 @click.option("--threads", "-t", type=int, default=get_n_available_cpus(), show_default=True,
               help="Number of threads to use.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
 def train_head(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, both_strands,
-               threads, verbose):
+               novelty, threads, verbose):
     """Train a classifier head for your own classes on the frozen encoder. LABELS is a TSV with the header
     seq_name<TAB>class and one row per labelled sequence of the INPUT FASTA (seq_name as nn-classification writes it).
     Writes <prefix>_head.npz (the epoch with the lowest validation loss), <prefix>_head_training.tsv and
@@ -150,6 +154,8 @@ def train_head(input, labels, output, epochs, batch_size, learning_rate, validat
     the reference."""
     from . import train_head as module
     extra = {"both_strands": True} if both_strands else {}
+    if novelty:
+        extra["novelty"] = True
     module.main(input, labels, output, epochs, batch_size, learning_rate, validation_fraction, class_weight, seed, threads,
                 verbose, **extra)
 

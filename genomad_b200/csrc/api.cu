@@ -27,6 +27,7 @@
 #include "clusters.cuh"
 #include "head.cuh"
 #include "regions.cuh"
+#include "novelty.cuh"
 
 using namespace gnm;
 
@@ -1442,6 +1443,7 @@ struct gnm_head {
   float *d1w = nullptr, *d1b = nullptr, *scale = nullptr, *shift = nullptr, *dwT_hi = nullptr, *dwT_lo = nullptr;
   float *d2w = nullptr, *d2b = nullptr;
   CUtensorMap tm_b[2];
+  double *nv_center = nullptr, *nv_whitening = nullptr, *nv_means = nullptr;   // novelty model (gnm_head_set_novelty)
 };
 
 // The head on the tensor cores from the TF32 halves of its input in hA_hi[1] / hA_lo[1] (dense layer 0's epilogue leaves h1's
@@ -2225,6 +2227,151 @@ extern "C" int gnm_head_segment_mean(gnm_handle* h, const float* d_probs, int C,
 extern "C" int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32_t* d_offsets, int n_contigs,
                                     float* d_sum, void* stream) {
   return head_segment_any(h, d_probs, C, d_offsets, n_contigs, d_sum, stream, false);
+}
+
+// ---- novelty (novelty.cuh)
+// Workspace of gnm_novelty_fit, in this order (each part 256-byte aligned): status, class-sum partials [blocks][C][512] fp64 and
+// counts [blocks][C], class means [C][512], center [512], counts [C], scatter partials [chunks][36][64][64] fp64, S, L and P
+// [512][512] fp64, whitened means [C][512].
+struct NvLayout {
+  size_t status, part, cnt, mu, center, counts, spart, S, L, P, m, total;
+  int n_blocks, n_chunks;
+};
+static NvLayout nv_layout(int64_t n_fit, int C) {
+  NvLayout l;
+  l.n_blocks = static_cast<int>((n_fit + kNvSumRows - 1) / kNvSumRows);
+  l.n_chunks = static_cast<int>((n_fit + kNvChunk - 1) / kNvChunk);
+  const size_t H = kHidden, c = static_cast<size_t>(C), nb = l.n_blocks, nc = l.n_chunks;
+  size_t o = 0;
+  l.status = o; o += nb_align(sizeof(NvStatus));
+  l.part = o; o += nb_align(nb * c * H * 8);
+  l.cnt = o; o += nb_align(nb * c * 8);
+  l.mu = o; o += nb_align(c * H * 8);
+  l.center = o; o += nb_align(H * 8);
+  l.counts = o; o += nb_align(c * 8);
+  l.spart = o; o += nb_align(nc * kNvTriTiles * kNvTile * kNvTile * 8);
+  l.S = o; o += nb_align(H * H * 8);
+  l.L = o; o += nb_align(H * H * 8);
+  l.P = o; o += nb_align(H * H * 8);
+  l.m = o; o += nb_align(c * H * 8);
+  l.total = o;
+  return l;
+}
+
+extern "C" size_t gnm_novelty_fit_workspace_bytes(int64_t n_fit, int C) {
+  if (n_fit < 1 || n_fit > (int64_t(1) << 40) || C < 2 || C > kNvMaxClasses) {
+    fail("gnm_novelty_fit_workspace_bytes: need 1 <= n_fit <= 2^40 and 2 <= C <= 32, not n_fit = " + std::to_string(n_fit) +
+         ", C = " + std::to_string(C));
+    return 0;
+  }
+  return nv_layout(n_fit, C).total;
+}
+
+extern "C" int gnm_novelty_fit(gnm_handle* h, const float* d_X, int64_t n_rows, const int64_t* d_idx, int64_t n_fit,
+                               const int32_t* d_labels, int C, double* h_center, double* h_whitening, double* h_means,
+                               double* h_min_pivot, double* h_class_means, double* h_scatter, void* d_work, size_t work_bytes,
+                               void* stream) {
+  const std::string fn = "gnm_novelty_fit";
+  if (!h) return fail(fn + ": null handle");
+  if (C < 2 || C > kNvMaxClasses) return fail(fn + ": C must be in [2, 32], not " + std::to_string(C));
+  if (n_fit < 1) return fail(fn + ": no fit row");
+  if (n_rows < 1) return fail(fn + ": n_rows must be >= 1");
+  if (!d_X || !d_idx || !d_labels || !d_work) return fail(fn + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(fn + ": d_work must be 256-byte aligned");
+  const size_t need = gnm_novelty_fit_workspace_bytes(n_fit, C);
+  if (need == 0) return 1;
+  if (work_bytes < need)
+    return fail(fn + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(need) +
+                " needed (gnm_novelty_fit_workspace_bytes)");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const NvLayout l = nv_layout(n_fit, C);
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  NvStatus* status = reinterpret_cast<NvStatus*>(w + l.status);
+  double *part = reinterpret_cast<double*>(w + l.part), *mu = reinterpret_cast<double*>(w + l.mu);
+  double *center = reinterpret_cast<double*>(w + l.center), *spart = reinterpret_cast<double*>(w + l.spart);
+  double *S = reinterpret_cast<double*>(w + l.S), *L = reinterpret_cast<double*>(w + l.L), *P = reinterpret_cast<double*>(w + l.P);
+  double* m = reinterpret_cast<double*>(w + l.m);
+  long long *cnt = reinterpret_cast<long long*>(w + l.cnt), *counts = reinterpret_cast<long long*>(w + l.counts);
+  GNM_CUDA(cudaMemsetAsync(status, 0, sizeof(NvStatus), st));
+  const int sum_smem = C * kHidden * 8;
+  GNM_CUDA(cudaFuncSetAttribute(nv_class_sums_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, sum_smem));
+  nv_class_sums_kernel<<<l.n_blocks, kHidden, sum_smem, st>>>(d_X, n_rows, d_idx, d_labels, n_fit, C, part, cnt, status);
+  if (check_launch(h, "nv_class_sums_kernel")) return 1;
+  nv_means_kernel<<<C + 1, kHidden, 0, st>>>(part, cnt, l.n_blocks, C, n_fit, mu, center, counts, status);
+  if (check_launch(h, "nv_means_kernel")) return 1;
+  nv_scatter_kernel<<<dim3(kNvTriTiles, l.n_chunks), kNvThreads, 0, st>>>(d_X, n_rows, d_idx, d_labels, n_fit, C, mu, spart, status);
+  if (check_launch(h, "nv_scatter_kernel")) return 1;
+  nv_scatter_reduce_kernel<<<dim3(kNvTriTiles, kNvTile * kNvTile / 256), 256, 0, st>>>(spart, l.n_chunks, n_fit, S);
+  if (check_launch(h, "nv_scatter_reduce_kernel")) return 1;
+  nv_factor_kernel<<<1, kNvFactorThreads, 0, st>>>(S, L, status);
+  if (check_launch(h, "nv_factor_kernel")) return 1;
+  nv_inverse_kernel<<<kHidden / 128, 128, 0, st>>>(L, P, status);
+  if (check_launch(h, "nv_inverse_kernel")) return 1;
+  nv_whiten_means_kernel<<<C, kHidden, 0, st>>>(P, mu, center, m, status);
+  if (check_launch(h, "nv_whiten_means_kernel")) return 1;
+  NvStatus hs;
+  GNM_CUDA(cudaMemcpyAsync(&hs, status, sizeof(NvStatus), cudaMemcpyDeviceToHost, st));
+  GNM_CUDA(cudaStreamSynchronize(st));
+  switch (hs.code) {
+    case kNvOk: break;
+    case kNvBadIndex: return fail(fn + ": a fit row index is outside [0, n_rows)");
+    case kNvBadLabel: return fail(fn + ": a fit row's label is outside [0, C)");
+    case kNvEmptyClass: return fail(fn + ": class " + std::to_string(hs.arg) + " has no fit row");
+    case kNvNoVariation: return fail(fn + ": the training windows have no within-class variation (tr S = 0)");
+    case kNvBadPivot:
+      return fail(fn + ": the shrunk covariance has a non-positive Cholesky pivot at column " + std::to_string(hs.arg));
+    default: return fail(fn + ": unknown status " + std::to_string(hs.code));
+  }
+  const size_t H = kHidden;
+  if (h_center) GNM_CUDA(cudaMemcpy(h_center, center, H * 8, cudaMemcpyDeviceToHost));
+  if (h_whitening) GNM_CUDA(cudaMemcpy(h_whitening, P, H * H * 8, cudaMemcpyDeviceToHost));
+  if (h_means) GNM_CUDA(cudaMemcpy(h_means, m, static_cast<size_t>(C) * H * 8, cudaMemcpyDeviceToHost));
+  if (h_class_means) GNM_CUDA(cudaMemcpy(h_class_means, mu, static_cast<size_t>(C) * H * 8, cudaMemcpyDeviceToHost));
+  if (h_scatter) GNM_CUDA(cudaMemcpy(h_scatter, S, H * H * 8, cudaMemcpyDeviceToHost));
+  if (h_min_pivot) *h_min_pivot = hs.min_pivot;
+  return 0;
+}
+
+extern "C" int gnm_head_set_novelty(gnm_handle* h, gnm_head* hd, const double* center, const double* whitening,
+                                    const double* means) {
+  const std::string fn = "gnm_head_set_novelty";
+  if (!h || !hd) return fail(fn + ": null handle");
+  if (!center || !whitening || !means) return fail(fn + ": null array");
+  const size_t H = kHidden, C = static_cast<size_t>(hd->C);
+  for (size_t i = 0; i < H; ++i)
+    if (!std::isfinite(center[i])) return fail(fn + ": center not finite at index " + std::to_string(i));
+  for (size_t i = 0; i < C * H; ++i)
+    if (!std::isfinite(means[i])) return fail(fn + ": means not finite at index " + std::to_string(i));
+  for (size_t i = 0; i < H; ++i)
+    for (size_t j = 0; j < H; ++j) {
+      const double v = whitening[i * H + j];
+      if (!std::isfinite(v)) return fail(fn + ": whitening not finite at (" + std::to_string(i) + ", " + std::to_string(j) + ")");
+      if (j > i && v != 0.0) return fail(fn + ": whitening is not lower triangular at (" + std::to_string(i) + ", " + std::to_string(j) + ")");
+      if (j == i && !(v > 0.0)) return fail(fn + ": whitening diagonal is not positive at " + std::to_string(i));
+    }
+  GNM_CUDA(cudaSetDevice(h->device));
+  if (!hd->nv_center) {
+    if (dev_alloc(hd, &hd->nv_center, H) || dev_alloc(hd, &hd->nv_whitening, H * H) || dev_alloc(hd, &hd->nv_means, C * H)) return 1;
+  }
+  GNM_CUDA(cudaMemcpy(hd->nv_center, center, H * 8, cudaMemcpyHostToDevice));
+  GNM_CUDA(cudaMemcpy(hd->nv_whitening, whitening, H * H * 8, cudaMemcpyHostToDevice));
+  GNM_CUDA(cudaMemcpy(hd->nv_means, means, C * H * 8, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+extern "C" int gnm_head_novelty(gnm_handle* h, const gnm_head* hd, const float* d_embed, int n, float* d_dist, void* stream) {
+  if (!h || !hd) return fail("gnm_head_novelty: null handle");
+  if (!hd->nv_center) return fail("gnm_head_novelty: the head has no novelty model (gnm_head_set_novelty)");
+  if (n < 0) return fail("gnm_head_novelty: negative row count");
+  if (n == 0) return 0;
+  if (!d_embed || !d_dist) return fail("gnm_head_novelty: null buffer");
+  GNM_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  GNM_CUDA(cudaFuncSetAttribute(nv_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kNvScoreSmem));
+  nv_score_kernel<<<(n + kNvTile - 1) / kNvTile, kNvThreads, kNvScoreSmem, st>>>(d_embed, n, hd->nv_center, hd->nv_whitening,
+                                                                               hd->nv_means, hd->C, d_dist);
+  return check_launch(h, "nv_score_kernel");
 }
 
 // ---- training

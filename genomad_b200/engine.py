@@ -128,6 +128,12 @@ EXPORTS = {
     "gnm_head_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_head_segment_mean": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_head_segment_sum": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "gnm_novelty_fit_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "gnm_novelty_fit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                  C.c_void_p]),
+    "gnm_head_set_novelty": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_head_novelty": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "gnm_head_train_create": (C.c_int, [C.c_int, C.POINTER(_HeadW), C.c_int, C.c_uint64, C.c_float, C.POINTER(C.c_void_p)]),
     "gnm_head_train_destroy": (C.c_int, [C.c_void_p]),
     "gnm_head_train_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
@@ -959,6 +965,67 @@ def head_param_count(C: int) -> int:
     return EMBED * EMBED + 3 * EMBED + EMBED * C + C
 
 
+class NoveltyFit(NamedTuple):
+    """A fitted novelty model (gnm_novelty_fit, include/gnm.h): center [512], whitening P [512, 512] (lower triangular),
+    means [C, 512] (whitened class means m_c), all float64; the smallest Cholesky pivot; and, with stats=True, the class means
+    mu_c [C, 512] and the scatter S [512, 512] (None otherwise)."""
+    center: np.ndarray
+    whitening: np.ndarray
+    means: np.ndarray
+    min_pivot: float
+    class_means: Optional[np.ndarray] = None
+    scatter: Optional[np.ndarray] = None
+
+
+def novelty_fit(clf: "Classifier", X, rows, labels, n_classes: int, stats: bool = False) -> NoveltyFit:
+    """Fit the novelty model on rows `rows` (int64 cuda [N]) of X (float32 cuda [n_rows, 512]) with labels (int32 cuda
+    [n_rows], the label of each row of X), on clf's device.  GnmError on an empty class, no within-class variation or a
+    non-positive pivot."""
+    t = clf._torch
+    assert X.dtype == t.float32 and X.dim() == 2 and X.shape[1] == EMBED and X.is_cuda and X.is_contiguous()
+    assert rows.dtype == t.int64 and labels.dtype == t.int32 and labels.numel() == X.shape[0]
+    C_ = int(n_classes)
+    n = int(rows.numel())
+    need = int(clf.lib.gnm_novelty_fit_workspace_bytes(max(n, 1), C_))
+    if need == 0:
+        raise GnmError(clf.lib.gnm_last_error().decode(errors="replace"))
+    work = t.empty(need + 256, dtype=t.uint8, device=X.device)
+    base = (-work.data_ptr()) % 256
+    center, whitening, means = np.empty(EMBED), np.empty((EMBED, EMBED)), np.empty((C_, EMBED))
+    mu = np.empty((C_, EMBED)) if stats else None
+    S = np.empty((EMBED, EMBED)) if stats else None
+    piv = C.c_double()
+    with t.cuda.device(clf.device):
+        _check(clf.lib, clf.lib.gnm_novelty_fit(clf._h, X.data_ptr(), X.shape[0], rows.contiguous().data_ptr(), n,
+                                                labels.contiguous().data_ptr(), C_, _ptr(center), _ptr(whitening),
+                                                _ptr(means), C.byref(piv), _ptr(mu) if stats else None,
+                                                _ptr(S) if stats else None, work.data_ptr() + base, need, clf._stream()))
+    return NoveltyFit(center, whitening, means, piv.value, mu, S)
+
+
+def novelty_scores(dist, counts, calibration):
+    """Per-sequence novelty from the per-contig mean window distances dist (float32 [n, C]), the window counts [n] and the
+    head's sorted calibration values (float32): (novelty float32 [n] = min_c dist, nearest_class int32 [n] = the argmin,
+    lowest index on ties, p_value float64 [n] = (1 + #{v in calibration : v >= novelty}) / (1 + |calibration|)).  A sequence
+    without a window gets novelty NaN, nearest_class -1 and p NaN."""
+    dist = np.asarray(dist, dtype=np.float32)
+    counts = np.asarray(counts).reshape(-1)
+    cal = np.asarray(calibration, dtype=np.float32).reshape(-1)
+    n = len(counts)
+    assert dist.ndim == 2 and len(dist) == n
+    has = counts > 0
+    nov = np.full(n, np.nan, np.float32)
+    nearest = np.full(n, -1, np.int32)
+    p = np.full(n, np.nan, np.float64)
+    if has.any():
+        d = dist[has]
+        nearest[has] = d.argmin(1)
+        nov[has] = d.min(1)
+        ge = len(cal) - np.searchsorted(cal, nov[has], side="left")
+        p[has] = (1.0 + ge) / (1.0 + len(cal))
+    return nov, nearest, p
+
+
 class Head:
     """A C-class head (weights.HeadFile, or a dict with arrays / class_names) on a Classifier's device and workspace: encoder
     embeddings -> class probabilities (gnm_head_forward), per-contig means and sums (gnm_head_segment_*).  Follows the
@@ -977,6 +1044,50 @@ class Head:
             msg = self.lib.gnm_last_error().decode(errors="replace")
             self.close()
             raise GnmError(msg)
+        self.calibration = None
+        nov = getattr(head, "novelty", None)
+        if nov is not None:
+            self.set_novelty(nov["novelty_center"], nov["novelty_whitening"], nov["novelty_means"], nov["novelty_calibration"])
+
+    @property
+    def has_novelty(self) -> bool:
+        return getattr(self, "_nv", None) is not None
+
+    def set_novelty(self, center, whitening, means, calibration=None):
+        """Attach a novelty model (float64 center [512], whitening [512, 512] lower triangular, whitened means [C, 512];
+        gnm_head_set_novelty) and, when given, its sorted float32 calibration values."""
+        self._nv = tuple(np.ascontiguousarray(a, dtype=np.float64) for a in (center, whitening, means))
+        assert self._nv[0].shape == (EMBED,) and self._nv[1].shape == (EMBED, EMBED) and self._nv[2].shape == (self.n_classes, EMBED)
+        with self.clf._torch.cuda.device(self.clf.device):
+            _check(self.lib, self.lib.gnm_head_set_novelty(self.clf._h, self._hd, *(_ptr(a) for a in self._nv)))
+        self.calibration = None if calibration is None else np.asarray(calibration, dtype=np.float32)
+
+    def novelty(self, embeddings, out=None):
+        """float32 cuda [n, 512] -> float32 [n, C]: each row's whitened squared distance to every class mean / 512
+        (gnm_head_novelty), into `out` when given."""
+        t = self.clf._torch
+        x = embeddings.contiguous()
+        assert x.dtype == t.float32 and x.dim() == 2 and x.shape[1] == EMBED and x.is_cuda
+        if out is None:
+            out = t.empty((x.shape[0], self.n_classes), dtype=t.float32, device=x.device)
+        assert out.shape == (x.shape[0], self.n_classes) and out.is_contiguous() and out.dtype == t.float32
+        if x.shape[0]:
+            _check(self.lib, self.lib.gnm_head_novelty(self.clf._h, self._hd, x.data_ptr(), x.shape[0], out.data_ptr(),
+                                                       self.clf._stream()))
+        return out
+
+    def novelty_contigs(self, seqs, single_window: bool = False):
+        """Contigs in, cuda tensors (per-contig mean window distances float32 [n_contigs, C], window counts int32
+        [n_contigs]) out: the windows of classify_contigs (forward strand), embedded, scored by novelty and averaged by
+        segment_mean.  novelty_scores turns them into (novelty, nearest_class, p_value)."""
+        clf, t = self.clf, self.clf._torch
+        seq, offs = clf.contig_buffers(seqs)
+        start, length, woff = clf.contig_windows(seq, offs, single_window)
+        if start.numel():
+            dist = self.novelty(clf.embed_windows(seq, start, length)[1])
+        else:
+            dist = t.zeros((0, self.n_classes), dtype=t.float32, device=seq.device)
+        return self.segment_mean(dist, woff), woff[1:] - woff[:-1]
 
     def close(self):
         if getattr(self, "_hd", None):

@@ -127,6 +127,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     allreduce, any width) and stored as head["preds"] (float32 [n_contigs, C], identical on all ranks).  With head["windows"]
     true, those rows are also collected on rank 0 in window order, as the class scores are with `window_probs`, and stored as
     head["window_preds"] (float32 [n_windows, C] on rank 0, None on the other ranks); with offsets None only that is done.
+    With head["novelty"] true (the head carries a novelty model), the head also scores each window's embedding by
+    Head.novelty into a second buffer of this rank's shard, reduced per contig the same way and stored as head["novelty_dist"]
+    (float32 [n_contigs, C], identical on all ranks).
     With `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
     """
     import torch
@@ -145,8 +148,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     def run(win, m, row):                                    # one chunk: windows win[:m] are rows [row, row + m) of the shard
         clf.classify_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12)
     scorer = head["head"] if head is not None else None
+    nov = scorer is not None and bool(head.get("novelty"))
     if scorer is not None:
         d_head = torch.empty((end - start, scorer.n_classes), dtype=torch.float32, device=dev)
+    if nov:
+        d_nov = torch.empty((end - start, scorer.n_classes), dtype=torch.float32, device=dev)
     if embeddings:
         shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
     if embeddings or scorer is not None or window_embeddings is not None:
@@ -157,6 +163,8 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, e.data_ptr())
                 if scorer is not None:
                     scorer.predict(e, out=d_head[row: row + m])
+                if nov:
+                    scorer.novelty(e, out=d_nov[row: row + m])
                 if embeddings:
                     shard.add(e)
                 sync()
@@ -192,12 +200,14 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 probs, attr = clf.attribute_ascii(d_win, attributions["target"])
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
-            if embeddings or (scorer is not None and not head_route):
+            if embeddings or nov or (scorer is not None and not head_route):
                 e = clf.embed_ascii(d_win)[1]
                 if embeddings:
                     shard.add(e)
                 if scorer is not None and not head_route:
                     scorer.predict(e, out=d_head[row: row + m])
+                if nov:
+                    scorer.novelty(e, out=d_nov[row: row + m])
             sync()
     futures = []
     with ThreadPoolExecutor(max_workers=1) as gpu:
@@ -222,6 +232,9 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
         if scorer is not None:
             head["preds"] = _reduce_rows(scorer.segment_mean, scorer.segment_sum, d_head, offsets, start, end, n, info,
                                          contig_reduce)
+            if nov:
+                head["novelty_dist"] = _reduce_rows(scorer.segment_mean, scorer.segment_sum, d_nov, offsets, start, end, n,
+                                                    info, contig_reduce)
     if window_probs:
         full = gdist.collect_window_probs(local_t, n, info)
         out.append(full.cpu().numpy() if full is not None else None)
@@ -534,6 +547,39 @@ def _write_head_strands(npz_path: Path, tsv_path: Path, names_key: str, names, f
             fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in (*a, *b, *c)) + "\n")
 
 
+_NOVELTY_HEADER = "seq_name\tnearest_class\tnovelty\tp_value\n"
+
+
+def _write_head_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, dist, counts, calibration, class_names,
+                        head_sha: str) -> None:
+    """<prefix>_nn_classification_head_novelty.{npz,tsv}: per sequence, the mean window distance to each of the head's classes
+    (distances float32 [n, C]), the smallest (novelty), its class (nearest_class, -1 / NA without a window) and the conformal
+    p-value against the head's calibration values (engine.novelty_scores), plus class_names and head_sha256."""
+    from .engine import novelty_scores
+    C = len(class_names)
+    dist = np.asarray(dist, dtype=np.float32).reshape(len(names), C)
+    nov, nearest, p = novelty_scores(dist, counts, calibration)
+    np.savez_compressed(npz_path, **{names_key: names, "distances": dist, "novelty": nov, "nearest_class": nearest,
+                                     "p_value": p, "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)})
+    with open(tsv_path, "w") as fout:
+        fout.write(_NOVELTY_HEADER)
+        for name, c, v, pv in zip(names, nearest, nov, p):
+            if c < 0:
+                fout.write(f"{name}\tNA\tNA\tNA\n")
+            else:
+                fout.write(f"{name}\t{class_names[c]}\t{float(v):.6g}\t{float(pv):.6g}\n")
+
+
+def _head_has_novelty(path) -> bool:
+    """Whether a --head file carries a novelty model (its keys present; load_head checks them)."""
+    from .weights import NOVELTY_KEYS
+    try:
+        with np.load(Path(path), allow_pickle=False) as z:
+            return any(k in z.files for k in NOVELTY_KEYS)
+    except Exception:
+        return False
+
+
 def _head_windows_current(npz_path: Path, tsv_path: Path, head_sha: str, stride: int) -> bool:
     """Both head window files exist and were written for this head at this stride."""
     if not _head_current(npz_path, tsv_path, head_sha):
@@ -790,6 +836,11 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         files += [outputs.nn_classification_head_windows_output, outputs.nn_classification_head_windows_npz_output]
         descr += ["window classification by the --head classifier: tabular format",
                   "window classification by the --head classifier: binary format"]
+    head_novelty = head is not None and _head_has_novelty(head)
+    if head_novelty:
+        files += [outputs.nn_classification_head_novelty_output, outputs.nn_classification_head_novelty_npz_output]
+        descr += ["novelty with respect to the --head classifier's classes: tabular format",
+                  "novelty with respect to the --head classifier's classes: binary format"]
     if head_attr_target:
         files.append(outputs.nn_classification_head_attributions_output)
         descr.append(f"window attributions of the --head classifier ({head_attr_target}{attr_method}): binary format")
@@ -825,6 +876,11 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                       outputs.provirus_nn_classification_head_windows_npz_output]
             descr += ["provirus window classification by the --head classifier: tabular format",
                       "provirus window classification by the --head classifier: binary format"]
+        if head_novelty:
+            files += [outputs.provirus_nn_classification_head_novelty_output,
+                      outputs.provirus_nn_classification_head_novelty_npz_output]
+            descr += ["provirus novelty with respect to the --head classifier's classes: tabular format",
+                      "provirus novelty with respect to the --head classifier's classes: binary format"]
         if head_attr_target:
             files.append(outputs.provirus_nn_classification_head_attributions_output)
             descr.append(f"provirus window attributions of the --head classifier ({head_attr_target}{attr_method}): "
@@ -866,7 +922,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output,
              outputs.nn_classification_head_attributions_output,
              outputs.nn_classification_head_strands_npz_output, outputs.nn_classification_head_strands_output,
-             outputs.nn_classification_head_windows_npz_output, outputs.nn_classification_head_windows_output)]
+             outputs.nn_classification_head_windows_npz_output, outputs.nn_classification_head_windows_output,
+             outputs.nn_classification_head_novelty_npz_output, outputs.nn_classification_head_novelty_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
@@ -879,7 +936,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                      outputs.provirus_nn_classification_head_strands_npz_output,
                      outputs.provirus_nn_classification_head_strands_output,
                      outputs.provirus_nn_classification_head_windows_npz_output,
-                     outputs.provirus_nn_classification_head_windows_output))
+                     outputs.provirus_nn_classification_head_windows_output,
+                     outputs.provirus_nn_classification_head_novelty_npz_output,
+                     outputs.provirus_nn_classification_head_novelty_output))
 
     plan = None
     info_writer = None
@@ -911,7 +970,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                       and (head_file is None or not write_window_scores
                            or _head_windows_current(j[21], j[22], head_sha, window_stride))
                       and (not head_attr_target
-                           or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))))
+                           or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))
+                      and (head_file is None or head_file.novelty is None or _head_current(j[23], j[24], head_sha))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -964,7 +1024,8 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
          win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path,
-         head_attr_path, head_strands_npz_path, head_strands_tsv_path, head_win_npz_path, head_win_tsv_path), \
+         head_attr_path, head_strands_npz_path, head_strands_tsv_path, head_win_npz_path, head_win_tsv_path,
+         head_nov_npz_path, head_nov_tsv_path), \
             (enc_skip, cls_skip), (parsed, index) \
             in zip(jobs, plan, staged):
         names = preds = emb = None
@@ -999,6 +1060,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     C = len(head_file.class_names)
                     hd = {"preds": np.zeros((len(index.names), C), np.float32), "window_preds": np.zeros((0, C), np.float32)}
                     hd["reverse_preds"] = hd["preds"]
+                    hd["novelty_dist"], hd["counts"] = hd["preds"], np.zeros(len(index.names), np.int64)
                 emb = np.zeros((len(index.names), 512), np.float32)
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
@@ -1010,6 +1072,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                 ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
                 if head_file is not None:
                     hd = {"head": head_scorer()}
+                    if head_file.novelty is not None:
+                        hd["novelty"] = True
+                        hd["counts"] = np.diff(np.asarray(index.offsets, np.int64))
                     ak["head"] = hd
                 if write_window_scores:
                     preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
@@ -1048,6 +1113,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                                             hd["reverse_preds"], head_file.class_names, head_sha)
                     console.log(f"{label} classification of both strands by the head written to "
                                 f"{head_strands_tsv_path.name} and {head_strands_npz_path.name}.")
+                if head_file.novelty is not None:
+                    if is_main:
+                        _write_head_novelty(head_nov_npz_path, head_nov_tsv_path, names_key, names, hd["novelty_dist"],
+                                            hd["counts"], head_file.novelty["novelty_calibration"], head_file.class_names,
+                                            head_sha)
+                    console.log(f"{label} novelty with respect to the head's classes (forward strand) written to "
+                                f"{head_nov_tsv_path.name} and {head_nov_npz_path.name}.")
             if write_window_scores:
                 if is_main:
                     _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,

@@ -14,6 +14,11 @@ With ``--both-strands`` the windows of the same records' reverse complements (nn
 are embedded too, into rows after the forward ones, and take the same labels: the head then learns from both strands, the
 split stays by sequence (both strands of a sequence on the same side), and a validation sequence is scored by the mean of its
 two strands' scores, as ``nn-classification --head --both-strands`` reports it.
+
+With ``--novelty`` a novelty model is fitted once the best epoch is chosen (engine.novelty_fit on the training rows of the
+embedding matrix: class means, shared covariance, whitening; DESIGN.md, "Head novelty") and calibrated on the validation
+sequences: the novelty of each, from its forward-strand windows through the same device path nn-classification --head takes
+(Head.novelty, then the head's segment mean, then the minimum over classes), sorted, is the head file's novelty_calibration.
 """
 from __future__ import annotations
 
@@ -185,9 +190,23 @@ def _make_head(clf, head_file):
     return Head(clf, head_file)
 
 
+def _fit_novelty(clf, X, rows, labels, n_classes):
+    """Factory (patched in CPU tests): engine.novelty_fit."""
+    from .engine import novelty_fit
+    return novelty_fit(clf, X, rows, labels, n_classes)
+
+
+def calibration_values(head, X, rows, offsets) -> np.ndarray:
+    """Sorted float32 novelty of the sequences whose windows are rows `rows` of X (int64 cuda, sequence by sequence, each
+    sequence's rows delimited by `offsets`, int32 cuda [n + 1]): Head.novelty, the head's segment mean, the minimum over
+    classes -- the values nn-classification --head computes for the same windows."""
+    dist = head.segment_mean(head.novelty(X[rows]), offsets).cpu().numpy()
+    return np.sort(dist.min(1)).astype(np.float32)
+
+
 def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int = 256, learning_rate: float = 1e-3,
          validation_fraction: float = 0.1, class_weight: str = "balanced", seed: int = 0, threads=None,
-         verbose: bool = True, both_strands: bool = False) -> None:
+         verbose: bool = True, both_strands: bool = False, novelty: bool = False) -> None:
     import torch
     from . import nn_classification as nnc
     from .engine import both_strands as both_strands_mean
@@ -200,6 +219,8 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
     if epochs < 1 or batch_size < 1 or not 0.0 <= validation_fraction < 1.0 or not learning_rate > 0 or seed < 0:
         raise ValueError("epochs >= 1, batch_size >= 1, 0 <= validation_fraction < 1, learning_rate > 0 and seed >= 0 "
                          "are required")
+    if novelty and validation_fraction == 0:
+        raise ValueError("--novelty needs validation sequences to calibrate against: use a validation fraction > 0")
     output_path.mkdir(parents=True, exist_ok=True)
     prefix = input_path.stem
     if sequence.is_compressed(input_path) != sequence.Compression.uncompressed:
@@ -245,6 +266,10 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
             console.error(f"class(es) without a sequence that has a window: {_listed(missing)}")
             sys.exit(1)
         val_seq = split_sequences(seq_class, C, validation_fraction, seed)
+        if novelty and not val_seq.any():
+            console.error("--novelty needs validation sequences to calibrate against, and this split holds none out (no class "
+                          "has two sequences with a window); label more sequences or train without --novelty")
+            sys.exit(1)
         # rows of X: the windows of the used records only, in file order; with both strands, then the same records' reverse
         # windows in file order (a record can have another number of windows on that strand: the N rule)
         strand_lists = [(RecordWindows(parsed, offsets, used), counts[used])]
@@ -329,6 +354,23 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
             if Xv is None or best is None or metrics[0] < best[1]:
                 best = (epoch, metrics[0], arrays)
     trainer.close()
-    _weights.save_head(npz_path, best[2], class_names, enc_w)
+    nov = None
+    if novelty:
+        train_d = torch.from_numpy(train_rows).to(dev)
+        fit = _fit_novelty(clf, X, train_d, labels_d, C)
+        head = _make_head(clf, _weights.HeadFile(best[2], class_names, enc_sha))
+        head.set_novelty(fit.center, fit.whitening, fit.means)
+        fwd = [rows[0][i] for i in val_idx]                  # the validation sequences' forward-strand rows
+        o = np.zeros(len(fwd) + 1, np.int32)
+        np.cumsum([len(r) for r in fwd], out=o[1:])
+        cal = calibration_values(head, X, torch.from_numpy(np.concatenate(fwd).astype(np.int64)).to(dev),
+                                 torch.from_numpy(o).to(dev))
+        head.close()
+        nov = {"novelty_center": fit.center, "novelty_whitening": fit.whitening, "novelty_means": fit.means,
+               "novelty_calibration": cal}
+        console.log(f"Novelty model fitted on {len(train_rows)} training windows (shrinkage alpha 0.01, smallest Cholesky pivot "
+                    f"{fit.min_pivot:.6g}) and calibrated on {len(cal)} validation sequences (novelty median "
+                    f"{float(np.median(cal)):.4g}, max {float(cal[-1]):.4g}).")
+    _weights.save_head(npz_path, best[2], class_names, enc_w, novelty=nov)
     console.log(f"Head of epoch {best[0]} written to {npz_path.name}; training record in {tsv_path.name}.")
     console.log("geNomad train-head finished!")

@@ -18,7 +18,7 @@ import ctypes as C
 import hashlib
 import re
 from pathlib import Path
-from typing import Dict, NamedTuple, Tuple
+from typing import Dict, NamedTuple, Optional, Tuple
 
 import numpy as np
 
@@ -126,10 +126,15 @@ SHIPPED_CLASSES = ("chromosome", "plasmid", "virus")
 _CLASS_NAME = re.compile(r"[A-Za-z0-9_.-]+")
 
 
+# A head file may also carry a novelty model (train-head --novelty; DESIGN.md, "Head novelty"): all four keys or none.
+NOVELTY_KEYS = ("novelty_center", "novelty_whitening", "novelty_means", "novelty_calibration")
+
+
 class HeadFile(NamedTuple):
     arrays: Dict[str, np.ndarray]   # short names of HEAD_KEYS -> float32 arrays; d2w [512, C], d2b [C]
     class_names: Tuple[str, ...]
     encoder_sha256: str
+    novelty: Optional[Dict[str, np.ndarray]] = None   # NOVELTY_KEYS -> arrays (check_novelty), or None
 
 
 def encoder_sha256(weights: Dict[str, np.ndarray]) -> str:
@@ -181,6 +186,38 @@ def _check_head_arrays(arrays, C: int) -> Dict[str, np.ndarray]:
     return out
 
 
+def check_novelty(novelty, C: int) -> Dict[str, np.ndarray]:
+    """The four novelty arrays, checked (ValueError naming the key): novelty_center float64 [512], novelty_whitening float64
+    [512, 512] lower triangular with a positive diagonal, novelty_means float64 [C, 512] (the whitened class means),
+    novelty_calibration float32 [n >= 1] sorted ascending; all finite."""
+    missing = [k for k in NOVELTY_KEYS if k not in novelty]
+    if missing:
+        raise ValueError(f"{missing[0]} missing: a novelty model needs all of {', '.join(NOVELTY_KEYS)}")
+    want = {"novelty_center": (np.float64, (512,)), "novelty_whitening": (np.float64, (512, 512)),
+            "novelty_means": (np.float64, (C, 512)), "novelty_calibration": (np.float32, None)}
+    out = {}
+    for key in NOVELTY_KEYS:
+        a = np.asarray(novelty[key])
+        dtype, shape = want[key]
+        if a.dtype != dtype:
+            raise ValueError(f"{key}: dtype {a.dtype}, expected {np.dtype(dtype)}")
+        if shape is not None and tuple(a.shape) != shape:
+            raise ValueError(f"{key}: shape {a.shape}, expected {shape}")
+        if shape is None and (a.ndim != 1 or a.size < 1):
+            raise ValueError(f"{key}: shape {a.shape}, expected [n] with n >= 1")
+        if not np.isfinite(a).all():
+            raise ValueError(f"{key}: not all finite")
+        out[key] = np.ascontiguousarray(a)
+    w = out["novelty_whitening"]
+    if np.triu(w, 1).any():
+        raise ValueError("novelty_whitening: not lower triangular")
+    if not (np.diagonal(w) > 0).all():
+        raise ValueError(f"novelty_whitening: diagonal not positive at {int(np.flatnonzero(~(np.diagonal(w) > 0))[0])}")
+    if (np.diff(out["novelty_calibration"]) < 0).any():
+        raise ValueError("novelty_calibration: not sorted ascending")
+    return out
+
+
 def load_head(path, weights: Dict[str, np.ndarray]) -> HeadFile:
     """Read and validate a head file against the encoder `weights` (load_weights()); ValueError naming the offending key."""
     with np.load(Path(path), allow_pickle=False) as z:
@@ -197,19 +234,26 @@ def load_head(path, weights: Dict[str, np.ndarray]) -> HeadFile:
             raise ValueError("encoder_sha256: expected one string")
         sha = str(sha)
         arrays = _check_head_arrays({s: z[KEYS[s][0]] for s in HEAD_KEYS if KEYS[s][0] in files}, len(names))
+        novelty = None
+        if any(k in files for k in NOVELTY_KEYS):
+            novelty = check_novelty({k: z[k] for k in NOVELTY_KEYS if k in files}, len(names))
     if sha != encoder_sha256(weights):
         raise ValueError("encoder_sha256: the head was trained on another encoder than the one loaded")
-    return HeadFile(arrays, names, sha)
+    return HeadFile(arrays, names, sha, novelty)
 
 
-def save_head(path, arrays: Dict[str, np.ndarray], class_names, weights: Dict[str, np.ndarray]) -> None:
-    """Write a head file.  The zip members carry a fixed timestamp, so equal heads give byte-identical files."""
+def save_head(path, arrays: Dict[str, np.ndarray], class_names, weights: Dict[str, np.ndarray], novelty=None) -> None:
+    """Write a head file, with the novelty model's four keys after the others when `novelty` is given.  The zip members carry
+    a fixed timestamp, so equal heads give byte-identical files."""
     import zipfile
     names = check_class_names(class_names)
     arrays = _check_head_arrays(arrays, len(names))
     members = [(KEYS[s][0], arrays[s]) for s in HEAD_KEYS]
     members += [("class_names", np.array(names, dtype=f"<U{max(len(x) for x in names)}")),
                 ("encoder_sha256", np.array(encoder_sha256(weights)))]
+    if novelty is not None:
+        novelty = check_novelty(novelty, len(names))
+        members += [(k, novelty[k]) for k in NOVELTY_KEYS]
     with zipfile.ZipFile(Path(path), "w", compression=zipfile.ZIP_STORED) as zf:
         for name, a in members:
             with zf.open(zipfile.ZipInfo(name + ".npy", date_time=(1980, 1, 1, 0, 0, 0)), "w", force_zip64=True) as f:

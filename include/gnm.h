@@ -674,6 +674,43 @@ int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32
                          void* stream);
 
 /*
+ * Head novelty: a Gaussian model of the embeddings a head was trained on, one mean per class and one shared covariance (Lee et
+ * al. 2018).  DESIGN.md, "Head novelty".  All of it in fp64, in a fixed order without atomics: a fit is bitwise reproducible
+ * for the same rows, and a row's distances do not depend on the batch it is scored in, its position there or n.
+ *   fit rows      x_i = d_X[d_idx[r]] (float [512], the gnm_embed_* rows), label y_i = d_labels[d_idx[r]] in [0, C), r < n_fit
+ *   means         mu_c = mean of class c's rows (block sums of 4096 rows, combined in block order);  N_c = 0 is an error
+ *                 center = (sum over c, in class order, of the class sums) / N
+ *   scatter       S = (1/N) sum_i (x_i - mu_{y_i})(x_i - mu_{y_i})^T, two-pass (x - mu centred in fp64 as the DMMA operand is
+ *                 loaded); lower 64 x 64 tiles only, K in chunks of 8192 rows combined in chunk order; S exactly symmetric
+ *   shrinkage     Sigma = (1 - 0.01) S + 0.01 (tr S / 512) I;  tr S = 0 is an error ("no within-class variation")
+ *   whitening     Sigma = L L^T (Cholesky, right-looking, one CTA; a pivot that is not > 0 is an error naming its column);
+ *                 P = L^-1 (lower triangular, forward substitution per column, k ascending)
+ *   whitened means  m_c = P (mu_c - center)
+ *   distance      D_c(x) = || P (x - center) - m_c ||^2 / 512 = || P (x - mu_c) ||^2 / 512 (about 1 for a typical training
+ *                 row), fp64, stored as float
+ *
+ * gnm_novelty_fit_workspace_bytes: bytes of d_work (256-byte aligned) for n_fit rows and C classes (0 on bad arguments);
+ *   about n_fit * (C * 512 * 8 / 4096 + 36 * 4096 * 8 / 8192) bytes + 6.3 MB.
+ * gnm_novelty_fit: d_X DEVICE float [n_rows][512], d_idx DEVICE int64 [n_fit] (rows of d_X), d_labels DEVICE int32 [n_rows]
+ *   (the d_idx / d_labels form of gnm_head_train_step).  Waits for `stream` and writes HOST fp64 arrays (any may be NULL):
+ *   h_center [512], h_whitening [512][512] = P (zeros above the diagonal), h_means [C][512] = m_c, h_min_pivot = the smallest
+ *   Cholesky pivot (a diagonal of Sigma after the earlier columns' updates, before its square root), and, for tests,
+ *   h_class_means [C][512] = mu_c and h_scatter [512][512] = S.  An index outside [0, n_rows) or a label outside [0, C) fails.
+ * gnm_head_set_novelty: attach a model (HOST fp64 center [512], whitening [512][512] lower triangular with a positive diagonal,
+ *   means [C][512] whitened) to a head; refuses non-finite values and a malformed whitening, naming the index.  Synchronous.
+ * gnm_head_novelty: embeddings DEVICE float [n][512] -> D DEVICE float [n][C] for the head's model.  One CTA per 64 rows:
+ *   Y = (x - center) P^T by DMMA in 64-column tiles in order (the k tiles above the diagonal skipped), each followed by an
+ *   epilogue adding sum_j (Y_j - m_cj)^2 over the tile's columns in order into a per-(row, class) fp64 sum; divided by 512.
+ *   Asynchronous on `stream`.  Per-sequence values: gnm_head_segment_mean of the rows.
+ */
+size_t gnm_novelty_fit_workspace_bytes(int64_t n_fit, int C);
+int gnm_novelty_fit(gnm_handle* h, const float* d_X, int64_t n_rows, const int64_t* d_idx, int64_t n_fit, const int32_t* d_labels,
+                    int C, double* h_center, double* h_whitening, double* h_means, double* h_min_pivot, double* h_class_means,
+                    double* h_scatter, void* d_work, size_t work_bytes, void* stream);
+int gnm_head_set_novelty(gnm_handle* h, gnm_head* head, const double* center, const double* whitening, const double* means);
+int gnm_head_novelty(gnm_handle* h, const gnm_head* head, const float* d_embed, int n, float* d_dist, void* stream);
+
+/*
  * Head training on cached embeddings (no encoder gradients).  Semantics, Keras 3 defaults with the reference's stack:
  *   training forward  z1 = x W1 + b1;  mu, var = batch mean and biased batch variance of z1 (per column);
  *                     y = gamma (z1 - mu) / sqrt(var + 1e-3) + beta;  h = relu(y) * keep / 0.8;  logits = h W2 + b2

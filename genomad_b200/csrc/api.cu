@@ -2319,6 +2319,7 @@ extern "C" int gnm_novelty_fit(gnm_handle* h, const float* d_X, int64_t n_rows, 
     case kNvBadLabel: return fail(fn + ": a fit row's label is outside [0, C)");
     case kNvEmptyClass: return fail(fn + ": class " + std::to_string(hs.arg) + " has no fit row");
     case kNvNoVariation: return fail(fn + ": the training windows have no within-class variation (tr S = 0)");
+    case kNvNonFinite: return fail(fn + ": a fit row has a non-finite value (NaN or infinity), so tr S is not finite");
     case kNvBadPivot:
       return fail(fn + ": the shrunk covariance has a non-positive Cholesky pivot at column " + std::to_string(hs.arg));
     default: return fail(fn + ": unknown status " + std::to_string(hs.code));

@@ -24,7 +24,7 @@ constexpr int kNvFactorThreads = 1024;
 constexpr int kNvScoreSmem = (2 * kNvTile * kNvMK + kNvTile * kNvYS + kNvTile * kNvMaxClasses + kNvMaxClasses * kNvTile) * 8;
 
 // Status of a fit, in device memory: the first error found (gnm_novelty_fit names it), the smallest pivot and tr S.
-enum { kNvOk = 0, kNvBadIndex = 1, kNvBadLabel = 2, kNvEmptyClass = 3, kNvNoVariation = 4, kNvBadPivot = 5 };
+enum { kNvOk = 0, kNvBadIndex = 1, kNvBadLabel = 2, kNvEmptyClass = 3, kNvNoVariation = 4, kNvBadPivot = 5, kNvNonFinite = 6 };
 struct NvStatus {
   int code;
   int arg;
@@ -213,7 +213,8 @@ nv_scatter_reduce_kernel(const double* __restrict__ part, int n_chunks, int64_t 
 }
 
 // One CTA: Sigma = (1 - alpha) S + alpha (tr S / 512) I, then its Cholesky factor L (lower; zeros above) in place of Sigma,
-// right-looking, column by column.  tr S <= 0 and a pivot that is not > 0 stop the fit (NvStatus).
+// right-looking, column by column.  A non-finite tr S (a fit row with a NaN or an infinity), tr S <= 0 and a pivot that is not
+// > 0 stop the fit (NvStatus).
 __global__ void __launch_bounds__(kNvFactorThreads)
 nv_factor_kernel(const double* __restrict__ S, double* __restrict__ L, NvStatus* st) {
   __shared__ double s_tr;
@@ -227,8 +228,8 @@ nv_factor_kernel(const double* __restrict__ S, double* __restrict__ L, NvStatus*
   }
   __syncthreads();
   const double tr = s_tr;
-  if (!(tr > 0.0) || !isfinite(tr)) {
-    if (tid == 0) st->code = kNvNoVariation;
+  if (!isfinite(tr) || !(tr > 0.0)) {
+    if (tid == 0) st->code = isfinite(tr) ? kNvNoVariation : kNvNonFinite;
     return;
   }
   const double shrink = kNvAlpha * (tr / kHidden);

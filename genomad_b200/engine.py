@@ -1007,13 +1007,13 @@ def novelty_scores(dist, counts, calibration):
     """Per-sequence novelty from the per-contig mean window distances dist (float32 [n, C]), the window counts [n] and the
     head's sorted calibration values (float32): (novelty float32 [n] = min_c dist, nearest_class int32 [n] = the argmin,
     lowest index on ties, p_value float64 [n] = (1 + #{v in calibration : v >= novelty}) / (1 + |calibration|)).  A sequence
-    without a window gets novelty NaN, nearest_class -1 and p NaN."""
+    without a window, or whose distances are not all finite, gets novelty NaN, nearest_class -1 and p NaN."""
     dist = np.asarray(dist, dtype=np.float32)
     counts = np.asarray(counts).reshape(-1)
     cal = np.asarray(calibration, dtype=np.float32).reshape(-1)
     n = len(counts)
     assert dist.ndim == 2 and len(dist) == n
-    has = counts > 0
+    has = (counts > 0) & np.isfinite(dist).all(1)
     nov = np.full(n, np.nan, np.float32)
     nearest = np.full(n, -1, np.int32)
     p = np.full(n, np.nan, np.float64)

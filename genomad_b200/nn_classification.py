@@ -553,7 +553,8 @@ _NOVELTY_HEADER = "seq_name\tnearest_class\tnovelty\tp_value\n"
 def _write_head_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, dist, counts, calibration, class_names,
                         head_sha: str) -> None:
     """<prefix>_nn_classification_head_novelty.{npz,tsv}: per sequence, the mean window distance to each of the head's classes
-    (distances float32 [n, C]), the smallest (novelty), its class (nearest_class, -1 / NA without a window) and the conformal
+    (distances float32 [n, C]), the smallest (novelty), its class (nearest_class; -1 / NA without a window or with a
+    non-finite distance) and the conformal
     p-value against the head's calibration values (engine.novelty_scores), plus class_names and head_sha256."""
     from .engine import novelty_scores
     C = len(class_names)

@@ -682,7 +682,8 @@ int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32
  *                 center = (sum over c, in class order, of the class sums) / N
  *   scatter       S = (1/N) sum_i (x_i - mu_{y_i})(x_i - mu_{y_i})^T, two-pass (x - mu centred in fp64 as the DMMA operand is
  *                 loaded); lower 64 x 64 tiles only, K in chunks of 8192 rows combined in chunk order; S exactly symmetric
- *   shrinkage     Sigma = (1 - 0.01) S + 0.01 (tr S / 512) I;  tr S = 0 is an error ("no within-class variation")
+ *   shrinkage     Sigma = (1 - 0.01) S + 0.01 (tr S / 512) I;  tr S = 0 is an error ("no within-class variation"), and so
+ *                 is a non-finite tr S ("a fit row has a non-finite value": a NaN or an infinity in a fit row)
  *   whitening     Sigma = L L^T (Cholesky, right-looking, one CTA; a pivot that is not > 0 is an error naming its column);
  *                 P = L^-1 (lower triangular, forward substitution per column, k ascending)
  *   whitened means  m_c = P (mu_c - center)
@@ -695,7 +696,8 @@ int gnm_head_segment_sum(gnm_handle* h, const float* d_probs, int C, const int32
  *   (the d_idx / d_labels form of gnm_head_train_step).  Waits for `stream` and writes HOST fp64 arrays (any may be NULL):
  *   h_center [512], h_whitening [512][512] = P (zeros above the diagonal), h_means [C][512] = m_c, h_min_pivot = the smallest
  *   Cholesky pivot (a diagonal of Sigma after the earlier columns' updates, before its square root), and, for tests,
- *   h_class_means [C][512] = mu_c and h_scatter [512][512] = S.  An index outside [0, n_rows) or a label outside [0, C) fails.
+ *   h_class_means [C][512] = mu_c and h_scatter [512][512] = S.  An index outside [0, n_rows), a label outside [0, C) or a
+ *   NaN or infinity in a fit row fails, each with its own message; the handle stays usable.
  * gnm_head_set_novelty: attach a model (HOST fp64 center [512], whitening [512][512] lower triangular with a positive diagonal,
  *   means [C][512] whitened) to a head; refuses non-finite values and a malformed whitening, naming the index.  Synchronous.
  * gnm_head_novelty: embeddings DEVICE float [n][512] -> D DEVICE float [n][C] for the head's model.  One CTA per 64 rows:

@@ -78,3 +78,106 @@ def whitening_bar(ref, N):
     P = rel * np.abs(ref["P"]).max()
     m = rel * (np.abs(ref["P"]) @ np.abs(ref["mu"] - ref["center"]).T).T.max() + rel * np.abs(ref["m"]).max()
     return P, m
+
+
+# ------------------------------------------------------------------------------------------------- derived per-step bounds
+# Each step of the fit is checked elementwise against its own computed inputs (the GPU's S, L, P, mu, center), with the
+# standard a-priori bounds of Higham, "Accuracy and Stability of Numerical Algorithms" (2nd ed.).  They do not depend on
+# kappa(Sigma), so a wrong small entry fails where a bar scaled by the largest entry would not.  |.| is elementwise.
+U32 = 2.0 ** -24                   # fp32 unit roundoff
+TINY32 = 2.0 ** -150               # half the smallest fp32 subnormal: the absolute rounding error of an fp32 store
+
+
+def gamma(k, u=U):
+    """gamma_k = k u / (1 - k u)."""
+    return k * u / (1 - k * u)
+
+
+def shrink(S):
+    """(A, tr) as nv_factor_kernel forms them from S: tr S summed over k = 0..511 in that order (bitwise the kernel's), then
+    A = (1 - alpha) S + alpha (tr / 512) I.  The kernel may contract the diagonal into an fma: A is within 2 u |A| of it."""
+    S = np.asarray(S, np.float64)
+    tr = 0.0
+    for k in range(DIM):
+        tr += float(S[k, k])
+    A = (1.0 - ALPHA) * S
+    A[np.diag_indices(DIM)] += ALPHA * (tr / DIM)
+    return A, tr
+
+
+def cholesky_ratio(L, A):
+    """max |L L^T - A| / bound over the lower triangle, bound = 2 gamma_513 |L| |L^T| + 2 u |A| (Thm 10.3, gamma_{n+1} for the
+    factorization, doubled for the host's own product; 2 u |A| for the shrinkage's fma)."""
+    L = np.tril(np.asarray(L, np.float64))
+    res = np.abs(L @ L.T - A)
+    bound = 2 * gamma(DIM + 1) * (np.abs(L) @ np.abs(L).T) + 2 * U * np.abs(A)
+    return _ratio(np.tril(res), np.tril(bound))
+
+
+def pivot_ratio(min_pivot, L):
+    """|min_pivot - min diag(L)^2| / (4 u min_pivot): the pivot is what the kernel took the square root of."""
+    d2 = np.diagonal(np.asarray(L, np.float64)) ** 2
+    return abs(min_pivot - d2.min()) / (4 * U * min_pivot)
+
+
+def inverse_ratio(L, P):
+    """max |L P - I| / (2 gamma_512 |L| |P|) (Thm 8.5 per column, doubled for the host's product)."""
+    L, P = np.tril(np.asarray(L, np.float64)), np.asarray(P, np.float64)
+    res = np.abs(L @ P - np.eye(DIM))
+    return _ratio(res, 2 * gamma(DIM) * (np.abs(L) @ np.abs(P)))
+
+
+def whiten_ratio(P, mu, center, m):
+    """max |m_c - P (mu_c - center)| / (2 gamma_513 |P| |mu_c - center|): the device's and the host's fp64 products."""
+    dm = np.asarray(mu, np.float64) - np.asarray(center, np.float64)
+    P = np.asarray(P, np.float64)
+    res = np.abs(np.asarray(m) - dm @ P.T)
+    return _ratio(res, 2 * gamma(DIM + 1) * (np.abs(dm) @ np.abs(P).T))
+
+
+def distance_bound(x, center, P, m):
+    """(D [n, C], bound [n, C]) for the window distances of the stored model (center, P, m): D from the fp64 oracle, and a bound
+    on |D_device - D| for a device that computes in fp64 and stores fp32.  With a = |x - center|, dY = gamma_514 |P| a (the
+    error of one fp64 Y = P (x - center)), r = |Y - m_c|:
+      fp64 = [sum_j (2 r_j dY_j + dY_j^2) + gamma_513 sum_j (r_j + dY_j)^2] / 512 + u D,
+    doubled because the oracle is an fp64 computation too, then 2^-24 of the value for the fp32 store and 2^-150 absolute."""
+    x = np.asarray(x, np.float64)
+    center, P, m = np.asarray(center, np.float64), np.asarray(P, np.float64), np.asarray(m, np.float64)
+    a = x - center
+    Y = a @ P.T
+    dY = gamma(DIM + 2) * (np.abs(a) @ np.abs(P).T)
+    D = np.empty((len(x), len(m)))
+    bound = np.empty_like(D)
+    for c in range(len(m)):
+        r = np.abs(Y - m[c])
+        D[:, c] = (r * r).sum(1) / DIM
+        b64 = ((2 * r * dY + dY * dY).sum(1) + gamma(DIM + 1) * ((r + dY) ** 2).sum(1)) / DIM + U * D[:, c]
+        bound[:, c] = 2 * b64 + U32 * (D[:, c] + 2 * b64) + TINY32
+    return D, bound
+
+
+def contig_bound(D, bound, offsets):
+    """Per-contig (mean [k, C], bound [k, C]) of window distances D with window bounds `bound` over the windows
+    offsets[i]:offsets[i+1], for the head reducer (one fp32 running sum in window order, then / n in fp32): the windows'
+    bounds, gamma_n (fp32) of the summed magnitudes for the running sum (n rather than n - 1 also covers this fp64 mean), and
+    2^-24 of the mean for the division."""
+    offsets = np.asarray(offsets)
+    k = len(offsets) - 1
+    mean, out = np.full((k, D.shape[1]), np.nan), np.full((k, D.shape[1]), np.nan)
+    for i in range(k):
+        b, e = int(offsets[i]), int(offsets[i + 1])
+        if e == b:
+            continue
+        n = e - b
+        mean[i] = D[b:e].sum(0) / n
+        tot = bound[b:e].sum(0) + gamma(n, U32) * np.abs(D[b:e]).sum(0) + bound[b:e].sum(0) * gamma(n, U32)
+        out[i] = tot / n + U32 * (np.abs(mean[i]) + tot / n) + TINY32
+    return mean, out
+
+
+def _ratio(err, bound):
+    """max err / bound, with 0 / 0 read as 0."""
+    err, bound = np.asarray(err), np.asarray(bound)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r = np.where(err == 0, 0.0, err / bound)
+    return float(r.max())

@@ -2,7 +2,7 @@
 Head novelty on an H100, against the fp64 oracle of tests/novelty_ref.py:
   * the fit (class means, center, scatter S, whitening P, whitened means m_c) on Gaussian clusters, post-ReLU-like sparse rows
     with dead columns, rows scaled from 1e-3 to 1e3 and a class with one row, at C in {2, 3, 32} and fit sizes at the tile and
-    chunk edges; the window distances of the fitted model within 1e-6 D + 1e-9;
+    chunk edges; the window distances of the fitted model within novelty_ref.distance_bound and 1e-6 D + 1e-9;
   * bitwise: two fits, and a row's distances under chunking, permutation and repeats;
   * errors: an empty class, no within-class variation;
   * end to end: train-head --novelty, then nn-classification --head (calibration membership, class predictions unchanged),
@@ -91,10 +91,10 @@ def check_distances(torch, clf, C, fit, x, label):
     h = head_with(clf, C, fit)
     got = h.novelty(torch.from_numpy(x).cuda()).cpu().numpy()
     h.close()
-    want = R.distances(x, fit.center, fit.whitening, fit.means)
+    want, bar = R.distance_bound(x, fit.center, fit.whitening, fit.means)
     err = np.abs(got.astype(np.float64) - want)
-    bar = 1e-6 * want + 1e-9
-    assert (err <= bar).all(), f"{label}: D off by {(err / bar).max():.3g} of its bar"
+    assert (err <= bar).all(), f"{label}: D off by {(err / bar).max():.3g} of its bound"
+    assert (err <= 1e-6 * want + 1e-9).all(), f"{label}: D off by more than 1e-6 D + 1e-9"
     return got
 
 

@@ -190,6 +190,31 @@ class NNOutputs:
     def provirus_nn_classification_head_attributions_output(self) -> Path:
         return self._nn("provirus_nn_classification_head_attributions.npz")
 
+    # ---- opt-in (--write-novelty-attributions, --write-window-novelty), not reference outputs: where and why a sequence is novel
+    @property
+    def nn_classification_head_novelty_attributions_output(self) -> Path:
+        return self._nn("nn_classification_head_novelty_attributions.npz")
+
+    @property
+    def provirus_nn_classification_head_novelty_attributions_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_novelty_attributions.npz")
+
+    @property
+    def nn_classification_head_novelty_windows_output(self) -> Path:
+        return self._nn("nn_classification_head_novelty_windows.tsv")
+
+    @property
+    def nn_classification_head_novelty_windows_npz_output(self) -> Path:
+        return self._nn("nn_classification_head_novelty_windows.npz")
+
+    @property
+    def provirus_nn_classification_head_novelty_windows_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_novelty_windows.tsv")
+
+    @property
+    def provirus_nn_classification_head_novelty_windows_npz_output(self) -> Path:
+        return self._nn("provirus_nn_classification_head_novelty_windows.npz")
+
     # ---- produced by find-proviruses, only read here (reference utils.py:280-297)
     @property
     def find_proviruses_dir(self) -> Path:

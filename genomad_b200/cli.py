@@ -89,9 +89,22 @@ def cli():
                    "class names) to <prefix>_nn_classification_head_attributions.npz, as --write-attributions does for the "
                    "shipped classes; --attribution-steps and --attribution-baseline apply to it. Cannot be combined with "
                    "--write-attributions. Not an option of the reference.")
+@click.option("--write-novelty-attributions", is_flag=True, default=False, show_default=True,
+              help="With a --head that carries a novelty model: also attribute every window's distance to its sequence's "
+                   "nearest class (the class of the novelty file) to the window's 4-mers, and write them to "
+                   "<prefix>_nn_classification_head_novelty_attributions.npz; --attribution-steps and --attribution-baseline "
+                   "apply to it. Cannot be combined with --write-attributions or --write-head-attributions. Costs one more "
+                   "pass over the windows. Not an option of the reference.")
+@click.option("--write-window-novelty", is_flag=True, default=False, show_default=True,
+              help="With a --head that carries a novelty model: also write every window's distance to each of the head's "
+                   "classes and its novelty (the smallest) to <prefix>_nn_classification_head_novelty_windows.{tsv,npz}, for "
+                   "the windows of the window-score files (--window-stride applies). There are no per-window p-values: the "
+                   "calibration set holds per-sequence means, whose quantiles do not describe single windows, whose "
+                   "distances spread wider. Not an option of the reference.")
 def nn_classification(input, output, single_window, batch_size, restart, threads, verbose, cleanup, write_tfrecords,
                       write_embeddings, write_window_scores, window_stride, write_attributions, attribution_steps,
-                      attribution_baseline, both_strands, head, write_head_attributions):
+                      attribution_baseline, both_strands, head, write_head_attributions, write_novelty_attributions,
+                      write_window_novelty):
     """Classify the sequences in the INPUT file (FASTA format) using the geNomad neural network and write
     the results to the OUTPUT directory."""
     import os
@@ -115,6 +128,10 @@ def nn_classification(input, output, single_window, batch_size, restart, threads
         extra["head"] = head
     if write_head_attributions is not None:
         extra["write_head_attributions"] = write_head_attributions
+    if write_novelty_attributions:
+        extra["write_novelty_attributions"] = True
+    if write_window_novelty:
+        extra["write_window_novelty"] = True
     module.main(input, output, single_window, batch_size, restart, threads, verbose, cleanup,
                 write_embeddings=True if write_embeddings else None, **extra)
 

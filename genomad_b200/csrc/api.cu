@@ -1470,6 +1470,9 @@ struct gnm_attr {
   float* g_out = nullptr; float* alpha = nullptr; float* g_logit = nullptr; float* g_mpi = nullptr;
   float* blockmax = nullptr; float* s_w = nullptr; float* probs = nullptr;
   float* unitmax = nullptr; float* s2 = nullptr;        // conv3 backward: max |s_w g_z2| per unit and warp; its power of two
+  double* nv_r = nullptr; float* nv_g = nullptr;        // novelty attributions: fp64 r = P (h1 - center) - m_c, fp32 g_h1
+  int32_t* nv_target = nullptr;                         //   each row's target class (uploaded per chunk)
+  float* nv_base = nullptr;                             //   the IG baseline's distances [C]
   uint8_t* wpackT[2] = {nullptr, nullptr};              // W2^T, W3^T packed like the forward's conv weights
   float out_scaleT[2] = {1.f, 1.f};
   float* wvT[2] = {nullptr, nullptr}; float* wqkT[2] = {nullptr, nullptr};
@@ -1541,6 +1544,10 @@ extern "C" int gnm_attr_create(gnm_handle* h, int max_batch, gnm_attr** out) {
   ATTR_ALLOC(a->unitmax, mb * kUnitsPerWin * 8 * sizeof(float));
   ATTR_ALLOC(a->s2, mb * sizeof(float));
   ATTR_ALLOC(a->probs, mb * 3 * sizeof(float));
+  ATTR_ALLOC(a->nv_r, mb * kHidden * sizeof(double));
+  ATTR_ALLOC(a->nv_g, mb * kHidden * sizeof(float));
+  ATTR_ALLOC(a->nv_target, mb * sizeof(int32_t));
+  ATTR_ALLOC(a->nv_base, kNvMaxClasses * sizeof(float));
 #undef ATTR_ALLOC
   // ---- weights, derived from the handle's device copies
   for (int L = 0; L < 2; ++L) {                         // conv2, conv3: W[j]^T in the forward's pack, same split and scale
@@ -1636,13 +1643,16 @@ static int launch_igloo_bwd(gnm_handle* h, gnm_attr* a, int s, int n, cudaStream
 // dense layer 0's epilogue left in hA_hi[1] / hA_lo[1] (head_forward_tc, as gnm_head_forward after its split).  Its hidden rows
 // replace the shipped ones in h2 and its probabilities [n][C] go to d_head_probs, or else to blockmax (376 B per window >= 128):
 // both are read by attr_head_backward_kernel, and blockmax is rewritten only after it, by IGLOO#1's backward.
+// With `novelty`, the gradient is instead that of the head's novelty distance D_c to each row's target class (a->nv_target,
+// uploaded by the caller): r and g_h1 in fp64 on the h1 rows the forward left (nv_residual_kernel, nv_grad_kernel), then g_out
+// (attr_novelty_backward_kernel); no head forward.  d_dist [n][C], when given, gets the rows' distances (nv_score_kernel).
 static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, int n, int target, float* d_probs, float* d_attr,
                           cudaStream_t st, const L1Interp* ig = nullptr, const gnm_head* hd = nullptr,
-                          float* d_head_probs = nullptr) {
+                          float* d_head_probs = nullptr, bool novelty = false, float* d_dist = nullptr) {
   float* probs = d_probs ? d_probs : a->probs;
   if (forward_step(h, d_ascii, nullptr, n, probs, nullptr, st, ig)) return 1;
   float* head_probs = d_head_probs ? d_head_probs : a->blockmax;
-  if (hd) {
+  if (hd && !novelty) {
     timer_mark(h, "attr_head_fwd", st);
     if (head_forward_tc(h, hd, n, head_probs, st)) return 1;
   }
@@ -1661,13 +1671,29 @@ static int attribute_step(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, in
   timer_mark(h, "attr_route0", st);
   if (launch_route(h, a, 0, a->tm_y1, n, st)) return 1;                      // y1
   timer_mark(h, "attr_head", st);
-  if (hd)
-    attr_head_backward_kernel<<<n, 256, 0, st>>>(head_probs, h->h1, h->h2, hd->d2w, hd->d1w, hd->scale, h->d0w, h->bn0_scale,
-                                                 attr_classes(target, hd->C), a->g_out);
-  else
-    attr_head_backward_kernel<<<n, 256, 0, st>>>(probs, h->h1, h->h2, h->d2w, h->d1w, h->bn1_scale, h->d0w, h->bn0_scale,
-                                                 attr_classes(target, 3), a->g_out);
-  if (check_launch(h, "attr_head_backward_kernel")) return 1;
+  if (novelty) {
+    const unsigned blocks = static_cast<unsigned>((n + kNvTile - 1) / kNvTile);
+    if (d_dist) {
+      nv_score_kernel<<<blocks, kNvThreads, kNvScoreSmem, st>>>(h->h1, n, hd->nv_center, hd->nv_whitening, hd->nv_means, hd->C,
+                                                                d_dist);
+      if (check_launch(h, "nv_score_kernel")) return 1;
+    }
+    nv_residual_kernel<<<blocks, kNvThreads, 0, st>>>(h->h1, n, hd->nv_center, hd->nv_whitening, hd->nv_means, a->nv_target,
+                                                      a->nv_r);
+    if (check_launch(h, "nv_residual_kernel")) return 1;
+    nv_grad_kernel<<<dim3(blocks, kNvTiles), kNvThreads, 0, st>>>(a->nv_r, n, hd->nv_whitening, a->nv_g);
+    if (check_launch(h, "nv_grad_kernel")) return 1;
+    attr_novelty_backward_kernel<<<n, 256, 0, st>>>(a->nv_g, h->h1, h->d0w, h->bn0_scale, a->g_out);
+    if (check_launch(h, "attr_novelty_backward_kernel")) return 1;
+  } else {
+    if (hd)
+      attr_head_backward_kernel<<<n, 256, 0, st>>>(head_probs, h->h1, h->h2, hd->d2w, hd->d1w, hd->scale, h->d0w,
+                                                   h->bn0_scale, attr_classes(target, hd->C), a->g_out);
+    else
+      attr_head_backward_kernel<<<n, 256, 0, st>>>(probs, h->h1, h->h2, h->d2w, h->d1w, h->bn1_scale, h->d0w, h->bn0_scale,
+                                                   attr_classes(target, 3), a->g_out);
+    if (check_launch(h, "attr_head_backward_kernel")) return 1;
+  }
   timer_mark(h, "attr_igloo1", st);
   if (launch_igloo_bwd(h, a, 1, n, st)) return 1;                            // -> fp32 g_z3, block maxima
   attr_pack_kernel<<<sgrid, 256, 0, st>>>(a->f32a, a->blockmax, a->s_w, a->gz3);
@@ -1709,6 +1735,7 @@ static int attr_debug_fetch(gnm_handle* h, const gnm_attr* a, const std::string&
     return check_launch(h, "reverse_rows_kernel");
   }
   if (k == "attr_g_out") { src = a->g_out; count = static_cast<size_t>(n) * 256; }
+  else if (k == "attr_g_h1") { src = a->nv_g; count = static_cast<size_t>(n) * kHidden; }
   else if (k == "attr_s_w") { src = a->s_w; count = n; }
   else if (k == "attr_s2") { src = a->s2; count = n; }
   else if (k == "attr_gy1") { src = a->gy1; count = rows * kC; }
@@ -1732,14 +1759,44 @@ static int check_target(const std::string& f, const gnm_head* hd, int target) {
   return 0;
 }
 
+// The novelty attribution calls' own arguments: HOST targets [n], DEVICE distances [n][C] and (IG) [n][2], each or NULL.
+struct NvAttrArgs {
+  const int32_t* h_target;
+  float* d_dist;
+  float* d_dist_target;
+};
+
+// the checks of the novelty attribution calls, before any launch: the head carries a model and every target is a class of it
+static int check_novelty(const std::string& f, const gnm_head* hd, const NvAttrArgs* nv, int n) {
+  if (!hd->nv_center) return fail(f + ": the head has no novelty model (gnm_head_set_novelty)");
+  if (n > 0 && !nv->h_target) return fail(f + ": null target array");
+  for (int i = 0; i < n; ++i)
+    if (nv->h_target[i] < 0 || nv->h_target[i] >= hd->C)
+      return fail(f + ": target[" + std::to_string(i) + "] = " + std::to_string(nv->h_target[i]) +
+                  " is not a class of the head, in [0, " + std::to_string(hd->C) + ")");
+  GNM_CUDA(cudaFuncSetAttribute(nv_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kNvScoreSmem));
+  return 0;
+}
+
+// targets of windows [0, m) of h_target, each repeated for its `rows` rows, to the context's target list (stream-ordered behind
+// the previous chunk's readers).  A copy from pageable memory may make the host wait for the stream first: 4 B per row, one
+// copy per chunk of up to 256 rows, so each chunk's launches are issued once the previous chunk has run.
+static int upload_targets(gnm_attr* a, const int32_t* h_target, int m, int rows, cudaStream_t st) {
+  std::vector<int32_t> v(static_cast<size_t>(m) * rows);
+  for (size_t i = 0; i < v.size(); ++i) v[i] = h_target[i / rows];
+  GNM_CUDA(cudaMemcpyAsync(a->nv_target, v.data(), v.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  return 0;
+}
+
 static int attribute_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
                          const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, float* d_probs, float* d_attr,
-                         void* stream, const gnm_head* hd = nullptr, float* d_head_probs = nullptr) {
+                         void* stream, const gnm_head* hd = nullptr, float* d_head_probs = nullptr,
+                         const NvAttrArgs* nv = nullptr) {
   const std::string f(fn);
   if (!h || !a) return fail(f + ": null handle or attribution context");
   if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
   if (n < 0) return fail(f + ": negative window count");
-  if (check_target(f, hd, target)) return 1;
+  if (nv ? check_novelty(f, hd, nv, n) : check_target(f, hd, target)) return 1;
   if (h->conv_impl != 0)
     return fail(f + ": attributions need the tensor-core path (conv_impl = 0); the fp32 validation kernels have no backward pass");
   if (h->debug_stop != 0) return fail(f + ": debug_stop must be 0");
@@ -1753,8 +1810,10 @@ static int attribute_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8
     const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
     if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
     float* head_probs = d_head_probs ? d_head_probs + static_cast<size_t>(off) * hd->C : nullptr;
+    float* dist = nv && nv->d_dist ? nv->d_dist + static_cast<size_t>(off) * hd->C : nullptr;
+    if (nv && upload_targets(a, nv->h_target + off, m, 1, st)) return 1;
     if (attribute_step(h, a, asc, m, target, probs_at(d_probs, off), d_attr + static_cast<size_t>(off) * kTok, st, nullptr, hd,
-                       head_probs)) return 1;
+                       head_probs, nv != nullptr, dist)) return 1;
   }
   return 0;
 }
@@ -1776,15 +1835,59 @@ extern "C" int gnm_attribute_windows(gnm_handle* h, gnm_attr* a, const uint8_t* 
 //   3. ig_reduce_kernel: IG = the rows' mean over k, ascending.
 // log p_c(x') is the same for every window: one one-row forward of the baseline per call, before the first chunk (only when
 // d_logp is given), so the debug buffers still hold the last chunk's rows afterwards.
+// attribute_ig_any's chunk loop for a head's novelty distance (checked by the caller): the same chunks, rows and mean over k,
+// with D_c in place of log p_c.  D_c(x') comes from the baseline's one-row forward before the first chunk, D_c(x) from each
+// chunk's own forward (bitwise gnm_head_novelty of the window's embedding); each window's target is repeated over its rows.
+static int attribute_novelty_ig(gnm_handle* h, gnm_attr* a, const uint8_t* d_ascii, const uint8_t* d_seq,
+                                const int64_t* d_win_start, const int32_t* d_win_len, int n, int steps, int baseline,
+                                float* d_probs, float* d_attr, cudaStream_t st, const gnm_head* hd, const NvAttrArgs* nv) {
+  const int per = a->max_batch / steps, C = hd->C;
+  if (nv->d_dist_target) {                                      // the baseline's distances to every class, a->nv_base [C]
+    const L1Interp base = {0, baseline};
+    if (forward_step(h, d_ascii ? d_ascii : h->in_stage[0], nullptr, 1, a->probs, nullptr, st, &base)) return 1;
+    nv_score_kernel<<<1, kNvThreads, kNvScoreSmem, st>>>(h->h1, 1, hd->nv_center, hd->nv_whitening, hd->nv_means, C, a->nv_base);
+    if (check_launch(h, "nv_score_kernel")) return 1;
+  }
+  const L1Interp ig = {steps, baseline};
+  for (int off = 0; off < n; off += per) {
+    const int m = std::min(per, n - off);
+    const uint8_t* asc = d_ascii ? d_ascii + static_cast<size_t>(off) * kWindow : h->in_stage[0];
+    if (!d_ascii && launch_gather_windows(h, d_seq, d_win_start + off, d_win_len + off, m, h->in_stage[0], st)) return 1;
+    if (upload_targets(a, nv->h_target + off, m, steps, st)) return 1;
+    if (d_probs || nv->d_dist || nv->d_dist_target) {
+      // the windows' own forward and distances: to d_dist or blockmax (scratch until the attribution step rewrites it)
+      float* probs = d_probs ? probs_at(d_probs, off) : a->probs;
+      float* dist = nv->d_dist ? nv->d_dist + static_cast<size_t>(off) * C : a->blockmax;
+      if (forward_step(h, asc, nullptr, m, probs, nullptr, st)) return 1;
+      nv_score_kernel<<<(m + kNvTile - 1) / kNvTile, kNvThreads, kNvScoreSmem, st>>>(h->h1, m, hd->nv_center, hd->nv_whitening,
+                                                                                     hd->nv_means, C, dist);
+      if (check_launch(h, "nv_score_kernel")) return 1;
+      if (nv->d_dist_target) {
+        float* out = nv->d_dist_target + static_cast<size_t>(off) * 2;
+        nv_pick_kernel<<<(m + 255) / 256, 256, 0, st>>>(dist, 0, m, C, a->nv_target, steps, out);
+        if (check_launch(h, "nv_pick_kernel")) return 1;
+        nv_pick_kernel<<<(m + 255) / 256, 256, 0, st>>>(a->nv_base, 1, m, C, a->nv_target, steps, out + 1);
+        if (check_launch(h, "nv_pick_kernel")) return 1;
+      }
+    }
+    if (attribute_step(h, a, asc, m * steps, 0, nullptr, nullptr, st, &ig, hd, nullptr, true)) return 1;
+    timer_mark(h, "ig_reduce", st);
+    ig_reduce_kernel<<<dim3((kTok + 255) / 256, m), 256, 0, st>>>(a->gy1, steps, d_attr + static_cast<size_t>(off) * kTok);
+    if (check_launch(h, "ig_reduce_kernel")) return 1;
+    timer_mark(h, "end", st);
+  }
+  return 0;
+}
+
 static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const uint8_t* d_ascii, const uint8_t* d_seq,
                             const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps, int baseline,
                             float* d_probs, float* d_logp, float* d_attr, void* stream, const gnm_head* hd = nullptr,
-                            float* d_head_probs = nullptr) {
+                            float* d_head_probs = nullptr, const NvAttrArgs* nv = nullptr) {
   const std::string f(fn);
   if (!h || !a) return fail(f + ": null handle or attribution context");
   if (a->h != h) return fail(f + ": the attribution context belongs to another handle");
   if (n < 0) return fail(f + ": negative window count");
-  if (check_target(f, hd, target)) return 1;
+  if (nv ? check_novelty(f, hd, nv, n) : check_target(f, hd, target)) return 1;
   if (steps < 1 || steps > a->max_batch)
     return fail(f + ": steps must be in [1, the attribution context's max_batch = " + std::to_string(a->max_batch) + "]");
   if (baseline != GNM_IG_BASELINE_ZERO && baseline != GNM_IG_BASELINE_N)
@@ -1799,6 +1902,8 @@ static int attribute_ig_any(gnm_handle* h, gnm_attr* a, const char* fn, const ui
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int per = a->max_batch / steps;                         // windows per chunk
   const int C = hd ? hd->C : 3;
+  if (nv) return attribute_novelty_ig(h, a, d_ascii, d_seq, d_win_start, d_win_len, n, steps, baseline, d_probs, d_attr, st, hd,
+                                      nv);
   if (d_logp) {                                                 // log p_c(x'), into column 1 of every window
     const L1Interp base = {0, baseline};
     if (forward_step(h, d_ascii ? d_ascii : h->in_stage[0], nullptr, 1, a->probs, nullptr, st, &base)) return 1;
@@ -1889,9 +1994,48 @@ extern "C" int gnm_attribute_head_ig_windows(gnm_handle* h, gnm_attr* a, const g
                           baseline, d_probs, d_logp, d_attr, stream, head, d_head_probs);
 }
 
+// ---- of a head's novelty distance to each window's target class (nv_residual_kernel, nv_grad_kernel)
+extern "C" int gnm_attribute_novelty_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                           const int32_t* h_target, float* d_probs, float* d_dist, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_novelty_ascii: null head");
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_novelty_ascii: null buffer");
+  const NvAttrArgs nv = {h_target, d_dist, nullptr};
+  return attribute_any(h, a, "gnm_attribute_novelty_ascii", d_ascii, nullptr, nullptr, nullptr, n, 0, d_probs, d_attr, stream,
+                       head, nullptr, &nv);
+}
+extern "C" int gnm_attribute_novelty_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                             const int64_t* d_win_start, const int32_t* d_win_len, int n, const int32_t* h_target,
+                                             float* d_probs, float* d_dist, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_novelty_windows: null head");
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_novelty_windows: null buffer");
+  const NvAttrArgs nv = {h_target, d_dist, nullptr};
+  return attribute_any(h, a, "gnm_attribute_novelty_windows", nullptr, d_seq, d_win_start, d_win_len, n, 0, d_probs, d_attr,
+                       stream, head, nullptr, &nv);
+}
+extern "C" int gnm_attribute_novelty_ig_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                              const int32_t* h_target, int steps, int baseline, float* d_probs, float* d_dist,
+                                              float* d_dist_target, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_novelty_ig_ascii: null head");
+  if (n > 0 && !d_ascii) return fail("gnm_attribute_novelty_ig_ascii: null buffer");
+  const NvAttrArgs nv = {h_target, d_dist, d_dist_target};
+  return attribute_ig_any(h, a, "gnm_attribute_novelty_ig_ascii", d_ascii, nullptr, nullptr, nullptr, n, 0, steps, baseline,
+                          d_probs, nullptr, d_attr, stream, head, nullptr, &nv);
+}
+extern "C" int gnm_attribute_novelty_ig_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                                const int64_t* d_win_start, const int32_t* d_win_len, int n,
+                                                const int32_t* h_target, int steps, int baseline, float* d_probs, float* d_dist,
+                                                float* d_dist_target, float* d_attr, void* stream) {
+  if (!head) return fail("gnm_attribute_novelty_ig_windows: null head");
+  if (n > 0 && (!d_seq || !d_win_start || !d_win_len)) return fail("gnm_attribute_novelty_ig_windows: null buffer");
+  const NvAttrArgs nv = {h_target, d_dist, d_dist_target};
+  return attribute_ig_any(h, a, "gnm_attribute_novelty_ig_windows", nullptr, d_seq, d_win_start, d_win_len, n, 0, steps,
+                          baseline, d_probs, nullptr, d_attr, stream, head, nullptr, &nv);
+}
+
 extern "C" long long gnm_attr_bytes_per_window(void) {
   return static_cast<long long>(kTok) * (3 * kRowBytes + 2 * kC * 4) + 2LL * kPooled * kC * 5 +
-         4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + kUnitsPerWin * 8 + 5);
+         4LL * (256 + 2 * kLogitsLd + kPatches + kAttrPosBlocks + kUnitsPerWin * 8 + 5) +
+         (8LL + 4LL) * kHidden + 4;                             // novelty attributions: r (fp64), g_h1, target
 }
 
 // ------------------------------------------------------------------------------------------------ embedding neighbours

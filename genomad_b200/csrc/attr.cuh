@@ -99,6 +99,31 @@ attr_head_backward_kernel(const float* __restrict__ probs,      // [n][C]
   }
 }
 
+// One window per CTA, 256 threads.  g_out[w][0..255] = d D_c / d h0 from g_h1 = d D_c / d h1 (nv_grad_kernel's fp32 rows): the
+// last stage of attr_head_backward_kernel, in its order.
+__global__ void __launch_bounds__(256)
+attr_novelty_backward_kernel(const float* __restrict__ g_h1,      // [n][512]
+                             const float* __restrict__ h1,        // [n][512] (post-ReLU)
+                             const float* __restrict__ d0w,       // [256][512]
+                             const float* __restrict__ bn0_scale, // [512]
+                             float* __restrict__ g_out) {
+  __shared__ float s_a0[kHidden];
+  const int w = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  for (int j = tid; j < kHidden; j += 256) {
+    const size_t o = static_cast<size_t>(w) * kHidden + j;
+    s_a0[j] = h1[o] > 0.f ? g_h1[o] * bn0_scale[j] : 0.f;
+  }
+  __syncthreads();
+  for (int m = warp; m < 256; m += 8) {                         // g_h0[m] = sum_j d0w[m][j] g_a0[j]
+    const float* row = d0w + static_cast<size_t>(m) * kHidden;
+    float a = 0.f;
+#pragma unroll 4
+    for (int j = lane; j < kHidden; j += 32) a = fmaf(row[j], s_a0[j], a);
+    a = warp_sum(a);
+    if (lane == 0) g_out[static_cast<size_t>(w) * 256 + m] = a;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ IGLOO: attention part
 // One window per CTA, 256 threads: alpha = softmax(logits) (as attention_kernel), g_alpha, g_logit -> [n][752] rows.
 __global__ void __launch_bounds__(256)

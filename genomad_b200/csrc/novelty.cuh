@@ -288,6 +288,36 @@ nv_whiten_means_kernel(const double* __restrict__ P, const double* __restrict__ 
   m[static_cast<size_t>(c) * kHidden + i] = s;
 }
 
+// Column tile ct of Y = (x - center) P^T for the 64 rows from row0 (rows >= n read as 0) into a warp's accumulators: k ascending
+// in k16 steps over the tiles up to the diagonal (P is zero above it).  sA, sB: [64][kNvMK] each.  nv_score_kernel and
+// nv_residual_kernel share it, so their Y are the same bits.
+__device__ __forceinline__ void nv_y_tile(double (&acc)[2][4][4], const float* __restrict__ x, int n, int64_t row0,
+                                          const double* __restrict__ center, const double* __restrict__ P, int ct, double* sA,
+                                          double* sB, int tid, int wm, int wn, int lane) {
+  const int lk = tid & 15, lr = tid >> 4;                // loader: column lk of rows lr, lr + 8, ...
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[mi][ni][i] = 0.0;
+  const int k_end = (ct + 1) * kNvTile;
+  for (int k0 = 0; k0 < k_end; k0 += kNvK) {
+    const double cen = center[k0 + lk];
+#pragma unroll
+    for (int q = 0; q < kNvTile / 8; ++q) {
+      const int r = lr + 8 * q;
+      const int64_t gr = row0 + r;
+      sA[r * kNvMK + lk] = gr < n ? static_cast<double>(x[gr * kHidden + k0 + lk]) - cen : 0.0;
+      sB[r * kNvMK + lk] = P[static_cast<size_t>(ct * kNvTile + r) * kHidden + k0 + lk];
+    }
+    __syncthreads();
+    nv_warp_step(acc, wm, wn, lane, [&](int m, int k) { return sA[m * kNvMK + k]; },
+                 [&](int k, int nn) { return sB[nn * kNvMK + k]; });
+    __syncthreads();
+  }
+}
+
 // D [n][C] (fp32) = || P (x - center) - m_c ||^2 / 512 per row, computed in fp64: per 64-row block, the column tiles of
 // Y = (x - center) P^T in order (k tiles above the diagonal, where P is zero, skipped), each followed by the epilogue that adds
 // sum_j (Y[r][j] - m_c[j])^2 over the tile's columns in column order into the (row, class) sum in shared memory.  A row's
@@ -304,30 +334,9 @@ nv_score_kernel(const float* __restrict__ x, int n, const double* __restrict__ c
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wm = warp >> 1, wn = warp & 1;
   const int64_t row0 = static_cast<int64_t>(blockIdx.x) * kNvTile;
   for (int p = tid; p < kNvTile * kNvMaxClasses; p += kNvThreads) sD[p] = 0.0;
-  const int lk = tid & 15, lr = tid >> 4;                // loader: column lk of rows lr, lr + 8, ...
   for (int ct = 0; ct < kNvTiles; ++ct) {
     double acc[2][4][4];
-#pragma unroll
-    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-      for (int ni = 0; ni < 4; ++ni)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) acc[mi][ni][i] = 0.0;
-    const int k_end = (ct + 1) * kNvTile;
-    for (int k0 = 0; k0 < k_end; k0 += kNvK) {
-      const double cen = center[k0 + lk];
-#pragma unroll
-      for (int q = 0; q < kNvTile / 8; ++q) {
-        const int r = lr + 8 * q;
-        const int64_t gr = row0 + r;
-        sA[r * kNvMK + lk] = gr < n ? static_cast<double>(x[gr * kHidden + k0 + lk]) - cen : 0.0;
-        sB[r * kNvMK + lk] = P[static_cast<size_t>(ct * kNvTile + r) * kHidden + k0 + lk];
-      }
-      __syncthreads();
-      nv_warp_step(acc, wm, wn, lane, [&](int m, int k) { return sA[m * kNvMK + k]; },
-                   [&](int k, int nn) { return sB[nn * kNvMK + k]; });
-      __syncthreads();
-    }
+    nv_y_tile(acc, x, n, row0, center, P, ct, sA, sB, tid, wm, wn, lane);
     const int g = lane >> 2, t = lane & 3;
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
@@ -355,6 +364,91 @@ nv_score_kernel(const float* __restrict__ x, int n, const double* __restrict__ c
     const int64_t gr = row0 + r;
     if (gr < n) out[gr * C + c] = static_cast<float>(sD[r * kNvMaxClasses + c] / kHidden);
   }
+}
+
+// ---- gradient of a window's distance to its target class (novelty attributions; DESIGN.md, "Head novelty")
+// r [n][512] (fp64) = P (x - center) - m_c, c = target[row]: nv_score_kernel's Y, and r[j] the same bits as the difference its
+// epilogue squares, stored straight from the accumulators.
+__global__ void __launch_bounds__(kNvThreads)
+nv_residual_kernel(const float* __restrict__ x, int n, const double* __restrict__ center, const double* __restrict__ P,
+                   const double* __restrict__ means, const int32_t* __restrict__ target, double* __restrict__ r) {
+  __shared__ double sA[kNvTile * kNvMK], sB[kNvTile * kNvMK];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wm = warp >> 1, wn = warp & 1, g = lane >> 2, t = lane & 3;
+  const int64_t row0 = static_cast<int64_t>(blockIdx.x) * kNvTile;
+  for (int ct = 0; ct < kNvTiles; ++ct) {
+    double acc[2][4][4];
+    nv_y_tile(acc, x, n, row0, center, P, ct, sA, sB, tid, wm, wn, lane);
+#pragma unroll
+    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+      for (int i = 0; i < 4; i += 2) {
+        const int64_t gr = row0 + wm * 32 + mi * 16 + g + 8 * (i >> 1);
+        if (gr >= n) continue;
+        const double* m = means + static_cast<size_t>(target[gr]) * kHidden + ct * kNvTile;
+        double* out = r + gr * kHidden + ct * kNvTile;
+#pragma unroll
+        for (int ni = 0; ni < 4; ++ni) {
+          const int j = wn * 32 + ni * 8 + 2 * t;
+          out[j] = acc[mi][ni][i] - m[j];
+          out[j + 1] = acc[mi][ni][i + 1] - m[j + 1];
+        }
+      }
+  }
+}
+
+// g [n][512] (fp32) = dD_c / dx = (2 / 512) P^T r, computed in fp64 and rounded once: block (64 rows, column tile cj),
+// g[j] = sum_{i >= j} r[i] P[i][j] over the k tiles from the diagonal down (P is zero above it), k ascending in k16 steps.
+__global__ void __launch_bounds__(kNvThreads)
+nv_grad_kernel(const double* __restrict__ r, int n, const double* __restrict__ P, float* __restrict__ g_out) {
+  __shared__ double sA[kNvTile * kNvMK], sB[kNvTile * kNvMK];   // [64 rows][k], [64 columns of g][k]
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wm = warp >> 1, wn = warp & 1;
+  const int64_t row0 = static_cast<int64_t>(blockIdx.x) * kNvTile;
+  const int cj = blockIdx.y;
+  double acc[2][4][4];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[mi][ni][i] = 0.0;
+  const int lk = tid & 15, lr = tid >> 4;                // A loader: column lk of rows lr, lr + 8, ...
+  const int bn = tid & 63, bk = tid >> 6;                // B loader: column bn of P rows k0 + bk, k0 + bk + 2, ...
+  for (int k0 = cj * kNvTile; k0 < kHidden; k0 += kNvK) {
+#pragma unroll
+    for (int q = 0; q < kNvTile / 8; ++q) {
+      const int m = lr + 8 * q;
+      const int64_t gr = row0 + m;
+      sA[m * kNvMK + lk] = gr < n ? r[gr * kHidden + k0 + lk] : 0.0;
+      const int k = bk + 2 * q;
+      sB[bn * kNvMK + k] = P[static_cast<size_t>(k0 + k) * kHidden + cj * kNvTile + bn];
+    }
+    __syncthreads();
+    nv_warp_step(acc, wm, wn, lane, [&](int m, int k) { return sA[m * kNvMK + k]; },
+                 [&](int k, int nn) { return sB[nn * kNvMK + k]; });
+    __syncthreads();
+  }
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < 4; ++ni)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int64_t gr = row0 + wm * 32 + mi * 16 + g + 8 * (i >> 1);
+        if (gr < n)
+          g_out[gr * kHidden + cj * kNvTile + wn * 32 + ni * 8 + 2 * t + (i & 1)] =
+              static_cast<float>(acc[mi][ni][i] * (2.0 / kHidden));
+      }
+}
+
+// out[2 i] = dist[i][target[i * t_stride]] (row 0 for every i when `broadcast`): a window's distance to its own target, from
+// its distance row (t_stride = the rows per window of the target list) or from the baseline's one row.
+__global__ void __launch_bounds__(256)
+nv_pick_kernel(const float* __restrict__ dist, int broadcast, int n, int C, const int32_t* __restrict__ target, int t_stride,
+               float* __restrict__ out) {
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  out[static_cast<size_t>(i) * 2] = dist[(broadcast ? 0 : static_cast<size_t>(i) * C) + target[static_cast<size_t>(i) * t_stride]];
 }
 
 }  // namespace gnm

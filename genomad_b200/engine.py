@@ -112,6 +112,15 @@ EXPORTS = {
     "gnm_attribute_head_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                                 C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_void_p]),
+    "gnm_attribute_novelty_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_novelty_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_novelty_ig_ascii": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                                 C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_attribute_novelty_ig_windows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]),
     "gnm_neighbours_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int]),
     "gnm_embedding_neighbours": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -446,7 +455,11 @@ class Attributions(NamedTuple):
     offsets: "object"         # int32 [n_contigs + 1], CSR
     attr: "object"            # float32 [W, 5997]: d log p_target / d one-hot token, token t = bases t .. t+3 of the window
     logp: "object" = None     # integrated gradients only: float32 [W, 2], log p_target(window), log p_target(baseline)
+                              # (novelty: D_target(window), D_target(baseline))
     head_probs: "object" = None   # Head.attribute_contigs / integrated_gradients_contigs: float32 [W, C], the head's scores
+                                  # (novelty: the window's distances to every class)
+    target: "object" = None   # Head.attribute_novelty_contigs / integrated_gradients_novelty_contigs: int32 [W], each window's
+                              # target, its sequence's nearest class
 
 
 CLASSES = ("chromosome", "plasmid", "virus")
@@ -952,7 +965,7 @@ class Classifier:
                   "conv_dbg": (self.get_option("num_sms"), 16), "routeq0": (n, 749, 128), "routeq1": (n, 749, 128),
                   "route0": (n, 749, 128), "route1": (n, 749, 128), "attr_y1": (n, TOKENS, 128), "attr_g_out": (n, 256),
                   "attr_s_w": (n,), "attr_s2": (n,), "attr_gz3": (n, TOKENS, 128), "attr_gz2": (n, TOKENS, 128),
-                  "attr_gy1": (n, TOKENS, 128), "attr_gz1": (n, TOKENS, 128)}
+                  "attr_gy1": (n, TOKENS, 128), "attr_gz1": (n, TOKENS, 128), "attr_g_h1": (n, EMBED)}
         dtype = t.uint8 if which in ("route0", "route1") else t.float32
         out = t.empty(shapes[which], dtype=dtype, device=self._dev())
         _check(self.lib, self.lib.gnm_debug_fetch(self._h, which.encode(), n, out.data_ptr(), self._stream()))
@@ -1255,6 +1268,137 @@ class Head:
         """attribute_contigs by integrated gradients, with logp [W, 2] of the head's class."""
         return self._contig_record(seqs, single_window,
                                    lambda s, b, l: self.integrated_gradients_windows(s, b, l, target, steps, baseline))
+
+    # ------------------------------------------------------------------ attributions of the novelty distance
+    def novelty_targets(self, target, n: int) -> np.ndarray:
+        """A class of the head (index or name) or an int array [n] of classes -> host int32 [n], each entry checked."""
+        if isinstance(target, (str, int, np.integer)):
+            return np.full(n, self.class_index(target), np.int32)
+        tg = target.cpu().numpy() if hasattr(target, "cpu") else np.asarray(target)
+        if tg.shape != (n,) or tg.dtype.kind not in "iu":
+            raise ValueError(f"target must be a class of the head or an integer array of {n} classes, not {tg.dtype} {tg.shape}")
+        bad = np.flatnonzero((tg < 0) | (tg >= self.n_classes))
+        if bad.size:
+            raise ValueError(f"target[{bad[0]}] = {tg[bad[0]]} is not a class of the head, in [0, {self.n_classes})")
+        return np.ascontiguousarray(tg, dtype=np.int32)
+
+    def _novelty_out(self, n, device, ig):
+        t = self.clf._torch
+        probs = t.empty((n, 3), dtype=t.float32, device=device)
+        dist = t.empty((n, self.n_classes), dtype=t.float32, device=device)
+        dist_target = t.empty((n, 2), dtype=t.float32, device=device) if ig else None
+        attr = t.empty((n, TOKENS), dtype=t.float32, device=device)
+        return probs, dist, dist_target, attr
+
+    def attribute_novelty_ascii(self, ascii_windows, target):
+        """uint8 cuda [n, 6000], target class(es) (a class of the head, or an int array [n]) -> (probabilities float32 [n, 3],
+        distances [n, C], attributions [n, 5997]): attr[i, t] = d D_c / d x[t, tok[t]] for window i's whitened distance D_c to
+        its target class c (gnm_attribute_novelty_ascii).  The probabilities are bitwise those of Classifier.predict_ascii, the
+        distances those of novelty(embed_ascii(...))."""
+        clf = self.clf
+        a = ascii_windows.contiguous()
+        assert a.dtype == clf._torch.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        n = a.shape[0]
+        tg = self.novelty_targets(target, n)
+        probs, dist, _, attr = self._novelty_out(n, a.device, False)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_novelty_ascii(clf._h, clf._attr_ctx(), self._hd, a.data_ptr(), n, _ptr(tg),
+                                                                  probs.data_ptr(), dist.data_ptr(), attr.data_ptr(),
+                                                                  clf._stream()))
+        return probs, dist, attr
+
+    def attribute_novelty_windows(self, seq_u8, win_start, win_len, target):
+        """Planned windows of a sequence buffer -> (probabilities [W, 3], distances [W, C], attributions [W, 5997])."""
+        clf, t = self.clf, self.clf._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        n = start.numel()
+        tg = self.novelty_targets(target, n)
+        probs, dist, _, attr = self._novelty_out(n, seq_u8.device, False)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_novelty_windows(clf._h, clf._attr_ctx(), self._hd, seq_u8.data_ptr(),
+                                                                    start.data_ptr(), length.data_ptr(), n, _ptr(tg),
+                                                                    probs.data_ptr(), dist.data_ptr(), attr.data_ptr(),
+                                                                    clf._stream()))
+        return probs, dist, attr
+
+    def integrated_gradients_novelty_ascii(self, ascii_windows, target, steps: int = IG_STEPS, baseline="zero"):
+        """uint8 cuda [n, 6000], target class(es) -> (probabilities [n, 3], distances [n, C], dist_target [n, 2] = (D_c(x),
+        D_c(x')), attributions [n, 5997]) by integrated gradients of D_c (gnm_attribute_novelty_ig_ascii; the rule of
+        Classifier.integrated_gradients_ascii).  The attributions add up to about D_c(x) - D_c(x')."""
+        clf = self.clf
+        a = ascii_windows.contiguous()
+        assert a.dtype == clf._torch.uint8 and a.dim() == 2 and a.shape[1] == WINDOW and a.is_cuda
+        n = a.shape[0]
+        tg = self.novelty_targets(target, n)
+        m, b = clf._ig_args(steps, baseline)
+        probs, dist, dist_target, attr = self._novelty_out(n, a.device, True)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_novelty_ig_ascii(clf._h, clf._attr_ctx(), self._hd, a.data_ptr(), n, _ptr(tg),
+                                                                     m, b, probs.data_ptr(), dist.data_ptr(),
+                                                                     dist_target.data_ptr(), attr.data_ptr(), clf._stream()))
+        return probs, dist, dist_target, attr
+
+    def integrated_gradients_novelty_windows(self, seq_u8, win_start, win_len, target, steps: int = IG_STEPS,
+                                             baseline="zero"):
+        """Planned windows of a sequence buffer -> (probabilities [W, 3], distances [W, C], dist_target [W, 2], attributions
+        [W, 5997]) by integrated gradients of D_c (see integrated_gradients_novelty_ascii)."""
+        clf, t = self.clf, self.clf._torch
+        start, length = win_start.contiguous(), win_len.contiguous()
+        assert start.dtype == t.int64 and length.dtype == t.int32 and start.numel() == length.numel()
+        n = start.numel()
+        tg = self.novelty_targets(target, n)
+        m, b = clf._ig_args(steps, baseline)
+        probs, dist, dist_target, attr = self._novelty_out(n, seq_u8.device, True)
+        if n:
+            _check(self.lib, self.lib.gnm_attribute_novelty_ig_windows(clf._h, clf._attr_ctx(), self._hd, seq_u8.data_ptr(),
+                                                                       start.data_ptr(), length.data_ptr(), n, _ptr(tg), m, b,
+                                                                       probs.data_ptr(), dist.data_ptr(),
+                                                                       dist_target.data_ptr(), attr.data_ptr(), clf._stream()))
+        return probs, dist, dist_target, attr
+
+    def nearest_window_targets(self, seqs, single_window: bool = False, names=None) -> np.ndarray:
+        """int32 [W]: each window of the contig pass gets its sequence's nearest class (novelty_contigs + novelty_scores).  A
+        sequence with windows but no nearest class (a distance that is not finite) is refused, named from `names` if given."""
+        if not self.has_novelty:
+            raise GnmError("the head has no novelty model (train-head --novelty)")
+        dist, counts = self.novelty_contigs(seqs, single_window)
+        counts = counts.cpu().numpy()
+        cal = self.calibration if self.calibration is not None else np.zeros(0, np.float32)
+        _, nearest, _ = novelty_scores(dist.cpu().numpy(), counts, cal)
+        bad = np.flatnonzero((nearest < 0) & (counts > 0))
+        if bad.size:
+            i = int(bad[0])
+            who = names[i] if names is not None else f"sequence {i}"
+            raise GnmError(f"{who}: its window distances are not finite, so it has no nearest class to attribute")
+        return np.repeat(nearest, counts).astype(np.int32)
+
+    def _novelty_record(self, seqs, single_window, attr_fn, names=None):
+        clf, t = self.clf, self.clf._torch
+        target = self.nearest_window_targets(seqs, single_window, names)
+        seq, offs = clf.contig_buffers(seqs)
+        start, length, woff = clf.contig_windows(seq, offs, single_window)
+        n = woff.numel() - 1
+        counts = (woff[1:] - woff[:-1]).to(t.int64)
+        contig = t.repeat_interleave(t.arange(n, dtype=t.int32, device=seq.device), counts)
+        out = attr_fn(seq, start, length, target)
+        rel = start - offs[:-1].index_select(0, contig.to(t.int64)) if start.numel() else start
+        dist_target = out[2] if len(out) == 4 else None
+        return Attributions(out[0], contig, rel, length, woff, out[-1], dist_target, out[1],
+                            t.from_numpy(target).to(seq.device))
+
+    def attribute_novelty_contigs(self, seqs, single_window: bool = False, names=None) -> "Attributions":
+        """Attributions of every window of the contig pass to its distance to its sequence's nearest class (the class the
+        novelty file reports), with head_probs the windows' distances [W, C] and target their class [W].  A sequence with
+        windows but no nearest class is refused, by its name in `names` when given."""
+        return self._novelty_record(seqs, single_window, self.attribute_novelty_windows, names)
+
+    def integrated_gradients_novelty_contigs(self, seqs, steps: int = IG_STEPS, baseline="zero",
+                                             single_window: bool = False, names=None) -> "Attributions":
+        """attribute_novelty_contigs by integrated gradients, with logp [W, 2] = (D_c(window), D_c(baseline))."""
+        return self._novelty_record(seqs, single_window,
+                                    lambda s, b, l, tg: self.integrated_gradients_novelty_windows(s, b, l, tg, steps, baseline),
+                                    names)
 
     def _segment(self, fn, probs, offsets, width):
         t = self.clf._torch

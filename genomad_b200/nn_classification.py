@@ -130,6 +130,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     With head["novelty"] true (the head carries a novelty model), the head also scores each window's embedding by
     Head.novelty into a second buffer of this rank's shard, reduced per contig the same way and stored as head["novelty_dist"]
     (float32 [n_contigs, C], identical on all ranks).
+    With attributions["novelty"] (int32 [n_windows], each window's target class, in global window order), the calls are the
+    head's novelty ones (Head.attribute_novelty_ascii / integrated_gradients_novelty_ascii) and each window's distance to its
+    target travels to rank 0 as attributions["distance"] (float32 [n_windows]), with IG's (D_c(x), D_c(x')) rows as
+    attributions["logp"].  With head["windows"] and head["novelty"] true, and head["window_novelty_wanted"] or no offsets, the
+    windows' novelty rows are collected on rank 0 too, as head["window_novelty"] (float32 [n_windows, C]).
     With `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
     """
     import torch
@@ -180,11 +185,23 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
             d_logp = torch.empty((end - start, 2), dtype=torch.float32, device=dev)
 
         head_route = bool(attributions.get("head"))
-        assert not head_route or scorer is not None
+        nov_targets = attributions.get("novelty")            # the novelty route: each window's target class, global order
+        assert not (head_route or nov_targets is not None) or scorer is not None
+        if nov_targets is not None:
+            d_distance = torch.empty((end - start, 1), dtype=torch.float32, device=dev)
 
         def run(win, m, row):                                # probabilities and attributions from the attribution calls
             d_win = torch.from_numpy(win[:m]).to(dev)
-            if head_route:                                   # the head's scores come out of the same call
+            if nov_targets is not None:                      # the head's novelty distance to each window's target
+                tg = np.ascontiguousarray(nov_targets[start + row: start + row + m], dtype=np.int32)
+                if ig_steps:
+                    probs, dist, dt, attr = scorer.integrated_gradients_novelty_ascii(d_win, tg, ig_steps,
+                                                                                      attributions["baseline"])
+                    d_logp[row: row + m].copy_(dt)
+                else:
+                    probs, dist, attr = scorer.attribute_novelty_ascii(d_win, tg)
+                d_distance[row: row + m].copy_(dist.gather(1, torch.from_numpy(tg).to(dist.device, torch.int64)[:, None]))
+            elif head_route:                                 # the head's scores come out of the same call
                 if ig_steps:
                     probs, head_probs, logp, attr = scorer.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
                                                                                       attributions["baseline"])
@@ -200,11 +217,11 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
                 probs, attr = clf.attribute_ascii(d_win, attributions["target"])
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
-            if embeddings or nov or (scorer is not None and not head_route):
+            if embeddings or nov or (scorer is not None and not head_route and nov_targets is None):
                 e = clf.embed_ascii(d_win)[1]
                 if embeddings:
                     shard.add(e)
-                if scorer is not None and not head_route:
+                if scorer is not None and not head_route and nov_targets is None:
                     scorer.predict(e, out=d_head[row: row + m])
                 if nov:
                     scorer.novelty(e, out=d_nov[row: row + m])
@@ -241,12 +258,18 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     if scorer is not None and head.get("windows"):
         full = gdist.collect_window_probs(d_head, n, info)
         head["window_preds"] = full.cpu().numpy() if full is not None else None
+        if nov and (offsets is None or head.get("window_novelty_wanted")):
+            full = gdist.collect_window_probs(d_nov, n, info)
+            head["window_novelty"] = full.cpu().numpy() if full is not None else None
     if attributions is not None:
         full = gdist.collect_window_probs(d_attr, n, info)
         attributions["attr"] = full.cpu().numpy() if full is not None else None
         if ig_steps:
             full = gdist.collect_window_probs(d_logp, n, info)
             attributions["logp"] = full.cpu().numpy() if full is not None else None
+        if nov_targets is not None:
+            full = gdist.collect_window_probs(d_distance, n, info)
+            attributions["distance"] = full.reshape(-1).cpu().numpy() if full is not None else None
     if not out:
         return None
     return out[0] if len(out) == 1 else tuple(out)
@@ -394,9 +417,11 @@ def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, i
     wl = parsed.windows(stride)
     try:
         if head is not None:
-            profile = {"head": head["head"], "windows": True}
+            profile = {"head": head["head"], "windows": True, "novelty": bool(head.get("window_novelty_wanted"))}
             probs = _classify_parsed(clf, wl, None, info, window_probs=True, head=profile)
             head["window_preds"] = profile["window_preds"]
+            if profile["novelty"]:
+                head["window_novelty"] = profile["window_novelty"]
         else:
             probs = _classify_parsed(clf, wl, None, info, window_probs=True)
         offsets, starts, lengths = wl.spans() if info.is_main else (None, None, None)
@@ -472,6 +497,25 @@ def head_attributions_target(value=None):
     if value is False or value is None or str(value).strip() in ("", "0"):
         return None
     return str(value).strip()
+
+
+def novelty_attributions_enabled(value=None) -> bool:
+    """``--write-novelty-attributions`` / GENOMAD_B200_NOVELTY_ATTRIBUTIONS=1 / main(..., write_novelty_attributions=True):
+    attribute each window's distance to its sequence's nearest class of the --head novelty model."""
+    if value is None:
+        return os.environ.get("GENOMAD_B200_NOVELTY_ATTRIBUTIONS", "0") not in ("", "0")
+    return bool(value)
+
+
+def window_novelty_enabled(value=None) -> bool:
+    """``--write-window-novelty`` / GENOMAD_B200_WINDOW_NOVELTY=1 / main(..., write_window_novelty=True): write every window's
+    distances to the --head novelty model's classes."""
+    if value is None:
+        return os.environ.get("GENOMAD_B200_WINDOW_NOVELTY", "0") not in ("", "0")
+    return bool(value)
+
+
+NOVELTY_TARGET = "nearest_class"
 
 
 def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr, steps: int = 0,
@@ -569,6 +613,60 @@ def _write_head_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, d
                 fout.write(f"{name}\tNA\tNA\tNA\n")
             else:
                 fout.write(f"{name}\t{class_names[c]}\t{float(v):.6g}\t{float(pv):.6g}\n")
+
+
+def _write_novelty_attributions(path: Path, names_key: str, names, offsets, starts, lengths, rec, steps: int, baseline: str,
+                                class_names, head_sha: str) -> None:
+    """<prefix>_nn_classification_head_novelty_attributions.npz: the attribution file's keys with target "nearest_class",
+    each window's target_class int32 [W] and distance float32 [W] (D of the window to that class), class_names, head_sha256;
+    with integrated gradients also method, steps, baseline and distance_target float32 [W, 2] = (D_c(x), D_c(x'))."""
+    extra = {"target_class": np.asarray(rec["target_class"], dtype=np.int32),
+             "distance": np.asarray(rec["distance"], dtype=np.float32).reshape(-1),
+             "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)}
+    if steps:
+        extra.update({"method": np.str_(IG_METHOD), "steps": np.int32(steps), "baseline": np.str_(baseline),
+                      "distance_target": np.asarray(rec["logp"], dtype=np.float32).reshape(-1, 2)})
+    _write_attributions(path, names_key, names, offsets, starts, lengths, NOVELTY_TARGET, rec["attr"], extra=extra)
+
+
+def _write_window_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, offsets, starts, lengths, dist, stride: int,
+                          class_names, head_sha: str, threads: int) -> None:
+    """<prefix>_nn_classification_head_novelty_windows.{npz,tsv}: the window-score files' windows and coordinate keys, each
+    window's distances float32 [W, C] to the head's classes, novelty [W] (the row minimum), nearest_class int32 [W] (lowest
+    index on ties; -1 and NaN for a row that is not all finite), window_stride, class_names and head_sha256.  The TSV holds
+    the coordinates, the novelty and one distance column per class."""
+    C = len(class_names)
+    offsets = np.asarray(offsets, dtype=np.int32)
+    dist = np.asarray(dist, dtype=np.float32).reshape(-1, C)
+    ok = np.isfinite(dist).all(1)
+    nov = np.full(len(dist), np.nan, np.float32)
+    nearest = np.full(len(dist), -1, np.int32)
+    if ok.any():
+        nov[ok] = dist[ok].min(1)
+        nearest[ok] = dist[ok].argmin(1)
+    np.savez(npz_path, **{names_key: names,
+                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+                          "window_start": np.asarray(starts, dtype=np.int64),
+                          "window_length": np.asarray(lengths, dtype=np.int32),
+                          "window_stride": np.int32(stride),
+                          "distances": dist, "novelty": nov, "nearest_class": nearest,
+                          "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)})
+    header = "seq_name\tstart\tend\tnovelty\t" + "\t".join(f"{c}_distance" for c in class_names) + "\n"
+    _write_window_tsv(tsv_path, names, offsets, starts, lengths, np.concatenate([nov[:, None], dist], 1), threads,
+                      header=header, n_cols=C + 1)
+
+
+def _novelty_window_targets(dist, counts, calibration, names) -> np.ndarray:
+    """int32 [W]: every window of the contig pass gets its sequence's nearest class (engine.novelty_scores of the novelty
+    file's distances).  A sequence with windows but no nearest class (a distance that is not finite) is refused by name."""
+    from .engine import GnmError, novelty_scores
+    counts = np.asarray(counts, np.int64)
+    _, nearest, _ = novelty_scores(dist, counts, calibration)
+    bad = np.flatnonzero((nearest < 0) & (counts > 0))
+    if bad.size:
+        raise GnmError(f"{names[int(bad[0])]}: its window distances to the head's classes are not finite, so it has no "
+                       "nearest class to attribute")
+    return np.repeat(nearest, counts).astype(np.int32)
 
 
 def _head_has_novelty(path) -> bool:
@@ -757,7 +855,8 @@ _attribution_steps, _attribution_baseline = attribution_steps, attribution_basel
 
 def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
          write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
-         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None, write_head_attributions=None):
+         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None, write_head_attributions=None,
+         write_novelty_attributions=None, write_window_novelty=None):
     import time as _time
     t_start = _time.perf_counter()
     last_timings.clear()
@@ -778,7 +877,16 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if head_attr_target is not None and attr_target:
         raise ValueError("--write-head-attributions and --write-attributions cannot be combined in one run: the contig pass "
                          "runs through one kind of attribution call")
-    any_attr = bool(attr_target or head_attr_target)
+    nov_attr = novelty_attributions_enabled(write_novelty_attributions)
+    window_nov = window_novelty_enabled(write_window_novelty)
+    if nov_attr and head is None:
+        raise ValueError("--write-novelty-attributions needs --head: it attributes the distance to the head's novelty model")
+    if nov_attr and (attr_target or head_attr_target):
+        raise ValueError("--write-novelty-attributions cannot be combined with --write-attributions or "
+                         "--write-head-attributions: a run writes one attribution file")
+    if window_nov and head is None:
+        raise ValueError("--write-window-novelty needs --head: it scores the windows by the head's novelty model")
+    any_attr = bool(attr_target or head_attr_target or nov_attr)
     # both options are validated whether or not they take effect; an option without effect is reported in the log
     steps_opt, baseline_opt = _attribution_steps(attribution_steps), _attribution_baseline(attribution_baseline)
     baseline_given = attribution_baseline is not None or bool(os.environ.get("GENOMAD_B200_ATTRIBUTION_BASELINE", "").strip())
@@ -845,6 +953,15 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     if head_attr_target:
         files.append(outputs.nn_classification_head_attributions_output)
         descr.append(f"window attributions of the --head classifier ({head_attr_target}{attr_method}): binary format")
+    if nov_attr:
+        files.append(outputs.nn_classification_head_novelty_attributions_output)
+        descr.append(f"window attributions of the distance to the nearest class of the --head novelty model{attr_method}: "
+                     "binary format")
+    if window_nov:
+        files += [outputs.nn_classification_head_novelty_windows_output,
+                  outputs.nn_classification_head_novelty_windows_npz_output]
+        descr += ["window novelty with respect to the --head classifier's classes: tabular format",
+                  "window novelty with respect to the --head classifier's classes: binary format"]
     if classify_proviruses:
         files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
                   outputs.provirus_nn_classification_npz_output]
@@ -886,6 +1003,15 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
             files.append(outputs.provirus_nn_classification_head_attributions_output)
             descr.append(f"provirus window attributions of the --head classifier ({head_attr_target}{attr_method}): "
                          "binary format")
+        if nov_attr:
+            files.append(outputs.provirus_nn_classification_head_novelty_attributions_output)
+            descr.append("provirus window attributions of the distance to the nearest class of the --head novelty model"
+                         f"{attr_method}: binary format")
+        if window_nov:
+            files += [outputs.provirus_nn_classification_head_novelty_windows_output,
+                      outputs.provirus_nn_classification_head_novelty_windows_npz_output]
+            descr += ["provirus window novelty with respect to the --head classifier's classes: tabular format",
+                      "provirus window novelty with respect to the --head classifier's classes: binary format"]
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
@@ -901,6 +1027,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if head_attr_target is not None and head_attr_target not in head_file.class_names:
             console.error(f"--write-head-attributions {head_attr_target}: not a class of {head} "
                           f"({', '.join(head_file.class_names)})")
+            sys.exit(1)
+        if (nov_attr or window_nov) and head_file.novelty is None:
+            opt = "--write-novelty-attributions" if nov_attr else "--write-window-novelty"
+            console.error(f"{opt}: {head} carries no novelty model (train-head --novelty)")
             sys.exit(1)
     ig_clf = None
     if ig_steps:                     # the steps must fit this device's attribution context: fail before any work
@@ -924,7 +1054,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
              outputs.nn_classification_head_attributions_output,
              outputs.nn_classification_head_strands_npz_output, outputs.nn_classification_head_strands_output,
              outputs.nn_classification_head_windows_npz_output, outputs.nn_classification_head_windows_output,
-             outputs.nn_classification_head_novelty_npz_output, outputs.nn_classification_head_novelty_output)]
+             outputs.nn_classification_head_novelty_npz_output, outputs.nn_classification_head_novelty_output,
+             outputs.nn_classification_head_novelty_attributions_output,
+             outputs.nn_classification_head_novelty_windows_npz_output,
+             outputs.nn_classification_head_novelty_windows_output)]
     if classify_proviruses:
         jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
                      outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
@@ -939,7 +1072,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                      outputs.provirus_nn_classification_head_windows_npz_output,
                      outputs.provirus_nn_classification_head_windows_output,
                      outputs.provirus_nn_classification_head_novelty_npz_output,
-                     outputs.provirus_nn_classification_head_novelty_output))
+                     outputs.provirus_nn_classification_head_novelty_output,
+                     outputs.provirus_nn_classification_head_novelty_attributions_output,
+                     outputs.provirus_nn_classification_head_novelty_windows_npz_output,
+                     outputs.provirus_nn_classification_head_novelty_windows_output))
 
     plan = None
     info_writer = None
@@ -972,7 +1108,10 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                            or _head_windows_current(j[21], j[22], head_sha, window_stride))
                       and (not head_attr_target
                            or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))
-                      and (head_file is None or head_file.novelty is None or _head_current(j[23], j[24], head_sha))))
+                      and (head_file is None or head_file.novelty is None or _head_current(j[23], j[24], head_sha))
+                      and (not nov_attr
+                           or _head_attributions_current(j[25], NOVELTY_TARGET, head_sha, ig_steps, ig_baseline))
+                      and (not window_nov or _head_windows_current(j[26], j[27], head_sha, window_stride))))
                 for j in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
@@ -1026,7 +1165,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
          win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path,
          head_attr_path, head_strands_npz_path, head_strands_tsv_path, head_win_npz_path, head_win_tsv_path,
-         head_nov_npz_path, head_nov_tsv_path), \
+         head_nov_npz_path, head_nov_tsv_path, nov_attr_path, win_nov_npz_path, win_nov_tsv_path), \
             (enc_skip, cls_skip), (parsed, index) \
             in zip(jobs, plan, staged):
         names = preds = emb = None
@@ -1062,11 +1201,15 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     hd = {"preds": np.zeros((len(index.names), C), np.float32), "window_preds": np.zeros((0, C), np.float32)}
                     hd["reverse_preds"] = hd["preds"]
                     hd["novelty_dist"], hd["counts"] = hd["preds"], np.zeros(len(index.names), np.int64)
+                    hd["window_novelty"] = hd["window_preds"]
                 emb = np.zeros((len(index.names), 512), np.float32)
                 win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
                        np.zeros((0, 3), np.float32))
                 if attr is not None:
                     attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), logp=np.zeros((0, 2), np.float32), spans=win[:3])
+                if nov_attr:
+                    nov_rec = {"attr": np.zeros((0, ATTR_TOKENS), np.float32), "logp": np.zeros((0, 2), np.float32),
+                               "distance": np.zeros(0, np.float32), "target_class": np.zeros(0, np.int32), "spans": win[:3]}
                 rev_preds, rev_emb = preds, emb
             else:
                 t_c = _time.perf_counter()
@@ -1076,8 +1219,9 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     if head_file.novelty is not None:
                         hd["novelty"] = True
                         hd["counts"] = np.diff(np.asarray(index.offsets, np.int64))
+                        hd["window_novelty_wanted"] = window_nov
                     ak["head"] = hd
-                if write_window_scores:
+                if write_window_scores or window_nov:
                     preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
                                                             contig_reduce, write_embeddings, **ak)
                 elif write_embeddings:
@@ -1086,6 +1230,22 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                     preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, **ak)
                 if attr is not None:
                     attr["spans"] = (index.offsets, *parsed.spans()) if is_main else None
+                if nov_attr:
+                    # a second pass over the contig pass's windows through the novelty attribution calls, each window
+                    # against its sequence's nearest class (head["novelty_dist"] is the same on every rank)
+                    t_n = _time.perf_counter()
+                    try:
+                        targets = _novelty_window_targets(hd["novelty_dist"], hd["counts"],
+                                                          head_file.novelty["novelty_calibration"], index.names)
+                    except Exception as e:
+                        console.error(str(e))
+                        sys.exit(1)
+                    nov_rec = {"target": NOVELTY_TARGET, "novelty": targets,
+                               **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
+                    _classify_parsed(classifier(), parsed, None, info, attributions=nov_rec, head={"head": head_scorer()})
+                    nov_rec["target_class"] = targets
+                    nov_rec["spans"] = (index.offsets, *parsed.spans()) if is_main else None
+                    last_timings[f"novelty_attributions_{what}_s"] = _time.perf_counter() - t_n
                 if strands:
                     rev_preds, rev_emb = _classify_reverse(classifier(), parsed, single_window, info, contig_reduce,
                                                            write_embeddings, head=hd)
@@ -1121,6 +1281,18 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                                             head_sha)
                     console.log(f"{label} novelty with respect to the head's classes (forward strand) written to "
                                 f"{head_nov_tsv_path.name} and {head_nov_npz_path.name}.")
+            if window_nov:
+                if is_main:
+                    _write_window_novelty(win_nov_npz_path, win_nov_tsv_path, names_key, names, *win[:3], hd["window_novelty"],
+                                          window_stride, head_file.class_names, head_sha, threads or 1)
+                console.log(f"{label} window novelty (stride {window_stride}) written to {win_nov_tsv_path.name} and "
+                            f"{win_nov_npz_path.name}.")
+            if nov_attr:
+                if is_main:
+                    _write_novelty_attributions(nov_attr_path, names_key, names, *nov_rec["spans"], nov_rec, ig_steps,
+                                                ig_baseline, head_file.class_names, head_sha)
+                console.log(f"{label} window attributions of the distance to the nearest class{attr_method} in binary "
+                            f"format written to {nov_attr_path.name}.")
             if write_window_scores:
                 if is_main:
                     _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,

@@ -413,7 +413,8 @@ int gnm_stage_times(gnm_handle* h, const char** names, float* ms, int* count);
  * written to d_dst; "routeq0","routeq1" [n][749][128] = the maxima the routing pass found (bitwise "q0","q1"); "attr_y1"
  * [n][5997][128] = its layer-1 copy (y1, bitwise what the forward's layer 1 wrote).  An attribution
  * call re-runs IGLOO#0's logits, so "logits" then holds the first IGLOO kernel's.  The backward pass's intermediates, same
- * conditions, positions in natural order: "attr_g_out" [n][256] = d log p_c / d h0 (unscaled); "attr_s_w" [n] = the per-window
+ * conditions, positions in natural order: "attr_g_out" [n][256] = d log p_c / d h0 (unscaled; d D_c / d h0 after a novelty
+ * attribution call); "attr_g_h1" [n][512] = d D_c / d h1 of the last novelty attribution chunk (fp32); "attr_s_w" [n] = the per-window
  * power of two s_w; "attr_s2" [n] = the power of two of conv3's backward output (max |s_w g_z2| s2 in [1, 2)); "attr_gz3",
  * "attr_gz2" [n][5997][128] = s_w g_z3 and s2 s_w g_z2 as the next conv reads them (the joined hi16 + lo8 of the operand rows);
  * "attr_gy1" [n][5997][128] = IGLOO#0's part of g_y1 (fp32, unscaled); "attr_gz1" [n][5997][128] = s_w g_z1 (fp32).  After an
@@ -534,6 +535,47 @@ int gnm_attribute_head_ig_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head
 int gnm_attribute_head_ig_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
                                   const int64_t* d_win_start, const int32_t* d_win_len, int n, int target, int steps, int baseline,
                                   float* d_probs, float* d_head_probs, float* d_logp, float* d_attr, void* stream);
+
+/*
+ * Novelty attributions: the same passes for a head's novelty distance (gnm_head_set_novelty, below) to a target class, so that
+ * a window flagged as novel can be explained.  For a window's encoder output h1 (gnm_embed_*) and its target class c:
+ *
+ *     r = P (h1 - center) - m_c;   D_c = ||r||^2 / 512;   g_h1 = dD_c / dh1 = (2 / 512) P^T r
+ *     attr[t] = d D_c / d x[t, tok[t]]     (D_c itself, not its log)
+ *
+ * r and g_h1 are computed in fp64 on the tensor cores (r's Y as gnm_head_novelty computes it; P^T r over the tiles where P is
+ * not zero, k ascending) and g_h1 is rounded to fp32 once; from there the pass is gnm_attribute_head_*'s from dense layer 0
+ * down, with the same routing rule and LeakyReLU branches.  No atomics: a window's row does not depend on its batch, its
+ * position in it, n or the chunking.  IG uses the same midpoint rule and baselines; sum_t IG[t] -> D_c(x) - D_c(x').
+ *
+ * gnm_attribute_novelty_ascii / _windows, gnm_attribute_novelty_ig_ascii / _ig_windows: arguments as gnm_attribute_head_*, except
+ *   head           a head created on h that carries a novelty model; one without is refused.
+ *   h_target       HOST int32 [n]: each window's target class.  Every entry is checked before any launch; one outside [0, C)
+ *                  is refused, naming its index.
+ *   d_probs        DEVICE float [n][3] or NULL: bitwise what gnm_forward_* returns.
+ *   d_dist         DEVICE float [n][C] or NULL: the windows' distances, bitwise gnm_head_novelty on the gnm_embed_* output of the
+ *                  same windows.
+ *   d_dist_target  (IG) DEVICE float [n][2] or NULL: D_c(x), bitwise d_dist[w][c], and D_c(x') from one one-row forward of the
+ *                  baseline per call.
+ *   Per chunk, three fp64 kernels (~1 MFLOP per window; 1.02x the time of gnm_attribute_head_* on an H100) instead of the
+ *   head's forward and backward; the context's memory holds
+ *   4 KB of r and 2 KB of g_h1 per window.  A gradient that is not finite is reported as for gnm_attribute_*.  Refused under
+ *   conv_impl = 1 or a debug_stop.  gnm_debug_fetch "attr_g_h1" [n][512] holds the last chunk's fp32 g_h1 rows.  Work is queued
+ *   on `stream`, but the call is not fully asynchronous: each chunk's targets are copied from pageable host memory, which can
+ *   make the host wait for the previous chunk's kernels before it issues the next chunk.
+ */
+int gnm_attribute_novelty_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                const int32_t* h_target, float* d_probs, float* d_dist, float* d_attr, void* stream);
+int gnm_attribute_novelty_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                  const int64_t* d_win_start, const int32_t* d_win_len, int n, const int32_t* h_target,
+                                  float* d_probs, float* d_dist, float* d_attr, void* stream);
+int gnm_attribute_novelty_ig_ascii(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_ascii, int n,
+                                   const int32_t* h_target, int steps, int baseline, float* d_probs, float* d_dist,
+                                   float* d_dist_target, float* d_attr, void* stream);
+int gnm_attribute_novelty_ig_windows(gnm_handle* h, gnm_attr* a, const gnm_head* head, const uint8_t* d_seq,
+                                     const int64_t* d_win_start, const int32_t* d_win_len, int n, const int32_t* h_target,
+                                     int steps, int baseline, float* d_probs, float* d_dist, float* d_dist_target, float* d_attr,
+                                     void* stream);
 
 /*
  * Embedding neighbours: for each query row, the k reference rows nearest in cosine similarity.  Rows are GNM_EMBED (512) fp32

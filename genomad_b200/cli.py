@@ -218,6 +218,29 @@ def embedding_clusters(input, output, min_similarity, both_strands, verbose):
     module.main(input, output, min_similarity, verbose, both_strands=both_strands)
 
 
+@cli.command(name="embedding-map", context_settings=CONTEXT_SETTINGS)
+@click.argument("input", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("-k", "k", type=int, default=15, show_default=True,
+              help="Neighbours of each sequence the map keeps close, other sequences only (1 to 64, fewer than the sequences; "
+                   "umap-learn's n_neighbors = k + 1).")
+@click.option("--epochs", type=int, default=None, show_default="500 for up to 10,000 sequences, else 200",
+              help="Layout epochs.")
+@click.option("--seed", type=int, default=0, show_default=True,
+              help="Seed of the initial noise and the negative samples: the same seed gives bitwise the same map.")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Map the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
+                   "--write-embeddings --both-strands), so a sequence and its reverse complement get the same point.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def embedding_map(input, output, k, epochs, seed, both_strands, verbose):
+    """Map the sequences of the INPUT embeddings file (nn-classification --write-embeddings output) onto two dimensions with
+    UMAP on the GPU, and write each sequence's coordinates to the OUTPUT directory as <prefix>_embedding_map.{tsv,npz}.
+    Not a module of the reference."""
+    from . import embedding_map as module
+    module.main(input, output, k, epochs, seed, verbose, both_strands=both_strands)
+
+
 @cli.command(name="window-regions", context_settings=CONTEXT_SETTINGS)
 @click.argument("windows", type=click.Path(path_type=Path, exists=True, dir_okay=False))
 @click.argument("output", type=click.Path(path_type=Path))

@@ -28,6 +28,7 @@
 #include "head.cuh"
 #include "regions.cuh"
 #include "novelty.cuh"
+#include "layout.cuh"
 
 using namespace gnm;
 
@@ -2676,5 +2677,162 @@ extern "C" int gnm_head_train_fetch(gnm_head_train* tr, const char* which, void*
   else return fail("gnm_head_train_fetch: unknown buffer " + k);
   GNM_CUDA(cudaMemcpyAsync(h_dst, src, bytes, cudaMemcpyDeviceToHost, st));
   GNM_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ embedding map (layout.cuh)
+// No handle: the current device, the caller's stream and buffers.
+static int mp_check_n(const std::string& fn, int64_t n) {
+  if (n < 2 || n > kNbRowMax) return fail(fn + ": n must be in [2, 2^30], not " + std::to_string(n));
+  return 0;
+}
+
+extern "C" int gnm_map_membership(const float* d_sim, const int64_t* d_idx, int64_t n, int k, double* d_mean_d, double* d_rho,
+                                  double* d_sigma, double* d_w, double* d_union, void* stream) {
+  const std::string fn = "gnm_map_membership";
+  if (mp_check_n(fn, n)) return 1;
+  if (k < 1 || k > kMpMaxK || k >= n) return fail(fn + ": k must be in [1, min(64, n - 1)], not " + std::to_string(k));
+  if (!d_sim || !d_idx || !d_mean_d || !d_rho || !d_sigma || !d_w || !d_union) return fail(fn + ": null buffer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nn = static_cast<int>(n);
+  mp_mean_kernel<<<1, kMpMeanThreads, 0, st>>>(d_sim, nn, k, d_mean_d);
+  GNM_CUDA(cudaGetLastError());
+  mp_sigma_kernel<<<(nn + 7) / 8, 256, 0, st>>>(d_sim, nn, k, d_mean_d, d_rho, d_sigma, d_w);
+  GNM_CUDA(cudaGetLastError());
+  const long long e = static_cast<long long>(n) * k;
+  mp_union_kernel<<<static_cast<unsigned>((e + 255) / 256), 256, 0, st>>>(reinterpret_cast<const long long*>(d_idx), d_w, nn, k,
+                                                                         d_union);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Workspace of gnm_map_pca, each part 256-byte aligned: the novelty fit's status, fit rows and labels, class-sum partials and
+// counts, mean, count and scatter partials at C = 1.
+struct MpPcaLayout {
+  size_t status, idx, labels, part, cnt, mu, counts, spart, total;
+  int n_blocks, n_chunks;
+};
+static MpPcaLayout mp_pca_layout(int64_t n) {
+  MpPcaLayout l;
+  l.n_blocks = static_cast<int>((n + kNvSumRows - 1) / kNvSumRows);
+  l.n_chunks = static_cast<int>((n + kNvChunk - 1) / kNvChunk);
+  const size_t H = kHidden, nr = static_cast<size_t>(n);
+  size_t o = 0;
+  l.status = o; o += nb_align(sizeof(NvStatus));
+  l.idx = o; o += nb_align(nr * 8);
+  l.labels = o; o += nb_align(nr * 4);
+  l.part = o; o += nb_align(static_cast<size_t>(l.n_blocks) * H * 8);
+  l.cnt = o; o += nb_align(static_cast<size_t>(l.n_blocks) * 8);
+  l.mu = o; o += nb_align(H * 8);
+  l.counts = o; o += nb_align(8);
+  l.spart = o; o += nb_align(static_cast<size_t>(l.n_chunks) * kNvTriTiles * kNvTile * kNvTile * 8);
+  l.total = o;
+  return l;
+}
+
+extern "C" size_t gnm_map_pca_workspace_bytes(int64_t n) {
+  if (mp_check_n("gnm_map_pca_workspace_bytes", n)) return 0;
+  return mp_pca_layout(n).total;
+}
+
+extern "C" int gnm_map_pca(const float* d_rows, int64_t n, float* d_xhat, double* d_center, double* d_S, double* d_V, void* d_work,
+                           size_t work_bytes, void* stream) {
+  const std::string fn = "gnm_map_pca";
+  if (mp_check_n(fn, n)) return 1;
+  if (!d_rows || !d_xhat || !d_center || !d_S || !d_V || !d_work) return fail(fn + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(fn + ": d_work must be 256-byte aligned");
+  const MpPcaLayout l = mp_pca_layout(n);
+  if (work_bytes < l.total)
+    return fail(fn + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(l.total) +
+                " needed (gnm_map_pca_workspace_bytes)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nn = static_cast<int>(n);
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  NvStatus* status = reinterpret_cast<NvStatus*>(w + l.status);
+  long long* idx = reinterpret_cast<long long*>(w + l.idx);
+  int* labels = reinterpret_cast<int*>(w + l.labels);
+  double *part = reinterpret_cast<double*>(w + l.part), *mu = reinterpret_cast<double*>(w + l.mu);
+  double* spart = reinterpret_cast<double*>(w + l.spart);
+  long long *cnt = reinterpret_cast<long long*>(w + l.cnt), *counts = reinterpret_cast<long long*>(w + l.counts);
+  GNM_CUDA(cudaMemsetAsync(status, 0, sizeof(NvStatus), st));
+  mp_normalize_kernel<<<(nn + 7) / 8, 256, 0, st>>>(d_rows, nn, d_xhat);
+  GNM_CUDA(cudaGetLastError());
+  mp_iota_kernel<<<(nn + 255) / 256, 256, 0, st>>>(nn, idx, labels);
+  GNM_CUDA(cudaGetLastError());
+  const int64_t* fit = reinterpret_cast<const int64_t*>(idx);
+  GNM_CUDA(cudaFuncSetAttribute(nv_class_sums_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHidden * 8));
+  nv_class_sums_kernel<<<l.n_blocks, kHidden, kHidden * 8, st>>>(d_xhat, n, fit, labels, n, 1, part, cnt, status);
+  GNM_CUDA(cudaGetLastError());
+  nv_means_kernel<<<2, kHidden, 0, st>>>(part, cnt, l.n_blocks, 1, n, mu, d_center, counts, status);
+  GNM_CUDA(cudaGetLastError());
+  nv_scatter_kernel<<<dim3(kNvTriTiles, l.n_chunks), kNvThreads, 0, st>>>(d_xhat, n, fit, labels, n, 1, mu, spart, status);
+  GNM_CUDA(cudaGetLastError());
+  nv_scatter_reduce_kernel<<<dim3(kNvTriTiles, kNvTile * kNvTile / 256), 256, 0, st>>>(spart, l.n_chunks, n, d_S);
+  GNM_CUDA(cudaGetLastError());
+  mp_eig_kernel<<<1, kMpEigThreads, 0, st>>>(d_S, d_V);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Workspace of gnm_map_init: the projections [n][2] fp64, then max |projection| and the per-axis extent (fp64).
+static size_t mp_init_ext_offset(int64_t n) { return nb_align(static_cast<size_t>(n) * 16); }
+
+extern "C" size_t gnm_map_init_workspace_bytes(int64_t n) {
+  if (mp_check_n("gnm_map_init_workspace_bytes", n)) return 0;
+  return mp_init_ext_offset(n) + 256;
+}
+
+extern "C" int gnm_map_init(const float* d_xhat, int64_t n, const double* d_center, const double* d_V, uint64_t seed, float* d_Y,
+                            void* d_work, size_t work_bytes, void* stream) {
+  const std::string fn = "gnm_map_init";
+  if (mp_check_n(fn, n)) return 1;
+  if (!d_xhat || !d_center || !d_V || !d_Y || !d_work) return fail(fn + ": null buffer");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(fn + ": d_work must be 256-byte aligned");
+  const size_t need = gnm_map_init_workspace_bytes(n);
+  if (work_bytes < need)
+    return fail(fn + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(need) +
+                " needed (gnm_map_init_workspace_bytes)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nn = static_cast<int>(n);
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  double* proj = reinterpret_cast<double*>(w);
+  double* ext = reinterpret_cast<double*>(w + mp_init_ext_offset(n));     // [0] max |proj|; [1..4] min x, min y, max x, max y
+  mp_project_kernel<<<(nn + 7) / 8, 256, 0, st>>>(d_xhat, nn, d_center, d_V, proj);
+  GNM_CUDA(cudaGetLastError());
+  mp_extent_kernel<<<1, 1024, 0, st>>>(proj, nullptr, 2 * static_cast<long long>(n), ext);
+  GNM_CUDA(cudaGetLastError());
+  const unsigned grid = static_cast<unsigned>((2 * n + 255) / 256);
+  mp_noise_kernel<<<grid, 256, 0, st>>>(proj, nn, ext, head_key(seed), d_Y);
+  GNM_CUDA(cudaGetLastError());
+  mp_extent_kernel<<<1, 1024, 0, st>>>(nullptr, d_Y, n, ext + 1);
+  GNM_CUDA(cudaGetLastError());
+  mp_rescale_kernel<<<grid, 256, 0, st>>>(d_Y, nn, ext + 1);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gnm_map_epochs(const int64_t* d_row_ptr, const int32_t* d_col, const double* d_eps, int64_t n, int epochs,
+                              int e_begin, int e_end, uint64_t seed, float* d_Y, float* d_Y_tmp, void* stream) {
+  const std::string fn = "gnm_map_epochs";
+  if (mp_check_n(fn, n)) return 1;
+  if (epochs < 1 || e_begin < 0 || e_end < e_begin || e_end > epochs)
+    return fail(fn + ": need epochs >= 1 and 0 <= e_begin <= e_end <= epochs, not " + std::to_string(epochs) + ", " +
+                std::to_string(e_begin) + ", " + std::to_string(e_end));
+  if (!d_row_ptr || !d_col || !d_eps || !d_Y || !d_Y_tmp) return fail(fn + ": null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_Y) | reinterpret_cast<uintptr_t>(d_Y_tmp)) % 8)
+    return fail(fn + ": d_Y and d_Y_tmp must be 8-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nn = static_cast<int>(n);
+  const uint32_t key = head_key(seed);
+  float2 *cur = reinterpret_cast<float2*>(d_Y), *nxt = reinterpret_cast<float2*>(d_Y_tmp);
+  for (int e = std::max(e_begin, 1); e < e_end; ++e) {            // epoch 0 samples no edge
+    const float alpha = static_cast<float>(1.0 - static_cast<double>(e) / epochs);
+    mp_epoch_kernel<<<(nn + 7) / 8, 256, 0, st>>>(reinterpret_cast<const long long*>(d_row_ptr), d_col, d_eps, nn, e,
+                                                  head_mix32(key ^ static_cast<uint32_t>(e)), alpha, cur, nxt);
+    GNM_CUDA(cudaGetLastError());
+    std::swap(cur, nxt);
+  }
+  if (cur != reinterpret_cast<float2*>(d_Y))
+    GNM_CUDA(cudaMemcpyAsync(d_Y, cur, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToDevice, st));
   return 0;
 }

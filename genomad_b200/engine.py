@@ -128,6 +128,16 @@ EXPORTS = {
     "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]),
+    "gnm_map_membership": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                     C.c_void_p, C.c_void_p]),
+    "gnm_map_pca_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "gnm_map_pca": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                              C.c_void_p]),
+    "gnm_map_init_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "gnm_map_init": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t,
+                               C.c_void_p]),
+    "gnm_map_epochs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
+                                 C.c_void_p, C.c_void_p]),
     "gnm_window_regions_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
     "gnm_window_regions": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -323,6 +333,160 @@ def cluster_block(rows, covered, min_similarity):
                                           work.data_ptr(), need, t.cuda.current_stream(x.device).cuda_stream))
         m = int(count.item())
     return reps[:m].long()
+
+
+MAP_A = 1.57694346               # 1 / (1 + a x^2b) least-squares fitted to umap-learn's curve at min_dist = 0.1, spread = 1
+MAP_B = 0.89506088
+
+
+def map_default_epochs(n: int) -> int:
+    """umap-learn's default: 500 layout epochs for at most 10,000 rows, else 200."""
+    return 500 if n <= 10000 else 200
+
+
+def map_check(n: int, k, epochs, seed) -> Tuple[int, int, int]:
+    """(k, epochs, seed) as ints, or ValueError: 1 <= k <= 64, k < n, epochs >= 1 (None: map_default_epochs), 0 <= seed < 2^64."""
+    k = int(k)
+    if not 1 <= k <= NEIGHBOURS_MAX_K:
+        raise ValueError(f"k must be in [1, {NEIGHBOURS_MAX_K}], not {k}")
+    if k >= n:
+        raise ValueError(f"k must be smaller than the number of sequences ({n:,}), not {k}")
+    epochs = map_default_epochs(n) if epochs is None else int(epochs)
+    if epochs < 1:
+        raise ValueError(f"epochs must be >= 1, not {epochs}")
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise ValueError(f"seed must be in [0, 2^64), not {seed}")
+    return k, epochs, seed
+
+
+class MapMembership(NamedTuple):
+    """Result of map_membership (cuda tensors, fp64; gnm_map_membership)."""
+    mean_d: "object"          # [1]
+    rho: "object"             # [n]
+    sigma: "object"           # [n]
+    w: "object"               # [n, k] directed memberships
+    union: "object"           # [n, k] fuzzy union at the entry that emits the pair, -1 elsewhere
+
+
+class MapGraph(NamedTuple):
+    """The layout graph (cuda tensors): both directions of every kept edge, each row sorted by column."""
+    row_ptr: "object"         # int64 [n + 1]
+    col: "object"             # int32 [nnz]
+    weight: "object"          # float64 [nnz]
+    eps: "object"             # float64 [nnz]: epochs per sample, max w / w
+
+
+def _stream(t, dev):
+    return t.cuda.current_stream(dev).cuda_stream
+
+
+def map_membership(sim, idx) -> MapMembership:
+    """Step 2 of the map: memberships and their fuzzy union from the all-vs-all lists of embedding_neighbours (sim float32
+    cuda [n, k], idx int64 cuda [n, k])."""
+    import torch as t
+    assert sim.dtype == t.float32 and idx.dtype == t.int64 and sim.is_cuda and sim.shape == idx.shape and sim.dim() == 2
+    n, k = sim.shape
+    sim, idx = sim.contiguous(), idx.contiguous()
+    f64 = dict(dtype=t.float64, device=sim.device)
+    out = MapMembership(t.empty(1, **f64), t.empty(n, **f64), t.empty(n, **f64), t.empty((n, k), **f64), t.empty((n, k), **f64))
+    lib = load_library()
+    with t.cuda.device(sim.device):
+        _check(lib, lib.gnm_map_membership(sim.data_ptr(), idx.data_ptr(), n, k, *(a.data_ptr() for a in out),
+                                           _stream(t, sim.device)))
+    return out
+
+
+def map_graph(union, idx, epochs: int) -> MapGraph:
+    """Step 3: drop union weights below max w / epochs, as umap-learn does, and store both directions of the rest as CSR rows
+    sorted by column, with the epochs per sample.  Integer bookkeeping with torch's stable sort and cumsum, on the device."""
+    import torch as t
+    n, k = union.shape
+    u = union.reshape(-1)
+    max_w = u.max()
+    e = t.nonzero(u >= max_w / epochs).flatten()
+    i, j, w = e // k, idx.reshape(-1)[e], u[e]
+    rows, cols, ws = t.cat([i, j]), t.cat([j, i]), t.cat([w, w])
+    order = t.sort(rows * n + cols, stable=True).indices
+    rows, cols, ws = rows[order], cols[order], ws[order]
+    row_ptr = t.zeros(n + 1, dtype=t.int64, device=union.device)
+    row_ptr[1:] = t.cumsum(t.bincount(rows, minlength=n), 0)
+    return MapGraph(row_ptr, cols.to(t.int32).contiguous(), ws.contiguous(), (max_w / ws).contiguous())
+
+
+def map_pca(rows):
+    """Step 4a: (xhat float32 [n, 512], center float64 [512], S float64 [512, 512], V float64 [2, 512]) of rows (float32 cuda
+    [n, 512]): the fp64-normalised rows, their mean and covariance, and its top-2 eigenvectors (gnm_map_pca)."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    n = x.shape[0]
+    lib = load_library()
+    dev = x.device
+    xhat = t.empty_like(x)
+    center = t.empty(EMBED, dtype=t.float64, device=dev)
+    S = t.empty((EMBED, EMBED), dtype=t.float64, device=dev)
+    V = t.empty((2, EMBED), dtype=t.float64, device=dev)
+    with t.cuda.device(dev):
+        need = int(lib.gnm_map_pca_workspace_bytes(n))
+        if need == 0:
+            _check(lib, 1)
+        work = t.empty(need, dtype=t.uint8, device=dev)
+        _check(lib, lib.gnm_map_pca(x.data_ptr(), n, xhat.data_ptr(), center.data_ptr(), S.data_ptr(), V.data_ptr(),
+                                    work.data_ptr(), need, _stream(t, dev)))
+    return xhat, center, S, V
+
+
+def map_init(xhat, center, V, seed: int, *, projection: bool = False):
+    """Step 4b: the initial layout float32 cuda [n, 2] (gnm_map_init).  projection=True also returns the fp64 projections
+    [n, 2] it was scaled from."""
+    import torch as t
+    n = xhat.shape[0]
+    dev = xhat.device
+    lib = load_library()
+    Y = t.empty((n, 2), dtype=t.float32, device=dev)
+    with t.cuda.device(dev):
+        need = int(lib.gnm_map_init_workspace_bytes(n))
+        if need == 0:
+            _check(lib, 1)
+        work = t.empty(need, dtype=t.uint8, device=dev)
+        _check(lib, lib.gnm_map_init(xhat.contiguous().data_ptr(), n, center.contiguous().data_ptr(), V.contiguous().data_ptr(),
+                                     int(seed), Y.data_ptr(), work.data_ptr(), need, _stream(t, dev)))
+        proj = work[: n * 16].view(t.float64).reshape(n, 2).clone() if projection else None
+    return (Y, proj) if projection else Y
+
+
+def map_epochs(graph: MapGraph, Y, epochs: int, seed: int, e_begin: int = 0, e_end: Optional[int] = None):
+    """Step 5: layout epochs e_begin .. e_end - 1 (default: all) of `epochs` from Y (float32 cuda [n, 2]); returns a new tensor
+    (gnm_map_epochs)."""
+    import torch as t
+    n = Y.shape[0]
+    e_end = epochs if e_end is None else int(e_end)
+    out = Y.contiguous().clone()
+    tmp = t.empty_like(out)
+    lib = load_library()
+    with t.cuda.device(Y.device):
+        _check(lib, lib.gnm_map_epochs(graph.row_ptr.data_ptr(), graph.col.data_ptr(), graph.eps.data_ptr(), n, int(epochs),
+                                       int(e_begin), e_end, int(seed), out.data_ptr(), tmp.data_ptr(), _stream(t, Y.device)))
+    return out
+
+
+def map_layout(rows, sim, idx, epochs: int, seed: int):
+    """Steps 2-5 from the rows and their all-vs-all neighbour lists: the map, float32 cuda [n, 2]."""
+    m = map_membership(sim, idx)
+    graph = map_graph(m.union, idx, epochs)
+    xhat, center, _, V = map_pca(rows)
+    Y = map_init(xhat, center, V, seed)
+    return map_epochs(graph, Y, epochs, seed)
+
+
+def embedding_map(rows, k: int = 15, epochs: Optional[int] = None, seed: int = 0):
+    """A 2-D UMAP layout of rows (float32 cuda [n, 512]) on one GPU: the all-vs-all k-nearest-neighbour lists
+    (embedding_neighbours), then map_layout.  Returns float32 cuda [n, 2].  DESIGN.md, "Embedding map"."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    k, epochs, seed = map_check(x.shape[0], k, epochs, seed)
+    sim, idx = embedding_neighbours(x, None, k)
+    return map_layout(x, sim, idx, epochs, seed)
 
 
 def both_strands(forward, reverse):

@@ -637,6 +637,54 @@ int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_cov
                       int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream);
 
 /*
+ * Embedding map: the stages of a 2-D UMAP layout (McInnes, Healy & Melville 2018) of n rows, 2 <= n <= 2^30, as umap-learn
+ * computes it with min_dist = 0.1 and spread = 1 (a = 1.57694346, b = 0.89506088), except where marked (dev).  DESIGN.md,
+ * "Embedding map".  No handle, no allocation: the current device, `stream` and the caller's buffers, all DEVICE.  Asynchronous.
+ *
+ * gnm_map_membership: from the all-vs-all lists of gnm_embedding_neighbours at k (1 <= k <= min(64, n - 1)), d_sim [n][k] and
+ *   d_idx [n][k], with d = 1 - s in fp64 (a zero row has s = 0 with every row, so its d is 1 everywhere and its list is the
+ *   lowest indices):
+ *     d_mean_d [1]     the mean d over all n k entries, summed in a fixed order;
+ *     d_rho [n]        the smallest d > 0 of the row, 0 if none;
+ *     d_sigma [n]      umap-learn's smooth_knn_dist bisection (64 steps, exit at |sum - target| < 1e-5, sigma doubled while the
+ *                      upper end is infinite) for sum_p f(d_ip - rho_i) = log2(k + 1), f(x) = exp(-x / sigma) for x > 0, else 1;
+ *                      then at least 1e-3 x the row's mean d, or x mean_d when rho_i = 0;
+ *     d_w [n][k]       w_ip = f(d_ip - rho_i) (fp64);
+ *     d_union [n][k]   for j = idx[i][p]: a + b - a b with a = w_ip and b = w_jq where idx[j][q] = i (0 if i is not in j's list),
+ *                      at the entry that emits the unordered pair {i, j} (the lower index when the entries are mutual, else the
+ *                      row that holds it), and -1 at every other entry.
+ * gnm_map_pca: (dev: a PCA initialisation, not spectral) d_xhat [n][512] fp32 = each row / its fp64 norm (a zero row stays
+ *   zero); d_center [512] and d_S [512][512] (fp64), the mean and covariance (1/n) sum (x^ - center)(x^ - center)^T from the
+ *   novelty fit's kernels at one class; d_V [2][512] (fp64), the top-2 eigenvectors of S by a fixed-step subspace iteration
+ *   from a fixed start, each signed so its largest-magnitude component is positive.  S = 0 leaves V at the start vectors.
+ *   gnm_map_pca_workspace_bytes(n): the bytes of d_work (256-byte aligned) it needs; 0 on invalid n.
+ * gnm_map_init: d_Y [n][2] fp32, the initial layout: p = (x^ - center) . v_c in fp64 (workspace bytes [0, 16 n)), scaled by
+ *   10 / max |p| (skipped when max |p| = 0) and rounded to fp32, plus (dev) the fp32 noise
+ *   (mix32(mix32(key ^ row) + axis) - 2^31 + 0.5) * 1e-4 / 2^31 with mix32 the lowbias32 hash and key = (seed * 0x9E3779B1 +
+ *   0x7F4A7C15) mod 2^32; then each axis mapped to [0, 10] by 10 (y - min) / (max - min) in fp32.
+ *   gnm_map_init_workspace_bytes(n): the bytes of d_work (256-byte aligned) it needs; 0 on invalid n.
+ * gnm_map_epochs: epochs e_begin .. e_end - 1 of `epochs` (dev: synchronous) on the CSR graph d_row_ptr [n + 1] int64,
+ *   d_col [nnz] int32 (both directions of every edge, each row sorted by column) and d_eps [nnz] fp64, the epochs per sample
+ *   max w / w.  Epoch e reads Y and writes the next Y: vertex i adds, in fp32 per term and in a fixed order, over each entry
+ *   (i, j) at CSR position p sampled at e (e >= 1 and floor(e / eps) > floor((e - 1) / eps) in fp64):
+ *     twice the attraction clip(-2ab d^(2(b-1)) / (1 + a d^2b) (y_i - y_j), +-4) (0 when d = 0), and
+ *     (dev) for s = 0..4 the repulsion of vertex m = mix32(mix32(mix32(key ^ e) + p mod 2^32) + s) mod n, skipped when m = i:
+ *     clip(2b / ((0.001 + d^2)(1 + a d^2b)) (y_i - y_m), +-4) (0 when d = 0);
+ *   then y_i += (1 - e / epochs) x the sum.  No atomics: the result is bitwise reproducible.  Epoch 0 samples nothing.  d_Y
+ *   holds the result; d_Y_tmp [n][2] is the second buffer.
+ */
+int gnm_map_membership(const float* d_sim, const int64_t* d_idx, int64_t n, int k, double* d_mean_d, double* d_rho,
+                       double* d_sigma, double* d_w, double* d_union, void* stream);
+size_t gnm_map_pca_workspace_bytes(int64_t n);
+int gnm_map_pca(const float* d_rows, int64_t n, float* d_xhat, double* d_center, double* d_S, double* d_V, void* d_work,
+                size_t work_bytes, void* stream);
+size_t gnm_map_init_workspace_bytes(int64_t n);
+int gnm_map_init(const float* d_xhat, int64_t n, const double* d_center, const double* d_V, uint64_t seed, float* d_Y,
+                 void* d_work, size_t work_bytes, void* stream);
+int gnm_map_epochs(const int64_t* d_row_ptr, const int32_t* d_col, const double* d_eps, int64_t n, int epochs, int e_begin,
+                   int e_end, uint64_t seed, float* d_Y, float* d_Y_tmp, void* stream);
+
+/*
  * Window regions: an HMM decode of each sequence's window-score profile (nn-classification --write-window-scores, or a head's)
  * into class regions.  No handle, no allocation: the current device and `stream`, the caller's workspace.  Asynchronous.
  * DESIGN.md, "Window regions" states the model; in short, for sequence windows w = 0..n-1 with scores p_w in R^C, starts a_w,

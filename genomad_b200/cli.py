@@ -188,14 +188,22 @@ def train_head(input, labels, output, epochs, batch_size, learning_rate, validat
 @click.option("--both-strands", is_flag=True, default=False, show_default=True,
               help="Search the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
                    "--write-embeddings --both-strands) of every input file, so a sequence and its reverse complement match.")
+@click.option("--index", "index", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
+              help="Search through this embedding-index file (embedding-index output) instead of comparing every pair: each "
+                   "sequence scans only the sequences of its --nprobe nearest lists. The index must have been built on the reference file (the query file without --reference) "
+                   "with the same --both-strands; checked before any work.")
+@click.option("--nprobe", type=int, default=None,
+              help="With --index: lists each sequence scans (1 to min(64, lists)); required with --index, since recall "
+                   "against the exact search depends on it. At nprobe = lists the result is the exact search's.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def embedding_neighbours(query, output, reference, neighbours, both_strands, verbose):
+def embedding_neighbours(query, output, reference, neighbours, both_strands, index, nprobe, verbose):
     """Find the nearest neighbours, in cosine similarity of the encoder embeddings, of every sequence of the QUERY embeddings
     file (nn-classification --write-embeddings output) and write them to the OUTPUT directory as
     <prefix>_embedding_neighbours.{tsv,npz}. Not a module of the reference."""
     from . import embedding_neighbours as module
-    module.main(query, reference, output, neighbours, verbose, both_strands=both_strands)
+    extra = {} if index is None and nprobe is None else {"index": index, "nprobe": nprobe}
+    module.main(query, reference, output, neighbours, verbose, both_strands=both_strands, **extra)
 
 
 @cli.command(name="embedding-clusters", context_settings=CONTEXT_SETTINGS)
@@ -231,14 +239,43 @@ def embedding_clusters(input, output, min_similarity, both_strands, verbose):
 @click.option("--both-strands", is_flag=True, default=False, show_default=True,
               help="Map the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
                    "--write-embeddings --both-strands), so a sequence and its reverse complement get the same point.")
+@click.option("--index", "index", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
+              help="Search through this embedding-index file (embedding-index output) instead of comparing every pair: each "
+                   "sequence scans only the sequences of its --nprobe nearest lists. The index must have been built on the INPUT file "
+                   "with the same --both-strands; checked before any work.")
+@click.option("--nprobe", type=int, default=None,
+              help="With --index: lists each sequence scans (1 to min(64, lists)); required with --index, since recall "
+                   "against the exact search depends on it. At nprobe = lists the result is the exact search's.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def embedding_map(input, output, k, epochs, seed, both_strands, verbose):
+def embedding_map(input, output, k, epochs, seed, both_strands, index, nprobe, verbose):
     """Map the sequences of the INPUT embeddings file (nn-classification --write-embeddings output) onto two dimensions with
     UMAP on the GPU, and write each sequence's coordinates to the OUTPUT directory as <prefix>_embedding_map.{tsv,npz}.
     Not a module of the reference."""
     from . import embedding_map as module
-    module.main(input, output, k, epochs, seed, verbose, both_strands=both_strands)
+    extra = {} if index is None and nprobe is None else {"index": index, "nprobe": nprobe}
+    module.main(input, output, k, epochs, seed, verbose, both_strands=both_strands, **extra)
+
+
+@cli.command(name="embedding-index", context_settings=CONTEXT_SETTINGS)
+@click.argument("reference", type=click.Path(path_type=Path, exists=True, dir_okay=False))
+@click.argument("output", type=click.Path(path_type=Path))
+@click.option("--lists", type=int, default=None, show_default="ceil(4 sqrt(n))",
+              help="Lists the sequences are split into by spherical k-means (1 to the number of sequences).")
+@click.option("--iterations", type=int, default=20, show_default=True, help="k-means iterations (>= 0).")
+@click.option("--seed", type=int, default=0, show_default=True,
+              help="Seed of the training sample and the initial centroids: the same seed gives bitwise the same index.")
+@click.option("--both-strands", is_flag=True, default=False, show_default=True,
+              help="Index the mean of both strands' embeddings (embeddings_both_strands); searches with the index must then "
+                   "use --both-strands too.")
+@click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
+              help="Display the execution log.")
+def embedding_index(reference, output, lists, iterations, seed, both_strands, verbose):
+    """Build an inverted-file index of the sequences of the REFERENCE embeddings file (nn-classification --write-embeddings
+    output) for embedding-neighbours --index and embedding-map --index, and write it to the OUTPUT directory as
+    <prefix>_embedding_index.npz. Runs in one process on one GPU (not a torchrun job). Not a module of the reference."""
+    from . import embedding_index as module
+    module.main(reference, output, lists, iterations, seed, verbose, both_strands=both_strands)
 
 
 @cli.command(name="window-regions", context_settings=CONTEXT_SETTINGS)

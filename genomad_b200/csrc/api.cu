@@ -11,6 +11,9 @@
 #include <string>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
 #include "../../include/gnm.h"
 #include "common.cuh"
 #include "encode.cuh"
@@ -29,6 +32,7 @@
 #include "regions.cuh"
 #include "novelty.cuh"
 #include "layout.cuh"
+#include "ivf.cuh"
 
 using namespace gnm;
 
@@ -2834,5 +2838,192 @@ extern "C" int gnm_map_epochs(const int64_t* d_row_ptr, const int32_t* d_col, co
   }
   if (cur != reinterpret_cast<float2*>(d_Y))
     GNM_CUDA(cudaMemcpyAsync(d_Y, cur, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ embedding index
+// Centroid helpers of the spherical k-means build: the rows normalised as gnm_map_pca normalises them (mp_normalize_kernel), and
+// a list's centroid as its rows' sum in row order (segment_sum_rows_kernel), normalised the same way.
+extern "C" int gnm_ivf_normalize(const float* d_rows, int64_t n, float* d_out, void* stream) {
+  if (n < 0 || n > kNbRowMax) return fail("gnm_ivf_normalize: n must be in [0, 2^30]");
+  if (n == 0) return 0;
+  if (!d_rows || !d_out) return fail("gnm_ivf_normalize: null buffer");
+  const int nn = static_cast<int>(n);
+  mp_normalize_kernel<<<(nn + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_rows, nn, d_out);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gnm_ivf_centroids(const float* d_xhat, const int32_t* d_offsets, int lists, float* d_sums, float* d_centroids,
+                                 void* stream) {
+  if (lists < 1) return fail("gnm_ivf_centroids: lists must be >= 1, not " + std::to_string(lists));
+  if (!d_xhat || !d_offsets || !d_sums || !d_centroids) return fail("gnm_ivf_centroids: null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_xhat) | reinterpret_cast<uintptr_t>(d_sums)) % 16)
+    return fail("gnm_ivf_centroids: d_xhat and d_sums must be 16-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  segment_sum_rows_kernel<<<lists, kSegRowThreads, 0, st>>>(d_xhat, d_offsets, nullptr, d_sums);
+  GNM_CUDA(cudaGetLastError());
+  mp_normalize_kernel<<<(lists + 7) / 8, 256, 0, st>>>(d_sums, lists, d_centroids);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int gnm_ivf_prepare(const float* d_rows, int64_t n, float* d_hi, float* d_lo, void* stream) {
+  if (n < 0 || n > kNbRowMax) return fail("gnm_ivf_prepare: n must be in [0, 2^30]");
+  if (n == 0) return 0;
+  if (!d_rows || !d_hi || !d_lo) return fail("gnm_ivf_prepare: null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_rows) | reinterpret_cast<uintptr_t>(d_hi) | reinterpret_cast<uintptr_t>(d_lo)) % 16)
+    return fail("gnm_ivf_prepare: d_rows, d_hi and d_lo must be 16-byte aligned");
+  const int nn = static_cast<int>(n);
+  nb_prep_kernel<<<(nn + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(d_rows, nn, d_hi, d_lo);
+  GNM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+namespace {
+struct IvfPlan {
+  long long parts = 0;                         // a bound on the partial lists: pairs x the most ranges of any list
+  int bits = 1;                                // sort key bits
+  size_t g_raw = 0, g_hi = 0, g_lo = 0, keys = 0, skeys = 0, vals = 0, svals = 0, slot = 0, self = 0, off = 0, pstart = 0,
+         items = 0, ibase = 0, cparts = 0, pbase = 0, cub = 0, cub_bytes = 0, p_sim = 0, p_idx = 0, bytes = 0;
+};
+}  // namespace
+
+static int ivf_check(const char* fn, int64_t n_pairs, int64_t n_ref, const int64_t* h_offsets, int lists, int k) {
+  const std::string f(fn);
+  if (k < 1 || k > kNbMaxK) return fail(f + ": k must be in [1, 64], not " + std::to_string(k));
+  if (lists < 1) return fail(f + ": lists must be >= 1, not " + std::to_string(lists));
+  if (n_pairs < 0 || n_pairs > kNbRowMax || n_ref < 0 || n_ref > kNbRowMax)
+    return fail(f + ": need 0 <= n_pairs <= 2^30 and 0 <= n_ref <= 2^30");
+  if (!h_offsets) return fail(f + ": null h_offsets");
+  if (h_offsets[0] != 0 || h_offsets[lists] != n_ref) return fail(f + ": offsets must start at 0 and end at n_ref");
+  for (int l = 0; l < lists; ++l)
+    if (h_offsets[l + 1] < h_offsets[l]) return fail(f + ": offsets must be non-decreasing (list " + std::to_string(l) + ")");
+  return 0;
+}
+
+// Every pair has at most the range count of the longest list, whatever the pairs are (duplicates included).
+static int ivf_plan(int64_t n_pairs, const int64_t* h_offsets, int lists, int k, IvfPlan* pl) {
+  IvfPlan p;
+  long long max_nr = 0;
+  for (int l = 0; l < lists; ++l) max_nr = std::max(max_nr, ivf_ranges(h_offsets[l + 1] - h_offsets[l]));
+  p.parts = n_pairs * max_nr;
+  while ((1LL << p.bits) <= lists) ++p.bits;
+  size_t sort_bytes = 0, scan_bytes = 0;
+  const int np = static_cast<int>(n_pairs);
+  GNM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, static_cast<const uint32_t*>(nullptr), static_cast<uint32_t*>(nullptr),
+                                           static_cast<const int32_t*>(nullptr), static_cast<int32_t*>(nullptr), np, 0, p.bits));
+  GNM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, static_cast<const long long*>(nullptr),
+                                         static_cast<long long*>(nullptr), lists + 1));
+  const size_t P = static_cast<size_t>(n_pairs), L1 = static_cast<size_t>(lists) + 1;
+  size_t o = 0;
+  p.g_raw = o; o += nb_align(P * kNbDim * 4);
+  p.g_hi = o; o += nb_align(P * kNbDim * 4);
+  p.g_lo = o; o += nb_align(P * kNbDim * 4);
+  p.keys = o; o += nb_align(P * 4);
+  p.skeys = o; o += nb_align(P * 4);
+  p.vals = o; o += nb_align(P * 4);
+  p.svals = o; o += nb_align(P * 4);
+  p.slot = o; o += nb_align(P * 4);
+  p.self = o; o += nb_align(P * 4);
+  p.off = o; o += nb_align(L1 * 8);
+  p.pstart = o; o += nb_align(L1 * 4);
+  p.items = o; o += nb_align(L1 * 8);
+  p.ibase = o; o += nb_align(L1 * 8);
+  p.cparts = o; o += nb_align(L1 * 8);
+  p.pbase = o; o += nb_align(L1 * 8);
+  p.cub_bytes = std::max(sort_bytes, scan_bytes);
+  p.cub = o; o += nb_align(p.cub_bytes);
+  p.p_sim = o; o += nb_align(static_cast<size_t>(p.parts) * k * 4);
+  p.p_idx = o; o += nb_align(static_cast<size_t>(p.parts) * k * 4);
+  p.bytes = o;
+  *pl = p;
+  return 0;
+}
+
+extern "C" size_t gnm_ivf_search_workspace_bytes(int64_t n_pairs, int64_t n_ref, const int64_t* h_offsets, int lists, int k) {
+  IvfPlan pl;
+  if (ivf_check("gnm_ivf_search_workspace_bytes", n_pairs, n_ref, h_offsets, lists, k) || ivf_plan(n_pairs, h_offsets, lists, k, &pl))
+    return 0;
+  return pl.bytes;
+}
+
+extern "C" int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list,
+                              int64_t n_pairs, const float* d_ref_hi, const float* d_ref_lo, int64_t n_ref, const int64_t* h_offsets,
+                              int lists, const int64_t* d_ref_index, int64_t self_index0, int k, float* d_sim, int64_t* d_idx,
+                              void* d_work, size_t work_bytes, void* stream) {
+  const char* fn = "gnm_ivf_search";
+  const std::string f(fn);
+  if (ivf_check(fn, n_pairs, n_ref, h_offsets, lists, k)) return 1;
+  if (n_query < 0 || n_query > kNbRowMax) return fail(f + ": n_query must be in [0, 2^30]");
+  if (self_index0 < -1) return fail(f + ": self_index0 must be -1 (no self-exclusion) or >= 0");
+  if (n_query == 0) return 0;
+  if (!d_sim || !d_idx || (n_pairs > 0 && (!d_query || !d_pair_query || !d_pair_list || !d_work)) ||
+      (n_ref > 0 && (!d_ref_hi || !d_ref_lo || !d_ref_index)))
+    return fail(f + ": null buffer");
+  if ((reinterpret_cast<uintptr_t>(d_query) | reinterpret_cast<uintptr_t>(d_ref_hi) | reinterpret_cast<uintptr_t>(d_ref_lo)) % 16)
+    return fail(f + ": d_query, d_ref_hi and d_ref_lo must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(f + ": d_work must be 256-byte aligned");
+  IvfPlan pl;
+  if (ivf_plan(n_pairs, h_offsets, lists, k, &pl)) return 1;
+  if (n_pairs > 0 && work_bytes < pl.bytes)
+    return fail(f + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(pl.bytes) +
+                " needed (gnm_ivf_search_workspace_bytes)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nq = static_cast<int>(n_query), nr = static_cast<int>(n_ref), np = static_cast<int>(n_pairs);
+  if (np == 0) {                                                  // no pair: every list padded
+    ivf_merge_kernel<<<(nq + 7) / 8, 256, 0, st>>>(nullptr, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr, nq,
+                                                   k, nullptr, d_sim, reinterpret_cast<long long*>(d_idx));
+    GNM_CUDA(cudaGetLastError());
+    return 0;
+  }
+  int dev = 0, sms = 0;
+  GNM_CUDA(cudaGetDevice(&dev));
+  GNM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  uint8_t* w = static_cast<uint8_t*>(d_work);
+  auto F = [&](size_t o) { return reinterpret_cast<float*>(w + o); };
+  auto U = [&](size_t o) { return reinterpret_cast<uint32_t*>(w + o); };
+  auto I = [&](size_t o) { return reinterpret_cast<int32_t*>(w + o); };
+  auto LL = [&](size_t o) { return reinterpret_cast<long long*>(w + o); };
+  long long* off = LL(pl.off);
+  GNM_CUDA(cudaMemcpyAsync(off, h_offsets, (static_cast<size_t>(lists) + 1) * 8, cudaMemcpyHostToDevice, st));
+  ivf_keys_kernel<<<(np + 255) / 256, 256, 0, st>>>(d_pair_query, d_pair_list, np, nq, lists, U(pl.keys), I(pl.vals));
+  GNM_CUDA(cudaGetLastError());
+  size_t cb = pl.cub_bytes;
+  GNM_CUDA(cub::DeviceRadixSort::SortPairs(w + pl.cub, cb, U(pl.keys), U(pl.skeys), I(pl.vals), I(pl.svals), np, 0, pl.bits, st));
+  ivf_lists_kernel<<<(lists + 1 + 255) / 256, 256, 0, st>>>(U(pl.skeys), np, off, lists, I(pl.pstart), LL(pl.items),
+                                                            LL(pl.cparts));
+  GNM_CUDA(cudaGetLastError());
+  cb = pl.cub_bytes;
+  GNM_CUDA(cub::DeviceScan::ExclusiveSum(w + pl.cub, cb, LL(pl.items), LL(pl.ibase), lists + 1, st));
+  cb = pl.cub_bytes;
+  GNM_CUDA(cub::DeviceScan::ExclusiveSum(w + pl.cub, cb, LL(pl.cparts), LL(pl.pbase), lists + 1, st));
+  ivf_gather_kernel<<<(np + 7) / 8, 256, 0, st>>>(d_query, d_pair_query, U(pl.skeys), I(pl.svals), np, I(pl.pstart), lists, off,
+                                                  reinterpret_cast<const long long*>(d_ref_index),
+                                                  static_cast<long long>(self_index0), F(pl.g_raw), I(pl.slot), I(pl.self));
+  GNM_CUDA(cudaGetLastError());
+  nb_prep_kernel<<<(np + 7) / 8, 256, 0, st>>>(F(pl.g_raw), np, F(pl.g_hi), F(pl.g_lo));
+  GNM_CUDA(cudaGetLastError());
+  if (nr > 0) {
+    PFN_encodeTiled enc = nullptr;
+    if (get_encode_fn(&enc)) return 1;
+    CUtensorMap tm[4];
+    if (make_f32_map(enc, &tm[0], F(pl.g_hi), kNbDim, np, kNbBM) || make_f32_map(enc, &tm[1], F(pl.g_lo), kNbDim, np, kNbBM) ||
+        make_f32_map(enc, &tm[2], const_cast<float*>(d_ref_hi), kNbDim, nr, kNbBN) ||
+        make_f32_map(enc, &tm[3], const_cast<float*>(d_ref_lo), kNbDim, nr, kNbBN))
+      return 1;
+    IvfSearchParams p;
+    p.part_sim = F(pl.p_sim); p.part_idx = I(pl.p_idx);
+    p.off = off; p.pstart = I(pl.pstart); p.ibase = LL(pl.ibase); p.pbase = LL(pl.pbase); p.self_col = I(pl.self);
+    p.lists = lists; p.k = k; p.status = nullptr;
+    const int smem = nb_smem_bytes(k);
+    GNM_CUDA(cudaFuncSetAttribute(ivf_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    ivf_search_kernel<<<sms, kNbThreads, smem, st>>>(tm[0], tm[1], tm[2], tm[3], p);   // persistent: items round robin
+    GNM_CUDA(cudaGetLastError());
+  }
+  ivf_merge_kernel<<<(nq + 7) / 8, 256, 0, st>>>(F(pl.p_sim), I(pl.p_idx), d_pair_query, d_pair_list, np, I(pl.slot), off,
+                                                 I(pl.pstart), LL(pl.pbase), nq, k, reinterpret_cast<const long long*>(d_ref_index),
+                                                 d_sim, reinterpret_cast<long long*>(d_idx));
+  GNM_CUDA(cudaGetLastError());
   return 0;
 }

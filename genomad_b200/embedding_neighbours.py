@@ -15,7 +15,11 @@ Outputs in OUTPUT, <prefix> = the query file's stem without ``_nn_classification
     <prefix>_embedding_neighbours.tsv   seq_name, rank (1-based), neighbour_name, cosine_similarity (6 decimals); padded
                                         entries (fewer than k references) are left out
     <prefix>_embedding_neighbours.npz   query_names, reference_names, neighbour_index int64 [n, k] (-1 = none),
-                                        similarity float32 [n, k] (-inf = none), k
+                                        similarity float32 [n, k] (-inf = none), k; with --index also nprobe and
+                                        index_sha256 (of the index file)
+
+With --index (an embedding-index file) each query scans only the rows of its nprobe nearest lists (engine.ivf_search); under
+torchrun each rank then takes a contiguous range of the lists, balanced by rows, and rank 0 merges in rank order as above.
 """
 from __future__ import annotations
 
@@ -91,17 +95,39 @@ def _device(info):
     return torch.device("cuda", info.local_rank) if torch.cuda.is_available() else torch.device("cpu")
 
 
-def search(query, reference, k: int, info) -> Optional[Tuple[np.ndarray, np.ndarray]]:
+def list_shard(offsets, world_size: int, rank: int) -> Tuple[int, int]:
+    """The contiguous range of an index's lists rank `rank` searches: the lists are split where the rows are, so every rank
+    gets about n / world_size rows."""
+    off = np.asarray(offsets, np.int64)
+    n, L = int(off[-1]), len(off) - 1
+    cut = lambda r: 0 if r == 0 else L if r == world_size else int(np.searchsorted(off, r * n // world_size, side="left"))
+    return cut(rank), max(cut(rank), cut(rank + 1))
+
+
+def search(query, reference, k: int, info, index=None, nprobe: Optional[int] = None) -> Optional[Tuple[np.ndarray, np.ndarray]]:
     """This rank's reference shard searched on the device, the lists gathered on rank 0 and merged there in rank order.
     Returns (sim float32 [n, k], idx int64 [n, k]) on rank 0, None on the others.  reference None: all-vs-all.  query and
-    reference are NumPy arrays, or tensors already on this rank's device (embedding_clusters keeps its rows there)."""
+    reference are NumPy arrays, or tensors already on this rank's device (embedding_clusters keeps its rows there).
+    index (embedding_index.read_index of the reference) and nprobe: search through the index instead; a rank's shard is then a
+    contiguous range of its lists (list_shard)."""
     import torch
     dev = _device(info)
     ref = query if reference is None else reference
-    s, e = dist.shard_bounds(ref.shape[0], info.world_size, info.rank)
     q = torch.as_tensor(query).to(dev)
-    r = torch.as_tensor(ref[s:e]).to(dev)
-    sim, idx = engine.embedding_neighbours(q, r, k, ref_index0=s, self_index0=0 if reference is None else -1)
+    if index is None:
+        s, e = dist.shard_bounds(ref.shape[0], info.world_size, info.rank)
+        r = torch.as_tensor(ref[s:e]).to(dev)
+        sim, idx = engine.embedding_neighbours(q, r, k, ref_index0=s, self_index0=0 if reference is None else -1)
+    else:
+        from . import embedding_index as EI
+        l0, l1 = list_shard(index["offsets"], info.world_size, info.rank)
+        if reference is None:                                  # the queries are the reference, already on the device
+            sim, idx = engine.ivf_search(q, None, EI.to_device(index, dev), k, nprobe, lists=(l0, l1))
+        else:                                                  # only the rows of this rank's lists, in list order
+            own = index["rows"][index["offsets"][l0]:index["offsets"][l1]]
+            r = torch.as_tensor(ref[torch.as_tensor(own)] if torch.is_tensor(ref) else ref[own]).to(dev)
+            sim, idx = engine.ivf_search(q, r, EI.to_device(index, dev), k, nprobe, self_index0=-1, lists=(l0, l1),
+                                         reference_shard=True)
     if info.world_size > 1:
         if not info.is_main:
             dist._p2p_send(sim.contiguous(), 0)
@@ -124,9 +150,11 @@ def write_tsv(path, query_names, reference_names, sim, idx) -> None:
                     fout.write(f"{qn}\t{rank}\t{reference_names[i]}\t{float(s):.6f}\n")
 
 
-def main(query_npz, reference_npz, output_dir, k: int = 10, verbose: bool = True, *, both_strands: bool = False):
+def main(query_npz, reference_npz, output_dir, k: int = 10, verbose: bool = True, *, both_strands: bool = False,
+         index=None, nprobe: Optional[int] = None):
     """both_strands: search the strand-averaged embeddings (BOTH_STRANDS_KEY) of every input file, so that a sequence and its
-    reverse complement have bitwise the same row."""
+    reverse complement have bitwise the same row.  index: an embedding-index file built on the reference file (the query file
+    for all-vs-all) with the same strand key, searched at nprobe lists per query (required with it)."""
     console = utils.HybridConsole(None, verbose)
     k = int(k)
     if not 1 <= k <= engine.NEIGHBOURS_MAX_K:
@@ -137,16 +165,25 @@ def main(query_npz, reference_npz, output_dir, k: int = 10, verbose: bool = True
         rnames, remb = read_embeddings(reference_npz, key)
     else:
         rnames, remb = qnames, None
+    ix = None
+    if index is not None:
+        from . import embedding_index as EI
+        ix = EI.read_index(index, rnames, qemb if remb is None else remb, key)
+        nprobe = EI.check_nprobe(nprobe, ix)
+    elif nprobe is not None:
+        raise ValueError("--nprobe applies only with --index")
     info = dist.init_process_group_if_needed()
     tsv_path, npz_path = output_paths(query_npz, output_dir)
     mode = f"against {len(rnames):,} reference sequences" if remb is not None else "all-vs-all"
-    console.log(f"Searching the {k} nearest neighbours of {len(qnames):,} sequences {mode}.")
-    res = search(qemb, remb, k, info)
+    via = "" if ix is None else f" through an index of {ix['lists']:,} lists ({nprobe} probed per query)"
+    console.log(f"Searching the {k} nearest neighbours of {len(qnames):,} sequences {mode}{via}.")
+    res = search(qemb, remb, k, info, ix, nprobe)
     if info.is_main:
         sim, idx = res
         Path(output_dir).mkdir(parents=True, exist_ok=True)
         write_tsv(tsv_path, qnames, rnames, sim, idx)
+        extra = {} if ix is None else {"nprobe": np.int64(nprobe), "index_sha256": np.str_(ix["sha256"])}
         np.savez(npz_path, query_names=qnames, reference_names=rnames, neighbour_index=idx.astype(np.int64),
-                 similarity=sim.astype(np.float32), k=np.int64(k))
+                 similarity=sim.astype(np.float32), k=np.int64(k), **extra)
         console.log(f"Neighbours written to {tsv_path.name} and {npz_path.name}.")
     dist.barrier(info)

@@ -125,6 +125,13 @@ EXPORTS = {
     "gnm_embedding_neighbours": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "gnm_neighbours_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p]),
+    "gnm_ivf_normalize": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "gnm_ivf_centroids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_ivf_prepare": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gnm_ivf_search_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int]),
+    "gnm_ivf_search": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                 C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                 C.c_void_p]),
     "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]),
@@ -290,6 +297,262 @@ def neighbours_merge(sim, idx, sim_b, idx_b):
     with t.cuda.device(sim.device):
         _check(lib, lib.gnm_neighbours_merge(sim.data_ptr(), idx.data_ptr(), sb.data_ptr(), ib.data_ptr(), sim.shape[0], k,
                                              t.cuda.current_stream(sim.device).cuda_stream))
+    return sim, idx
+
+
+IVF_MAX_PROBE = 64
+IVF_TRAIN_PER_LIST = 256         # training rows per list at most (the first 256 L rows of the hashed order)
+IVF_QUERY_BYTES = 1 << 31        # per gnm_ivf_search call: the live (query, list) pairs' rows, halves and partial lists
+IVF_REF_ROWS = NEIGHBOURS_CHUNK  # reference rows per gnm_ivf_search call: whole lists, or pieces of a longer list
+
+
+class IvfIndex(NamedTuple):
+    """An inverted-file index of n reference rows (cuda tensors; DESIGN.md, "Embedding index")."""
+    centroids: "object"       # float32 [L, 512], unit rows (or zero)
+    rows: "object"            # int64 [n]: the reference rows in (list, row) order
+    offsets: "object"         # int64 [L + 1]: list l is rows[offsets[l]:offsets[l + 1]]
+
+
+def ivf_default_lists(n: int) -> int:
+    """ceil(4 sqrt(n)), at most n: the usual rule of thumb for the list count (Johnson, Douze & Jegou 2019)."""
+    import math
+    r = math.isqrt(16 * n)
+    return min(n, r + (r * r < 16 * n))
+
+
+def ivf_check(n: int, lists, iterations, seed) -> Tuple[int, int, int]:
+    """(lists, iterations, seed) as ints, or ValueError: 1 <= lists <= n, iterations >= 0, 0 <= seed < 2^64."""
+    lists, iterations, seed = int(lists), int(iterations), int(seed)
+    if not 1 <= lists <= n:
+        raise ValueError(f"lists must be in [1, {n:,}] (the reference rows), not {lists}")
+    if iterations < 0:
+        raise ValueError(f"iterations must be >= 0, not {iterations}")
+    if not 0 <= seed < 1 << 64:
+        raise ValueError(f"seed must be in [0, 2^64), not {seed}")
+    return lists, iterations, seed
+
+
+def ivf_nprobe(nprobe, lists: int) -> int:
+    nprobe = int(nprobe)
+    if not 1 <= nprobe <= min(IVF_MAX_PROBE, lists):
+        raise ValueError(f"nprobe must be in [1, {min(IVF_MAX_PROBE, lists)}] (at most 64 and the index's {lists:,} lists), "
+                         f"not {nprobe}")
+    return nprobe
+
+
+def ivf_training_rows(n: int, lists: int, seed: int, device):
+    """The training rows, int64 cuda [min(n, 256 lists)]: rows in the order of (mix32(key ^ row), row), key = synth._keys(seed)[0]."""
+    import torch as t
+    from .synth import _keys, _mix32
+    r = t.arange(n, dtype=t.int64, device=device)
+    h = _mix32((r & 0xFFFFFFFF) ^ _keys(seed)[0])
+    return t.sort(h, stable=True).indices[: min(n, IVF_TRAIN_PER_LIST * lists)]
+
+
+def ivf_normalize(rows):
+    """rows / their fp64 norm, rounded to fp32 (gnm_ivf_normalize): float32 cuda [n, 512]."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    out = t.empty_like(x)
+    lib = load_library()
+    with t.cuda.device(x.device):
+        _check(lib, lib.gnm_ivf_normalize(x.data_ptr(), x.shape[0], out.data_ptr(), _stream(t, x.device)))
+    return out
+
+
+def ivf_assign(rows, centroids):
+    """Each row's k = 1 centroid under s, the row as the query: (similarity float32 [n], list int64 [n]), cuda.  The queries
+    are searched NEIGHBOURS_CHUNK rows per call; each row's result does not depend on the others."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    sims, lists = [], []
+    for a in range(0, x.shape[0], NEIGHBOURS_CHUNK):
+        s, i = embedding_neighbours(x[a:a + NEIGHBOURS_CHUNK], centroids, 1)
+        sims.append(s[:, 0]); lists.append(i[:, 0])
+    if not sims:
+        return t.empty(0, dtype=t.float32, device=x.device), t.empty(0, dtype=t.int64, device=x.device)
+    return t.cat(sims), t.cat(lists)
+
+
+def ivf_layout(assign, lists: int):
+    """(rows int64 [n], offsets int64 [lists + 1]): the row indices stably sorted by their list."""
+    import torch as t
+    order = t.sort(assign, stable=True).indices
+    offsets = t.zeros(lists + 1, dtype=t.int64, device=assign.device)
+    offsets[1:] = t.cumsum(t.bincount(assign, minlength=lists), 0)
+    return order, offsets
+
+
+def ivf_centroids(xhat, assign, lists: int):
+    """The normalised sums of each list's normalised rows, summed in row order after a stable sort by list (gnm_ivf_centroids):
+    float32 cuda [lists, 512]; an empty list gives the zero row."""
+    import torch as t
+    order, offsets = ivf_layout(assign, lists)
+    xs = xhat.index_select(0, order).contiguous()
+    off32 = offsets.to(t.int32)
+    sums = t.empty((lists, EMBED), dtype=t.float32, device=xhat.device)
+    cent = t.empty_like(sums)
+    lib = load_library()
+    with t.cuda.device(xhat.device):
+        _check(lib, lib.gnm_ivf_centroids(xs.data_ptr(), off32.data_ptr(), lists, sums.data_ptr(), cent.data_ptr(),
+                                          _stream(t, xhat.device)))
+    return cent
+
+
+def ivf_reseed(centroids, xhat, train, best, assign):
+    """Empty lists, in ascending order, each take the normalised training row not yet taken with the lowest best similarity
+    (ties: the lowest row).  train: the training rows' indices; best, assign: their k = 1 search.  Returns (centroids, the
+    reseeded lists int64)."""
+    import torch as t
+    lists = centroids.shape[0]
+    empty = t.nonzero(t.bincount(assign, minlength=lists) == 0).flatten()
+    if empty.numel() == 0:
+        return centroids, empty
+    by_row = t.sort(train, stable=True).indices
+    order = by_row[t.sort(best[by_row], stable=True).indices]
+    out = centroids.clone()
+    out[empty] = xhat[order[: empty.numel()]]
+    return out, empty
+
+
+def ivf_build(rows, lists: int, iterations: int = 20, seed: int = 0) -> IvfIndex:
+    """Spherical k-means of rows (float32 cuda [n, 512]) into `lists` lists, and the layout of every row (include/gnm.h,
+    "Embedding index").  The same rows, lists, iterations and seed give a bitwise identical index."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    lists, iterations, seed = ivf_check(x.shape[0], lists, iterations, seed)
+    train = ivf_training_rows(x.shape[0], lists, seed, x.device)
+    xhat = ivf_normalize(x.index_select(0, train).contiguous())
+    cent = xhat[:lists].clone()
+    for _ in range(iterations):
+        best, assign = ivf_assign(xhat, cent)
+        cent = ivf_centroids(xhat, assign, lists)
+        cent, _ = ivf_reseed(cent, xhat, train, best, assign)
+    _, assign = ivf_assign(x, cent)
+    order, offsets = ivf_layout(assign, lists)
+    return IvfIndex(cent, order, offsets)
+
+
+def ivf_chunks(offsets, l_begin: int, l_end: int, max_rows: int = NEIGHBOURS_CHUNK):
+    """The reference chunks of lists [l_begin, l_end) for gnm_ivf_search: (l0, l1, a, b) = lists l0 .. l1 - 1, index rows
+    [a, b); consecutive whole lists up to max_rows rows, a longer list alone in pieces of max_rows rows."""
+    off = [int(v) for v in offsets]
+    out, l = [], l_begin
+    while l < l_end:
+        if off[l + 1] - off[l] > max_rows:
+            out += [(l, l + 1, a, min(a + max_rows, off[l + 1])) for a in range(off[l], off[l + 1], max_rows)]
+            l += 1
+            continue
+        e = l + 1
+        while e < l_end and off[e + 1] - off[l] <= max_rows:
+            e += 1
+        out.append((l, e, off[l], off[e]))
+        l = e
+    return out
+
+
+def ivf_probes(query, centroids, nprobe: int):
+    """Each query's nprobe nearest centroids under the total order: int32 cuda [nq, nprobe] (embedding_neighbours, NEIGHBOURS_CHUNK
+    queries per call, so its workspace does not grow with the queries; each query's result does not depend on the others)."""
+    import torch as t
+    out = t.empty((query.shape[0], nprobe), dtype=t.int32, device=query.device)
+    for a in range(0, query.shape[0], NEIGHBOURS_CHUNK):
+        out[a:a + NEIGHBOURS_CHUNK] = embedding_neighbours(query[a:a + NEIGHBOURS_CHUNK], centroids, nprobe)[1]
+    return out
+
+
+def ivf_check_probes(probes, nq: int, nprobe: int, lists: int):
+    """ValueError unless probes is an integer cuda tensor [nq, nprobe] of list ids in [0, lists), distinct within each row."""
+    import torch as t
+    if tuple(probes.shape) != (nq, nprobe) or probes.dtype not in (t.int32, t.int64):
+        raise ValueError(f"probes must be integers [{nq}, {nprobe}], not {probes.dtype} {list(probes.shape)}")
+    if nq and nprobe and (int(probes.min()) < 0 or int(probes.max()) >= lists):
+        raise ValueError(f"probes must be list ids in [0, {lists})")
+    if nq and nprobe > 1 and bool((t.diff(t.sort(probes, 1).values, dim=1) == 0).any()):
+        raise ValueError("probes must be distinct within each row")
+    return probes.to(t.int32)
+
+
+def ivf_search(query, reference, index: IvfIndex, k: int, nprobe: int, *, ref_index0: int = 0,
+               self_index0: Optional[int] = None, lists: Optional[Tuple[int, int]] = None, probes=None,
+               reference_shard: bool = False):
+    """The k nearest rows of every query among the rows of its nprobe nearest lists (gnm_ivf_search), shaped and ordered like
+    embedding_neighbours: (sim float32 [nq, k], idx int64 [nq, k]), cuda, padded with (-inf, -1).  reference None: all-vs-all
+    over the query rows (self_index0 defaults to ref_index0).  Indices are ref_index0 + reference row.  lists=(l0, l1) searches
+    only those lists of the probes (a rank's share); reference_shard: `reference` then holds only the rows of those lists, in
+    list order (index.rows[offsets[l0]:offsets[l1]]).  probes: precomputed ivf_probes, checked.  At nprobe = L the result is
+    bitwise embedding_neighbours.
+
+    Each reference chunk (ivf_chunks) is prepared once (gnm_ivf_prepare); its live pairs, the (query, list) pairs whose list
+    lies in the chunk, go to gnm_ivf_search in query ranges of at most about IVF_QUERY_BYTES of workspace."""
+    import torch as t
+    k = _neighbours_k(k)
+    q = _neighbours_args(t, query, "query")
+    ref = q if reference is None else _neighbours_args(t, reference, "reference")
+    self0 = (ref_index0 if reference is None else -1) if self_index0 is None else int(self_index0)
+    L = index.centroids.shape[0]
+    nprobe = ivf_nprobe(nprobe, L)
+    dev = q.device
+    nq = q.shape[0]
+    off = index.offsets.cpu().numpy().astype(np.int64)
+    l0_, l1_ = (0, L) if lists is None else (int(lists[0]), int(lists[1]))
+    if not 0 <= l0_ <= l1_ <= L:
+        raise ValueError(f"lists must be a range inside [0, {L}], not {lists}")
+    base = int(off[l0_]) if reference_shard else 0
+    want = int(off[l1_] - off[l0_]) if reference_shard else index.rows.shape[0]
+    if ref.shape[0] != want:
+        raise ValueError(f"the index holds {want:,} rows here, the reference {ref.shape[0]:,}")
+    probes = ivf_probes(q, index.centroids.to(dev), nprobe) if probes is None else ivf_check_probes(probes.to(dev), nq, nprobe, L)
+    rows = index.rows.to(dev)
+    sim = t.full((nq, k), float("-inf"), dtype=t.float32, device=dev)
+    idx = t.full((nq, k), -1, dtype=t.int64, device=dev)
+    s_out, i_out = t.empty_like(sim), t.empty_like(idx)
+    lib = load_library()
+    work = t.empty(0, dtype=t.uint8, device=dev)
+    halves = t.empty(0, dtype=t.float32, device=dev)
+    with t.cuda.device(dev):
+        stream = _stream(t, dev)
+        for l0, l1, a, b in ivf_chunks(off, l0_, l1_, IVF_REF_ROWS):
+            lp = probes.to(t.int64) - l0
+            live = (lp >= 0) & (lp < l1 - l0)
+            cum = t.cumsum(live.sum(1), 0)
+            total = int(cum[-1]) if nq else 0
+            if total == 0 or b == a:
+                continue
+            ridx = rows[a:b]
+            r = ref[a - base:b - base] if reference_shard else ref.index_select(0, ridx).contiguous()
+            if halves.numel() < 2 * (b - a) * EMBED:
+                halves = t.empty(2 * (b - a) * EMBED, dtype=t.float32, device=dev)
+            hi, lo = halves[: (b - a) * EMBED], halves[(b - a) * EMBED: 2 * (b - a) * EMBED]
+            _check(lib, lib.gnm_ivf_prepare(r.data_ptr(), b - a, hi.data_ptr(), lo.data_ptr(), stream))
+            gidx = (ridx + int(ref_index0)).contiguous()
+            h_off = np.ascontiguousarray(np.clip(off[l0:l1 + 1], a, b) - a, dtype=np.int64)
+            qi, ji = t.nonzero(live, as_tuple=True)                                # query-major: pairs in query order
+            pq, pl = qi.to(t.int32), lp[qi, ji].to(t.int32)
+            # pairs per call: a range of whole queries of at most pc + nprobe pairs
+            pc = max(total, nprobe)                               # >= nprobe: every range holds a whole query
+            while pc > nprobe and lib.gnm_ivf_search_workspace_bytes(pc + nprobe, b - a, _ptr(h_off), l1 - l0, k) > IVF_QUERY_BYTES:
+                pc = max(nprobe, (pc + 1) // 2)
+            cuts = t.searchsorted(cum, t.arange(pc, total, pc, device=dev), right=True).tolist()
+            bounds = [0] + cuts + [nq]
+            pstart = [0] + cum[t.tensor(bounds[1:], device=dev) - 1].tolist()
+            for c in range(len(bounds) - 1):
+                qa, qb, pa, pb = bounds[c], bounds[c + 1], int(pstart[c]), int(pstart[c + 1])
+                if pb == pa:
+                    continue
+                need = int(lib.gnm_ivf_search_workspace_bytes(pb - pa, b - a, _ptr(h_off), l1 - l0, k))
+                if need == 0:
+                    _check(lib, 1)
+                if need > work.numel():
+                    work = t.empty(need, dtype=t.uint8, device=dev)
+                cq = (pq[pa:pb] - qa).contiguous()
+                cl = pl[pa:pb].contiguous()
+                _check(lib, lib.gnm_ivf_search(q[qa:qb].data_ptr(), qb - qa, cq.data_ptr(), cl.data_ptr(), pb - pa, hi.data_ptr(),
+                                               lo.data_ptr(), b - a, _ptr(h_off), l1 - l0, gidx.data_ptr(),
+                                               self0 + qa if self0 >= 0 else -1, k, s_out.data_ptr(), i_out.data_ptr(),
+                                               work.data_ptr(), need, stream))
+                _check(lib, lib.gnm_neighbours_merge(sim[qa:qb].data_ptr(), idx[qa:qb].data_ptr(), s_out.data_ptr(),
+                                                     i_out.data_ptr(), qb - qa, k, stream))
     return sim, idx
 
 

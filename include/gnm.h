@@ -610,6 +610,56 @@ int gnm_neighbours_merge(float* d_sim, int64_t* d_idx, const float* d_sim_b, con
                          void* stream);
 
 /*
+ * Embedding index: an inverted-file (IVF) search over reference rows split into L lists by spherical k-means.  s(q, r) is the
+ * similarity gnm_embedding_neighbours returns for query q and reference r; "the total order" is its (s descending, index
+ * ascending).  DESIGN.md, "Embedding index".
+ *
+ * Build (spherical k-means, Dhillon & Modha 2001; engine.ivf_build drives it with the calls below), from n reference rows, L lists
+ * (1 <= L <= n), I iterations and a seed:
+ *   training rows   the first min(n, 256 L) rows in the order of (mix32(key ^ row), row) ascending, mix32 the lowbias32 hash and
+ *                   key = (seed * 0x9E3779B1 + 0x7F4A7C15) mod 2^32 (gnm_map_init's key);
+ *   initial         centroid l = training row l of that order, normalised (gnm_ivf_normalize);
+ *   each iteration  every training row is assigned its k = 1 centroid under s, the row as the query (gnm_embedding_neighbours);
+ *                   the normalised training rows are stably sorted by list and centroid l = normalise(sum of its rows in that
+ *                   order) (gnm_ivf_centroids); then, in ascending list order, each empty list takes as its centroid the
+ *                   normalised training row, not yet taken, of lowest best similarity (ties: the lowest row);
+ *   layout          every reference row is assigned as above; rows [n] int64 = the rows in (list, row) order, offsets [L + 1].
+ * The same rows, L, I and seed give a bitwise identical index.
+ *
+ * Search: probes(q) = q's top-nprobe centroids under the total order (gnm_embedding_neighbours of the queries against the
+ * centroids, 1 <= nprobe <= min(64, L)); the result is the top-k under the total order of {(s(q, r), r) : r in a probed list,
+ * r not q's self index}, padded with (-inf, -1).  At nprobe = L it is bitwise gnm_embedding_neighbours; it does not depend on the
+ * query order, the query or reference chunking, or the GPU count.
+ *
+ * gnm_ivf_normalize: d_out [n][512] = each row / its fp64 norm, rounded to fp32 (a zero row stays zero), as gnm_map_pca's x^.
+ * gnm_ivf_centroids: d_centroids [lists][512] = the normalised fp32 sums (row order) of the rows d_xhat[d_offsets[l] ..
+ *   d_offsets[l + 1]) (int32 offsets [lists + 1]); an empty list gives the zero row.  d_sums [lists][512] is scratch.
+ * gnm_ivf_prepare: d_hi, d_lo [n][512] = the TF32 halves of gnm_embedding_neighbours' operands (the row normalised by its fp32
+ *   norm, then split), row by row: a reference chunk's halves, made once and searched by any number of gnm_ivf_search calls.
+ * gnm_ivf_search: one reference chunk of an index against the live (query, list) pairs of some queries.
+ *   d_ref_hi / d_ref_lo [n_ref][512]   gnm_ivf_prepare of reference rows in list order, list l at rows [h_offsets[l],
+ *                                      h_offsets[l + 1]) (h_offsets: HOST int64 [lists + 1] from 0 to n_ref, checked before any
+ *                                      launch), with global indices d_ref_index [n_ref] (DEVICE int64) ascending within each list;
+ *   d_pair_query, d_pair_list [n_pairs] DEVICE int32: pair e asks for the rows of list d_pair_list[e] for query d_pair_query[e],
+ *                                      in ascending query order; each (query, list) at most once.  A pair whose list is outside
+ *                                      [0, lists) or whose query is outside [0, n_query) is dropped.
+ *   result  d_sim / d_idx [n_query][k]: for query q of d_query [n_query][512], the top-k under the total order of the rows of its
+ *           pairs' lists, global indices from d_ref_index, excluding global index self_index0 + q when self_index0 >= 0; a query
+ *           without pairs gets a padded list.
+ *   1 <= k <= 64, n_pairs, n_query, n_ref <= 2^30.  Asynchronous; d_work 256-byte aligned.
+ * gnm_ivf_search_workspace_bytes: the bytes of d_work a call with n_pairs pairs needs (0 on invalid arguments): each pair's query
+ *   row and halves (6 KB) and a partial list of 8 k bytes per 1,536-row range of the longest list, whatever the pairs are.
+ */
+int gnm_ivf_normalize(const float* d_rows, int64_t n, float* d_out, void* stream);
+int gnm_ivf_centroids(const float* d_xhat, const int32_t* d_offsets, int lists, float* d_sums, float* d_centroids, void* stream);
+int gnm_ivf_prepare(const float* d_rows, int64_t n, float* d_hi, float* d_lo, void* stream);
+size_t gnm_ivf_search_workspace_bytes(int64_t n_pairs, int64_t n_ref, const int64_t* h_offsets, int lists, int k);
+int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list, int64_t n_pairs,
+                   const float* d_ref_hi, const float* d_ref_lo, int64_t n_ref, const int64_t* h_offsets, int lists,
+                   const int64_t* d_ref_index, int64_t self_index0, int k, float* d_sim, int64_t* d_idx, void* d_work,
+                   size_t work_bytes, void* stream);
+
+/*
  * Embedding clusters: one block step of greedy clustering at a cosine threshold t.  Rows are processed in file order, block by
  * block; row j is a representative iff s(j, i) < t for every representative i < j, where s(a, b) is the similarity
  * gnm_embedding_neighbours returns for QUERY row a and REFERENCE row b (s is not bitwise symmetric: the row being placed is

@@ -18,6 +18,7 @@ from __future__ import annotations
 import os
 import shutil
 import sys
+from dataclasses import dataclass, replace
 from pathlib import Path
 
 import numpy as np
@@ -90,52 +91,77 @@ def _device(clf):
     return torch.device("cuda", clf.device)
 
 
-def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather",
-                     embeddings: bool = False, window_probs: bool = False, attributions: "dict | None" = None,
-                     head: "dict | None" = None, window_embeddings=None):
+@dataclass(frozen=True)
+class AttributionSpec:
+    """What a chunk pass attributes to 4-mers: a class of the classifier (`target`), a class of the request's head (`target`,
+    `head` true), or each window's distance to its target class of the head's novelty model (`novelty_targets`, int32
+    [n_windows] in global window order).  `steps` >= 1 selects integrated gradients from `baseline`."""
+    target: "str | None" = None
+    head: bool = False
+    novelty_targets: "np.ndarray | None" = None
+    steps: int = 0
+    baseline: str = "zero"
+
+
+@dataclass(frozen=True)
+class ChunkRequest:
+    """What a chunk pass computes besides the class scores.  `head` (engine.Head) scores every window's embedding, and with
+    `novelty` also its distances to the head's novelty classes.  `window_probs`, `window_head` and `window_novelty` collect
+    those per-window rows on rank 0 in window order.  `window_embeddings` (float32 cuda [shard windows, 512]) keeps each
+    window's embedding in its row."""
+    embeddings: bool = False
+    head: object = None
+    novelty: bool = False
+    window_probs: bool = False
+    window_head: bool = False
+    window_novelty: bool = False
+    attribution: "AttributionSpec | None" = None
+    window_embeddings: object = None
+
+
+@dataclass(frozen=True)
+class ChunkResult:
+    """A chunk pass's results.  Per contig (only with offsets), identical on all ranks: preds float32 [n_contigs, 3],
+    head_preds and novelty [n_contigs, C]; embeddings [n_contigs, 512] on rank 0.  Per window, on rank 0 (None on the other
+    ranks): window_probs [n_windows, 3], head_window_preds and window_novelty [n_windows, C], attributions [n_windows, 5997],
+    logp [n_windows, 2] (integrated gradients: log p_target, or the novelty distance, at the window and at the baseline) and
+    distance [n_windows] (the novelty route: each window's distance to its target class)."""
+    preds: "np.ndarray | None" = None
+    embeddings: "np.ndarray | None" = None
+    head_preds: "np.ndarray | None" = None
+    novelty: "np.ndarray | None" = None
+    window_probs: "np.ndarray | None" = None
+    head_window_preds: "np.ndarray | None" = None
+    window_novelty: "np.ndarray | None" = None
+    attributions: "np.ndarray | None" = None
+    logp: "np.ndarray | None" = None
+    distance: "np.ndarray | None" = None
+
+
+def _chunk_pass(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather",
+                req: ChunkRequest = ChunkRequest()) -> ChunkResult:
     """
-    Indexed FASTA -> float32 [n_contigs, 3] per-contig mean (identical on all ranks).
+    Indexed FASTA -> per-contig means of the class scores (and of whatever `req` asks for), reduced over `offsets`, or with
+    offsets None only the per-window rows `req` collects.
 
     `parsed` is the window source: a ParsedFasta (the reference's windows) or a sequence.WindowList (windows at another
     stride); all the loop needs is n_windows, export_windows and release_before.
 
     This rank's contiguous block of the global window list is streamed in chunks: the native reader fills one pinned
     chunk straight from the mmap'ed file (upper-case + pad, multi-threaded) while the GPU classifies the previous one
-    (gnm_classify_host on a worker thread; the C call releases the GIL) into a pinned result buffer, so neither copy
-    direction blocks the host.  Windows never exist on disk, and file pages behind the cursor are released.
+    (on a worker thread; the C calls release the GIL) into a pinned result buffer, so neither copy direction blocks the
+    host.  Windows never exist on disk, and file pages behind the cursor are released.
 
-    With `embeddings`, every chunk goes through gnm_embed_host instead (same probabilities, plus the encoder output of each
-    window in a device chunk buffer), is summed per contig right away (segment_sum_rows, carried from chunk to chunk) and
-    the per-contig means are combined over the ranks by the carry chain of genomad_b200.dist; returns (means, embeddings),
-    the embeddings float32 [n_contigs, 512] on rank 0 and None on the other ranks.
-
-    With `window_probs`, the per-window probabilities float32 [n_windows, 3] are collected on rank 0 (None on the other
-    ranks) and returned last.  With offsets None there is no per-contig reduction: only those are returned.
-
-    With `attributions` ({"target": class name}), every chunk goes through the attribution calls instead
-    (Classifier.attribute_ascii: the same forward step, so bitwise the same probabilities, plus each window's 5,997
-    attributions in a device buffer of this rank's shard); they are collected on rank 0 in window order and stored as
-    attributions["attr"] (float32 [n_windows, 5997] on rank 0, None on the other ranks).  With attributions["steps"] >= 1 the
-    calls are the integrated-gradients ones (Classifier.integrated_gradients_ascii, same probabilities), and the rows of
-    log p_target at the window and at the baseline travel to rank 0 the same way, as attributions["logp"] (float32 [n_windows, 2]).
-    With attributions["head"] true, the target is a class of the `head` and the calls are the head's (Head.attribute_ascii /
-    integrated_gradients_ascii): one call gives the probabilities, the head's scores of the windows (bitwise Head.predict of
-    their embeddings) and the attributions of the head's log p_target, so the chunk takes no other route.
-
-    With `head` ({"head": engine.Head}), every chunk takes the embedding route and the head scores each window's embedding on
-    the device into a buffer of this rank's shard; they are reduced per contig by the routes of the class scores (gather or
-    allreduce, any width) and stored as head["preds"] (float32 [n_contigs, C], identical on all ranks).  With head["windows"]
-    true, those rows are also collected on rank 0 in window order, as the class scores are with `window_probs`, and stored as
-    head["window_preds"] (float32 [n_windows, C] on rank 0, None on the other ranks); with offsets None only that is done.
-    With head["novelty"] true (the head carries a novelty model), the head also scores each window's embedding by
-    Head.novelty into a second buffer of this rank's shard, reduced per contig the same way and stored as head["novelty_dist"]
-    (float32 [n_contigs, C], identical on all ranks).
-    With attributions["novelty"] (int32 [n_windows], each window's target class, in global window order), the calls are the
-    head's novelty ones (Head.attribute_novelty_ascii / integrated_gradients_novelty_ascii) and each window's distance to its
-    target travels to rank 0 as attributions["distance"] (float32 [n_windows]), with IG's (D_c(x), D_c(x')) rows as
-    attributions["logp"].  With head["windows"] and head["novelty"] true, and head["window_novelty_wanted"] or no offsets, the
-    windows' novelty rows are collected on rank 0 too, as head["window_novelty"] (float32 [n_windows, C]).
-    With `window_embeddings` (float32 cuda [shard windows, 512]), each window's embedding is kept in its row of that matrix.
+    Each chunk takes one route:
+    * gnm_classify_host, when nothing but the class scores is asked for;
+    * gnm_embed_host (the same probabilities, plus each window's encoder output on the device), with embeddings, a head or
+      window_embeddings: the head scores the embeddings on the device, and the embeddings are summed per contig right away
+      (segment_sum_rows, carried from chunk to chunk) and combined over the ranks by genomad_b200.dist's carry chain;
+    * with an attribution, the classifier's or the head's attribution calls (the same forward step, so bitwise the same
+      probabilities; a head route call also gives the head's scores), plus Classifier.embed_ascii only for embeddings,
+      novelty or head scores that call does not give.
+    Per-window rows live in device buffers of this rank's shard and are reduced per contig by the routes of the class
+    scores (gather or allreduce, any width) or collected on rank 0 in window order.
     """
     import torch
     from concurrent.futures import ThreadPoolExecutor
@@ -145,87 +171,80 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
     keep, bufs = zip(*(_pinned_chunk(min(chunk, max(1, end - start))) for _ in range(2)))
     out_t = _pinned_probs(max(1, end - start))
     dev = _device(clf)
+    scorer, nov, att, embeddings = req.head, req.head is not None and req.novelty, req.attribution, req.embeddings
 
     def sync():
         if dev.type == "cuda":
             torch.cuda.current_stream(dev).synchronize()
 
-    def run(win, m, row):                                    # one chunk: windows win[:m] are rows [row, row + m) of the shard
-        clf.classify_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12)
-    scorer = head["head"] if head is not None else None
-    nov = scorer is not None and bool(head.get("novelty"))
     if scorer is not None:
         d_head = torch.empty((end - start, scorer.n_classes), dtype=torch.float32, device=dev)
     if nov:
         d_nov = torch.empty((end - start, scorer.n_classes), dtype=torch.float32, device=dev)
     if embeddings:
         shard = gdist.EmbeddingShard(offsets, start, end, clf.segment_sum_rows, device=dev)
-    if embeddings or scorer is not None or window_embeddings is not None:
-        d_emb = torch.empty((min(chunk, max(1, end - start)), 512), dtype=torch.float32, device=dev)
-        if attributions is None and (scorer is not None or window_embeddings is not None):
-            def run(win, m, row):                            # the worker owns d_emb: one chunk at a time
-                e = window_embeddings[row: row + m] if window_embeddings is not None else d_emb[:m]
-                clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, e.data_ptr())
-                if scorer is not None:
-                    scorer.predict(e, out=d_head[row: row + m])
-                if nov:
-                    scorer.novelty(e, out=d_nov[row: row + m])
-                if embeddings:
-                    shard.add(e)
-                sync()
-        elif attributions is None:
-            def run(win, m, row):                            # the worker owns d_emb: one chunk at a time
-                clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, d_emb.data_ptr())
-                shard.add(d_emb[:m])
-                sync()
-    if attributions is not None:
-        d_attr = torch.empty((end - start, ATTR_TOKENS), dtype=torch.float32, device=dev)
-        ig_steps = attributions.get("steps") or 0
-        if ig_steps:
-            d_logp = torch.empty((end - start, 2), dtype=torch.float32, device=dev)
 
-        head_route = bool(attributions.get("head"))
-        nov_targets = attributions.get("novelty")            # the novelty route: each window's target class, global order
-        assert not (head_route or nov_targets is not None) or scorer is not None
+    if att is not None:
+        d_attr = torch.empty((end - start, ATTR_TOKENS), dtype=torch.float32, device=dev)
+        if att.steps:
+            d_logp = torch.empty((end - start, 2), dtype=torch.float32, device=dev)
+        nov_targets = att.novelty_targets
+        assert not (att.head or nov_targets is not None) or scorer is not None
         if nov_targets is not None:
             d_distance = torch.empty((end - start, 1), dtype=torch.float32, device=dev)
+        head_by_embedding = scorer is not None and not att.head and nov_targets is None
 
-        def run(win, m, row):                                # probabilities and attributions from the attribution calls
+        def run(win, m, row):                                # one chunk: windows win[:m] are rows [row, row + m) of the shard
             d_win = torch.from_numpy(win[:m]).to(dev)
             if nov_targets is not None:                      # the head's novelty distance to each window's target
                 tg = np.ascontiguousarray(nov_targets[start + row: start + row + m], dtype=np.int32)
-                if ig_steps:
-                    probs, dist, dt, attr = scorer.integrated_gradients_novelty_ascii(d_win, tg, ig_steps,
-                                                                                      attributions["baseline"])
+                if att.steps:
+                    probs, dist, dt, attr = scorer.integrated_gradients_novelty_ascii(d_win, tg, att.steps, att.baseline)
                     d_logp[row: row + m].copy_(dt)
                 else:
                     probs, dist, attr = scorer.attribute_novelty_ascii(d_win, tg)
                 d_distance[row: row + m].copy_(dist.gather(1, torch.from_numpy(tg).to(dist.device, torch.int64)[:, None]))
-            elif head_route:                                 # the head's scores come out of the same call
-                if ig_steps:
-                    probs, head_probs, logp, attr = scorer.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
-                                                                                      attributions["baseline"])
+            elif att.head:                                   # the head's scores come out of the same call
+                if att.steps:
+                    probs, head_probs, logp, attr = scorer.integrated_gradients_ascii(d_win, att.target, att.steps,
+                                                                                      att.baseline)
                     d_logp[row: row + m].copy_(logp)
                 else:
-                    probs, head_probs, attr = scorer.attribute_ascii(d_win, attributions["target"])
+                    probs, head_probs, attr = scorer.attribute_ascii(d_win, att.target)
                 d_head[row: row + m].copy_(head_probs)
-            elif ig_steps:
-                probs, logp, attr = clf.integrated_gradients_ascii(d_win, attributions["target"], ig_steps,
-                                                                   attributions["baseline"])
+            elif att.steps:
+                probs, logp, attr = clf.integrated_gradients_ascii(d_win, att.target, att.steps, att.baseline)
                 d_logp[row: row + m].copy_(logp)
             else:
-                probs, attr = clf.attribute_ascii(d_win, attributions["target"])
+                probs, attr = clf.attribute_ascii(d_win, att.target)
             out_t[row: row + m].copy_(probs)
             d_attr[row: row + m].copy_(attr)
-            if embeddings or nov or (scorer is not None and not head_route and nov_targets is None):
+            if embeddings or nov or head_by_embedding:
                 e = clf.embed_ascii(d_win)[1]
                 if embeddings:
                     shard.add(e)
-                if scorer is not None and not head_route and nov_targets is None:
+                if head_by_embedding:
                     scorer.predict(e, out=d_head[row: row + m])
                 if nov:
                     scorer.novelty(e, out=d_nov[row: row + m])
             sync()
+    elif embeddings or scorer is not None or req.window_embeddings is not None:
+        if req.window_embeddings is None:
+            d_emb = torch.empty((min(chunk, max(1, end - start)), 512), dtype=torch.float32, device=dev)
+
+        def run(win, m, row):                                # the worker owns d_emb: one chunk at a time
+            e = req.window_embeddings[row: row + m] if req.window_embeddings is not None else d_emb[:m]
+            clf.embed_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12, e.data_ptr())
+            if scorer is not None:
+                scorer.predict(e, out=d_head[row: row + m])
+            if nov:
+                scorer.novelty(e, out=d_nov[row: row + m])
+            if embeddings:
+                shard.add(e)
+            sync()
+    else:
+        def run(win, m, row):
+            clf.classify_host_into(win.ctypes.data, m, out_t.data_ptr() + row * 12)
     futures = []
     with ThreadPoolExecutor(max_workers=1) as gpu:
         for i, a in enumerate(range(start, end, chunk)):
@@ -239,40 +258,57 @@ def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: 
             f.result()
     del keep
     local_t = out_t[: end - start].to(dev, non_blocking=True)
-    out = []
+
+    def collect(rows):                                       # per-window rows -> rank 0, in window order
+        full = gdist.collect_window_probs(rows, n, info)
+        return full.cpu().numpy() if full is not None else None
+
+    def reduce(mean, total, rows):
+        return _reduce_rows(mean, total, rows, offsets, start, end, n, info, contig_reduce)
+    res = {}
     if offsets is not None:
-        out.append(_reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce))
+        res["preds"] = _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
         if embeddings:
             lo, means = shard.finish(info)
             emb = gdist.gather_contig_means(lo, means, len(offsets) - 1, info)
-            out.append(emb.cpu().numpy() if emb is not None else None)
+            res["embeddings"] = emb.cpu().numpy() if emb is not None else None
         if scorer is not None:
-            head["preds"] = _reduce_rows(scorer.segment_mean, scorer.segment_sum, d_head, offsets, start, end, n, info,
-                                         contig_reduce)
+            res["head_preds"] = reduce(scorer.segment_mean, scorer.segment_sum, d_head)
             if nov:
-                head["novelty_dist"] = _reduce_rows(scorer.segment_mean, scorer.segment_sum, d_nov, offsets, start, end, n,
-                                                    info, contig_reduce)
-    if window_probs:
-        full = gdist.collect_window_probs(local_t, n, info)
-        out.append(full.cpu().numpy() if full is not None else None)
-    if scorer is not None and head.get("windows"):
-        full = gdist.collect_window_probs(d_head, n, info)
-        head["window_preds"] = full.cpu().numpy() if full is not None else None
-        if nov and (offsets is None or head.get("window_novelty_wanted")):
-            full = gdist.collect_window_probs(d_nov, n, info)
-            head["window_novelty"] = full.cpu().numpy() if full is not None else None
-    if attributions is not None:
-        full = gdist.collect_window_probs(d_attr, n, info)
-        attributions["attr"] = full.cpu().numpy() if full is not None else None
-        if ig_steps:
-            full = gdist.collect_window_probs(d_logp, n, info)
-            attributions["logp"] = full.cpu().numpy() if full is not None else None
+                res["novelty"] = reduce(scorer.segment_mean, scorer.segment_sum, d_nov)
+    if req.window_probs:
+        res["window_probs"] = collect(local_t)
+    if scorer is not None and req.window_head:
+        res["head_window_preds"] = collect(d_head)
+        if nov and req.window_novelty:
+            res["window_novelty"] = collect(d_nov)
+    if att is not None:
+        res["attributions"] = collect(d_attr)
+        if att.steps:
+            res["logp"] = collect(d_logp)
         if nov_targets is not None:
-            full = gdist.collect_window_probs(d_distance, n, info)
-            attributions["distance"] = full.reshape(-1).cpu().numpy() if full is not None else None
-    if not out:
-        return None
-    return out[0] if len(out) == 1 else tuple(out)
+            distance = collect(d_distance)
+            res["distance"] = distance.reshape(-1) if distance is not None else None
+    return ChunkResult(**res)
+
+
+def _classify_parsed(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str = "gather", embeddings: bool = False):
+    """Per-contig class scores float32 [n_contigs, 3] (identical on all ranks), and with `embeddings` the pair (scores,
+    per-contig mean embeddings float32 [n_contigs, 512] on rank 0, None on the other ranks): the chunk pass when nothing else
+    is asked for.  It is the seam where tests substitute the classification of a whole window source."""
+    res = _chunk_pass(clf, parsed, offsets, info, contig_reduce, ChunkRequest(embeddings=embeddings))
+    return (res.preds, res.embeddings) if embeddings else res.preds
+
+
+def _contig_pass(clf, parsed, offsets, info: gdist.DistInfo, contig_reduce: str, req: ChunkRequest) -> ChunkResult:
+    """_chunk_pass of a per-contig request; one that asks for the class scores and embeddings only goes through
+    _classify_parsed."""
+    if req.head is not None or req.attribution is not None:
+        return _chunk_pass(clf, parsed, offsets, info, contig_reduce, req)
+    if req.embeddings:
+        preds, emb = _classify_parsed(clf, parsed, offsets, info, contig_reduce, embeddings=True)
+        return ChunkResult(preds=preds, embeddings=emb)
+    return ChunkResult(preds=_classify_parsed(clf, parsed, offsets, info, contig_reduce))
 
 
 def _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce) -> np.ndarray:
@@ -305,11 +341,24 @@ def _classify_windows(clf, windows: np.ndarray, offsets: np.ndarray, info: gdist
     return _reduce_probs(clf, local_t, offsets, start, end, n, info, contig_reduce)
 
 
-def _write_tsv(path: Path, names, preds) -> None:
+def _write_score_tsv(path: Path, header: str, names, rows) -> None:
+    """One line per sequence: its name, then every score of its row with the digits of f"{x:.4f}"."""
     with open(path, "w") as fout:
-        fout.write(_HEADER)
-        for name, s in zip(names, preds):
-            fout.write(f"{name}\t{float(s[0]):.4f}\t{float(s[1]):.4f}\t{float(s[2]):.4f}\n")
+        fout.write(header)
+        for name, row in zip(names, rows):
+            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in row) + "\n")
+
+
+def _write_tsv(path: Path, names, preds) -> None:
+    _write_score_tsv(path, _HEADER, names, preds)
+
+
+def _window_coords(offsets, starts, lengths) -> dict:
+    """The coordinate keys of every per-window file: each window's contig, 0-based start and length."""
+    offsets = np.asarray(offsets, dtype=np.int32)
+    return {"window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
+            "window_start": np.asarray(starts, dtype=np.int64),
+            "window_length": np.asarray(lengths, dtype=np.int32)}
 
 
 _WINDOW_HEADER = "seq_name\tstart\tend\tchromosome_score\tplasmid_score\tvirus_score\n"
@@ -351,11 +400,7 @@ def _write_window_tsv(path: Path, names, offsets, starts, lengths, probs, thread
 
 def _write_window_scores(npz_path: Path, tsv_path: Path, names_key: str, names, offsets, starts, lengths, probs, stride: int,
                          threads: int) -> None:
-    offsets = np.asarray(offsets, dtype=np.int32)
-    np.savez(npz_path, **{names_key: names,
-                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
-                          "window_start": np.asarray(starts, dtype=np.int64),
-                          "window_length": np.asarray(lengths, dtype=np.int32),
+    np.savez(npz_path, **{names_key: names, **_window_coords(offsets, starts, lengths),
                           "predictions": np.asarray(probs, dtype=np.float32).reshape(-1, 3),
                           "window_stride": np.int32(stride)})
     _write_window_tsv(tsv_path, names, offsets, starts, lengths, probs, threads)
@@ -366,12 +411,8 @@ def _write_head_windows(npz_path: Path, tsv_path: Path, names_key: str, names, o
     """<prefix>_nn_classification_head_windows.{npz,tsv}: the window-score files' windows and keys, with the head's scores
     float32 [W, C] as predictions, plus class_names and head_sha256."""
     C = len(class_names)
-    offsets = np.asarray(offsets, dtype=np.int32)
     preds = np.asarray(preds, dtype=np.float32).reshape(-1, C)
-    np.savez(npz_path, **{names_key: names,
-                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
-                          "window_start": np.asarray(starts, dtype=np.int64),
-                          "window_length": np.asarray(lengths, dtype=np.int32),
+    np.savez(npz_path, **{names_key: names, **_window_coords(offsets, starts, lengths),
                           "predictions": preds,
                           "window_stride": np.int32(stride),
                           "class_names": np.array(class_names),
@@ -380,54 +421,28 @@ def _write_head_windows(npz_path: Path, tsv_path: Path, names_key: str, names, o
     _write_window_tsv(tsv_path, names, offsets, starts, lengths, preds, threads, header=header, n_cols=C)
 
 
-def _window_scores_current(npz_path: Path, tsv_path: Path, stride: int) -> bool:
-    """Both window-score files exist and were written at this stride."""
-    if not (npz_path.exists() and tsv_path.exists()):
-        return False
-    try:
-        with np.load(npz_path) as z:
-            return int(z["window_stride"]) == stride
-    except Exception:
-        return False
-
-
-def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, embeddings: bool,
-                         attributions=None, head=None):
-    """Per-contig scores (+ embeddings) and the per-window scores at `stride`: (preds, emb or None, offsets, starts, lengths,
-    probs); the window arrays are None off rank 0.  At stride 6000 without --single-window the profile windows are the
-    contig pass's own windows and their probabilities come out of that pass; otherwise a second pass classifies the list.
-    With `head`, the head's scores of the same windows are stored as head["window_preds"] (rank 0): the contig pass's own
-    rows, or the second pass's, which then takes the embedding route with the head (the same probabilities, bitwise)."""
-    emb = None
-    ak = {"attributions": attributions} if attributions is not None else {}      # option off: the call of before
-    if head is not None:
-        ak["head"] = head
-        head["windows"] = stride == sequence.WINDOW and not single_window
+def _classify_windows_of(clf, parsed, index, stride: int, single_window: bool, info, contig_reduce, req: ChunkRequest,
+                         window_novelty: bool = False):
+    """The contig pass of `req`, plus the class scores of every window at `stride` (and with a head, the head's scores and,
+    with `window_novelty`, its novelty rows): (ChunkResult, (offsets, starts, lengths) of those windows on rank 0).  At
+    stride 6000 without --single-window the profile windows are the contig pass's own windows and their rows come out of that
+    pass; otherwise a second pass over the window list collects them, with the head taking the embedding route (the same
+    probabilities, bitwise)."""
+    head = req.head is not None
     if stride == sequence.WINDOW and not single_window:
-        res = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=embeddings, window_probs=True, **ak)
-        preds, probs = res[0], res[-1]
-        if embeddings:
-            emb = res[1]
-        starts, lengths = parsed.spans() if info.is_main else (None, None)
-        return preds, emb, index.offsets, starts, lengths, probs
-    if embeddings:
-        preds, emb = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, embeddings=True, **ak)
-    else:
-        preds = _classify_parsed(clf, parsed, index.offsets, info, contig_reduce, **ak)
+        res = _chunk_pass(clf, parsed, index.offsets, info, contig_reduce,
+                          replace(req, window_probs=True, window_head=head, window_novelty=window_novelty))
+        return res, (index.offsets, *(parsed.spans() if info.is_main else (None, None)))
+    res = _chunk_pass(clf, parsed, index.offsets, info, contig_reduce, req)
     wl = parsed.windows(stride)
     try:
-        if head is not None:
-            profile = {"head": head["head"], "windows": True, "novelty": bool(head.get("window_novelty_wanted"))}
-            probs = _classify_parsed(clf, wl, None, info, window_probs=True, head=profile)
-            head["window_preds"] = profile["window_preds"]
-            if profile["novelty"]:
-                head["window_novelty"] = profile["window_novelty"]
-        else:
-            probs = _classify_parsed(clf, wl, None, info, window_probs=True)
-        offsets, starts, lengths = wl.spans() if info.is_main else (None, None, None)
+        prof = _chunk_pass(clf, wl, None, info, req=ChunkRequest(window_probs=True, head=req.head, window_head=head,
+                                                                 novelty=window_novelty, window_novelty=window_novelty))
+        spans = wl.spans() if info.is_main else (None, None, None)
     finally:
         wl.close()
-    return preds, emb, offsets, starts, lengths, probs
+    return replace(res, window_probs=prof.window_probs, head_window_preds=prof.head_window_preds,
+                   window_novelty=prof.window_novelty), spans
 
 
 ATTR_TOKENS = 5997
@@ -521,11 +536,7 @@ NOVELTY_TARGET = "nearest_class"
 def _write_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target: str, attr, steps: int = 0,
                         baseline: str = "zero", logp=None, extra=None) -> None:
     # np.savez, as for the embeddings: 24 KB of fp32 per window barely compresses
-    offsets = np.asarray(offsets, dtype=np.int32)
-    keys = {names_key: names,
-            "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
-            "window_start": np.asarray(starts, dtype=np.int64),
-            "window_length": np.asarray(lengths, dtype=np.int32),
+    keys = {names_key: names, **_window_coords(offsets, starts, lengths),
             "target": np.str_(target),
             "attributions": np.asarray(attr, dtype=np.float32).reshape(-1, ATTR_TOKENS)}
     if steps:                                       # integrated gradients; a gradient x input file keeps the keys above only
@@ -535,30 +546,17 @@ def _write_attributions(path: Path, names_key: str, names, offsets, starts, leng
     np.savez(path, **keys)
 
 
-def _attributions_current(path: Path, target: str, steps: int = 0, baseline: str = "zero") -> bool:
-    """The attributions file exists and was written for this class by this method (a file without "method" is gradient x
-    input), with these integrated-gradients steps and baseline."""
-    if not path.exists():
-        return False
-    try:
-        with np.load(path) as z:
-            if str(z["target"]) != target:
-                return False
-            method = str(z["method"]) if "method" in z.files else "gradient_x_input"
-            if not steps:
-                return method == "gradient_x_input"
-            return method == IG_METHOD and int(z["steps"]) == steps and str(z["baseline"]) == baseline
-    except Exception:
-        return False
+# the value of a key that an output file may lack: an attributions file without "method" is gradient x input
+_NPZ_ABSENT = {"method": "gradient_x_input"}
 
 
-def _head_attributions_current(path: Path, target: str, head_sha: str, steps: int = 0, baseline: str = "zero") -> bool:
-    """The head attributions file is current for this class, method, steps and baseline, and was written for this head."""
-    if not _attributions_current(path, target, steps, baseline):
+def _npz_current(paths, npz_path: Path, **keys) -> bool:
+    """Every file of `paths` exists and the NPZ file `npz_path` holds each of `keys` with that value."""
+    if not all(p.exists() for p in paths):
         return False
     try:
-        with np.load(path) as z:
-            return str(z["head_sha256"]) == head_sha
+        with np.load(npz_path) as z:
+            return all((z[k].item() if k in z.files else _NPZ_ABSENT.get(k)) == v for k, v in keys.items())
     except Exception:
         return False
 
@@ -568,10 +566,7 @@ def _write_head(npz_path: Path, tsv_path: Path, names_key: str, names, preds, cl
     preds = np.asarray(preds, dtype=np.float32).reshape(len(names), len(class_names))
     np.savez_compressed(npz_path, **{names_key: names, "predictions": preds, "class_names": np.array(class_names),
                                      "head_sha256": np.str_(head_sha)})
-    with open(tsv_path, "w") as fout:
-        fout.write("seq_name\t" + "\t".join(f"{c}_score" for c in class_names) + "\n")
-        for name, row in zip(names, preds):
-            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in row) + "\n")
+    _write_score_tsv(tsv_path, "seq_name\t" + "\t".join(f"{c}_score" for c in class_names) + "\n", names, preds)
 
 
 def _write_head_strands(npz_path: Path, tsv_path: Path, names_key: str, names, forward, reverse, class_names,
@@ -585,10 +580,8 @@ def _write_head_strands(npz_path: Path, tsv_path: Path, names_key: str, names, f
     both = both_strands(fwd, rev)
     np.savez_compressed(npz_path, **{names_key: names, "forward": fwd, "reverse": rev, "both_strands": both,
                                      "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)})
-    with open(tsv_path, "w") as fout:
-        fout.write("seq_name\t" + "\t".join(f"{c}_score_{s}" for s in STRANDS for c in class_names) + "\n")
-        for name, a, b, c in zip(names, fwd, rev, both):
-            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in (*a, *b, *c)) + "\n")
+    _write_score_tsv(tsv_path, "seq_name\t" + "\t".join(f"{c}_score_{s}" for s in STRANDS for c in class_names) + "\n",
+                     names, np.concatenate([fwd, rev, both], 1))
 
 
 _NOVELTY_HEADER = "seq_name\tnearest_class\tnovelty\tp_value\n"
@@ -615,18 +608,18 @@ def _write_head_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, d
                 fout.write(f"{name}\t{class_names[c]}\t{float(v):.6g}\t{float(pv):.6g}\n")
 
 
-def _write_novelty_attributions(path: Path, names_key: str, names, offsets, starts, lengths, rec, steps: int, baseline: str,
-                                class_names, head_sha: str) -> None:
+def _write_novelty_attributions(path: Path, names_key: str, names, offsets, starts, lengths, target_class, res: ChunkResult,
+                                steps: int, baseline: str, class_names, head_sha: str) -> None:
     """<prefix>_nn_classification_head_novelty_attributions.npz: the attribution file's keys with target "nearest_class",
     each window's target_class int32 [W] and distance float32 [W] (D of the window to that class), class_names, head_sha256;
     with integrated gradients also method, steps, baseline and distance_target float32 [W, 2] = (D_c(x), D_c(x'))."""
-    extra = {"target_class": np.asarray(rec["target_class"], dtype=np.int32),
-             "distance": np.asarray(rec["distance"], dtype=np.float32).reshape(-1),
+    extra = {"target_class": np.asarray(target_class, dtype=np.int32),
+             "distance": np.asarray(res.distance, dtype=np.float32).reshape(-1),
              "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)}
     if steps:
         extra.update({"method": np.str_(IG_METHOD), "steps": np.int32(steps), "baseline": np.str_(baseline),
-                      "distance_target": np.asarray(rec["logp"], dtype=np.float32).reshape(-1, 2)})
-    _write_attributions(path, names_key, names, offsets, starts, lengths, NOVELTY_TARGET, rec["attr"], extra=extra)
+                      "distance_target": np.asarray(res.logp, dtype=np.float32).reshape(-1, 2)})
+    _write_attributions(path, names_key, names, offsets, starts, lengths, NOVELTY_TARGET, res.attributions, extra=extra)
 
 
 def _write_window_novelty(npz_path: Path, tsv_path: Path, names_key: str, names, offsets, starts, lengths, dist, stride: int,
@@ -636,7 +629,6 @@ def _write_window_novelty(npz_path: Path, tsv_path: Path, names_key: str, names,
     index on ties; -1 and NaN for a row that is not all finite), window_stride, class_names and head_sha256.  The TSV holds
     the coordinates, the novelty and one distance column per class."""
     C = len(class_names)
-    offsets = np.asarray(offsets, dtype=np.int32)
     dist = np.asarray(dist, dtype=np.float32).reshape(-1, C)
     ok = np.isfinite(dist).all(1)
     nov = np.full(len(dist), np.nan, np.float32)
@@ -644,10 +636,7 @@ def _write_window_novelty(npz_path: Path, tsv_path: Path, names_key: str, names,
     if ok.any():
         nov[ok] = dist[ok].min(1)
         nearest[ok] = dist[ok].argmin(1)
-    np.savez(npz_path, **{names_key: names,
-                          "window_contig": np.repeat(np.arange(len(offsets) - 1, dtype=np.int32), np.diff(offsets)),
-                          "window_start": np.asarray(starts, dtype=np.int64),
-                          "window_length": np.asarray(lengths, dtype=np.int32),
+    np.savez(npz_path, **{names_key: names, **_window_coords(offsets, starts, lengths),
                           "window_stride": np.int32(stride),
                           "distances": dist, "novelty": nov, "nearest_class": nearest,
                           "class_names": np.array(class_names), "head_sha256": np.str_(head_sha)})
@@ -675,28 +664,6 @@ def _head_has_novelty(path) -> bool:
     try:
         with np.load(Path(path), allow_pickle=False) as z:
             return any(k in z.files for k in NOVELTY_KEYS)
-    except Exception:
-        return False
-
-
-def _head_windows_current(npz_path: Path, tsv_path: Path, head_sha: str, stride: int) -> bool:
-    """Both head window files exist and were written for this head at this stride."""
-    if not _head_current(npz_path, tsv_path, head_sha):
-        return False
-    try:
-        with np.load(npz_path) as z:
-            return int(z["window_stride"]) == stride
-    except Exception:
-        return False
-
-
-def _head_current(npz_path: Path, tsv_path: Path, head_sha: str) -> bool:
-    """Both head files exist and were written for the head file with this sha256."""
-    if not (npz_path.exists() and tsv_path.exists()):
-        return False
-    try:
-        with np.load(npz_path) as z:
-            return str(z["head_sha256"]) == head_sha
     except Exception:
         return False
 
@@ -777,10 +744,7 @@ def _write_strands(npz_path: Path, tsv_path: Path, names_key: str, names, forwar
     fwd, rev = np.asarray(forward, dtype=np.float32), np.asarray(reverse, dtype=np.float32)
     both = both_strands(fwd, rev)
     np.savez_compressed(npz_path, **{names_key: names, "forward": fwd, "reverse": rev, "both_strands": both})
-    with open(tsv_path, "w") as fout:
-        fout.write(_STRANDS_HEADER)
-        for name, a, b, c in zip(names, fwd, rev, both):
-            fout.write(f"{name}" + "".join(f"\t{float(x):.4f}" for x in (*a, *b, *c)) + "\n")
+    _write_score_tsv(tsv_path, _STRANDS_HEADER, names, np.concatenate([fwd, rev, both], 1))
 
 
 def _strands_current(npz_path: Path, tsv_path: Path, emb_path: Path, embeddings: bool) -> bool:
@@ -796,25 +760,13 @@ def _strands_current(npz_path: Path, tsv_path: Path, emb_path: Path, embeddings:
         return False
 
 
-def _classify_reverse(clf, parsed, single_window: bool, info, contig_reduce, embeddings: bool, head=None):
+def _classify_reverse(clf, parsed, single_window: bool, info, contig_reduce, req: ChunkRequest) -> ChunkResult:
     """The reverse strand: the windows of every record's reverse complement (sequence.WindowList, reverse=True) through the
     forward pass's chunk loop, per-contig reduction, embedding carry chain and multi-GPU routes.  A record keeps its row: it
-    has at least one window on either strand.  Returns (preds, embeddings or None).  With `head` ({"head": engine.Head}), the
-    list takes the embedding route with the head, as the forward pass does, and the head's per-contig means of the reverse
-    windows are stored as head["reverse_preds"] (float32 [n_contigs, C], identical on all ranks)."""
+    has at least one window on either strand."""
     wl = parsed.windows(sequence.WINDOW, single_window, reverse=True)
-    hk = {}
-    if head is not None:
-        hk["head"] = rev_head = {"head": head["head"]}
     try:
-        offsets = wl.spans()[0]
-        if embeddings:
-            res = _classify_parsed(clf, wl, offsets, info, contig_reduce, embeddings=True, **hk)
-        else:
-            res = _classify_parsed(clf, wl, offsets, info, contig_reduce, **hk), None
-        if head is not None:
-            head["reverse_preds"] = rev_head["preds"]
-        return res
+        return _contig_pass(clf, wl, wl.spans()[0], info, contig_reduce, req)
     finally:
         wl.close()
 
@@ -853,16 +805,35 @@ def contig_reduce_mode(default: str = "gather") -> str:
 _attribution_steps, _attribution_baseline = attribution_steps, attribution_baseline
 
 
-def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
-         write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
-         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None, write_head_attributions=None,
-         write_novelty_attributions=None, write_window_novelty=None):
-    import time as _time
-    t_start = _time.perf_counter()
-    last_timings.clear()
-    input_path, output_path = Path(input_path), Path(output_path)
-    info = gdist.init_process_group_if_needed()
-    is_main = info.is_main
+@dataclass(frozen=True)
+class _Options:
+    """nn-classification's options, parsed and checked once.  attr_kind is the one attribution file of the run: "classifier",
+    "head" or "novelty" (attr_target then is NOVELTY_TARGET); head_file and head_sha are set once the --head file is loaded."""
+    contig_reduce: str
+    embeddings: bool
+    strands: bool
+    window_scores: bool
+    stride: int
+    attr_kind: "str | None"
+    attr_target: "str | None"
+    steps: int
+    baseline: str
+    window_novelty: bool
+    head: object
+    head_novelty: bool
+    notes: tuple
+    threads: int
+    head_file: object = None
+    head_sha: "str | None" = None
+
+    @property
+    def attr_method(self) -> str:
+        return f", integrated gradients, {self.steps} steps, baseline {self.baseline}" if self.steps else ""
+
+
+def _parse_options(threads, contig_reduce, write_embeddings, write_window_scores, window_stride, write_attributions,
+                   attribution_steps, attribution_baseline, both_strands, head, write_head_attributions,
+                   write_novelty_attributions, write_window_novelty) -> _Options:
     contig_reduce = contig_reduce or contig_reduce_mode()
     write_embeddings = embeddings_enabled() if write_embeddings is None else bool(write_embeddings)
     strands = both_strands_enabled() if both_strands is None else bool(both_strands)
@@ -886,21 +857,195 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                          "--write-head-attributions: a run writes one attribution file")
     if window_nov and head is None:
         raise ValueError("--write-window-novelty needs --head: it scores the windows by the head's novelty model")
-    any_attr = bool(attr_target or head_attr_target or nov_attr)
+    attr_kind = "classifier" if attr_target else "head" if head_attr_target else "novelty" if nov_attr else None
     # both options are validated whether or not they take effect; an option without effect is reported in the log
     steps_opt, baseline_opt = _attribution_steps(attribution_steps), _attribution_baseline(attribution_baseline)
     baseline_given = attribution_baseline is not None or bool(os.environ.get("GENOMAD_B200_ATTRIBUTION_BASELINE", "").strip())
-    ig_notes = []
-    if not any_attr and (steps_opt or baseline_given):
-        ig_notes.append("--attribution-steps / --attribution-baseline have no effect without --write-attributions or "
-                        "--write-head-attributions.")
-    elif any_attr and baseline_given and not steps_opt:
-        ig_notes.append("--attribution-baseline has no effect with --attribution-steps 0 (gradient x input).")
-    ig_steps = steps_opt if any_attr else 0
-    ig_baseline = baseline_opt if ig_steps else "zero"
-    attr_method = f", integrated gradients, {ig_steps} steps, baseline {ig_baseline}" if ig_steps else ""
+    notes = []
+    if not attr_kind and (steps_opt or baseline_given):
+        notes.append("--attribution-steps / --attribution-baseline have no effect without --write-attributions or "
+                     "--write-head-attributions.")
+    elif attr_kind and baseline_given and not steps_opt:
+        notes.append("--attribution-baseline has no effect with --attribution-steps 0 (gradient x input).")
+    steps = steps_opt if attr_kind else 0
     if not 1 <= window_stride <= sequence.WINDOW:
         raise ValueError(f"window_stride must be in [1, {sequence.WINDOW}], not {window_stride}")
+    return _Options(contig_reduce=contig_reduce, embeddings=write_embeddings, strands=strands,
+                    window_scores=write_window_scores, stride=window_stride, attr_kind=attr_kind,
+                    attr_target={"classifier": attr_target, "head": head_attr_target, "novelty": NOVELTY_TARGET}.get(attr_kind),
+                    steps=steps, baseline=baseline_opt if steps else "zero", window_novelty=window_nov, head=head,
+                    head_novelty=head is not None and _head_has_novelty(head), notes=tuple(notes),
+                    threads=threads or 1)
+
+
+@dataclass(frozen=True)
+class _Job:
+    """One classification of the module: the input's sequences, or find-proviruses' proviruses.  Its output paths are the
+    NNOutputs properties of the sequence job's names with `prefix` in front."""
+    what: str
+    noun: str
+    fasta: Path
+    enc_dir: Path
+    id_path: Path
+    names_key: str
+    ids_key: str
+    must_have_windows: bool
+    outputs: NNOutputs
+    prefix: str
+
+    def path(self, name: str) -> Path:
+        return getattr(self.outputs, self.prefix + name)
+
+    @property
+    def label(self) -> str:                  # the reference's log wording (nn_classification.py:333, 351, 407, 425)
+        return "Sequence" if self.what == "sequence" else "Provirus"
+
+
+@dataclass
+class _Classified:
+    """One job's classification, as the writers read it on rank 0: the contig pass (fwd), the reverse strand's (rev), the
+    pass whose attributions are written (attr), the windows of the window files and of the attribution files (offsets,
+    starts, lengths), the head's window count per sequence and each window's novelty target class."""
+    names: object
+    fwd: ChunkResult
+    rev: "ChunkResult | None" = None
+    attr: "ChunkResult | None" = None
+    windows: tuple = (None, None, None)
+    spans: tuple = (None, None, None)
+    counts: "np.ndarray | None" = None
+    target_class: "np.ndarray | None" = None
+
+    @classmethod
+    def empty(cls, names, n_classes: int) -> "_Classified":
+        """A job without windows: zero scores and embeddings per sequence, no window rows."""
+        n, C = len(names), n_classes
+        rows = np.zeros((n, C), np.float32)
+        none = np.zeros((0, C), np.float32)
+        fwd = ChunkResult(preds=np.zeros((n, 3), np.float32), embeddings=np.zeros((n, 512), np.float32), head_preds=rows,
+                          novelty=rows, window_probs=np.zeros((0, 3), np.float32), head_window_preds=none,
+                          window_novelty=none, attributions=np.zeros((0, ATTR_TOKENS), np.float32),
+                          logp=np.zeros((0, 2), np.float32), distance=np.zeros(0, np.float32))
+        spans = (np.zeros(n + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32))
+        return cls(names, fwd, fwd, fwd, spans, spans, np.zeros(n, np.int64), np.zeros(0, np.int32))
+
+
+@dataclass(frozen=True)
+class _Product:
+    """One opt-in output of a job: the NNOutputs properties of its files (a .tsv is described as tabular, a .npz as binary),
+    when it is written, its header description and log line (str.format templates of _Product.fields), whether a previous
+    run's files are current, and its writer (rank 0)."""
+    files: tuple
+    enabled: object
+    descr: str
+    log: str
+    current: object
+    write: object
+
+    def fields(self, o: _Options, job: _Job) -> dict:
+        named = {job.path(f).suffix[1:]: job.path(f).name for f in self.files}
+        return {"p": "" if job.what == "sequence" else "provirus ", "noun": job.noun, "label": job.label, "stride": o.stride,
+                "target": o.attr_target, "method": o.attr_method, **named}
+
+
+def _attributions_keys(o: _Options, **keys) -> dict:
+    """The keys that make an attributions file current: its class, method and integrated-gradients steps and baseline."""
+    if not o.steps:
+        return {"target": o.attr_target, "method": "gradient_x_input", **keys}
+    return {"target": o.attr_target, "method": IG_METHOD, "steps": o.steps, "baseline": o.baseline, **keys}
+
+
+def _write_attributions_of(o: _Options, j: _Job, r: _Classified, npz: Path, extra=None) -> None:
+    _write_attributions(npz, j.names_key, r.names, *r.spans, o.attr_target, r.attr.attributions, o.steps, o.baseline,
+                        r.attr.logp, extra=extra)
+
+
+# Every opt-in output of a job, in the order the header lists them and the module writes them.  `current` and `write` take
+# the options, the job and (write) its _Classified, then the row's files.
+_PRODUCTS = (
+    _Product(("nn_classification_embeddings_output",), lambda o: o.embeddings,
+             "{noun} embeddings", "{label} embeddings in binary format written to {npz}.",
+             lambda o, j, npz: npz.exists(),
+             lambda o, j, r, npz: _write_embeddings(npz, j.names_key, r.names, r.fwd.embeddings,
+                                                    r.rev.embeddings if o.strands else None)),
+    _Product(("nn_classification_windows_output", "nn_classification_windows_npz_output"), lambda o: o.window_scores,
+             "{p}window classification", "{label} window scores (stride {stride}) written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, window_stride=o.stride),
+             lambda o, j, r, tsv, npz: _write_window_scores(npz, tsv, j.names_key, r.names, *r.windows, r.fwd.window_probs,
+                                                            o.stride, o.threads)),
+    _Product(("nn_classification_attributions_output",), lambda o: o.attr_kind == "classifier",
+             "{p}window attributions ({target}{method})",
+             "{label} window attributions ({target}{method}) in binary format written to {npz}.",
+             lambda o, j, npz: _npz_current((npz,), npz, **_attributions_keys(o)),
+             _write_attributions_of),
+    _Product(("nn_classification_strands_output", "nn_classification_strands_npz_output"), lambda o: o.strands,
+             "{p}classification of both strands", "{label} classification of both strands written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _strands_current(npz, tsv, j.path("nn_classification_embeddings_output"), o.embeddings),
+             lambda o, j, r, tsv, npz: _write_strands(npz, tsv, j.names_key, r.names, r.fwd.preds.astype(np.float32),
+                                                      r.rev.preds)),
+    _Product(("nn_classification_head_output", "nn_classification_head_npz_output"), lambda o: o.head is not None,
+             "{p}classification by the --head classifier", "{label} classification by the head written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, head_sha256=o.head_sha),
+             lambda o, j, r, tsv, npz: _write_head(npz, tsv, j.names_key, r.names, r.fwd.head_preds, o.head_file.class_names,
+                                                   o.head_sha)),
+    _Product(("nn_classification_head_strands_output", "nn_classification_head_strands_npz_output"),
+             lambda o: o.head is not None and o.strands,
+             "{p}classification of both strands by the --head classifier",
+             "{label} classification of both strands by the head written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, head_sha256=o.head_sha),
+             lambda o, j, r, tsv, npz: _write_head_strands(npz, tsv, j.names_key, r.names, r.fwd.head_preds,
+                                                           r.rev.head_preds, o.head_file.class_names, o.head_sha)),
+    _Product(("nn_classification_head_windows_output", "nn_classification_head_windows_npz_output"),
+             lambda o: o.head is not None and o.window_scores,
+             "{p}window classification by the --head classifier",
+             "{label} window scores of the head (stride {stride}) written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, head_sha256=o.head_sha, window_stride=o.stride),
+             lambda o, j, r, tsv, npz: _write_head_windows(npz, tsv, j.names_key, r.names, *r.windows,
+                                                           r.fwd.head_window_preds, o.stride, o.head_file.class_names,
+                                                           o.head_sha, o.threads)),
+    _Product(("nn_classification_head_novelty_output", "nn_classification_head_novelty_npz_output"),
+             lambda o: o.head_novelty,
+             "{p}novelty with respect to the --head classifier's classes",
+             "{label} novelty with respect to the head's classes (forward strand) written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, head_sha256=o.head_sha),
+             lambda o, j, r, tsv, npz: _write_head_novelty(npz, tsv, j.names_key, r.names, r.fwd.novelty, r.counts,
+                                                           o.head_file.novelty["novelty_calibration"],
+                                                           o.head_file.class_names, o.head_sha)),
+    _Product(("nn_classification_head_attributions_output",), lambda o: o.attr_kind == "head",
+             "{p}window attributions of the --head classifier ({target}{method})",
+             "{label} window attributions of the head ({target}{method}) in binary format written to {npz}.",
+             lambda o, j, npz: _npz_current((npz,), npz, **_attributions_keys(o, head_sha256=o.head_sha)),
+             lambda o, j, r, npz: _write_attributions_of(o, j, r, npz, extra={
+                 "head_sha256": np.str_(o.head_sha), "class_names": np.array(o.head_file.class_names)})),
+    _Product(("nn_classification_head_novelty_attributions_output",), lambda o: o.attr_kind == "novelty",
+             "{p}window attributions of the distance to the nearest class of the --head novelty model{method}",
+             "{label} window attributions of the distance to the nearest class{method} in binary format written to {npz}.",
+             lambda o, j, npz: _npz_current((npz,), npz, **_attributions_keys(o, head_sha256=o.head_sha)),
+             lambda o, j, r, npz: _write_novelty_attributions(npz, j.names_key, r.names, *r.spans, r.target_class, r.attr,
+                                                              o.steps, o.baseline, o.head_file.class_names, o.head_sha)),
+    _Product(("nn_classification_head_novelty_windows_output", "nn_classification_head_novelty_windows_npz_output"),
+             lambda o: o.window_novelty,
+             "{p}window novelty with respect to the --head classifier's classes",
+             "{label} window novelty (stride {stride}) written to {tsv} and {npz}.",
+             lambda o, j, tsv, npz: _npz_current((tsv, npz), npz, head_sha256=o.head_sha, window_stride=o.stride),
+             lambda o, j, r, tsv, npz: _write_window_novelty(npz, tsv, j.names_key, r.names, *r.windows,
+                                                             r.fwd.window_novelty, o.stride, o.head_file.class_names,
+                                                             o.head_sha, o.threads)),
+)
+
+
+def main(input_path, output_path, single_window, batch_size, restart, threads, verbose, cleanup, *, contig_reduce=None,
+         write_embeddings=None, write_window_scores=None, window_stride=None, write_attributions=None,
+         attribution_steps=None, attribution_baseline=None, both_strands=None, head=None, write_head_attributions=None,
+         write_novelty_attributions=None, write_window_novelty=None):
+    import time as _time
+    t_start = _time.perf_counter()
+    last_timings.clear()
+    input_path, output_path = Path(input_path), Path(output_path)
+    info = gdist.init_process_group_if_needed()
+    is_main = info.is_main
+    opts = _parse_options(threads, contig_reduce, write_embeddings, write_window_scores, window_stride, write_attributions,
+                          attribution_steps, attribution_baseline, both_strands, head, write_head_attributions,
+                          write_novelty_attributions, write_window_novelty)
     if is_main:
         utils.start_md5(input_path)                      # hashed in the background while the file is indexed (rank 0 only)
     if not output_path.is_dir() and is_main:
@@ -917,125 +1062,45 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     classify_proviruses = gdist.broadcast_object(
         utils.check_provirus_execution(prefix, input_path, output_path) if is_main else None, info)
 
-    files = [outputs.nn_classification_execution_info, outputs.encoded_sequences_dir,
-             outputs.nn_classification_output, outputs.nn_classification_npz_output]
-    descr = ["execution parameters", "directory containing encoded sequence data",
-             "contig classification: tabular format", "contig classification: binary format"]
-    if write_embeddings:
-        files.append(outputs.nn_classification_embeddings_output)
-        descr.append("contig embeddings: binary format")
-    if write_window_scores:
-        files += [outputs.nn_classification_windows_output, outputs.nn_classification_windows_npz_output]
-        descr += ["window classification: tabular format", "window classification: binary format"]
-    if attr_target:
-        files.append(outputs.nn_classification_attributions_output)
-        descr.append(f"window attributions ({attr_target}{attr_method}): binary format")
-    if strands:
-        files += [outputs.nn_classification_strands_output, outputs.nn_classification_strands_npz_output]
-        descr += ["classification of both strands: tabular format", "classification of both strands: binary format"]
-    if head is not None:
-        files += [outputs.nn_classification_head_output, outputs.nn_classification_head_npz_output]
-        descr += ["classification by the --head classifier: tabular format",
-                  "classification by the --head classifier: binary format"]
-    if head is not None and strands:
-        files += [outputs.nn_classification_head_strands_output, outputs.nn_classification_head_strands_npz_output]
-        descr += ["classification of both strands by the --head classifier: tabular format",
-                  "classification of both strands by the --head classifier: binary format"]
-    if head is not None and write_window_scores:
-        files += [outputs.nn_classification_head_windows_output, outputs.nn_classification_head_windows_npz_output]
-        descr += ["window classification by the --head classifier: tabular format",
-                  "window classification by the --head classifier: binary format"]
-    head_novelty = head is not None and _head_has_novelty(head)
-    if head_novelty:
-        files += [outputs.nn_classification_head_novelty_output, outputs.nn_classification_head_novelty_npz_output]
-        descr += ["novelty with respect to the --head classifier's classes: tabular format",
-                  "novelty with respect to the --head classifier's classes: binary format"]
-    if head_attr_target:
-        files.append(outputs.nn_classification_head_attributions_output)
-        descr.append(f"window attributions of the --head classifier ({head_attr_target}{attr_method}): binary format")
-    if nov_attr:
-        files.append(outputs.nn_classification_head_novelty_attributions_output)
-        descr.append(f"window attributions of the distance to the nearest class of the --head novelty model{attr_method}: "
-                     "binary format")
-    if window_nov:
-        files += [outputs.nn_classification_head_novelty_windows_output,
-                  outputs.nn_classification_head_novelty_windows_npz_output]
-        descr += ["window novelty with respect to the --head classifier's classes: tabular format",
-                  "window novelty with respect to the --head classifier's classes: binary format"]
+    jobs = [_Job("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
+                 "contig_names", "contig_ids", True, outputs, "")]
     if classify_proviruses:
-        files += [outputs.encoded_proviruses_dir, outputs.provirus_nn_classification_output,
-                  outputs.provirus_nn_classification_npz_output]
-        descr += ["directory containing encoded sequence data", "provirus classification: tabular format",
-                  "provirus classification: binary format"]
-        if write_embeddings:
-            files.append(outputs.provirus_nn_classification_embeddings_output)
-            descr.append("provirus embeddings: binary format")
-        if write_window_scores:
-            files += [outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_windows_npz_output]
-            descr += ["provirus window classification: tabular format", "provirus window classification: binary format"]
-        if attr_target:
-            files.append(outputs.provirus_nn_classification_attributions_output)
-            descr.append(f"provirus window attributions ({attr_target}{attr_method}): binary format")
-        if strands:
-            files += [outputs.provirus_nn_classification_strands_output, outputs.provirus_nn_classification_strands_npz_output]
-            descr += ["provirus classification of both strands: tabular format",
-                      "provirus classification of both strands: binary format"]
-        if head is not None:
-            files += [outputs.provirus_nn_classification_head_output, outputs.provirus_nn_classification_head_npz_output]
-            descr += ["provirus classification by the --head classifier: tabular format",
-                      "provirus classification by the --head classifier: binary format"]
-        if head is not None and strands:
-            files += [outputs.provirus_nn_classification_head_strands_output,
-                      outputs.provirus_nn_classification_head_strands_npz_output]
-            descr += ["provirus classification of both strands by the --head classifier: tabular format",
-                      "provirus classification of both strands by the --head classifier: binary format"]
-        if head is not None and write_window_scores:
-            files += [outputs.provirus_nn_classification_head_windows_output,
-                      outputs.provirus_nn_classification_head_windows_npz_output]
-            descr += ["provirus window classification by the --head classifier: tabular format",
-                      "provirus window classification by the --head classifier: binary format"]
-        if head_novelty:
-            files += [outputs.provirus_nn_classification_head_novelty_output,
-                      outputs.provirus_nn_classification_head_novelty_npz_output]
-            descr += ["provirus novelty with respect to the --head classifier's classes: tabular format",
-                      "provirus novelty with respect to the --head classifier's classes: binary format"]
-        if head_attr_target:
-            files.append(outputs.provirus_nn_classification_head_attributions_output)
-            descr.append(f"provirus window attributions of the --head classifier ({head_attr_target}{attr_method}): "
-                         "binary format")
-        if nov_attr:
-            files.append(outputs.provirus_nn_classification_head_novelty_attributions_output)
-            descr.append("provirus window attributions of the distance to the nearest class of the --head novelty model"
-                         f"{attr_method}: binary format")
-        if window_nov:
-            files += [outputs.provirus_nn_classification_head_novelty_windows_output,
-                      outputs.provirus_nn_classification_head_novelty_windows_npz_output]
-            descr += ["provirus window novelty with respect to the --head classifier's classes: tabular format",
-                      "provirus window novelty with respect to the --head classifier's classes: binary format"]
+        jobs.append(_Job("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
+                         outputs.provirus_window_id_output, "provirus_names", "provirus_ids", False, outputs, "provirus_"))
+    products = [p for p in _PRODUCTS if p.enabled(opts)]
+    files, descr = [outputs.nn_classification_execution_info], ["execution parameters"]
+    for job in jobs:
+        files += [job.enc_dir, job.path("nn_classification_output"), job.path("nn_classification_npz_output")]
+        descr += ["directory containing encoded sequence data", f"{job.noun} classification: tabular format",
+                  f"{job.noun} classification: binary format"]
+        for p in products:
+            files += [job.path(f) for f in p.files]
+            descr += [p.descr.format(**p.fields(opts, job)) + (": tabular format" if job.path(f).suffix == ".tsv"
+                                                               else ": binary format") for f in p.files]
     utils.display_header(console, __version__, "nn-classification",
                          "This will classify the input sequences into chromosome, plasmid, or virus based on the "
                          "nucleotide sequence.", outputs.nn_classification_dir, files, descr)
-    for note in ig_notes:
+    for note in opts.notes:
         console.log(f"Warning: {note}")
-    head_file = head_sha = None
     if head is not None:             # a head for another encoder (or a malformed file) is refused before any work
         try:
             head_file, head_sha = _load_head_file(head)
         except (OSError, ValueError, KeyError) as e:
             console.error(f"{head} is not a usable head file: {e}")
             sys.exit(1)
-        if head_attr_target is not None and head_attr_target not in head_file.class_names:
-            console.error(f"--write-head-attributions {head_attr_target}: not a class of {head} "
+        if opts.attr_kind == "head" and opts.attr_target not in head_file.class_names:
+            console.error(f"--write-head-attributions {opts.attr_target}: not a class of {head} "
                           f"({', '.join(head_file.class_names)})")
             sys.exit(1)
-        if (nov_attr or window_nov) and head_file.novelty is None:
-            opt = "--write-novelty-attributions" if nov_attr else "--write-window-novelty"
+        if (opts.attr_kind == "novelty" or opts.window_novelty) and head_file.novelty is None:
+            opt = "--write-novelty-attributions" if opts.attr_kind == "novelty" else "--write-window-novelty"
             console.error(f"{opt}: {head} carries no novelty model (train-head --novelty)")
             sys.exit(1)
+        opts = replace(opts, head_file=head_file, head_sha=head_sha)
     ig_clf = None
-    if ig_steps:                     # the steps must fit this device's attribution context: fail before any work
+    if opts.steps:                   # the steps must fit this device's attribution context: fail before any work
         ig_clf = _make_classifier(batch_size, info.local_rank)
-        _check_ig_steps_fit(ig_clf, ig_steps)
+        _check_ig_steps_fit(ig_clf, opts.steps)
 
     parsed_input = sequence.ParsedFasta(input_path, single_window, threads)      # one native index pass: check + windows
     last_timings["index_s"] = _time.perf_counter() - t_start
@@ -1044,38 +1109,6 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
                       "Please check your input FASTA file and execute genomad nn-classification again.")
         sys.exit(1)
     console.log("Executing genomad nn-classification.")
-
-    jobs = [("sequence", "contig", input_path, outputs.encoded_sequences_dir, outputs.seq_window_id_output,
-             "contig_names", "contig_ids", outputs.nn_classification_npz_output, outputs.nn_classification_output, True,
-             outputs.nn_classification_embeddings_output, outputs.nn_classification_windows_npz_output,
-             outputs.nn_classification_windows_output, outputs.nn_classification_attributions_output,
-             outputs.nn_classification_strands_npz_output, outputs.nn_classification_strands_output,
-             outputs.nn_classification_head_npz_output, outputs.nn_classification_head_output,
-             outputs.nn_classification_head_attributions_output,
-             outputs.nn_classification_head_strands_npz_output, outputs.nn_classification_head_strands_output,
-             outputs.nn_classification_head_windows_npz_output, outputs.nn_classification_head_windows_output,
-             outputs.nn_classification_head_novelty_npz_output, outputs.nn_classification_head_novelty_output,
-             outputs.nn_classification_head_novelty_attributions_output,
-             outputs.nn_classification_head_novelty_windows_npz_output,
-             outputs.nn_classification_head_novelty_windows_output)]
-    if classify_proviruses:
-        jobs.append(("provirus", "provirus", outputs.find_proviruses_nucleotide_output, outputs.encoded_proviruses_dir,
-                     outputs.provirus_window_id_output, "provirus_names", "provirus_ids",
-                     outputs.provirus_nn_classification_npz_output, outputs.provirus_nn_classification_output, False,
-                     outputs.provirus_nn_classification_embeddings_output, outputs.provirus_nn_classification_windows_npz_output,
-                     outputs.provirus_nn_classification_windows_output, outputs.provirus_nn_classification_attributions_output,
-                     outputs.provirus_nn_classification_strands_npz_output, outputs.provirus_nn_classification_strands_output,
-                     outputs.provirus_nn_classification_head_npz_output, outputs.provirus_nn_classification_head_output,
-                     outputs.provirus_nn_classification_head_attributions_output,
-                     outputs.provirus_nn_classification_head_strands_npz_output,
-                     outputs.provirus_nn_classification_head_strands_output,
-                     outputs.provirus_nn_classification_head_windows_npz_output,
-                     outputs.provirus_nn_classification_head_windows_output,
-                     outputs.provirus_nn_classification_head_novelty_npz_output,
-                     outputs.provirus_nn_classification_head_novelty_output,
-                     outputs.provirus_nn_classification_head_novelty_attributions_output,
-                     outputs.provirus_nn_classification_head_novelty_windows_npz_output,
-                     outputs.provirus_nn_classification_head_novelty_windows_output))
 
     plan = None
     info_writer = None
@@ -1092,27 +1125,13 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
         if not outputs.nn_classification_dir.is_dir():
             console.log(f"Creating the {outputs.nn_classification_dir} directory.")
             outputs.nn_classification_dir.mkdir()
-        # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten
-        # (with embeddings or window scores requested, a classification whose embeddings file is missing, or whose window
-        # scores are missing or were written at another stride, or whose attributions are missing or were written for another
-        # class, or whose strand files are missing, or whose head files are missing or were written for another head or
-        # stride, is redone: same predictions, bit for bit)
-        plan = [(bool(skip and j[4].exists()),
-                 bool(skip and j[7].exists() and (not write_embeddings or j[10].exists())
-                      and (not write_window_scores or _window_scores_current(j[11], j[12], window_stride))
-                      and (not attr_target or _attributions_current(j[13], attr_target, ig_steps, ig_baseline))
-                      and (not strands or _strands_current(j[14], j[15], j[10], write_embeddings))
-                      and (head_file is None or _head_current(j[16], j[17], head_sha))
-                      and (head_file is None or not strands or _head_current(j[19], j[20], head_sha))
-                      and (head_file is None or not write_window_scores
-                           or _head_windows_current(j[21], j[22], head_sha, window_stride))
-                      and (not head_attr_target
-                           or _head_attributions_current(j[18], head_attr_target, head_sha, ig_steps, ig_baseline))
-                      and (head_file is None or head_file.novelty is None or _head_current(j[23], j[24], head_sha))
-                      and (not nov_attr
-                           or _head_attributions_current(j[25], NOVELTY_TARGET, head_sha, ig_steps, ig_baseline))
-                      and (not window_nov or _head_windows_current(j[26], j[27], head_sha, window_stride))))
-                for j in jobs]
+        # per job: (skip the encoding stage, skip the classification) -- decided BEFORE anything is rewritten; a
+        # classification any of whose opt-in outputs is missing or was written for other options is redone (same
+        # predictions, bit for bit)
+        plan = [(bool(skip and job.id_path.exists()),
+                 bool(skip and job.path("nn_classification_npz_output").exists()
+                      and all(p.current(opts, job, *map(job.path, p.files)) for p in products)))
+                for job in jobs]
         # The execution info carries the input's md5 (aggregated-classification cross-checks it).  md5 is sequential
         # (~0.6 GB/s): writing the JSON here, as the reference does, would hold the GPUs back until the whole file is hashed,
         # so it is written by a helper thread as soon as the background hash is done and joined before main() returns.
@@ -1142,7 +1161,7 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     def head_scorer():
         nonlocal scorer
         if scorer is None:
-            scorer = _make_head(classifier(), head_file)
+            scorer = _make_head(classifier(), opts.head_file)
         return scorer
 
     if not all(cls_skip for _, cls_skip in plan) and ig_clf is None:
@@ -1151,182 +1170,56 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     # ---- stage 1, every job: "encode" (here: record the window -> sequence map; the windows themselves are streamed to the GPU in
     # stage 2).  Like the reference, sequences AND proviruses are encoded before either is classified (nn_classification.py:215-281).
     staged = []
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path, *_), \
-            (enc_skip, cls_skip) in zip(jobs, plan):
+    for job, (enc_skip, cls_skip) in zip(jobs, plan):
         parsed = index = None
         if enc_skip:
-            console.log(f"{enc_dir.name} was found. Skipping {what} encoding.")
+            console.log(f"{job.enc_dir.name} was found. Skipping {job.what} encoding.")
         else:
-            parsed = parsed_input if what == "sequence" else sequence.ParsedFasta(fasta, single_window, threads)
-            index = _encode_stage(console, enc_dir, id_path, names_key, ids_key, what, is_main, parsed, classifier)
+            parsed = parsed_input if job.what == "sequence" else sequence.ParsedFasta(job.fasta, single_window, threads)
+            index = _encode_stage(console, job.enc_dir, job.id_path, job.names_key, job.ids_key, job.what, is_main, parsed,
+                                  classifier)
         staged.append((parsed, index))
 
     # ---- stage 2, every job: classify, write NPZ, clean up, write TSV (nn_classification.py:283-353, 355-425)
-    for (what, noun, fasta, enc_dir, id_path, names_key, ids_key, npz_path, tsv_path, must_have_windows, emb_path,
-         win_npz_path, win_tsv_path, attr_path, strands_npz_path, strands_tsv_path, head_npz_path, head_tsv_path,
-         head_attr_path, head_strands_npz_path, head_strands_tsv_path, head_win_npz_path, head_win_tsv_path,
-         head_nov_npz_path, head_nov_tsv_path, nov_attr_path, win_nov_npz_path, win_nov_tsv_path), \
-            (enc_skip, cls_skip), (parsed, index) \
-            in zip(jobs, plan, staged):
-        names = preds = emb = None
-        rev_preds = rev_emb = None      # --both-strands: the reverse strand's scores and embeddings
-        attr = None                     # the contig pass runs through the attribution calls
-        if attr_target:
-            attr = {"target": attr_target, **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
-        elif head_attr_target:          # the same, through the head's attribution calls
-            attr = {"target": head_attr_target, "head": True,
-                    **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
-        win = None                      # (offsets, starts, lengths, probs) of the window scores, on rank 0
-        hd = None                       # --head: the chunk loop also scores every window with the head
-        label = "Sequence" if what == "sequence" else "Provirus"      # the reference's log wording (nn_classification.py:333, 351, 407, 425)
+    for job, (enc_skip, cls_skip), (parsed, index) in zip(jobs, plan, staged):
+        what, npz_path, tsv_path = job.what, job.path("nn_classification_npz_output"), job.path("nn_classification_output")
         # ---- classify
         if cls_skip:
             console.log(f"{npz_path.name} was found. Skipping {what} classification.")
+            names = preds = None
             if is_main:
                 z = np.load(npz_path)
-                names, preds = z[names_key], z["predictions"]
+                names, preds = z[job.names_key], z["predictions"]
         else:
             if parsed is None:
-                parsed = parsed_input if what == "sequence" else sequence.ParsedFasta(fasta, single_window, threads)
+                parsed = parsed_input if what == "sequence" else sequence.ParsedFasta(job.fasta, single_window, threads)
                 index = parsed.index()
             if parsed.n_windows == 0:
-                if must_have_windows:
+                if job.must_have_windows:
                     console.error("No sequences were found. Please check your input FASTA.")
                     if info_writer is not None:
                         info_writer.join()                    # the reference has written the JSON by this point
                     sys.exit(1)
-                names, preds = index.names, np.zeros((len(index.names), 3), np.float32)
-                if head_file is not None:
-                    C = len(head_file.class_names)
-                    hd = {"preds": np.zeros((len(index.names), C), np.float32), "window_preds": np.zeros((0, C), np.float32)}
-                    hd["reverse_preds"] = hd["preds"]
-                    hd["novelty_dist"], hd["counts"] = hd["preds"], np.zeros(len(index.names), np.int64)
-                    hd["window_novelty"] = hd["window_preds"]
-                emb = np.zeros((len(index.names), 512), np.float32)
-                win = (np.zeros(len(index.names) + 1, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int32),
-                       np.zeros((0, 3), np.float32))
-                if attr is not None:
-                    attr.update(attr=np.zeros((0, ATTR_TOKENS), np.float32), logp=np.zeros((0, 2), np.float32), spans=win[:3])
-                if nov_attr:
-                    nov_rec = {"attr": np.zeros((0, ATTR_TOKENS), np.float32), "logp": np.zeros((0, 2), np.float32),
-                               "distance": np.zeros(0, np.float32), "target_class": np.zeros(0, np.int32), "spans": win[:3]}
-                rev_preds, rev_emb = preds, emb
+                r = _Classified.empty(index.names, len(opts.head_file.class_names) if opts.head_file else 0)
             else:
-                t_c = _time.perf_counter()
-                ak = {"attributions": attr} if attr is not None else {}      # option off: the calls of before
-                if head_file is not None:
-                    hd = {"head": head_scorer()}
-                    if head_file.novelty is not None:
-                        hd["novelty"] = True
-                        hd["counts"] = np.diff(np.asarray(index.offsets, np.int64))
-                        hd["window_novelty_wanted"] = window_nov
-                    ak["head"] = hd
-                if write_window_scores or window_nov:
-                    preds, emb, *win = _classify_windows_of(classifier(), parsed, index, window_stride, single_window, info,
-                                                            contig_reduce, write_embeddings, **ak)
-                elif write_embeddings:
-                    preds, emb = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, embeddings=True, **ak)
-                else:
-                    preds = _classify_parsed(classifier(), parsed, index.offsets, info, contig_reduce, **ak)
-                if attr is not None:
-                    attr["spans"] = (index.offsets, *parsed.spans()) if is_main else None
-                if nov_attr:
-                    # a second pass over the contig pass's windows through the novelty attribution calls, each window
-                    # against its sequence's nearest class (head["novelty_dist"] is the same on every rank)
-                    t_n = _time.perf_counter()
-                    try:
-                        targets = _novelty_window_targets(hd["novelty_dist"], hd["counts"],
-                                                          head_file.novelty["novelty_calibration"], index.names)
-                    except Exception as e:
-                        console.error(str(e))
-                        sys.exit(1)
-                    nov_rec = {"target": NOVELTY_TARGET, "novelty": targets,
-                               **({"steps": ig_steps, "baseline": ig_baseline} if ig_steps else {})}
-                    _classify_parsed(classifier(), parsed, None, info, attributions=nov_rec, head={"head": head_scorer()})
-                    nov_rec["target_class"] = targets
-                    nov_rec["spans"] = (index.offsets, *parsed.spans()) if is_main else None
-                    last_timings[f"novelty_attributions_{what}_s"] = _time.perf_counter() - t_n
-                if strands:
-                    rev_preds, rev_emb = _classify_reverse(classifier(), parsed, single_window, info, contig_reduce,
-                                                           write_embeddings, head=hd)
-                last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
-                names = index.names
+                r = _classify_job(opts, classifier, head_scorer, parsed, index, single_window, info, what, console)
+            names, preds = r.names, r.fwd.preds
             console.log(f"{'Sequences' if what == 'sequence' else 'Proviruses'} classified.")
             if is_main:
-                np.savez_compressed(npz_path, **{names_key: names, "predictions": preds.astype(np.float32)})
-            console.log(f"{label} classification in binary format written to {npz_path.name}.")
-            if write_embeddings:
+                np.savez_compressed(npz_path, **{job.names_key: names, "predictions": preds.astype(np.float32)})
+            console.log(f"{job.label} classification in binary format written to {npz_path.name}.")
+            for p in products:
                 if is_main:
-                    _write_embeddings(emb_path, names_key, names, emb, rev_emb if strands else None)
-                console.log(f"{label} embeddings in binary format written to {emb_path.name}.")
-            if strands:
-                if is_main:
-                    _write_strands(strands_npz_path, strands_tsv_path, names_key, names, preds.astype(np.float32), rev_preds)
-                console.log(f"{label} classification of both strands written to {strands_tsv_path.name} and "
-                            f"{strands_npz_path.name}.")
-            if hd is not None:
-                if is_main:
-                    _write_head(head_npz_path, head_tsv_path, names_key, names, hd["preds"], head_file.class_names, head_sha)
-                console.log(f"{label} classification by the head written to {head_tsv_path.name} and {head_npz_path.name}.")
-                if strands:
-                    if is_main:
-                        _write_head_strands(head_strands_npz_path, head_strands_tsv_path, names_key, names, hd["preds"],
-                                            hd["reverse_preds"], head_file.class_names, head_sha)
-                    console.log(f"{label} classification of both strands by the head written to "
-                                f"{head_strands_tsv_path.name} and {head_strands_npz_path.name}.")
-                if head_file.novelty is not None:
-                    if is_main:
-                        _write_head_novelty(head_nov_npz_path, head_nov_tsv_path, names_key, names, hd["novelty_dist"],
-                                            hd["counts"], head_file.novelty["novelty_calibration"], head_file.class_names,
-                                            head_sha)
-                    console.log(f"{label} novelty with respect to the head's classes (forward strand) written to "
-                                f"{head_nov_tsv_path.name} and {head_nov_npz_path.name}.")
-            if window_nov:
-                if is_main:
-                    _write_window_novelty(win_nov_npz_path, win_nov_tsv_path, names_key, names, *win[:3], hd["window_novelty"],
-                                          window_stride, head_file.class_names, head_sha, threads or 1)
-                console.log(f"{label} window novelty (stride {window_stride}) written to {win_nov_tsv_path.name} and "
-                            f"{win_nov_npz_path.name}.")
-            if nov_attr:
-                if is_main:
-                    _write_novelty_attributions(nov_attr_path, names_key, names, *nov_rec["spans"], nov_rec, ig_steps,
-                                                ig_baseline, head_file.class_names, head_sha)
-                console.log(f"{label} window attributions of the distance to the nearest class{attr_method} in binary "
-                            f"format written to {nov_attr_path.name}.")
-            if write_window_scores:
-                if is_main:
-                    _write_window_scores(win_npz_path, win_tsv_path, names_key, names, *win, window_stride,
-                                         threads or 1)
-                console.log(f"{label} window scores (stride {window_stride}) written to {win_tsv_path.name} and "
-                            f"{win_npz_path.name}.")
-                if hd is not None:
-                    if is_main:
-                        _write_head_windows(head_win_npz_path, head_win_tsv_path, names_key, names, *win[:3],
-                                            hd["window_preds"], window_stride, head_file.class_names, head_sha, threads or 1)
-                    console.log(f"{label} window scores of the head (stride {window_stride}) written to "
-                                f"{head_win_tsv_path.name} and {head_win_npz_path.name}.")
-            if attr is not None and head_attr_target:
-                if is_main:
-                    _write_attributions(head_attr_path, names_key, names, *attr["spans"], head_attr_target, attr["attr"],
-                                        ig_steps, ig_baseline, attr.get("logp"),
-                                        extra={"head_sha256": np.str_(head_sha),
-                                               "class_names": np.array(head_file.class_names)})
-                console.log(f"{label} window attributions of the head ({head_attr_target}{attr_method}) in binary format "
-                            f"written to {head_attr_path.name}.")
-            elif attr is not None:
-                if is_main:
-                    _write_attributions(attr_path, names_key, names, *attr["spans"], attr_target, attr["attr"], ig_steps,
-                                        ig_baseline, attr.get("logp"))
-                console.log(f"{label} window attributions ({attr_target}{attr_method}) in binary format written to "
-                            f"{attr_path.name}.")
+                    p.write(opts, job, r, *map(job.path, p.files))
+                console.log(p.log.format(**p.fields(opts, job)))
         if parsed is not None:
             parsed.close()
-        if cleanup and is_main and enc_dir.is_dir():
+        if cleanup and is_main and job.enc_dir.is_dir():
             console.log(f"Deleting encoded {what} data.")
-            shutil.rmtree(enc_dir)
+            shutil.rmtree(job.enc_dir)
         if is_main:
             _write_tsv(tsv_path, names, preds)
-        console.log(f"{label} classification in tabular format written to {tsv_path.name}.")
+        console.log(f"{job.label} classification in tabular format written to {tsv_path.name}.")
 
     clf_pool.shutdown(wait=True)
     t_j = _time.perf_counter()
@@ -1336,3 +1229,47 @@ def main(input_path, output_path, single_window, batch_size, restart, threads, v
     gdist.barrier(info)
     last_timings["total_s"] = _time.perf_counter() - t_start                                   # rank 0 has written everything before any rank returns
     console.log("geNomad nn-classification finished!")
+
+
+def _classify_job(opts: _Options, classifier, head_scorer, parsed, index, single_window: bool, info, what: str,
+                  console) -> _Classified:
+    """The passes of one job with windows: the contig pass (with the window profile when window files are written), the
+    novelty attribution pass and the reverse strand."""
+    import time as _time
+    t_c = _time.perf_counter()
+    scorer = head_scorer() if opts.head is not None else None
+    clf = classifier()
+    att = None                       # the contig pass runs through the classifier's or the head's attribution calls
+    if opts.attr_kind in ("classifier", "head"):
+        att = AttributionSpec(opts.attr_target, opts.attr_kind == "head", steps=opts.steps, baseline=opts.baseline)
+    req = ChunkRequest(embeddings=opts.embeddings, head=scorer, novelty=opts.head_novelty, attribution=att)
+    windows = spans = (None, None, None)
+    counts = target_class = rev = None
+    if opts.window_scores or opts.window_novelty:
+        fwd, windows = _classify_windows_of(clf, parsed, index, opts.stride, single_window, info, opts.contig_reduce, req,
+                                            opts.window_novelty)
+    else:
+        fwd = _contig_pass(clf, parsed, index.offsets, info, opts.contig_reduce, req)
+    attr = fwd
+    if opts.attr_kind and info.is_main:
+        spans = (index.offsets, *parsed.spans())
+    if opts.head_novelty:
+        counts = np.diff(np.asarray(index.offsets, np.int64))
+    if opts.attr_kind == "novelty":
+        # a second pass over the contig pass's windows through the novelty attribution calls, each window against its
+        # sequence's nearest class (the per-contig novelty is the same on every rank)
+        t_n = _time.perf_counter()
+        try:
+            target_class = _novelty_window_targets(fwd.novelty, counts, opts.head_file.novelty["novelty_calibration"],
+                                                   index.names)
+        except Exception as e:
+            console.error(str(e))
+            sys.exit(1)
+        att = AttributionSpec(novelty_targets=target_class, steps=opts.steps, baseline=opts.baseline)
+        attr = _chunk_pass(clf, parsed, None, info, req=ChunkRequest(head=scorer, attribution=att))
+        last_timings[f"novelty_attributions_{what}_s"] = _time.perf_counter() - t_n
+    if opts.strands:
+        rev = _classify_reverse(clf, parsed, single_window, info, opts.contig_reduce,
+                                ChunkRequest(embeddings=opts.embeddings, head=scorer))
+    last_timings[f"classify_{what}_s"] = _time.perf_counter() - t_c          # incl. waiting for the CUDA context
+    return _Classified(index.names, fwd, rev, attr, windows, spans, counts, target_class)

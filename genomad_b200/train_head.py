@@ -307,7 +307,7 @@ def main(input_path, labels_path, output_path, epochs: int = 10, batch_size: int
         console.log(f"Computing the encoder embeddings of {W} windows.")
         row = 0
         for src, _ in strand_lists:
-            nnc._classify_parsed(clf, src, None, info, window_embeddings=X[row: row + src.n_windows])
+            nnc._chunk_pass(clf, src, None, info, req=nnc.ChunkRequest(window_embeddings=X[row: row + src.n_windows]))
             row += src.n_windows
     finally:
         if rev_list is not None:

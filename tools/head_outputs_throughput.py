@@ -42,7 +42,7 @@ def timed_train(torch, train_head, nnc, fa, labels, out, both):
     """(embedding s, [epoch s]) of one train-head run: the chunk-loop passes, each ended by a device synchronise, and the time
     from one epoch's weight read (after its last step) to the next, which covers a validation and an epoch's steps."""
     marks = {"embed": 0.0, "epochs": []}
-    classify = nnc._classify_parsed
+    classify = nnc._chunk_pass
 
     def classify_timed(*a, **k):
         t0 = time.perf_counter()
@@ -52,7 +52,7 @@ def timed_train(torch, train_head, nnc, fa, labels, out, both):
         marks["last"] = time.perf_counter()
         return r
 
-    nnc._classify_parsed = classify_timed
+    nnc._chunk_pass = classify_timed
     trainer_make = train_head._make_trainer
 
     def trainer_timed(*a, **k):
@@ -71,7 +71,7 @@ def timed_train(torch, train_head, nnc, fa, labels, out, both):
     try:
         train_head.main(fa, labels, out, epochs=3, batch_size=256, seed=0, verbose=False, both_strands=both)
     finally:
-        nnc._classify_parsed, train_head._make_trainer = classify, trainer_make
+        nnc._chunk_pass, train_head._make_trainer = classify, trainer_make
     return marks["embed"], marks["epochs"]
 
 

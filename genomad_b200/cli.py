@@ -215,15 +215,23 @@ def embedding_neighbours(query, output, reference, neighbours, both_strands, ind
 @click.option("--both-strands", is_flag=True, default=False, show_default=True,
               help="Cluster the mean of both strands' embeddings (embeddings_both_strands, written by nn-classification "
                    "--write-embeddings --both-strands), so a sequence and its reverse complement share a cluster.")
+@click.option("--index", "index", type=click.Path(path_type=Path, exists=True, dir_okay=False), default=None,
+              help="Cluster through this embedding-index file (embedding-index output) instead of comparing every sequence with "
+                   "every representative: a sequence is compared only with the representatives of its --nprobe nearest lists. "
+                   "The index must have been built on the INPUT file (with --both-strands if given here).")
+@click.option("--nprobe", type=int, default=None,
+              help="With --index: lists each sequence is compared in (1 to min(64, lists)); required with --index. At "
+                   "nprobe = lists the clusters are the exact ones.")
 @click.option("--verbose/--quiet", "-v/-q", is_flag=True, default=True, show_default=True,
               help="Display the execution log.")
-def embedding_clusters(input, output, min_similarity, both_strands, verbose):
+def embedding_clusters(input, output, min_similarity, both_strands, index, nprobe, verbose):
     """Cluster the sequences of the INPUT embeddings file (nn-classification --write-embeddings output) greedily, in file
     order, at a cosine similarity threshold of the encoder embeddings, and write each sequence's representative to the OUTPUT
     directory as <prefix>_embedding_clusters.{tsv,npz}. A representative is the first member of its cluster in file order.
     Not a module of the reference."""
     from . import embedding_clusters as module
-    module.main(input, output, min_similarity, verbose, both_strands=both_strands)
+    extra = {} if index is None and nprobe is None else {"index": index, "nprobe": nprobe}
+    module.main(input, output, min_similarity, verbose, both_strands=both_strands, **extra)
 
 
 @cli.command(name="embedding-map", context_settings=CONTEXT_SETTINGS)

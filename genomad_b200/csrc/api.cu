@@ -2173,9 +2173,11 @@ extern "C" size_t gnm_cluster_block_workspace_bytes(int64_t n_block) {
   return cl_mask_offset(n_block) + nb_align(static_cast<size_t>(n_block) * cl_words(n_block) * 4);
 }
 
-extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
-                                 int32_t* d_new_reps, int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream) {
-  const char* fn = "gnm_cluster_block";
+// d_probes null: every pair of the block is compared (gnm_cluster_block); else only pairs whose representative's home list is
+// one of the row's probes (gnm_cluster_block_probed)
+static int cluster_block_any(const char* fn, const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
+                             const int32_t* d_probes, int nprobe, const int32_t* d_home, int32_t* d_new_reps, int32_t* d_n_new,
+                             void* d_work, size_t work_bytes, cudaStream_t st) {
   if (n_block < 0 || n_block > kClMaxBlock)
     return fail(std::string(fn) + ": n_block must be in [0, " + std::to_string(kClMaxBlock) + "], not " + std::to_string(n_block));
   if (!(min_similarity > 0.f && min_similarity <= 1.f))
@@ -2187,7 +2189,6 @@ extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uin
   if (work_bytes < need)
     return fail(std::string(fn) + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(need) +
                 " needed (gnm_cluster_block_workspace_bytes)");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int n = static_cast<int>(n_block), words = cl_words(n);
   uint8_t* w = static_cast<uint8_t*>(d_work);
   float* hi = reinterpret_cast<float*>(w);
@@ -2209,10 +2210,31 @@ extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uin
     dim3 grid((rt + kClMaskTiles - 1) / kClMaskTiles, (n + kNbBM - 1) / kNbBM);
     nb_mask_kernel<<<grid, kNbThreads, kClMaskSmem, st>>>(tm[0], tm[1], tm[2], tm[3], p);
     GNM_CUDA(cudaGetLastError());
+    if (d_probes) {
+      const long long cells = static_cast<long long>(n) * words;
+      cl_probe_filter_kernel<<<static_cast<unsigned>((cells + 255) / 256), 256, 0, st>>>(mask, n, words, d_probes, nprobe, d_home);
+      GNM_CUDA(cudaGetLastError());
+    }
   }
   cl_resolve_kernel<<<1, kClThreads, 0, st>>>(mask, n, words, d_covered, d_new_reps, d_n_new);
   GNM_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
+                                 int32_t* d_new_reps, int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream) {
+  return cluster_block_any("gnm_cluster_block", d_rows, n_block, d_covered, min_similarity, nullptr, 0, nullptr, d_new_reps, d_n_new,
+                           d_work, work_bytes, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int gnm_cluster_block_probed(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
+                                        const int32_t* d_probes, int nprobe, const int32_t* d_home, int32_t* d_new_reps,
+                                        int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream) {
+  const char* fn = "gnm_cluster_block_probed";
+  if (nprobe < 1 || nprobe > kIvfMaxProbe) return fail(std::string(fn) + ": nprobe must be in [1, 64], not " + std::to_string(nprobe));
+  if (n_block > 0 && (!d_probes || !d_home)) return fail(std::string(fn) + ": null buffer");
+  return cluster_block_any(fn, d_rows, n_block, d_covered, min_similarity, d_probes, nprobe, d_home, d_new_reps, d_n_new, d_work,
+                           work_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // ------------------------------------------------------------------------------------------------ window regions (regions.cuh)
@@ -2903,7 +2925,8 @@ static int ivf_check(const char* fn, int64_t n_pairs, int64_t n_ref, const int64
 }
 
 // Every pair has at most the range count of the longest list, whatever the pairs are (duplicates included).
-static int ivf_plan(int64_t n_pairs, const int64_t* h_offsets, int lists, int k, IvfPlan* pl) {
+// grow: `off` also holds the lists' ends (gnm_ivf_search_ranges)
+static int ivf_plan(int64_t n_pairs, const int64_t* h_offsets, int lists, int k, IvfPlan* pl, bool grow = false) {
   IvfPlan p;
   long long max_nr = 0;
   for (int l = 0; l < lists; ++l) max_nr = std::max(max_nr, ivf_ranges(h_offsets[l + 1] - h_offsets[l]));
@@ -2926,7 +2949,7 @@ static int ivf_plan(int64_t n_pairs, const int64_t* h_offsets, int lists, int k,
   p.svals = o; o += nb_align(P * 4);
   p.slot = o; o += nb_align(P * 4);
   p.self = o; o += nb_align(P * 4);
-  p.off = o; o += nb_align(L1 * 8);
+  p.off = o; o += nb_align((grow ? L1 + lists : L1) * 8);
   p.pstart = o; o += nb_align(L1 * 4);
   p.items = o; o += nb_align(L1 * 8);
   p.ibase = o; o += nb_align(L1 * 8);
@@ -2948,27 +2971,28 @@ extern "C" size_t gnm_ivf_search_workspace_bytes(int64_t n_pairs, int64_t n_ref,
   return pl.bytes;
 }
 
-extern "C" int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list,
-                              int64_t n_pairs, const float* d_ref_hi, const float* d_ref_lo, int64_t n_ref, const int64_t* h_offsets,
-                              int lists, const int64_t* d_ref_index, int64_t self_index0, int k, float* d_sim, int64_t* d_idx,
-                              void* d_work, size_t work_bytes, void* stream) {
-  const char* fn = "gnm_ivf_search";
+// kGrow: list l holds the rows [h_offsets[l], d_end[l]) (gnm_ivf_search_ranges), else [h_offsets[l], h_offsets[l + 1])
+template <bool kGrow>
+static int ivf_search_any(const char* fn, const float* d_query, int64_t n_query, const int32_t* d_pair_query,
+                          const int32_t* d_pair_list, int64_t n_pairs, const float* d_ref_hi, const float* d_ref_lo, int64_t n_ref,
+                          const int64_t* h_offsets, const int64_t* d_end, int lists, const int64_t* d_ref_index, int64_t self_index0,
+                          int k, float* d_sim, int64_t* d_idx, void* d_work, size_t work_bytes, void* stream) {
   const std::string f(fn);
   if (ivf_check(fn, n_pairs, n_ref, h_offsets, lists, k)) return 1;
   if (n_query < 0 || n_query > kNbRowMax) return fail(f + ": n_query must be in [0, 2^30]");
   if (self_index0 < -1) return fail(f + ": self_index0 must be -1 (no self-exclusion) or >= 0");
   if (n_query == 0) return 0;
   if (!d_sim || !d_idx || (n_pairs > 0 && (!d_query || !d_pair_query || !d_pair_list || !d_work)) ||
-      (n_ref > 0 && (!d_ref_hi || !d_ref_lo || !d_ref_index)))
+      (n_ref > 0 && (!d_ref_hi || !d_ref_lo || !d_ref_index)) || (kGrow && n_pairs > 0 && !d_end))
     return fail(f + ": null buffer");
   if ((reinterpret_cast<uintptr_t>(d_query) | reinterpret_cast<uintptr_t>(d_ref_hi) | reinterpret_cast<uintptr_t>(d_ref_lo)) % 16)
     return fail(f + ": d_query, d_ref_hi and d_ref_lo must be 16-byte aligned");
   if (reinterpret_cast<uintptr_t>(d_work) % 256) return fail(f + ": d_work must be 256-byte aligned");
   IvfPlan pl;
-  if (ivf_plan(n_pairs, h_offsets, lists, k, &pl)) return 1;
+  if (ivf_plan(n_pairs, h_offsets, lists, k, &pl, kGrow)) return 1;
   if (n_pairs > 0 && work_bytes < pl.bytes)
-    return fail(f + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(pl.bytes) +
-                " needed (gnm_ivf_search_workspace_bytes)");
+    return fail(f + ": workspace too small: " + std::to_string(work_bytes) + " bytes, " + std::to_string(pl.bytes) + " needed (" + f +
+                "_workspace_bytes)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int nq = static_cast<int>(n_query), nr = static_cast<int>(n_ref), np = static_cast<int>(n_pairs);
   if (np == 0) {                                                  // no pair: every list padded
@@ -2987,12 +3011,16 @@ extern "C" int gnm_ivf_search(const float* d_query, int64_t n_query, const int32
   auto LL = [&](size_t o) { return reinterpret_cast<long long*>(w + o); };
   long long* off = LL(pl.off);
   GNM_CUDA(cudaMemcpyAsync(off, h_offsets, (static_cast<size_t>(lists) + 1) * 8, cudaMemcpyHostToDevice, st));
+  if (kGrow) {
+    ivf_ends_kernel<<<(lists + 255) / 256, 256, 0, st>>>(reinterpret_cast<const long long*>(d_end), lists, off);
+    GNM_CUDA(cudaGetLastError());
+  }
   ivf_keys_kernel<<<(np + 255) / 256, 256, 0, st>>>(d_pair_query, d_pair_list, np, nq, lists, U(pl.keys), I(pl.vals));
   GNM_CUDA(cudaGetLastError());
   size_t cb = pl.cub_bytes;
   GNM_CUDA(cub::DeviceRadixSort::SortPairs(w + pl.cub, cb, U(pl.keys), U(pl.skeys), I(pl.vals), I(pl.svals), np, 0, pl.bits, st));
-  ivf_lists_kernel<<<(lists + 1 + 255) / 256, 256, 0, st>>>(U(pl.skeys), np, off, lists, I(pl.pstart), LL(pl.items),
-                                                            LL(pl.cparts));
+  (kGrow ? ivf_grow_lists_kernel : ivf_lists_kernel)<<<(lists + 1 + 255) / 256, 256, 0, st>>>(U(pl.skeys), np, off, lists,
+                                                                                              I(pl.pstart), LL(pl.items), LL(pl.cparts));
   GNM_CUDA(cudaGetLastError());
   cb = pl.cub_bytes;
   GNM_CUDA(cub::DeviceScan::ExclusiveSum(w + pl.cub, cb, LL(pl.items), LL(pl.ibase), lists + 1, st));
@@ -3017,13 +3045,44 @@ extern "C" int gnm_ivf_search(const float* d_query, int64_t n_query, const int32
     p.off = off; p.pstart = I(pl.pstart); p.ibase = LL(pl.ibase); p.pbase = LL(pl.pbase); p.self_col = I(pl.self);
     p.lists = lists; p.k = k; p.status = nullptr;
     const int smem = nb_smem_bytes(k);
-    GNM_CUDA(cudaFuncSetAttribute(ivf_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ivf_search_kernel<<<sms, kNbThreads, smem, st>>>(tm[0], tm[1], tm[2], tm[3], p);   // persistent: items round robin
+    auto kernel = kGrow ? ivf_grow_search_kernel : ivf_search_kernel;
+    GNM_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    kernel<<<sms, kNbThreads, smem, st>>>(tm[0], tm[1], tm[2], tm[3], p);   // persistent: items round robin
     GNM_CUDA(cudaGetLastError());
   }
-  ivf_merge_kernel<<<(nq + 7) / 8, 256, 0, st>>>(F(pl.p_sim), I(pl.p_idx), d_pair_query, d_pair_list, np, I(pl.slot), off,
-                                                 I(pl.pstart), LL(pl.pbase), nq, k, reinterpret_cast<const long long*>(d_ref_index),
-                                                 d_sim, reinterpret_cast<long long*>(d_idx));
+  if (kGrow)
+    ivf_grow_merge_kernel<<<(nq + 7) / 8, 256, 0, st>>>(F(pl.p_sim), I(pl.p_idx), d_pair_query, d_pair_list, np, I(pl.slot), off, lists,
+                                                        I(pl.pstart), LL(pl.pbase), nq, k,
+                                                        reinterpret_cast<const long long*>(d_ref_index), d_sim,
+                                                        reinterpret_cast<long long*>(d_idx));
+  else
+    ivf_merge_kernel<<<(nq + 7) / 8, 256, 0, st>>>(F(pl.p_sim), I(pl.p_idx), d_pair_query, d_pair_list, np, I(pl.slot), off,
+                                                   I(pl.pstart), LL(pl.pbase), nq, k, reinterpret_cast<const long long*>(d_ref_index),
+                                                   d_sim, reinterpret_cast<long long*>(d_idx));
   GNM_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list,
+                              int64_t n_pairs, const float* d_ref_hi, const float* d_ref_lo, int64_t n_ref, const int64_t* h_offsets,
+                              int lists, const int64_t* d_ref_index, int64_t self_index0, int k, float* d_sim, int64_t* d_idx,
+                              void* d_work, size_t work_bytes, void* stream) {
+  return ivf_search_any<false>("gnm_ivf_search", d_query, n_query, d_pair_query, d_pair_list, n_pairs, d_ref_hi, d_ref_lo, n_ref,
+                               h_offsets, nullptr, lists, d_ref_index, self_index0, k, d_sim, d_idx, d_work, work_bytes, stream);
+}
+
+extern "C" size_t gnm_ivf_search_ranges_workspace_bytes(int64_t n_pairs, int64_t n_slots, const int64_t* h_offsets, int lists, int k) {
+  IvfPlan pl;
+  if (ivf_check("gnm_ivf_search_ranges_workspace_bytes", n_pairs, n_slots, h_offsets, lists, k) ||
+      ivf_plan(n_pairs, h_offsets, lists, k, &pl, true))
+    return 0;
+  return pl.bytes;
+}
+
+extern "C" int gnm_ivf_search_ranges(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list,
+                                     int64_t n_pairs, const float* d_slot_hi, const float* d_slot_lo, int64_t n_slots,
+                                     const int64_t* h_offsets, const int64_t* d_end, int lists, const int64_t* d_slot_index, int k,
+                                     float* d_sim, int64_t* d_idx, void* d_work, size_t work_bytes, void* stream) {
+  return ivf_search_any<true>("gnm_ivf_search_ranges", d_query, n_query, d_pair_query, d_pair_list, n_pairs, d_slot_hi, d_slot_lo,
+                              n_slots, h_offsets, d_end, lists, d_slot_index, -1, k, d_sim, d_idx, d_work, work_bytes, stream);
 }

@@ -10,6 +10,9 @@
 //                      representative and no mask bit (j, i) has i a representative of this block.  The 8 warps stage 32 mask rows
 //                      at a time in shared memory; warp 0 decides them in order, holding the block's representative bitmap in
 //                      registers (lane L: words L + 32 q).
+//   cl_probe_filter_kernel  (gnm_cluster_block_probed, between the two) clears mask bit (j, i) unless row i's home list is one of
+//                      row j's probes, so row j is compared only with the representatives its probed lists hold.  One thread per
+//                      mask word below the diagonal; only set bits are checked, and at a high threshold few are set.
 //
 // DESIGN.md, "Embedding clusters".
 #pragma once
@@ -81,6 +84,25 @@ nb_mask_kernel(const __grid_constant__ CUtensorMap tm_q_hi, const __grid_constan
       }
     }
   }
+}
+
+// mask word (j, w) with a column i < j: bit i kept iff home[i] is one of probes[j][0 .. nprobe)
+__global__ void __launch_bounds__(256) cl_probe_filter_kernel(uint32_t* __restrict__ mask, int n, int words,
+                                                              const int32_t* __restrict__ probes, int nprobe,
+                                                              const int32_t* __restrict__ home) {
+  const long long x = static_cast<long long>(blockIdx.x) * 256 + threadIdx.x;
+  if (x >= static_cast<long long>(n) * words) return;
+  const int j = static_cast<int>(x / words), w = static_cast<int>(x - static_cast<long long>(j) * words);
+  if (32 * w >= j) return;                                                 // no column i < j: not written by nb_mask_kernel
+  const uint32_t bits = mask[x];
+  uint32_t keep = bits;
+  for (uint32_t b = bits; b; b &= b - 1) {
+    const int i = 32 * w + __ffs(b) - 1, h = home[i];
+    bool probed = false;
+    for (int q = 0; q < nprobe && !probed; ++q) probed = probes[static_cast<size_t>(j) * nprobe + q] == h;
+    if (!probed) keep &= ~(1u << (i & 31));
+  }
+  if (keep != bits) mask[x] = keep;
 }
 
 __global__ void __launch_bounds__(kClThreads, 1)

@@ -132,6 +132,12 @@ EXPORTS = {
     "gnm_ivf_search": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                  C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                  C.c_void_p]),
+    "gnm_ivf_search_ranges_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int]),
+    "gnm_ivf_search_ranges": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+    "gnm_cluster_block_probed": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "gnm_cluster_block_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "gnm_cluster_block": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                     C.c_void_p]),
@@ -557,6 +563,7 @@ def ivf_search(query, reference, index: IvfIndex, k: int, nprobe: int, *, ref_in
 
 
 CLUSTER_MAX_BLOCK = 8192         # rows per gnm_cluster_block call: a threshold mask of 8 MB
+CLUSTER_SLOT_BYTES = 2 * EMBED * 4 + 8   # per representative slot: its TF32 halves and its global row index
 
 
 def cluster_threshold(min_similarity) -> float:
@@ -596,6 +603,128 @@ def cluster_block(rows, covered, min_similarity):
                                           work.data_ptr(), need, t.cuda.current_stream(x.device).cuda_stream))
         m = int(count.item())
     return reps[:m].long()
+
+
+def cluster_block_probed(rows, covered, min_similarity, probes, home):
+    """cluster_block, comparing row j only with the block's representatives i whose home list is one of j's probes
+    (gnm_cluster_block_probed): probes int32 cuda [n, nprobe] (the block rows' ivf_probes), home int32 cuda [n] (the list the
+    index places each block row in)."""
+    import torch as t
+    x = _neighbours_args(t, rows, "rows")
+    n = x.shape[0]
+    if n > CLUSTER_MAX_BLOCK:
+        raise ValueError(f"a block holds at most {CLUSTER_MAX_BLOCK} rows, not {n}")
+    assert covered.dtype == t.uint8 and covered.shape == (n,) and covered.device == x.device, \
+        "covered: uint8 tensor [n] on the rows' device expected"
+    assert probes.dtype == t.int32 and probes.dim() == 2 and probes.shape[0] == n and probes.device == x.device, \
+        "probes: int32 tensor [n, nprobe] on the rows' device expected"
+    assert home.dtype == t.int32 and home.shape == (n,) and home.device == x.device, "home: int32 tensor [n] expected"
+    thr = cluster_threshold(min_similarity)
+    cov, pr, hm = covered.contiguous(), probes.contiguous(), home.contiguous()
+    lib = load_library()
+    with t.cuda.device(x.device):
+        need = int(lib.gnm_cluster_block_workspace_bytes(n))
+        if need == 0 and n:
+            _check(lib, 1)
+        work = t.empty(need, dtype=t.uint8, device=x.device)
+        reps = t.empty(max(n, 1), dtype=t.int32, device=x.device)
+        count = t.empty(1, dtype=t.int32, device=x.device)
+        _check(lib, lib.gnm_cluster_block_probed(x.data_ptr(), n, cov.data_ptr(), thr, pr.data_ptr(), pr.shape[1], hm.data_ptr(),
+                                                 reps.data_ptr(), count.data_ptr(), work.data_ptr(), need,
+                                                 _stream(t, x.device)))
+        m = int(count.item())
+    return reps[:m].long()
+
+
+class ClusterSlots(NamedTuple):
+    """The slots of the representatives of lists [l0, l0 + m) of an index (gnm_ivf_search_ranges, include/gnm.h): list l0 + j owns
+    slots [offsets[j], offsets[j + 1]) and holds the representatives in slots [offsets[j], end[j]), in ascending row order."""
+    l0: int
+    offsets: np.ndarray       # host int64 [m + 1] from 0: the capacities, the index's list sizes
+    end: "object"             # cuda int64 [m]
+    hi: "object"              # cuda float32 [slots, 512]: the representatives' TF32 halves (gnm_ivf_prepare)
+    lo: "object"
+    index: "object"           # cuda int64 [slots]: their global rows
+
+
+def cluster_slots(offsets, l0: int, l1: int, device) -> ClusterSlots:
+    """Empty slots for the representatives of lists [l0, l1) of an index with these offsets (int64 [L + 1])."""
+    import torch as t
+    off = np.asarray(offsets, np.int64)[l0:l1 + 1]
+    off = np.ascontiguousarray(off - off[0])
+    cap = int(off[-1])
+    return ClusterSlots(int(l0), off, t.from_numpy(off[:-1].copy()).to(device),
+                        t.empty((cap, EMBED), dtype=t.float32, device=device), t.empty((cap, EMBED), dtype=t.float32, device=device),
+                        t.empty(cap, dtype=t.int64, device=device))
+
+
+def cluster_slots_counts(slots: ClusterSlots):
+    """The representatives each list holds: int64 cuda [m]."""
+    import torch as t
+    return slots.end - t.from_numpy(slots.offsets[:-1]).to(slots.end.device)
+
+
+def cluster_slots_append(slots: ClusterSlots, rows, gidx, home) -> None:
+    """Append new representatives: rows float32 cuda [r, 512] with global rows gidx (int64 [r], ascending, after every row the
+    slots hold) and home lists home (int [r]); those of other lists are skipped.  Only the new slots are written."""
+    import torch as t
+    m = slots.end.shape[0]
+    j = home.to(t.int64) - slots.l0
+    own = t.nonzero((j >= 0) & (j < m)).flatten()
+    if own.numel() == 0:
+        return
+    j = j[own]
+    order = t.sort(j, stable=True).indices
+    js = j[order]
+    rank = t.arange(js.numel(), device=js.device) - t.searchsorted(js, js)
+    pos = slots.end[js] + rank
+    x = _neighbours_args(t, rows.index_select(0, own[order]), "rows")
+    hi, lo = t.empty_like(x), t.empty_like(x)
+    lib = load_library()
+    with t.cuda.device(x.device):
+        _check(lib, lib.gnm_ivf_prepare(x.data_ptr(), x.shape[0], hi.data_ptr(), lo.data_ptr(), _stream(t, x.device)))
+    slots.hi.index_copy_(0, pos, hi)
+    slots.lo.index_copy_(0, pos, lo)
+    slots.index.index_copy_(0, pos, gidx[own[order]])
+    slots.end.add_(t.bincount(j, minlength=m))
+
+
+def cluster_slots_search(slots: ClusterSlots, query, probes):
+    """Each query's nearest representative among those of its probed lists that these slots hold (gnm_ivf_search_ranges at
+    k = 1): (sim float32 [nq, 1], idx int64 [nq, 1] global rows), cuda, (-inf, -1) where there is none.  probes: int32 cuda
+    [nq, nprobe]; lists outside the slots' are skipped.  The queries go in ranges of at most about IVF_QUERY_BYTES of workspace,
+    sized from the capacities, so no call waits for the device."""
+    import torch as t
+    q = _neighbours_args(t, query, "query")
+    nq, nprobe = probes.shape
+    dev = q.device
+    m = slots.end.shape[0]
+    sim = t.full((nq, 1), float("-inf"), dtype=t.float32, device=dev)
+    idx = t.full((nq, 1), -1, dtype=t.int64, device=dev)
+    if nq == 0 or slots.offsets[-1] == 0:
+        return sim, idx
+    lib = load_library()
+    off = slots.offsets
+    ws = lambda pairs: int(lib.gnm_ivf_search_ranges_workspace_bytes(pairs, int(off[-1]), _ptr(off), m, 1))
+    qc = nq
+    while qc > 1 and ws(qc * nprobe) > IVF_QUERY_BYTES:
+        qc = (qc + 1) // 2
+    need = ws(min(qc, nq) * nprobe)
+    if need == 0:
+        _check(lib, 1)
+    work = t.empty(need, dtype=t.uint8, device=dev)
+    pl_all = (probes.to(t.int32) - slots.l0).contiguous()
+    with t.cuda.device(dev):
+        stream = _stream(t, dev)
+        for a in range(0, nq, qc):
+            b = min(nq, a + qc)
+            pq = t.arange(b - a, dtype=t.int32, device=dev).repeat_interleave(nprobe)
+            pl = pl_all[a:b].reshape(-1)
+            _check(lib, lib.gnm_ivf_search_ranges(q[a:b].data_ptr(), b - a, pq.data_ptr(), pl.data_ptr(), pq.numel(),
+                                                  slots.hi.data_ptr(), slots.lo.data_ptr(), int(off[-1]), _ptr(off),
+                                                  slots.end.data_ptr(), m, slots.index.data_ptr(), 1, sim[a:b].data_ptr(),
+                                                  idx[a:b].data_ptr(), work.data_ptr(), need, stream))
+    return sim, idx
 
 
 MAP_A = 1.57694346               # 1 / (1 + a x^2b) least-squares fitted to umap-learn's curve at min_dist = 0.1, spread = 1

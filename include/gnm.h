@@ -660,6 +660,24 @@ int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_
                    size_t work_bytes, void* stream);
 
 /*
+ * Growing lists: the search of a clustering through an index (embedding-clusters --index), whose lists of representatives grow
+ * block by block.  The representatives live in slots laid out like the index: list l owns slots [h_offsets[l], h_offsets[l + 1])
+ * (HOST int64 [lists + 1] from 0 to n_slots, the index offsets: the capacities), and holds at any time the prefix
+ * [h_offsets[l], d_end[l]) (DEVICE int64 [lists], clamped to the list's slots), filled in ascending global index.  Appending
+ * writes only the new slots' halves (gnm_ivf_prepare): nothing placed earlier moves.
+ * gnm_ivf_search_ranges: gnm_ivf_search with list l read as [h_offsets[l], d_end[l]) and no self-exclusion; d_slot_hi / d_slot_lo
+ *   [n_slots][512] are the slots' halves, d_slot_index [n_slots] their global indices (read only inside the prefixes).  Same
+ *   pairs, order, padding and bitwise similarities as gnm_ivf_search; it runs the same kernels, instantiated to read d_end.
+ * gnm_ivf_search_ranges_workspace_bytes: as gnm_ivf_search_workspace_bytes, sized from the capacities, so it holds for any d_end
+ *   and the caller needs no device-to-host copy of the ends.
+ */
+size_t gnm_ivf_search_ranges_workspace_bytes(int64_t n_pairs, int64_t n_slots, const int64_t* h_offsets, int lists, int k);
+int gnm_ivf_search_ranges(const float* d_query, int64_t n_query, const int32_t* d_pair_query, const int32_t* d_pair_list,
+                          int64_t n_pairs, const float* d_slot_hi, const float* d_slot_lo, int64_t n_slots, const int64_t* h_offsets,
+                          const int64_t* d_end, int lists, const int64_t* d_slot_index, int k, float* d_sim, int64_t* d_idx,
+                          void* d_work, size_t work_bytes, void* stream);
+
+/*
  * Embedding clusters: one block step of greedy clustering at a cosine threshold t.  Rows are processed in file order, block by
  * block; row j is a representative iff s(j, i) < t for every representative i < j, where s(a, b) is the similarity
  * gnm_embedding_neighbours returns for QUERY row a and REFERENCE row b (s is not bitwise symmetric: the row being placed is
@@ -685,6 +703,22 @@ int gnm_ivf_search(const float* d_query, int64_t n_query, const int32_t* d_pair_
 size_t gnm_cluster_block_workspace_bytes(int64_t n_block);
 int gnm_cluster_block(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity, int32_t* d_new_reps,
                       int32_t* d_n_new, void* d_work, size_t work_bytes, void* stream);
+
+/*
+ * Clustering through an index (embedding-clusters --index; DESIGN.md, "Embedding clusters through the index").  With home(i) the
+ * list the index places row i in and P(j) row j's nprobe nearest centroids under the total order (P(j)[0] = home(j)):
+ *   row j is a representative iff s(j, i) < t for every representative i < j with home(i) in P(j);
+ *   every other row joins the first representative under the total order among the representatives i with home(i) in P(j).
+ * At nprobe = L this is the exact greedy clustering above.  The caller finds the covered rows with gnm_ivf_search_ranges at k = 1
+ * against the earlier blocks' representatives in the row's probed lists.
+ * gnm_cluster_block_probed: gnm_cluster_block, except that the in-block comparison (j, i) counts only when home(i) is one of j's
+ *   probes: d_probes DEVICE int32 [n_block][nprobe] (row j's probes), d_home DEVICE int32 [n_block], 1 <= nprobe <= 64.  The
+ *   threshold mask is the same; a filter kernel clears its other bits before the rows are decided.  Workspace:
+ *   gnm_cluster_block_workspace_bytes.
+ */
+int gnm_cluster_block_probed(const float* d_rows, int64_t n_block, const uint8_t* d_covered, float min_similarity,
+                             const int32_t* d_probes, int nprobe, const int32_t* d_home, int32_t* d_new_reps, int32_t* d_n_new,
+                             void* d_work, size_t work_bytes, void* stream);
 
 /*
  * Embedding map: the stages of a 2-D UMAP layout (McInnes, Healy & Melville 2018) of n rows, 2 <= n <= 2^30, as umap-learn
